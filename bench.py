@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- denoising steps/sec of the U-Net hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- denoising steps/sec of the U-Net hot path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|torch-gpu] [--workload cfg3|cfg2a|cfg1|cfg5]
     (N > 1: launched by torch.distributed.run, one rank per GPU)
@@ -13,8 +13,9 @@ Prints ONE JSON line (rank 0).
   value        whole-job steps/s with inputs resident in HBM: the captured step (CUDA graph) replayed K times, noise drawn
                on the device inside the graph, image / timestep updated in place.
   e2e          the same step driven with HOST (pinned) buffers: x, t and the noise copied in, x' copied out, every step.
-  roofline     the dominant kernel (tcgen05 3x3 implicit-GEMM convolution): ALGORITHMIC conv FLOPs of its launches divided
-               by their CUDA-event durations (launches timed one by one in an eager step), against MEASURED_PEAKS.json.
+  roofline     the dominant kernel (wgmma 3x3 implicit-GEMM convolution): ALGORITHMIC conv FLOPs of its launches divided
+               by their CUDA-event durations (launches timed one by one in an eager step), against MEASURED_PEAKS.json
+               (else the H100 SXM data-sheet dense FP16 rate).
   secondary    the other BASELINE.json configurations, same metric: cfg 1 (tiny), cfg 2a / 2b (base U-Net, weak, b=64/GPU),
                cfg 4 (cascade base64 + SR256, classifier-free guidance w=7, GLOBAL batch 128 = strong scaling: 128/N per
                GPU) and cfg 5 (SR 256->1024 dim=256, GLOBAL batch 16 = strong scaling), each with its whole-step fraction
@@ -25,6 +26,9 @@ Prints ONE JSON line (rank 0).
                autocast -- "the only existing kernels to beat on the same box" (SURVEY.md 2.1).
 `--impl reference` times the CPU path alone (the reference has no other implementation of this path); `--impl torch-gpu`
 prints the stock-PyTorch-on-GPU line alone.
+`--dump-outputs DIR` writes, after the timed steps, what the timed path returned in its last step as float32: with one GPU
+the image state x (DIR/x.npy), with several the all-gathered finalized images of every rank (DIR/images.npy).  Inputs,
+weights and the device noise are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -132,7 +136,7 @@ class ClockSampler:
 # ------------------------------------------------------------------------------------------------ CPU baseline
 def physical_cores():
     """Physical cores this process may run on: distinct SMT sibling sets among os.sched_getaffinity(0).  (One thread per
-    physical core: on the 2 x 32-core HT hosts of the B200 boxes 128 threads are ~200x slower than 64.)"""
+    physical core: on hosts with SMT, oversubscribing the hardware threads made the run ~200x slower.)"""
     cpus = sorted(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else list(range(os.cpu_count() or 1))
     sets = set()
     for c in cpus:
@@ -326,8 +330,10 @@ def main():
     ap.add_argument("--kernel-table", default=None, help="write a CUPTI per-kernel time table of 3 steps to this path")
     ap.add_argument("--pdl", type=int, default=None, help="programmatic dependent launch on (1) / off (0)")
     ap.add_argument("--profiler-range", action="store_true",
-                    help="cudaProfilerStart/Stop around the timed steps (for `ncu --profile-from-start off`: launch lists of exactly K steps)")
+                    help="cudaProfilerStart/Stop around the timed steps (launch lists of exactly K steps for an external profiler)")
     ap.add_argument("--gn-f16", action="store_true", help="GroupNorm inputs in fp16 (faster, 1.05e-3 instead of 9e-4 rel-L2)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the timed step's output of its last replay as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -341,7 +347,7 @@ def main():
     B = wl["batch"]
     config = {"workload": f"{args.workload}: {wl['desc']}", "batch_per_gpu": B, "global_batch": B * world,
               "image_size": wl["size"], "cond_scale": 1.0, "parallelism": f"dp{world} (batch-sharded sampling)",
-              "l2": "per-step working set (activations + 1.4 GB fp16 weights) >> 126 MB L2, no explicit flush needed",
+              "l2": "per-step working set (activations + 1.4 GB fp16 weights) >> 50 MB L2, no explicit flush needed",
               "algorithmic_gflop_per_image_forward": GFLOP_PER_IMG.get(args.workload)}
 
     # ------------------------------------------------------------------------------------ reference arm (CPU)
@@ -382,7 +388,7 @@ def main():
                           "torch_gpu": r}))
         return
 
-    # ------------------------------------------------------------------------------------ our arm (B200)
+    # ------------------------------------------------------------------------------------ our arm (H100)
     if world > 1:
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=dev)
@@ -403,8 +409,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
-    burst_tf = peaks.get("bf16_tflops") or 1650.0
+    peak_tf = peaks.get("bf16_tflops_sustained") or 989.0      # H100 SXM data sheet, dense FP16/BF16 (700 W)
+    burst_tf = peaks.get("bf16_tflops") or 989.0
 
     def build(wl_, base_cfg=None):
         """Imagen whose LAST U-Net is the one under test.  SR U-Nets sit behind a base stage (Imagen treats unets[0] as
@@ -451,7 +457,7 @@ def main():
         print(f"[bench] launches/step={launches_per_step}; first step (weight pack + allocator) {first_step_s:.2f} s, "
               f"eager step {eager_step_s * 1e3:.1f} ms", file=sys.stderr, flush=True)
 
-        # per-kernel timing of the dominant kernel (tcgen05 implicit GEMM): CUDA events around every launch of one eager step
+        # per-kernel timing of the dominant kernel (wgmma implicit GEMM): CUDA events around every launch of one eager step
         conv = measure_conv_kernels(imagen, unet, x, t_dev, shape, kw, dev)
 
         # steady state: the captured step, replayed (device-resident inputs, noise drawn inside the graph)
@@ -505,6 +511,12 @@ def main():
         assert torch.isfinite(state()).all(), "non-finite output"
         peak_mem = torch.cuda.max_memory_allocated(dev) / 2 ** 30
         print(f"[bench] device-resident: {ms / args.steps:.2f} ms/step", file=sys.stderr, flush=True)
+        if args.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            # one GPU: the step's image state; several: the timed path's all-gathered, finalized images of every rank
+            out = state() if world == 1 else gathered
+            np.save(os.path.join(args.dump_outputs, "x.npy" if world == 1 else "images.npy"), out.detach().float().cpu().numpy())
 
         if args.kernel_table and rank == 0:
             kernel_table(lambda: [replay() for _ in range(3)], 3, args.kernel_table)
@@ -672,7 +684,7 @@ def main():
             dt = (time.perf_counter() - t0) / 3
             row = {"ms_per_training_step": dt * 1e3, "batch": tb, "loss": float(loss.detach()), "params_m": sum(p.numel() for p in tu.parameters()) / 1e6,
                    "workload": f"base U-Net dim 128, mults (1,2,4), 64x64, b={tb}: Imagen.forward + backward + Adam step (eager; convs and the "
-                               "attention projections forward, data gradient and weight gradient on tcgen05 with fp16 operands; GroupNorm / "
+                               "attention projections forward, data gradient and weight gradient on wgmma with fp16 operands; GroupNorm / "
                                "LayerNorm / attention-core backward fp32)"}
             del loss        # a live loss keeps the parameters' gradient accumulators (bound to the default stream) alive: not capturable
             import gc
@@ -766,13 +778,6 @@ def main():
     d_achieved = d["alg_flops"] / (d["ms"] / 1000.0) / 1e12 if d["ms"] > 0 else 0.0
     a_achieved = a["alg_flops"] / (a["ms"] / 1000.0) / 1e12 if a["ms"] > 0 else 0.0
     traffic, traffic_src = None, None
-    for cand in ("r02_dominant_dram.json",):
-        try:
-            prof = json.load(open(os.path.join(ROOT, "profiles", cand)))
-            if args.workload == "cfg3" and B == 32 and prof.get("launches") == d["n"]:
-                traffic, traffic_src = prof["dram_bytes_per_launch"], cand
-        except Exception:
-            pass
     ms_step = ms / args.steps
     roofline = {"bound": "tensor",
                 "kernel": conv["dominant_name"],
@@ -781,8 +786,7 @@ def main():
                 "achieved": d_achieved, "peak": burst_tf, "unit": "TFLOP/s", "frac": d_achieved / burst_tf,
                 "frac_of_sustained_peak": d_achieved / peak_tf,
                 "traffic": traffic,
-                "traffic_unit": f"DRAM bytes per launch (ncu, profiles/{traffic_src})" if traffic_src else
-                                "null: no committed ncu DRAM capture matches this build's launch count",
+                "traffic_unit": "null: DRAM traffic is not measured",
                 "algorithmic_flops_per_launch": d["alg_flops"] / d["n"] if d["n"] else None,
                 "executed_flops_per_launch": d["exe_flops"] / d["n"] if d["n"] else None,
                 "algorithmic_bytes_per_launch": d["bytes"] / d["n"] if d["n"] else None,
@@ -798,7 +802,7 @@ def main():
                                       "executed_tflop_per_step": a["exe_flops"] / 1e12},
                 "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst, kernel timed alone) for `frac`; bf16_tflops_sustained "
                                "(kernel inside a long step) for `whole_step_frac` and `frac_of_sustained_peak`"
-                               if peaks else "fallback 1.65 / 1.4 PFLOP/s (B200_PROFILING.md)",
+                               if peaks else "fallback 989 TFLOP/s (H100 SXM data sheet, dense FP16, 700 W)",
                 "whole_step_tflops_per_gpu": step_tflops, "whole_step_frac": step_tflops / peak_tf,
                 "whole_step_peak": peak_tf}
     result = {
@@ -876,9 +880,9 @@ def kernel_table(fn, steps, path):
 
 
 def measure_conv_kernels(imagen, unet, x, t_dev, shape, kw, dev):
-    """Run one eager step with CUDA events around every tcgen05 conv launch.  Returns totals over all conv launches and,
-    separately, over the launches of the dominant kernel family (conv3x3_halo_t_kernel / its fused-GroupNorm form: 3x3 / 15x1
-    stride-1 convs with C_out % 128 == 0 on a 32x8- or 16x16-tileable grid -- the selection rule of csrc/conv_tc.cu).
+    """Run one eager step with CUDA events around every wgmma conv launch.  Returns totals over all conv launches and,
+    separately, over the launches of the dominant family (3x3 / 15x1 stride-1 convs and 2x2 sub-pixel phases with
+    C_out % 128 == 0 on a 32x8- or 16x16-tileable grid, the folded res_conv and fused-GroupNorm forms included).
     FLOPs are counted twice: ALGORITHMIC (what the reference's conv computes) and EXECUTED (what the lowering issues)."""
     from minimagen_b200 import ops as ops_mod
     real = ops_mod.get_ops()
@@ -887,8 +891,8 @@ def measure_conv_kernels(imagen, unet, x, t_dev, shape, kw, dev):
     stem_alg_per_pixel = sum(2.0 * c.kernel_size[0] ** 2 * c.in_channels * c.out_channels for c in stem.convs)
 
     def is_halo_t(H, W, c_out, kh, kw_, mode):
-        if 2 <= mode <= 5:          # sub-pixel phase on the swapped-operand kernel's Sub geometry
-            return c_out % 128 == 0 and H % 32 == 0 and W % 8 == 0 and W != 16 and not os.environ.get("MI_SUBPIX_PAIR")
+        if 2 <= mode <= 5:          # sub-pixel phase of the up-sampling conv
+            return c_out % 128 == 0 and H % 32 == 0 and W % 8 == 0 and W != 16
         return (mode == 0 and (kh, kw_) in ((3, 3), (15, 1)) and c_out % 128 == 0 and
                 ((W == 16 and H % 16 == 0 and kh == 3) or (H % 32 == 0 and W % 8 == 0 and W != 16)))
 
@@ -959,11 +963,11 @@ def measure_conv_kernels(imagen, unet, x, t_dev, shape, kw, dev):
         for key in (("all", "dominant") if dom else ("all",)):
             r = res[key]
             r["ms"] += ms; r["alg_flops"] += alg; r["exe_flops"] += exe; r["n"] += 1; r["bytes"] += nb
-    res["dominant_name"] = ("conv3x3_halo_t_kernel family (tcgen05 swapped-operand halo conv: 3x3, 3x3 + folded 1x1 res_conv, 15x1 "
-                            "stem, 2x2 sub-pixel phases; incl. the fused GroupNorm-prologue form when enabled)")
+    res["dominant_name"] = ("conv_wg_kernel, 3x3-class launches (3x3, 3x3 + folded 1x1 res_conv, 15x1 stem, 2x2 sub-pixel "
+                            "phases; incl. the fused GroupNorm-prologue form when enabled)")
     if res["dominant"]["n"] == 0:
         res["dominant"] = res["all"]
-        res["dominant_name"] = "tcgen05 implicit-GEMM convolutions (all launches)"
+        res["dominant_name"] = "wgmma implicit-GEMM convolutions (all launches)"
     return res
 
 

@@ -1,5 +1,5 @@
 /*
- * minimagen_b200 -- C ABI of the B200-native (sm_100a) kernels behind MinImagen's U-Net denoising hot path.
+ * minimagen_b200 -- C ABI of the H100-native (sm_90a) kernels behind MinImagen's U-Net denoising hot path.
  *
  * This header is the drop-in boundary: plain `extern "C"` entry points, raw device pointers + sizes + a CUDA stream
  * (passed as void*), no torch types.  The reference is pure Python/PyTorch, so the "FFI" a maintainer would bind is
@@ -48,7 +48,7 @@ int mi_pack_conv_weight_f16(const float* w_oihw, int c_out, int c_in, int kh, in
 int mi_pack_conv_weight_dgrad_f16(const float* w_oihw, int c_out, int c_in, int kh, int kw, void* out_f16, void* stream);
 
 /* ------------------------------------------------------------------------------------------------- convolution
- * Tensor-core (tcgen05 + TMA + TMEM) implicit-GEMM convolution / linear layer.
+ * Tensor-core (wgmma + TMA) implicit-GEMM convolution / linear layer.
  * Replaces nn.Conv2d / nn.Linear forward at: layers.py:129,145 (Block.project 3x3), layers.py:415,439 (res_conv 1x1),
  * layers.py:319 (Downsample 4x4 stride 2), layers.py:514 (Upsample conv 3x3), layers.py:157,160 (ChanFeedForward 1x1),
  * layers.py:41-42,48 and :213-214,217 (attention to_q / to_kv / to_out), Unet.py:234 (Parallel 3x3 + 1x1).
@@ -89,14 +89,14 @@ int mi_conv2d_igemm_f16(const void* act_f16, int B, int H, int W, int lda, int c
                         const float* bias, const float* residual, float* out_f32, void* out_f16, double* out_stats,
                         long long out_sb, long long out_sh, long long out_sw, long long out_sc, int n_valid,
                         int block_n, int* err_flag, void* workspace, long long workspace_bytes, void* stream);
-/* ResnetBlock.forward's tail (layers.py:437-439)  block2.project(h) + res_conv(x)  as ONE launch of the swapped-operand 3x3
+/* ResnetBlock.forward's tail (layers.py:437-439)  block2.project(h) + res_conv(x)  as ONE launch of the implicit-GEMM
  * kernel: after the nine taps of the 3x3 conv over `act` (the GroupNorm/SiLU operand of block2), the 1x1 res_conv rides in the
- * same accumulator as x_cin/64 extra K chunks read at the centre tap of x's halo tile -- no separate 1x1 launch, no fp32
+ * same accumulator as x_cin/64 extra K chunks read at the centre tap of x -- no separate 1x1 launch, no fp32
  * round trip of the residual branch through HBM.  w_f16 = [c_out][9*c_in + x_cin]: each row is the packed 3x3 weight followed
  * by the 1x1 weight; bias = the sum of both convs' biases.  Both operands may be virtual concats (act2 / x_act2 hold channels
  * >= c_in1 / x_cin1, the skip scale folded into the weight columns).  Outputs [B][H][W][c_out] contiguous; residual, out_stats
  * as mi_conv2d_igemm_f16.  Requirements: mi_conv3x3_res1x1_supported (H % 32 == 0 and W % 8 == 0, or W == 16 and H % 16 == 0;
- * c_in % 64 == 0, x_cin % 64 == 0, c_out % 128 == 0). */
+ * c_in % 64 == 0, x_cin % 64 == 0, c_out % 128 == 0, and the grid tileable into 128-pixel tiles). */
 int mi_conv3x3_res1x1_supported(int H, int W, int c_in, int c_out, int x_cin);
 int mi_conv3x3_res1x1_f16(const void* act_f16, int B, int H, int W, int lda, int c_in, const void* act2_f16, int lda2,
                           int c_in1, const void* x_f16, int ldx, int x_cin, const void* x2_f16, int ldx2, int x_cin1,
@@ -107,13 +107,13 @@ int mi_conv3x3_res1x1_f16(const void* act_f16, int B, int H, int W, int lda, int
 long long mi_conv2d_igemm_workspace_bytes(void);
 
 /* Fused Block.forward (layers.py:131-145): GroupNorm -> (scale + 1, shift) -> SiLU -> Conv2d 3x3 in ONE kernel; the
- * normalised tensor never exists in HBM.  The swapped-operand 3x3 halo convolution (weights = M, 256 pixels = N) with the TMA
- * load of its activation halo replaced by a prologue: eight warps read the raw fp32 NHWC input (optionally the virtual
+ * normalised tensor never exists in HBM.  The implicit-GEMM convolution with the TMA load of its
+ * activation tile replaced by a prologue: the producer warpgroup reads the raw fp32 NHWC input (optionally the virtual
  * concat cat(src0, src1*scale1), Unet.py:445) straight from global memory, apply y = SiLU(x*A[b,c] + B[b,c]) (GroupNorm
  * mean/rstd from the producers' 16-channel block statistics stats0/stats1 = out_stats of the convs that wrote src0/src1,
- * affine, FiLM and skip scale folded into A, B) and write the fp16 operand directly in the 128B-swizzled layout tcgen05.mma
+ * affine, FiLM and skip scale folded into A, B) and write the fp16 operand directly in the 128B-swizzled layout wgmma
  * reads; zero padding is applied to the ACTIVATED tensor.  Epilogue as mi_conv2d_igemm_f16 (bias, fp32 residual, fp32/fp16
- * outputs [B][H][W][c_out] contiguous, out_stats).  Requirements: mi_conv3x3_gn_supported (H % 32 == 0, W % 8 == 0,
+ * outputs [B][H][W][c_out] contiguous, out_stats).  Requirements: mi_conv3x3_gn_supported (H % 32 == 0, W % 8 == 0, H*W >= 128,
  * c0 % 64 == 0, c1 % 64 == 0, c_out % 128 == 0, (c0+c1)/groups % 16 == 0). */
 int mi_conv3x3_gn_supported(int H, int W, int c0, int c1, int c_out, int groups);
 int mi_conv3x3_gn_silu_f16(const float* src0, int c0, const float* src1, int c1, float scale1, int B, int H, int W,
@@ -208,12 +208,11 @@ int mi_resize_separable(const float* in, long long planes, int h_in, int w_in, f
  * multi-query Attention.forward (layers.py:52-104) with kv_head_stride = 0.  q must already carry the dim_head**-0.5
  * scale.  Key 0 is the learned null_kv [2][64] fp32 (layers.py:65-67,232-235); key_mask: uint8 [B][m] or NULL
  * (masked_fill(~mask, -FLT_MAX), layers.py:92-95,242-245).  q/out: [B][n][ld] with head h at column h*64.
- * workspace (optional, 128-byte aligned, size from mi_attention_workspace_bytes): lends the tcgen05 kernels room for the
+ * workspace (optional, 128-byte aligned, size from mi_attention_workspace_bytes): lends the wgmma kernel room for the
  * null-prepended padded K, the transposed V and the key-validity bits (null key, key_mask, padding); it is used when
- * n % 128 == 0, m >= 128 and q is batch-contiguous (q_bs == n*ldq) -- S = QK^T and O = PV then run as tcgen05.mma with TMEM
- * accumulators in ONE sweep over the keys (lazily rescaled reference maximum), the softmax in between reads S from TMEM and
- * hands P to the second GEMM through tensor memory; two query tiles per CTA when n % 256 == 0.  Otherwise (or with workspace
- * NULL) a mma.sync kernel runs. */
+ * n % 128 == 0, m >= 128 and q is batch-contiguous (q_bs == n*ldq) -- S = QK^T and O = PV then run as wgmma with
+ * register accumulators and an online softmax in between (P stays in registers as the A operand of the second GEMM).
+ * Otherwise (or with workspace NULL) a mma.sync kernel runs. */
 long long mi_attention_workspace_bytes(int B, int heads, int kv_head_stride, int m);
 int mi_attention_fwd(const void* q_f16, long long q_bs, int ldq, const void* k_f16, const void* v_f16, long long kv_bs,
                      int ldkv, int kv_head_stride, const float* null_kv, const uint8_t* key_mask, int B, int heads,

@@ -1,4 +1,4 @@
-"""Cascaded text-to-image diffusion sampler, B200-native (reference: minimagen/Imagen.py).
+"""Cascaded text-to-image diffusion sampler, H100-native (reference: minimagen/Imagen.py).
 
 Same class surface as the reference's `Imagen` (constructor `Imagen.py:27-42`, `.sample` `:424-433`, `.forward` `:575-582`,
 `.device`, `.unets`, `.noise_schedulers`, `.lowres_noise_schedule`, `state_dict` / `load_state_dict` overrides), same
@@ -138,10 +138,10 @@ class Imagen(nn.Module):
         self.register_buffer('_temp', torch.tensor([0.]), persistent=False)
         self.to(next(self.unets.parameters()).device)
 
-        # B200 additions (not part of the reference surface)
+        # additions (not part of the reference surface)
         self.use_cuda_graph = True       # replay each denoising step from a captured CUDA graph
         self.noise_fn: Callable = None   # see module docstring
-        self.cfg_batched = False         # classifier-free guidance as ONE 2B-sample forward (not yet measured on B200)
+        self.cfg_batched = False         # classifier-free guidance as ONE 2B-sample forward (not measured)
         self._graphs = {}
         self.max_cached_graphs = 4
 
@@ -196,7 +196,7 @@ class Imagen(nn.Module):
     @contextmanager
     def _one_unet_in_gpu(self, unet_number=None, unet=None):
         """Reference behaviour (Imagen.py:235-259) moves every other U-Net to the CPU for the duration of a stage.
-        With 180 GB of HBM per B200 all U-Nets of the cascade stay resident (cfg 5's 2.85 B-parameter SR U-Net is
+        On an 80 GB H100 all U-Nets of the cascade stay resident (cfg 5's 2.85 B-parameter SR U-Net is
         11.4 GB in fp32), so this only makes sure the requested one is on the sampling device."""
         assert exists(unet_number) ^ exists(unet)
         if exists(unet_number):
@@ -497,10 +497,10 @@ class Imagen(nn.Module):
             return self.loss_fn(pred, noise)
 
     def graphed_train_step(self, optimizer, images, *, text_embeds, text_masks=None, unet_number: int = None, warmup: int = 3):
-        """B200-side addition (no reference counterpart): capture `loss = self(images, ...); loss.backward(); optimizer.step()`
+        """Addition without a reference counterpart: capture `loss = self(images, ...); loss.backward(); optimizer.step()`
         for this batch SHAPE in ONE CUDA graph and return `step(images, text_embeds, text_masks=None) -> loss` that copies a new
         batch into the graph's static buffers and replays it.  An eager step of this path is bound by its ~2000 host-side
-        launches (b = 8: 39 ms eager vs 18.5 ms replayed, `profiles/r02_train_step_vs_torch.txt`); the timestep / noise /
+        launches; the timestep / noise /
         conditioning-dropout draws are in-graph RNG calls, so every replay sees fresh randomness.  `optimizer` must be
         capturable (e.g. `torch.optim.Adam(params, lr, capturable=True)`); gradients are left in `.grad` after each step.
         Drop references to losses of earlier EAGER steps first (`del loss`): a live autograd graph keeps the parameters' gradient

@@ -1,11 +1,11 @@
-"""Denoising U-Net, B200-native (reference: minimagen/Unet.py).
+"""Denoising U-Net, H100-native (reference: minimagen/Unet.py).
 
 Same class surface as the reference -- constructor signature (`Unet.py:31-48`), attributes (`lowres_cond`, `channels`,
 `channels_out`, `text_embed_dim`, `max_text_len`, `_locals`), methods (`forward`, `forward_with_cond_scale`,
 `_cast_model_parameters`, `_generate_t_tokens`, `_text_condition`), presets (`Base`, `Super`, `BaseTest`, `SuperTest`)
 and an identical `state_dict()` key set, so checkpoints written by the reference load unchanged
-(`generate.py:102`) -- but `forward` executes hand-written sm_100a kernels through the C ABI
-(include/minimagen_b200.h): NHWC fp32 residual stream, fp16 tensor-core operands with fp32 TMEM accumulation.
+(`generate.py:102`) -- but `forward` executes hand-written sm_90a kernels through the C ABI
+(include/minimagen_b200.h): NHWC fp32 residual stream, fp16 tensor-core operands with fp32 accumulation.
 """
 from typing import Union
 
@@ -221,7 +221,7 @@ class Unet(nn.Module):
             main.wait_stream(s)
         return out
 
-    batch_streams = 1          # number of concurrent batch slices in forward (measured: no gain on B200, see DESIGN.md)
+    batch_streams = 1          # number of concurrent batch slices in forward
     min_chunk_batch = 8
 
     def _batch_chunks(self, B, is_cuda):

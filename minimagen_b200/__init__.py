@@ -1,4 +1,4 @@
-"""minimagen_b200 -- B200-native (sm_100a) implementation of MinImagen's U-Net denoising hot path.
+"""minimagen_b200 -- H100-native (sm_90a) implementation of MinImagen's U-Net denoising hot path.
 
 Drop-in module layout (same names as the reference package `minimagen`):
     minimagen_b200.Unet             Unet, Base, Super, BaseTest, SuperTest

@@ -4,7 +4,7 @@
 U-Net runs `minimagen_b200.train_path.unet_forward_train`, which is built from the Functions below.  Each Function's forward
 is the same kernel the sampling path uses (tensor-core implicit GEMM for tensor-core-shaped convs, fp32 kernels otherwise);
 each backward calls the backward entry points of the ABI (csrc/backward.cu) -- or, for the data gradient of a tensor-core-
-shaped 3x3 / 1x1 conv, the forward tcgen05 kernel itself on the flipped, in/out-transposed packed weight.
+shaped 3x3 / 1x1 conv, the forward wgmma kernel itself on the flipped, in/out-transposed packed weight.
 
 Activations here are plain fp32 NHWC tensors `[B, H, W, C]` (rows `[R, C]` for token ops); torch is only the tape.
 """
@@ -84,7 +84,7 @@ class Conv2dFn(torch.autograd.Function):
             dx = torch.empty_like(x)
             if tc and same and Cout % 64 == 0 and Cin % 16 == 0 and ops.igemm_supported(H, W, Cout, Cin):
                 # data gradient of a 'same' conv = the same conv of dy with the taps flipped and in/out channels swapped:
-                # runs on the forward tcgen05 implicit-GEMM kernel
+                # runs on the forward wgmma implicit-GEMM kernel
                 g16 = dy16()
                 ops.conv_igemm(g16, B, H, W, Cout, 0, Cout, ops.pack_conv_weight_dgrad(w), Cin, kh, kw, 0, None, None, dx, None,
                                (H * W * Cin, W * Cin, Cin))
@@ -107,7 +107,7 @@ class Conv2dFn(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             dw = torch.empty_like(w, memory_format=torch.contiguous_format)
             if tc and (same or down) and ops.conv_wgrad_tc_supported(Ho, Wo, Cin, Cout, kh, kw, stride):
-                # contraction over the pixels on tcgen05: fp16 NHWC dy and x are both MN-major operands (csrc/wgrad_tc.cu)
+                # contraction over the pixels on wgmma: fp16 NHWC dy and x are both MN-major operands (csrc/wgrad_tc.cu)
                 x16 = ctx.x16
                 if x16 is None:
                     x16 = torch.empty((B, 1, H, W, Cin), dtype=F16, device=x.device)
@@ -199,7 +199,7 @@ class LayerNormFn(torch.autograd.Function):
 class LinearFn(torch.autograd.Function):
     """y = x @ W^T + b on rows; x [M, K] fp32, W the nn.Linear weight [N, K].  Tensor-core-shaped problems (M >= 256, K % 64 == 0,
     N % 16 == 0: the attention projections over image tokens and over the text / time context) run as 1x1 convs of a
-    (Mp/128) x 128 "image" (Mp = M rounded up to 128 with zero rows) on the tcgen05 implicit-GEMM kernel with fp16 operands --
+    (Mp/128) x 128 "image" (Mp = M rounded up to 128 with zero rows) on the wgmma implicit-GEMM kernel with fp16 operands --
     forward, dX (transposed packed weight) and dW (contraction over the rows on the weight-gradient kernel, csrc/wgrad_tc.cu);
     everything else (time / text MLPs on B rows, ragged widths) stays fp32."""
 

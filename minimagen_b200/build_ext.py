@@ -1,7 +1,7 @@
-"""In-tree build of the sm_100a kernel library (no torch involved): nvcc -> minimagen_b200/lib/libminimagen_b200.so.
+"""In-tree build of the sm_90a kernel library (no torch involved): nvcc -> minimagen_b200/lib/libminimagen_b200.so.
 
-nvcc cross-compiles without a GPU, so this runs on the CPU-only build container; the resulting .so travels to the GPU
-box with the repo snapshot.  Rebuilds only when a source is newer than the library.
+nvcc cross-compiles without a GPU, so the library can be built on a machine without one.  Rebuilds only when a source
+is newer than the library.
 """
 import os
 import subprocess
@@ -11,8 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libminimagen_b200.so")
-SOURCES = ["capi.cu", "conv_tc.cu", "conv_gn.cu", "conv_gn_pair.cu", "conv_direct.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "step.cu", "backward.cu", "wgrad_tc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+SOURCES = ["capi.cu", "conv_tc.cu", "conv_direct.cu", "elementwise.cu", "attention.cu", "attention_tc.cu", "step.cu", "backward.cu", "wgrad_tc.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

@@ -4,7 +4,7 @@
 // One kernel: S = Q K^T (Q pre-scaled by dim_head^-0.5 via the packed to_q weight), optional key mask
 // (masked_fill(~mask, -FLT_MAX), null key never masked), softmax in fp32 (online / flash style, the b x h x n x j score
 // tensor the reference materialises is never written), O = P V.  Tensor-core math via mma.sync.m16n8k16 (fp16 in,
-// fp32 accumulate); the GEMM-heavy projections around it run on the tcgen05 path (conv_tc.cu).
+// fp32 accumulate); the GEMM-heavy projections around it run on the wgmma path (conv_tc.cu).
 //
 // CTA = 4 warps = 64 query rows of one (batch, head); key blocks of 64 staged in shared memory (V transposed).
 #include <cuda_fp16.h>

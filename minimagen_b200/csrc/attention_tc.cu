@@ -1,63 +1,45 @@
-// Attention core on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), head dim 64, no mask.
+// Attention core on the Hopper tensor cores (wgmma + TMA + mbarrier), head dim 64.
 //
 // Replaces the softmax(q k^T) v core of Attention.forward (layers.py:56-104; one shared k/v head = multi-query) and
 // CrossAttention.forward (layers.py:226-251; per-head k/v over the text tokens), both with the learned null key/value
 // prepended (layers.py:67-70, :240-242).  q arrives pre-scaled (dim_head**-0.5 folded into to_q).
 //
-// One CTA = 128 queries of one (batch, head).  Keys are processed in blocks of 128:
-//   S = Q K_j^T        tcgen05.mma  M = 128 queries, N = 128 keys, K = 64   -> TMEM (fp32, double-buffered)
-//   P = exp(S - max)   16 softmax warps: one query row x 32 / 64 keys per thread (tcgen05.ld), fp16 P written back to
-//                      TENSOR MEMORY (tcgen05.st, two keys per 32-bit column) where the next MMA reads it as its A operand
-//   O += P V_j         tcgen05.mma  M = 128 queries, N = 64, K = 128 keys, A from TMEM    -> TMEM
-// (P used to go through shared memory: 64 KB written and 64 KB re-read per key block on the 128 B/clk port, and an N = 64 MMA
-// with A in shared memory costs ~119 clk against the 32-clk floor it reaches with A in tensor memory.)
-// ONE sweep over the keys (kOnline, the default): P is taken relative to a per-row REFERENCE maximum m_ref that is only
-// raised -- and O (in TMEM) and the partial row sums rescaled by exp(m_old - m_new) -- when some row of the CTA sees a score
-// more than 2^8 above its reference (lazy rescaling: P stays <= 256, far inside fp16; the decision is one `bar.red.or` per
-// key block, the rescale itself happens in the first block and then almost never).  The earlier two-sweep form (exact row
-// maximum from a first S-only sweep; 1.5x the QK^T work) is kept as kOnline = false for comparison (MI_ATTN_TWO_SWEEP=1).  K comes from a padded copy with the null key
-// prepended, V from a TRANSPOSED padded copy (keys contiguous = the K-major B operand of the second GEMM); both are
-// written by attn_prep_kernel into a caller-provided workspace.  Warp roles: 0-15 softmax / epilogue (four warps per
-// TMEM lane quarter, each owning 32 keys of every block and 16 dims of the output), 16 TMA producer, 17 MMA issuer + TMEM
-// allocator.
+// One CTA = 128 queries of one (batch, head); warpgroup 0 is the TMA producer (Q once, then K and V^T blocks of 128 keys
+// through a two-stage mbarrier ring), warpgroups 1 and 2 each own 64 of the queries:
+//   S = Q K_j^T       wgmma m64n128k16, Q and K from shared memory, S in registers (fp32)
+//   P = exp(S - m)    online softmax in registers: running row maximum m, O and the row sums rescaled when m rises
+//   O += P V_j        wgmma m64n64k16 with P as the register A operand (the S accumulator layout IS the A fragment
+//                     layout, so P never leaves the registers), V^T from shared memory
+// K comes from a padded copy with the null key prepended, V from a TRANSPOSED padded copy (keys contiguous = the K-major B
+// operand of the second GEMM); both, and the key-validity bits (null key, key_mask, padding), are written by
+// attn_prep_kernel into a caller-provided workspace.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "kernels.cuh"
 #include "launch.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace mi {
 
 namespace {
 
-constexpr int kD = 64, kBQ = 128;
-constexpr int kSoftmaxWarps = 16;                    // four per TMEM lane quarter, each owning a quarter of every key block
-constexpr int kThreads = 32 * (kSoftmaxWarps + 2);    // + TMA producer (warp 16) + MMA issuer / TMEM allocator (warp 17)
+constexpr int kD = 64, kBQ = 128, kBK = 128;
+constexpr int kThreads = 384;
+constexpr int kStages = 2;
 constexpr uint32_t kQBytes = kBQ * kD * 2;            // 16 KB
-constexpr uint32_t kTmemCols = 512;                   // S tiles in [0,256), O in [256,320), P (fp16 pairs) in [320,448)
-constexpr uint32_t kTmemO = 256, kTmemP = 320;
-
-// BK = keys per block = N of the S = Q K^T instruction.  128: S and P double-buffered (short key sequences pad less);
-// 256: one S tile, one P tile, but N = 256 instructions (long self-attention sequences, +10 % at 4096 tokens).
-template <int BK>
-struct AC {
-    static constexpr int kSBuf = BK == 128 ? 2 : 1;            // S tiles in TMEM (512 columns: kSBuf * BK for S + 64 for O)
-    static constexpr int kPBuf = BK == 128 ? 2 : 1;            // P tiles in tensor memory (BK / 2 columns each)
-    static constexpr int kChunks = BK / 64;                    // 64-key (128-byte) swizzle chunks per block
-    static constexpr uint32_t kKBytes = BK * kD * 2;
-    static constexpr uint32_t kVBytes = kD * BK * 2;           // kChunks x [64 dims][64 keys]
-    static constexpr uint32_t kSmemBytes = kQBytes + 2 * kKBytes + 2 * kVBytes + 1024 + 256 + 2048;
-};
+constexpr uint32_t kKBytes = kBK * kD * 2;            // 16 KB: [128 keys][64 dims]
+constexpr uint32_t kVBytes = kD * kBK * 2;            // 16 KB: two [64 dims][64 keys] chunks
+constexpr uint32_t kStageBytes = kKBytes + kVBytes;
+constexpr uint32_t kSmemBytes = kQBytes + kStages * kStageBytes + 1024 + 256;
 
 // ------------------------------------------------------------------------------------------------ operand preparation
 // Kp[bh][key][64]: key 0 = null key, keys 1..m = k, keys > m = 0.   Vt[bh][dim][key]: the same, transposed.
 // valid[b][key / 32]: bit (key % 32) = this padded key takes part in the softmax -- the null key always, key 1..m unless the
-// caller's key mask (b, m; layers.py:86-93 / :242-245) clears it, the padding never.  The attention kernels read one or two words
-// per thread and key block: the fast path when all bits are set, per-key tests otherwise (masked keys and the padded tail alike).
+// caller's key mask (b, m; layers.py:86-93 / :242-245) clears it, the padding never.
 __global__ void __launch_bounds__(256)
 attn_prep_kernel(const __half* __restrict__ k, const __half* __restrict__ v, long long kv_bs, int ldkv, int kv_hs,
                  const float* __restrict__ null_kv, int hkv, int m, int Mp, __half* __restrict__ Kp,
@@ -93,737 +75,202 @@ attn_prep_kernel(const __half* __restrict__ k, const __half* __restrict__ v, lon
 }
 
 struct AttnArgs {
-    int n, heads, hkv, Mp, nblk, kv_len, batch;       // kv_len = m + 1 valid (padded) keys
+    int n, heads, hkv, Mp, nblk;
     __half* out; long long o_bs; int ldo;
-    int poly;                                  // 1: every fourth exp on the FMA pipe (ex2_poly)
     const uint32_t* valid;                     // [B][Mp / 32] key validity bits (attn_prep_kernel)
     int* err;
 };
-
-// 2^x on the FMA / ALU pipes (Cody-Waite split + degree-3 minimax polynomial, max relative error 7.5e-5 -- P is rounded to
-// fp16, 4.9e-4, right after): used for every fourth key so that the 16-per-clock MUFU pipe is not the only exp unit.
-__device__ __forceinline__ float ex2_poly(float x) {
-    x = fmaxf(x, -120.f);
-    const float xr = x + 12582912.f;                  // 1.5 * 2^23: the low mantissa bits now hold round(x)
-    const float f = x - (xr - 12582912.f);            // [-0.5, 0.5]
-    float p = fmaf(f, 0.0551714078f, 0.242610753f);
-    p = fmaf(p, f, 0.693260968f);
-    p = fmaf(p, f, 0.999928117f);
-    return __int_as_float(__float_as_int(p) + (__float_as_int(xr) << 23));     // p * 2^round(x)
-}
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <int kBK, bool kOnline>
 __global__ void __launch_bounds__(kThreads, 1)
-attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+attn_wg_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnArgs a) {
-    pdl_trigger();
-    using C = AC<kBK>;
-    constexpr int kSBuf = C::kSBuf, kPBuf = C::kPBuf, kChunks = C::kChunks;
-    constexpr uint32_t kKBytes = C::kKBytes, kVBytes = C::kVBytes;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sQ = smem;
-    uint8_t* sK = sQ + kQBytes;                 // [2]
-    uint8_t* sV = sK + 2 * kKBytes;             // [2]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + 2 * kVBytes);
+    uint8_t* sKV = sQ + kQBytes;                // [kStages] x (K block, V^T block)
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + kStages * kStageBytes);
     uint64_t* q_full = bars;
-    uint64_t* k_full = bars + 1;                // [2]
-    uint64_t* k_empty = bars + 3;
-    uint64_t* v_full = bars + 5;
-    uint64_t* v_empty = bars + 7;
-    uint64_t* s_full = bars + 9;
-    uint64_t* s_empty = bars + 11;
-    uint64_t* p_full = bars + 13;
-    uint64_t* p_empty = bars + 15;
-    uint64_t* o_full = bars + 17;
-    uint64_t* pv_done = bars + 19;              // one phase per key block: P V_j (and everything before it) has completed
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 18);
-    float* s_xchg = reinterpret_cast<float*>(bars + 20);     // [4][128]: row max / row sum exchange between the column parts
+    uint64_t* full_bar = bars + 1;              // [kStages]
+    uint64_t* empty_bar = bars + 1 + kStages;   // [kStages]: one arrival per consumer warpgroup
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int q0 = blockIdx.x * kBQ, h = blockIdx.y, b = blockIdx.z;
-    const int bh = b * a.hkv + (a.hkv == 1 ? 0 : h);
+    const int hk = a.hkv == 1 ? 0 : h;
+    const int kv_row0 = (b * a.hkv + hk) * a.Mp;     // first padded key of this (batch, kv head) in Kp
+    const int vt_row0 = (b * a.hkv + hk) * kD;       // first dim row of this (batch, kv head) in Vt
     int* err = a.err;
 
-    if (warp == kSoftmaxWarps && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tmQ);
         ptx::prefetch_tensormap(&tmK);
         ptx::prefetch_tensormap(&tmV);
-    }
-    if (warp == kSoftmaxWarps + 1 && lane == 0) {
         ptx::mbar_init(q_full, 1);
-        ptx::mbar_init(o_full, 1);
-        ptx::mbar_init(pv_done, 1);
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&k_full[i], 1); ptx::mbar_init(&k_empty[i], 1);
-            ptx::mbar_init(&v_full[i], 1); ptx::mbar_init(&v_empty[i], 1);
-            ptx::mbar_init(&s_full[i], 1); ptx::mbar_init(&s_empty[i], 32 * kSoftmaxWarps);
-            ptx::mbar_init(&p_full[i], 32 * kSoftmaxWarps); ptx::mbar_init(&p_empty[i], 1);
-        }
+        for (int i = 0; i < kStages; ++i) { ptx::mbar_init(&full_bar[i], 1); ptx::mbar_init(&empty_bar[i], 2); }
         ptx::fence_barrier_init();
     }
-    if (warp == kSoftmaxWarps + 1) {
-        ptx::tmem_alloc(tmem_ptr_smem, kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     pdl_wait();
 
-    const int nblk = a.nblk;
-
-    if (warp == kSoftmaxWarps) {
+    if (wg == 0) {
         // ===================== TMA producer =====================
-        if (ptx::elect_one()) {
-            ptx::mbar_arrive_expect_tx(q_full, kQBytes);
-            ptx::tma_load_2d(&tmQ, q_full, sQ, h * kD, b * a.n + q0);
-        }
-        int ik = 0, iv = 0;
-        for (int pass = kOnline ? 1 : 0; pass < 2; ++pass) {
-            for (int j = 0; j < nblk; ++j) {
-                {
-                    const int s = ik & 1;
-                    ptx::mbar_wait(&k_empty[s], ((ik >> 1) & 1) ^ 1, err, 4100 + s);
-                    if (ptx::elect_one()) {
-                        ptx::mbar_arrive_expect_tx(&k_full[s], kKBytes);
-                        ptx::tma_load_2d(&tmK, &k_full[s], sK + s * kKBytes, 0, bh * a.Mp + j * kBK);
-                    }
-                    ++ik;
-                }
-                if (pass == 1) {
-                    const int s = iv & 1;
-                    ptx::mbar_wait(&v_empty[s], ((iv >> 1) & 1) ^ 1, err, 4200 + s);
-                    if (ptx::elect_one()) {
-                        ptx::mbar_arrive_expect_tx(&v_full[s], kVBytes);
-#pragma unroll
-                        for (int c = 0; c < kChunks; ++c)
-                            ptx::tma_load_2d(&tmV, &v_full[s], sV + s * kVBytes + c * (kVBytes / kChunks), j * kBK + c * 64,
-                                             bh * kD);
-                    }
-                    ++iv;
-                }
-            }
-        }
-    } else if (warp == kSoftmaxWarps + 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc_s = ptx::make_idesc_f16(kBQ, kBK, 0);
-        constexpr uint32_t idesc_o = ptx::make_idesc_f16(kBQ, kD, 0);
-        const uint32_t tmem_o = tmem_base + kTmemO;
-        ptx::mbar_wait(q_full, 0, err, 4300);
-        int ik = 0, is = 0, ip = 0, iv = 0;
-        auto issue_qk = [&]() {
-            const int ks = ik & 1, ss = is % kSBuf;
-            ptx::mbar_wait(&k_full[ks], (ik >> 1) & 1, err, 4310 + ks);
-            ptx::mbar_wait(&s_empty[ss], ((is / kSBuf) & 1) ^ 1, err, 4320 + ss);
-            ptx::tc_fence_after();
+        if (warp == 0) {
             if (ptx::elect_one()) {
-                const uint64_t da = ptx::make_kmajor_sw128_desc(ptx::smem_u32(sQ));
-                const uint64_t db = ptx::make_kmajor_sw128_desc(ptx::smem_u32(sK + ks * kKBytes));
-#pragma unroll
-                for (int k = 0; k < kD / 16; ++k)
-                    ptx::umma_f16(tmem_base + ss * kBK, da + 2 * k, db + 2 * k, idesc_s, k != 0);
-                ptx::umma_commit(&k_empty[ks]);
-                ptx::umma_commit(&s_full[ss]);
+                ptx::mbar_arrive_expect_tx(q_full, kQBytes);
+                ptx::tma_load_2d(&tmQ, q_full, sQ, h * kD, b * a.n + q0);
             }
-            ++ik; ++is;
-        };
-        // two-sweep form only -- sweep 1: S only (row maxima)
-        if (!kOnline)
-            for (int j = 0; j < nblk; ++j) issue_qk();
-        // main sweep: S of block j+1 is issued before P V of block j so the softmax warps always have work
-        issue_qk();
-        for (int j = 0; j < nblk; ++j) {
-            if (j + 1 < nblk) issue_qk();
-            const int ps = ip % kPBuf, vs = iv & 1;
-            ptx::mbar_wait(&p_full[ps], (ip / kPBuf) & 1, err, 4330 + ps);
-            ptx::mbar_wait(&v_full[vs], (iv >> 1) & 1, err, 4340 + vs);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-#pragma unroll
-                for (int c = 0; c < kChunks; ++c) {
-                    const uint32_t ta = tmem_base + kTmemP + ps * (kBK / 2) + c * 32;      // 64 keys = 32 columns of fp16 pairs
-                    const uint64_t db = ptx::make_kmajor_sw128_desc(ptx::smem_u32(sV + vs * kVBytes + c * (kVBytes / kChunks)));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_f16_ts(tmem_o, ta + 8 * k, db + 2 * k, idesc_o, (j | c | k) != 0);
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int j = 0; j < a.nblk; ++j) {
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 8100 + stage);
+                if (ptx::elect_one()) {
+                    uint8_t* sK = sKV + stage * kStageBytes;
+                    uint8_t* sV = sK + kKBytes;
+                    ptx::mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+                    ptx::tma_load_2d(&tmK, &full_bar[stage], sK, 0, kv_row0 + j * kBK);
+                    ptx::tma_load_2d(&tmV, &full_bar[stage], sV, j * kBK, vt_row0);
+                    ptx::tma_load_2d(&tmV, &full_bar[stage], sV + kVBytes / 2, j * kBK + 64, vt_row0);
                 }
-                ptx::umma_commit(&p_empty[ps]);
-                ptx::umma_commit(&v_empty[vs]);
-                if (kOnline) ptx::umma_commit(pv_done);
-                if (j + 1 == nblk) ptx::umma_commit(o_full);
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
-            ++ip; ++iv;
+            pdl_trigger();
         }
-    } else {
-        // ===================== softmax / epilogue: one query row x kPer keys of every block per thread ================
-        constexpr int kPer = kBK / 4;                  // 32 or 64 keys per thread and block
-        const int q4 = warp & 3, part = warp >> 2;     // TMEM lane quarter, key columns [kPer*part, kPer*part + kPer)
-        const int row = q4 * 32 + lane;
-        const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q4 * 32) << 16);
-        const int c_lo = part * kPer;
-        constexpr float kLog2e = 1.4426950408889634f;
-        const int qbar = 1 + q4;                      // named barrier of this lane quarter: its four warps own the same 32 rows
-        int is = 0, ip = 0;
-        // ---- sweep 1: exact row maximum (four independent running maxima: no long dependent chain)
-        float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-        for (int j = 0; !kOnline && j < nblk; ++j, ++is) {
-            const int ss = is % kSBuf;
-            ptx::mbar_wait(&s_full[ss], (is / kSBuf) & 1, err, 4400 + ss);
-            ptx::tc_fence_after();
-            uint32_t v[kPer];
+        return;
+    }
+
+    // ===================== consumers: queries [64 cw, 64 cw + 64) of the tile =====================
+    // fragment element 4j + 2r + e of S (resp. O) = row 16 wq + lane/4 + 8r, key (resp. dim) 8j + 2(lane%4) + e
+    const int cw = wg - 1, wq = warp & 3;
+    constexpr float kLog2e = 1.4426950408889634f;
+    float o[kD / 2];
 #pragma unroll
-            for (int c = 0; c < kPer; c += 16) ptx::tmem_ld_x16(lane_addr + ss * kBK + c_lo + c, *reinterpret_cast<uint32_t(*)[16]>(&v[c]));
-            ptx::tmem_ld_wait();
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&s_empty[ss]);                     // S is in registers: release the buffer early
-            const uint32_t* vw = a.valid + (long long)b * (a.Mp / 32) + (j * kBK + c_lo) / 32;
-            uint32_t vb[kPer / 32];
-            bool all_ok = true;
+    for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const uint32_t* vrow = a.valid + (long long)b * (a.Mp / 32);
+    const uint64_t dq = ptx::make_sw128_desc(ptx::smem_u32(sQ + cw * (64 * 128)));
+    ptx::mbar_wait(q_full, 0, err, 8200);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int j = 0; j < a.nblk; ++j) {
+        ptx::mbar_wait(&full_bar[stage], phase, err, 8300 + stage);
+        const uint32_t sK = ptx::smem_u32(sKV + stage * kStageBytes);
+        const uint32_t sV = sK + kKBytes;
+        float s[kBK / 2];
+        const uint64_t dk = ptx::make_sw128_desc(sK);
+        ptx::wg_fence();
 #pragma unroll
-            for (int w = 0; w < kPer / 32; ++w) { vb[w] = __ldg(vw + w); all_ok = all_ok && vb[w] == 0xffffffffu; }
-            if (all_ok) {                                       // no masked / padded key among this thread's keys of the block
+        for (int k = 0; k < kD / 16; ++k) ptx::Wgmma<kBK, 0>::run(s, dq + 2 * k, dk + 2 * k, k != 0);
+        ptx::wg_commit();
+        ptx::wg_wait<0>();
+        ptx::wg_fence_regs(s);
+
+        // key validity of this block (null key, mask, padding): all-ones words take the fast path
+        uint32_t vb[kBK / 32];
+        bool tail = false;
 #pragma unroll
-                for (int i = 0; i < kPer; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[i]));
-            } else {
+        for (int w = 0; w < kBK / 32; ++w) { vb[w] = __ldg(vrow + j * (kBK / 32) + w); tail = tail || vb[w] != 0xffffffffu; }
+        if (tail) {
 #pragma unroll
-                for (int i = 0; i < kPer; ++i)
-                    if ((vb[i >> 5] >> (i & 31)) & 1u) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[i]));
+            for (int i = 0; i < kBK / 2; ++i) {
+                const int key = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+                if (!((vb[key >> 5] >> (key & 31)) & 1u)) s[i] = -INFINITY;
             }
         }
-        float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-        if (!kOnline) {
-            s_xchg[part * 128 + row] = mx;
-            asm volatile("bar.sync %0, 128;" ::"r"(qbar) : "memory");      // the four warps of this lane quarter
-            mx = fmaxf(fmaxf(s_xchg[row], s_xchg[128 + row]), fmaxf(s_xchg[256 + row], s_xchg[384 + row]));   // key 0 (null) is valid
+        float scale[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int jj = 0; jj < kBK / 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * r], s[4 * jj + 2 * r + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_run[r], mx);
+            // a row whose keys so far are all masked keeps m = -inf: no contribution, nothing to rescale
+            scale[r] = m_new == -INFINITY ? 1.f : ptx::ex2_approx((m_run[r] - m_new) * kLog2e);
+            m_run[r] = m_new;
         }
-        float m_ref = mx;                                       // kOnline: -inf until the first block sets it
-        float mneg = -mx * kLog2e;
-        // ---- sweep 2: P = exp(S - max) -> shared memory (fp16, swizzled), row sums in four partial accumulators
-        float l4[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int j = 0; j < nblk; ++j, ++is, ++ip) {
-            const int ss = is % kSBuf, ps = ip % kPBuf;
-            ptx::mbar_wait(&s_full[ss], (is / kSBuf) & 1, err, 4410 + ss);
-            ptx::tc_fence_after();
-            uint32_t v[kPer];
+        uint32_t p[kBK / 16][4];
+        float lsum[2] = {0.f, 0.f};
 #pragma unroll
-            for (int c = 0; c < kPer; c += 16) ptx::tmem_ld_x16(lane_addr + ss * kBK + c_lo + c, *reinterpret_cast<uint32_t(*)[16]>(&v[c]));
-            ptx::tmem_ld_wait();
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&s_empty[ss]);
-            // key validity bits of this thread's keys: "tail" = some key of them is masked or padding (warp-uniform)
-            uint32_t vb[kPer / 32];
-            bool tail = false;
-            {
-                const uint32_t* vw = a.valid + (long long)b * (a.Mp / 32) + (j * kBK + c_lo) / 32;
+        for (int jj = 0; jj < kBK / 8; ++jj) {
 #pragma unroll
-                for (int w = 0; w < kPer / 32; ++w) { vb[w] = __ldg(vw + w); tail = tail || vb[w] != 0xffffffffu; }
+            for (int r = 0; r < 2; ++r) {
+                const float mneg = m_run[r] == -INFINITY ? 0.f : -m_run[r] * kLog2e;
+                const float p0 = ptx::ex2_approx(fmaf(s[4 * jj + 2 * r], kLog2e, mneg));
+                const float p1 = ptx::ex2_approx(fmaf(s[4 * jj + 2 * r + 1], kLog2e, mneg));
+                lsum[r] += p0 + p1;
+                // A fragment of k-step jj/2: regs {row r0 keys 0-7, row r1 keys 0-7, row r0 keys 8-15, row r1 keys 8-15}
+                p[jj >> 1][(jj & 1) * 2 + r] = pack_h2(p0, p1);
             }
-            if (kOnline) {
-                // lazy reference maximum: does any row of the CTA see a score more than 2^8 above its reference?
-                float b4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-                if (!tail) {
-#pragma unroll
-                    for (int i = 0; i < kPer; ++i) b4[i & 3] = fmaxf(b4[i & 3], __uint_as_float(v[i]));
-                } else {
-#pragma unroll
-                    for (int i = 0; i < kPer; ++i)
-                        if ((vb[i >> 5] >> (i & 31)) & 1u) b4[i & 3] = fmaxf(b4[i & 3], __uint_as_float(v[i]));
-                }
-                const float bm = fmaxf(fmaxf(b4[0], b4[1]), fmaxf(b4[2], b4[3]));
-                const uint32_t need = (bm - m_ref) * kLog2e > 8.f ? 1u : 0u;     // m_ref = -inf in block 0: true wherever bm is finite
-                uint32_t any;
-                asm volatile(
-                    "{\n\t.reg .pred p, q;\n\tsetp.ne.u32 q, %1, 0;\n\tbar.red.or.pred p, %2, 128, q;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                    : "=r"(any) : "r"(need), "r"(qbar) : "memory");
-                if (any) {                                                       // uniform over the four warps of the lane quarter
-                    s_xchg[part * 128 + row] = bm;
-                    asm volatile("bar.sync %0, 128;" ::"r"(qbar) : "memory");
-                    const float bmr = fmaxf(fmaxf(s_xchg[row], s_xchg[128 + row]), fmaxf(s_xchg[256 + row], s_xchg[384 + row]));
-                    const float m_new = fmaxf(m_ref, bmr);
-                    const float factor = m_ref == -INFINITY ? 0.f : ptx::ex2_approx((m_ref - m_new) * kLog2e);
-                    if (j > 0) {
-                        // O holds sum_k exp(s - m_ref) v: wait until P V of the previous block has landed, rescale this thread's
-                        // 16 dims of its row in place (rows whose reference did not move multiply by exactly 1)
-                        ptx::mbar_wait(pv_done, (j - 1) & 1, err, 4430);
-                        ptx::tc_fence_after();
-                        uint32_t o[16];
-                        ptx::tmem_ld_x16(lane_addr + kTmemO + part * 16, o);
-                        ptx::tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-                        ptx::tmem_st_x16(lane_addr + kTmemO + part * 16, o);
-                        ptx::tmem_st_wait();
-                        ptx::tc_fence_before();
-                    }
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) l4[i] *= factor;
-                    m_ref = m_new;
-                    mneg = -m_new * kLog2e;
-                }
-            }
-            uint32_t pk[kPer / 2];                              // fp16 pairs (low half = the even key)
-            if (!tail && a.poly) {                              // uniform branches: MUFU for three keys, FMA-pipe polynomial for the fourth
-#pragma unroll
-                for (int i = 0; i < kPer; i += 2) {
-                    const float p0 = ptx::ex2_approx(fmaf(__uint_as_float(v[i]), kLog2e, mneg));
-                    const float x1 = fmaf(__uint_as_float(v[i + 1]), kLog2e, mneg);
-                    const float p1 = (i & 2) ? ex2_poly(x1) : ptx::ex2_approx(x1);
-                    l4[i & 3] += p0;
-                    l4[(i + 1) & 3] += p1;
-                    pk[i >> 1] = pack_h2(p0, p1);
-                }
-            } else if (!tail) {                                 // the per-key bound check only in the last block
-#pragma unroll
-                for (int i = 0; i < kPer; i += 2) {
-                    const float p0 = ptx::ex2_approx(fmaf(__uint_as_float(v[i]), kLog2e, mneg));
-                    const float p1 = ptx::ex2_approx(fmaf(__uint_as_float(v[i + 1]), kLog2e, mneg));
-                    l4[i & 3] += p0;
-                    l4[(i + 1) & 3] += p1;
-                    pk[i >> 1] = pack_h2(p0, p1);
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < kPer; i += 2) {
-                    float p0 = ptx::ex2_approx(fmaf(__uint_as_float(v[i]), kLog2e, mneg));
-                    float p1 = ptx::ex2_approx(fmaf(__uint_as_float(v[i + 1]), kLog2e, mneg));
-                    if (!((vb[i >> 5] >> (i & 31)) & 1u)) p0 = 0.f;
-                    if (!((vb[(i + 1) >> 5] >> ((i + 1) & 31)) & 1u)) p1 = 0.f;
-                    l4[i & 3] += p0;
-                    l4[(i + 1) & 3] += p1;
-                    pk[i >> 1] = pack_h2(p0, p1);
-                }
-            }
-            // keys [c_lo, c_lo + kPer) of this thread's row -> columns c_lo/2 .. of the P tile (A operand of the P V MMA)
-            ptx::mbar_wait(&p_empty[ps], ((ip / kPBuf) & 1) ^ 1, err, 4420 + ps);
-            ptx::tc_fence_after();
-#pragma unroll
-            for (int g = 0; g < kPer / 32; ++g)
-                ptx::tmem_st_x16(lane_addr + kTmemP + ps * (kBK / 2) + (c_lo >> 1) + 16 * g,
-                                 *reinterpret_cast<const uint32_t(*)[16]>(&pk[16 * g]));
-            ptx::tmem_st_wait();
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&p_full[ps]);
         }
-        float l = (l4[0] + l4[1]) + (l4[2] + l4[3]);
-        asm volatile("bar.sync %0, 128;" ::"r"(qbar) : "memory");          // this quarter has read the maxima
-        s_xchg[part * 128 + row] = l;
-        asm volatile("bar.sync %0, 128;" ::"r"(qbar) : "memory");
-        l = (s_xchg[row] + s_xchg[128 + row]) + (s_xchg[256 + row] + s_xchg[384 + row]);
-        // ---- epilogue: O / l -> fp16 [b][q0 + row][h*64 + 16*part ..]
-        ptx::mbar_wait(o_full, 0, err, 4500);
-        ptx::tc_fence_after();
+#pragma unroll
+        for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * scale[r] + lsum[r];
+#pragma unroll
+        for (int i = 0; i < kD / 2; ++i) o[i] *= scale[(i >> 1) & 1];
+
+        ptx::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < kBK / 16; ++kk) {
+            // 16 keys: chunk kk / 4 of V^T ([64 dims][64 keys]), 32-byte step kk % 4 inside the 128-byte rows
+            const uint64_t dv = ptx::make_sw128_desc(sV + (kk >> 2) * (kVBytes / 2)) + 2 * (kk & 3);
+            ptx::WgmmaRS<kD>::run(o, p[kk], dv, 1);
+        }
+        ptx::wg_commit();
+        ptx::wg_wait<0>();
+        ptx::wg_fence_regs(o);
+        if ((threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[stage]);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+
+    // ---- epilogue: O / l, fp16, head h's 64 columns of the output rows
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        float l = l_run[r];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
         const float inv = 1.f / l;
-        __half* orow = a.out + (long long)b * a.o_bs + (long long)(q0 + row) * a.ldo + h * kD + part * 16;
-        {
-            uint32_t v0[16];
-            ptx::tmem_ld_x16(lane_addr + kTmemO + part * 16, v0);
-            ptx::tmem_ld_wait();
+        const int row = q0 + cw * 64 + wq * 16 + (lane >> 2) + 8 * r;
+        __half* orow = a.out + (long long)b * a.o_bs + (long long)row * a.ldo + h * kD + 2 * (lane & 3);
 #pragma unroll
-            for (int g = 0; g < 2; ++g) {
-                uint4 w0;
-                w0.x = pack_h2(__uint_as_float(v0[8 * g + 0]) * inv, __uint_as_float(v0[8 * g + 1]) * inv);
-                w0.y = pack_h2(__uint_as_float(v0[8 * g + 2]) * inv, __uint_as_float(v0[8 * g + 3]) * inv);
-                w0.z = pack_h2(__uint_as_float(v0[8 * g + 4]) * inv, __uint_as_float(v0[8 * g + 5]) * inv);
-                w0.w = pack_h2(__uint_as_float(v0[8 * g + 6]) * inv, __uint_as_float(v0[8 * g + 7]) * inv);
-                *reinterpret_cast<uint4*>(orow + 8 * g) = w0;
-            }
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == kSoftmaxWarps + 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, kTmemCols);
-    }
-}
-
-
-// =====================================================================================================================
-// Two query tiles per CTA, ping-ponged (n % 256 == 0): the softmax side is the bound of this kernel (MUFU 16 exp/clk/SM,
-// ncu: r02_attention_tc_study.md) and with one query tile the four warps of an SM sub-partition own the same rows and move in
-// lock-step, so the MUFU pipe idles while they wait for S, load it, take maxima and store P.  Here a CTA owns 256 queries as
-// tiles A and B, each with its own eight softmax warps (two per sub-partition and tile), S / P / O regions in tensor memory
-//   S_A [0,128)  S_B [128,256)  O_A [256,320)  O_B [320,384)  P_A [384,448)  P_B [448,512)      (128-key blocks)
-// and the MMA warp issues  QK_A(j+1), PV_A(j), QK_B(j+1), PV_B(j), ...: tile B's S arrives one P.V + one Q.K^T later than
-// tile A's, which keeps the two groups half a block apart -- one computes exps while the other loads / stores / synchronises.
-// (Tried: one issuing warp PER tile -- without the enforced order the two groups drift into phase, 3746 vs 3206 us at 4096 --
-// and QK_A(j+1), QK_B(j+1), PV_A(j), PV_B(j): both groups in phase again, 3492 vs 3304 us.)
-// K_j / V_j are loaded once for both tiles (three-stage rings).  Same lazy-rescale single sweep, P in tensor memory, every
-// fourth exp on the FMA pipe as attn_tc_kernel.  The CTAs are PERSISTENT: one per SM, streaming over the (query pair-tile, head,
-// batch) work items with Q double-buffered and O handed from the MMA warp to the epilogue and back through o_full / o_empty, so
-// the set-up of a work item (Q / first K loads, pipeline fill) overlaps the tail of the previous one -- +25 % on the three-block
-// cross-attention shapes.
-constexpr int kBQ2 = 256, kBK2 = 128, kStages2 = 3;
-constexpr int kThreads2 = kThreads;
-constexpr uint32_t kK2Bytes = kBK2 * kD * 2, kV2Bytes = kD * kBK2 * 2;       // 16 KB each
-constexpr uint32_t kSmem2Bytes = 4 * kQBytes + kStages2 * (kK2Bytes + kV2Bytes) + 1024 + 512 + 4096;
-
-__global__ void __launch_bounds__(kThreads2, 1)
-attn_tc2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnArgs a) {
-    pdl_trigger();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sQ = smem;                                  // [2 work items in flight][2 tiles]
-    uint8_t* sK = sQ + 4 * kQBytes;                      // [kStages2]
-    uint8_t* sV = sK + kStages2 * kK2Bytes;              // [kStages2]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kStages2 * kV2Bytes);
-    uint64_t* q_full = bars + 26;                        // [2]  (bars + 0 unused)
-    uint64_t* q_empty = bars + 28;                       // [2]
-    uint64_t* o_empty = bars + 30;                       // [2 tiles]
-    uint64_t* k_full = bars + 1;                         // [3]
-    uint64_t* k_empty = bars + 4;                        // [3]
-    uint64_t* v_full = bars + 7;                         // [3]
-    uint64_t* v_empty = bars + 10;                       // [3]
-    uint64_t* s_full = bars + 13;                        // [2 tiles]
-    uint64_t* s_empty = bars + 15;
-    uint64_t* p_full = bars + 17;
-    uint64_t* p_empty = bars + 19;
-    uint64_t* pv_done = bars + 21;
-    uint64_t* o_full = bars + 23;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 32);
-    float* s_xchg = reinterpret_cast<float*>(bars + 64);  // [2 tiles][2 parts][128 rows]
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int* err = a.err;
-    // persistent CTA: work item w = (query pair-tile, head, batch), w = blockIdx.x, blockIdx.x + gridDim.x, ...; all barrier
-    // phases run on GLOBAL counters (work index i, key-block index gj = i * nblk + j) so that the producer and the MMA warp stream
-    // straight into the next work item while the softmax warps finish the current one (Q double-buffered, O handed over through
-    // o_full / o_empty)
-    const int q_tiles = a.n / kBQ2;
-    const int total_work = q_tiles * a.heads * a.batch;
-
-    if (warp == kSoftmaxWarps && lane == 0) {
-        ptx::prefetch_tensormap(&tmQ);
-        ptx::prefetch_tensormap(&tmK);
-        ptx::prefetch_tensormap(&tmV);
-    }
-    if (warp == kSoftmaxWarps + 1 && lane == 0) {
-        for (int i = 0; i < 2; ++i) { ptx::mbar_init(&q_full[i], 1); ptx::mbar_init(&q_empty[i], 1); }
-        for (int i = 0; i < kStages2; ++i) {
-            ptx::mbar_init(&k_full[i], 1); ptx::mbar_init(&k_empty[i], 1);
-            ptx::mbar_init(&v_full[i], 1); ptx::mbar_init(&v_empty[i], 1);
-        }
-        for (int t = 0; t < 2; ++t) {
-            ptx::mbar_init(&s_full[t], 1); ptx::mbar_init(&s_empty[t], 32 * kSoftmaxWarps / 2);
-            ptx::mbar_init(&p_full[t], 32 * kSoftmaxWarps / 2); ptx::mbar_init(&p_empty[t], 1);
-            ptx::mbar_init(&pv_done[t], 1); ptx::mbar_init(&o_full[t], 1);
-            ptx::mbar_init(&o_empty[t], 32 * kSoftmaxWarps / 2);
-        }
-        ptx::fence_barrier_init();
-    }
-    if (warp == kSoftmaxWarps + 1) {
-        ptx::tmem_alloc(tmem_ptr_smem, kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    pdl_wait();
-
-    const int nblk = a.nblk;
-
-    if (warp == kSoftmaxWarps) {
-        // ===================== TMA producer: Q tiles once, then K_j and V_j for both tiles =====================
-        int st = 0;
-        uint32_t ph = 0;
-        int i = 0;
-        for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++i) {
-            const int q0 = (w % q_tiles) * kBQ2, h = (w / q_tiles) % a.heads, b = w / (q_tiles * a.heads);
-            const int bh = b * a.hkv + (a.hkv == 1 ? 0 : h);
-            const int qb = i & 1;
-            ptx::mbar_wait(&q_empty[qb], ((i >> 1) & 1) ^ 1, err, 5050 + qb);
-            if (ptx::elect_one()) {
-                ptx::mbar_arrive_expect_tx(&q_full[qb], 2 * kQBytes);
-                ptx::tma_load_2d(&tmQ, &q_full[qb], sQ + qb * 2 * kQBytes, h * kD, b * a.n + q0);
-                ptx::tma_load_2d(&tmQ, &q_full[qb], sQ + qb * 2 * kQBytes + kQBytes, h * kD, b * a.n + q0 + kBQ);
-            }
-            for (int j = 0; j < nblk; ++j) {
-                ptx::mbar_wait(&k_empty[st], ph ^ 1, err, 5100 + st);
-                if (ptx::elect_one()) {
-                    ptx::mbar_arrive_expect_tx(&k_full[st], kK2Bytes);
-                    ptx::tma_load_2d(&tmK, &k_full[st], sK + st * kK2Bytes, 0, bh * a.Mp + j * kBK2);
-                }
-                ptx::mbar_wait(&v_empty[st], ph ^ 1, err, 5200 + st);
-                if (ptx::elect_one()) {
-                    ptx::mbar_arrive_expect_tx(&v_full[st], kV2Bytes);
-                    ptx::tma_load_2d(&tmV, &v_full[st], sV + st * kV2Bytes, j * kBK2, bh * kD);
-                    ptx::tma_load_2d(&tmV, &v_full[st], sV + st * kV2Bytes + kV2Bytes / 2, j * kBK2 + 64, bh * kD);
-                }
-                if (++st == kStages2) { st = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp == kSoftmaxWarps + 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc_s = ptx::make_idesc_f16(kBQ, kBK2, 0);
-        constexpr uint32_t idesc_o = ptx::make_idesc_f16(kBQ, kD, 0);
-        int i = 0, gbase = 0, qb = 0;                    // work index, global index of this work item's first key block, Q buffer
-        // S_t(j) = Q_t K_j^T; `last` = the later of the two users of K_j releases its stage
-        auto issue_qk = [&](int t, int jl, bool last) {
-            const int j = gbase + jl;                    // global key-block index: ring stage and barrier phases
-            const int st = j % kStages2;
-            ptx::mbar_wait(&k_full[st], (j / kStages2) & 1, err, 5310 + st);
-            ptx::mbar_wait(&s_empty[t], (j & 1) ^ 1, err, 5320 + t);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                const uint64_t da = ptx::make_kmajor_sw128_desc(ptx::smem_u32(sQ + qb * 2 * kQBytes + t * kQBytes));
-                const uint64_t db = ptx::make_kmajor_sw128_desc(ptx::smem_u32(sK + st * kK2Bytes));
-#pragma unroll
-                for (int k = 0; k < kD / 16; ++k)
-                    ptx::umma_f16(tmem_base + t * kBK2, da + 2 * k, db + 2 * k, idesc_s, k != 0);
-                if (last) ptx::umma_commit(&k_empty[st]);
-                if (last && jl + 1 == nblk) ptx::umma_commit(&q_empty[qb]);      // both tiles' last Q K^T: the Q buffer is free
-                ptx::umma_commit(&s_full[t]);
-            }
-        };
-        // O_t += P_t(j) V_j
-        auto issue_pv = [&](int t, int jl, bool last) {
-            const int j = gbase + jl;
-            const int st = j % kStages2;
-            ptx::mbar_wait(&p_full[t], j & 1, err, 5330 + t);
-            ptx::mbar_wait(&v_full[st], (j / kStages2) & 1, err, 5340 + st);
-            if (jl == 0) ptx::mbar_wait(&o_empty[t], (i & 1) ^ 1, err, 5350 + t);   // the previous work item's O has been read out
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    const uint32_t ta = tmem_base + 384 + t * 64 + c * 32;
-                    const uint64_t db = ptx::make_kmajor_sw128_desc(ptx::smem_u32(sV + st * kV2Bytes + c * (kV2Bytes / 2)));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_f16_ts(tmem_base + 256 + t * 64, ta + 8 * k, db + 2 * k, idesc_o, (jl | c | k) != 0);
-                }
-                ptx::umma_commit(&p_empty[t]);
-                ptx::umma_commit(&pv_done[t]);
-                if (last) ptx::umma_commit(&v_empty[st]);
-                if (jl + 1 == nblk) ptx::umma_commit(&o_full[t]);
-            }
-        };
-        for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++i, gbase += nblk) {
-            qb = i & 1;
-            ptx::mbar_wait(&q_full[qb], (i >> 1) & 1, err, 5300 + qb);
-            issue_qk(0, 0, false);
-            issue_qk(1, 0, true);
-            for (int j = 0; j < nblk; ++j) {
-                if (j + 1 < nblk) issue_qk(0, j + 1, false);
-                issue_pv(0, j, false);
-                if (j + 1 < nblk) issue_qk(1, j + 1, true);
-                issue_pv(1, j, true);
-            }
-        }
-    } else {
-        // ===================== softmax / epilogue: tile = warp / 8, one query row x 64 keys of every block per thread ==========
-        constexpr int kPer = kBK2 / 2;
-        const int tile = warp >> 3, part = (warp >> 2) & 1, q4 = warp & 3;
-        const int row = q4 * 32 + lane;
-        const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q4 * 32) << 16);
-        const uint32_t tS = lane_addr + tile * kBK2, tO = lane_addr + 256 + tile * 64, tP = lane_addr + 384 + tile * 64;
-        const int c_lo = part * kPer;
-        const int qbar = 1 + tile * 4 + q4;            // named barrier of the two warps that share these 32 rows
-        float* xch = s_xchg + tile * 256;              // [2 parts][128 rows]
-        constexpr float kLog2e = 1.4426950408889634f;
-        int i = 0, gbase = 0;
-        for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++i, gbase += nblk) {
-            const int q0 = (w % q_tiles) * kBQ2, h = (w / q_tiles) % a.heads, b = w / (q_tiles * a.heads);
-            float m_ref = -INFINITY, mneg = 0.f;
-            float l4[4] = {0.f, 0.f, 0.f, 0.f};
-            for (int j = 0; j < nblk; ++j) {
-                const int gj = gbase + j;                            // global key-block index: barrier phases
-                ptx::mbar_wait(&s_full[tile], gj & 1, err, 5400 + tile);
-                ptx::tc_fence_after();
-                uint32_t v[kPer];
-    #pragma unroll
-                for (int c = 0; c < kPer; c += 16) ptx::tmem_ld_x16(tS + c_lo + c, *reinterpret_cast<uint32_t(*)[16]>(&v[c]));
-                ptx::tmem_ld_wait();
-                ptx::tc_fence_before();
-                ptx::mbar_arrive(&s_empty[tile]);                   // S is in registers: Q K^T of the next block may start
-                uint32_t vb[kPer / 32];                             // key validity bits of this thread's 64 keys
-                bool tail = false;                                  // some key masked or padding (warp-uniform)
-                {
-                    const uint32_t* vw = a.valid + (long long)b * (a.Mp / 32) + (j * kBK2 + c_lo) / 32;
-    #pragma unroll
-                    for (int w = 0; w < kPer / 32; ++w) { vb[w] = __ldg(vw + w); tail = tail || vb[w] != 0xffffffffu; }
-                }
-                {
-                    float b4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-                    if (!tail) {
-    #pragma unroll
-                        for (int i = 0; i < kPer; ++i) b4[i & 3] = fmaxf(b4[i & 3], __uint_as_float(v[i]));
-                    } else {
-    #pragma unroll
-                        for (int i = 0; i < kPer; ++i)
-                            if ((vb[i >> 5] >> (i & 31)) & 1u) b4[i & 3] = fmaxf(b4[i & 3], __uint_as_float(v[i]));
-                    }
-                    const float bm = fmaxf(fmaxf(b4[0], b4[1]), fmaxf(b4[2], b4[3]));
-                    const uint32_t need = (bm - m_ref) * kLog2e > 8.f ? 1u : 0u;
-                    uint32_t any;
-                    asm volatile(
-                        "{\n\t.reg .pred p, q;\n\tsetp.ne.u32 q, %1, 0;\n\tbar.red.or.pred p, %2, 64, q;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                        : "=r"(any) : "r"(need), "r"(qbar) : "memory");
-                    if (any) {
-                        xch[part * 128 + row] = bm;
-                        asm volatile("bar.sync %0, 64;" ::"r"(qbar) : "memory");
-                        const float m_new = fmaxf(m_ref, fmaxf(xch[row], xch[128 + row]));
-                        const float factor = m_ref == -INFINITY ? 0.f : ptx::ex2_approx((m_ref - m_new) * kLog2e);
-                        if (j > 0) {
-                            ptx::mbar_wait(&pv_done[tile], (gj - 1) & 1, err, 5430 + tile);
-                            ptx::tc_fence_after();
-    #pragma unroll
-                            for (int g = 0; g < 2; ++g) {
-                                uint32_t o[16];
-                                ptx::tmem_ld_x16(tO + part * 32 + 16 * g, o);
-                                ptx::tmem_ld_wait();
-    #pragma unroll
-                                for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * factor);
-                                ptx::tmem_st_x16(tO + part * 32 + 16 * g, o);
-                            }
-                            ptx::tmem_st_wait();
-                            ptx::tc_fence_before();
-                        }
-    #pragma unroll
-                        for (int i = 0; i < 4; ++i) l4[i] *= factor;
-                        m_ref = m_new;
-                        mneg = -m_new * kLog2e;
-                    }
-                }
-                uint32_t pk[kPer / 2];
-                if (!tail && a.poly) {
-    #pragma unroll
-                    for (int i = 0; i < kPer; i += 2) {
-                        const float p0 = ptx::ex2_approx(fmaf(__uint_as_float(v[i]), kLog2e, mneg));
-                        const float x1 = fmaf(__uint_as_float(v[i + 1]), kLog2e, mneg);
-                        const float p1 = (i & 2) ? ex2_poly(x1) : ptx::ex2_approx(x1);
-                        l4[i & 3] += p0;
-                        l4[(i + 1) & 3] += p1;
-                        pk[i >> 1] = pack_h2(p0, p1);
-                    }
-                } else if (!tail) {
-    #pragma unroll
-                    for (int i = 0; i < kPer; i += 2) {
-                        const float p0 = ptx::ex2_approx(fmaf(__uint_as_float(v[i]), kLog2e, mneg));
-                        const float p1 = ptx::ex2_approx(fmaf(__uint_as_float(v[i + 1]), kLog2e, mneg));
-                        l4[i & 3] += p0;
-                        l4[(i + 1) & 3] += p1;
-                        pk[i >> 1] = pack_h2(p0, p1);
-                    }
-                } else {
-    #pragma unroll
-                    for (int i = 0; i < kPer; i += 2) {
-                        float p0 = ptx::ex2_approx(fmaf(__uint_as_float(v[i]), kLog2e, mneg));
-                        float p1 = ptx::ex2_approx(fmaf(__uint_as_float(v[i + 1]), kLog2e, mneg));
-                        if (!((vb[i >> 5] >> (i & 31)) & 1u)) p0 = 0.f;
-                        if (!((vb[(i + 1) >> 5] >> ((i + 1) & 31)) & 1u)) p1 = 0.f;
-                        l4[i & 3] += p0;
-                        l4[(i + 1) & 3] += p1;
-                        pk[i >> 1] = pack_h2(p0, p1);
-                    }
-                }
-                ptx::mbar_wait(&p_empty[tile], (gj & 1) ^ 1, err, 5420 + tile);
-                ptx::tc_fence_after();
-    #pragma unroll
-                for (int g = 0; g < kPer / 32; ++g)
-                    ptx::tmem_st_x16(tP + (c_lo >> 1) + 16 * g, *reinterpret_cast<const uint32_t(*)[16]>(&pk[16 * g]));
-                ptx::tmem_st_wait();
-                ptx::tc_fence_before();
-                ptx::mbar_arrive(&p_full[tile]);
-            }
-            float l = (l4[0] + l4[1]) + (l4[2] + l4[3]);
-            asm volatile("bar.sync %0, 64;" ::"r"(qbar) : "memory");
-            xch[part * 128 + row] = l;
-            asm volatile("bar.sync %0, 64;" ::"r"(qbar) : "memory");
-            l = xch[row] + xch[128 + row];
-            // ---- epilogue: O / l -> fp16 [b][q0 + tile*128 + row][h*64 + 32*part ..]
-            ptx::mbar_wait(&o_full[tile], i & 1, err, 5500 + tile);
-            ptx::tc_fence_after();
-            const float inv = 1.f / l;
-            __half* orow = a.out + (long long)b * a.o_bs + (long long)(q0 + tile * kBQ + row) * a.ldo + h * kD + part * 32;
-            uint32_t v0[32];
-            ptx::tmem_ld_x16(tO + part * 32, *reinterpret_cast<uint32_t(*)[16]>(&v0[0]));
-            ptx::tmem_ld_x16(tO + part * 32 + 16, *reinterpret_cast<uint32_t(*)[16]>(&v0[16]));
-            ptx::tmem_ld_wait();
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&o_empty[tile]);                       // O is in registers: the next work item's P V may overwrite it
-    #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                uint4 w0;
-                w0.x = pack_h2(__uint_as_float(v0[8 * g + 0]) * inv, __uint_as_float(v0[8 * g + 1]) * inv);
-                w0.y = pack_h2(__uint_as_float(v0[8 * g + 2]) * inv, __uint_as_float(v0[8 * g + 3]) * inv);
-                w0.z = pack_h2(__uint_as_float(v0[8 * g + 4]) * inv, __uint_as_float(v0[8 * g + 5]) * inv);
-                w0.w = pack_h2(__uint_as_float(v0[8 * g + 6]) * inv, __uint_as_float(v0[8 * g + 7]) * inv);
-                *reinterpret_cast<uint4*>(orow + 8 * g) = w0;
-            }
-        }       // work items
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == kSoftmaxWarps + 1) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, kTmemCols);
+        for (int jj = 0; jj < kD / 8; ++jj)
+            *reinterpret_cast<uint32_t*>(orow + 8 * jj) = pack_h2(o[4 * jj + 2 * r] * inv, o[4 * jj + 2 * r + 1] * inv);
     }
 }
 
 }  // namespace
 
-// key-block size: 256-key blocks pay off on long sequences, 128-key blocks pad short ones less
-static inline int attn_block_keys(int m) { return m >= 1024 ? 256 : 128; }
-
 long long attention_tc_workspace_bytes(int B, int heads, int kv_hs, int m) {
     const int hkv = kv_hs == 0 ? 1 : heads;
-    const int bk = attn_block_keys(m) > kBK2 ? attn_block_keys(m) : kBK2;       // the larger padding covers both kernels
-    const long long Mp = ((long long)(m + 1) + bk - 1) / bk * bk;
+    const long long Mp = ((long long)(m + 1) + kBK - 1) / kBK * kBK;
     return 2 * (long long)B * hkv * Mp * kD * (long long)sizeof(__half) + (long long)B * (Mp / 32) * (long long)sizeof(uint32_t);
 }
 
-bool attention_tc_supported(int n, int ldq, int ldo, long long q_bs, const void* mask) {
-    (void)mask;                  // key masks are handled in-kernel (validity bits written by attn_prep_kernel)
+bool attention_tc_supported(int n, int ldq, int ldo, long long q_bs) {
     return n > 0 && (n % kBQ) == 0 && (ldq % 8) == 0 && (ldo % 8) == 0 && q_bs == (long long)n * ldq;
-}
-
-template <int BK, bool ONLINE>
-static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnArgs& a, dim3 grid,
-                       cudaStream_t st) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(attn_tc_kernel<BK, ONLINE>, cudaFuncAttributeMaxDynamicSharedMemorySize, AC<BK>::kSmemBytes) !=
-            cudaSuccess)
-            return -10;
-        attr_set = true;
-    }
-    launch_k(attn_tc_kernel<BK, ONLINE>, grid, kThreads, AC<BK>::kSmemBytes, st, tmQ, tmK, tmV, a);
-    return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
 int attention_tc_fwd(const __half* q, long long q_bs, int ldq, const __half* k, const __half* v, long long kv_bs, int ldkv,
                      int kv_hs, const float* null_kv, const uint8_t* key_mask, int B, int heads, int n, int m, __half* out,
-                     long long o_bs, int ldo,
-                     void* workspace, long long workspace_bytes, int* err_flag, cudaStream_t st) {
-    if (!attention_tc_supported(n, ldq, ldo, q_bs, nullptr) || (o_bs % 8) || (reinterpret_cast<uintptr_t>(q) & 15) ||
+                     long long o_bs, int ldo, void* workspace, long long workspace_bytes, int* err_flag, cudaStream_t st) {
+    if (!attention_tc_supported(n, ldq, ldo, q_bs) || (o_bs % 8) || (reinterpret_cast<uintptr_t>(q) & 15) ||
         (reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(workspace) & 127))
         return -1;
     if (workspace_bytes < attention_tc_workspace_bytes(B, heads, kv_hs, m)) return -1;
     PFN_tmaEncodeTiled enc = get_tma_encode();
-    if (!enc) return -5;
+    if (!enc) return -1;
     const int hkv = kv_hs == 0 ? 1 : heads;
-    static const bool pair_ok = [] { const char* e = getenv("MI_ATTN_PAIR"); return !(e && e[0] == '0'); }();
-    const bool two_tiles = pair_ok && n % kBQ2 == 0;         // two query tiles per CTA, 128-key blocks (attn_tc2_kernel)
-    const int bk = two_tiles ? kBK2 : attn_block_keys(m);
-    const int Mp = (m + 1 + bk - 1) / bk * bk;
+    const int Mp = (m + 1 + kBK - 1) / kBK * kBK;
     __half* Kp = reinterpret_cast<__half*>(workspace);
     __half* Vt = Kp + (long long)B * hkv * Mp * kD;
     uint32_t* valid = reinterpret_cast<uint32_t*>(Vt + (long long)B * hkv * Mp * kD);      // [B][Mp / 32]
-    {
-        dim3 grid(Mp / 64, B * hkv);
-        launch_k(attn_prep_kernel, grid, 256, 0, st, k, v, kv_bs, ldkv, kv_hs, null_kv, hkv, m, Mp, Kp, Vt, key_mask, valid);
-        if (cudaGetLastError() != cudaSuccess) return -2;
-    }
+    launch_k(attn_prep_kernel, dim3(Mp / 64, B * hkv), 256, 0, st, k, v, kv_bs, ldkv, kv_hs, null_kv, hkv, m, Mp, Kp, Vt,
+             key_mask, valid);
+    if (cudaGetLastError() != cudaSuccess) return -2;
+
     CUtensorMap tmQ, tmK, tmV;
     cuuint32_t estr[2] = {1, 1};
     {
@@ -833,16 +280,16 @@ int attention_tc_fwd(const __half* q, long long q_bs, int ldq, const __half* k, 
         if (enc(&tmQ, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(q), dim, str, box, estr,
                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return -6;
+            return -1;
     }
     {
         cuuint64_t dim[2] = {kD, (cuuint64_t)B * hkv * Mp};
         cuuint64_t str[1] = {kD * 2};
-        cuuint32_t box[2] = {kD, (cuuint32_t)bk};
+        cuuint32_t box[2] = {kD, kBK};
         if (enc(&tmK, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, Kp, dim, str, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) !=
             CUDA_SUCCESS)
-            return -6;
+            return -1;
     }
     {
         cuuint64_t dim[2] = {(cuuint64_t)Mp, (cuuint64_t)B * hkv * kD};
@@ -851,34 +298,19 @@ int attention_tc_fwd(const __half* q, long long q_bs, int ldq, const __half* k, 
         if (enc(&tmV, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, Vt, dim, str, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) !=
             CUDA_SUCCESS)
-            return -6;
+            return -1;
     }
     AttnArgs a{};
-    a.n = n; a.heads = heads; a.hkv = hkv; a.Mp = Mp; a.nblk = Mp / bk; a.kv_len = m + 1; a.batch = B;
-    a.out = out; a.o_bs = o_bs; a.ldo = ldo; a.err = err_flag;
-    static const int poly = [] { const char* e = getenv("MI_ATTN_POLY"); return e ? atoi(e) : 1; }();    // MI_ATTN_POLY=0: MUFU only
-    a.poly = poly;
-    a.valid = valid;
-    if (two_tiles) {
-        static bool attr_set2 = false;
-        if (!attr_set2) {
-            if (cudaFuncSetAttribute(attn_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem2Bytes) != cudaSuccess) return -10;
-            attr_set2 = true;
-        }
-        // persistent CTAs (one per SM) stream over the (query pair-tile, head, batch) work items; MI_ATTN_PERSISTENT=0: one each
-        static const bool persistent = [] { const char* e = getenv("MI_ATTN_PERSISTENT"); return !(e && e[0] == '0'); }();
-        int dev = 0, num_sms = 148;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-        const long long total_work = (long long)(n / kBQ2) * heads * B;
-        const unsigned grid2 = (unsigned)(persistent && total_work > num_sms ? num_sms : total_work);
-        launch_k(attn_tc2_kernel, dim3(grid2), kThreads2, kSmem2Bytes, st, tmQ, tmK, tmV, a);
-        return cudaGetLastError() == cudaSuccess ? 0 : -2;
+    a.n = n; a.heads = heads; a.hkv = hkv; a.Mp = Mp; a.nblk = Mp / kBK;
+    a.out = out; a.o_bs = o_bs; a.ldo = ldo; a.valid = valid; a.err = err_flag;
+    static bool attr_set = false;
+    if (!attr_set) {
+        if (cudaFuncSetAttribute(attn_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
+            return -2;
+        attr_set = true;
     }
-    dim3 grid(n / kBQ, heads, B);
-    static const bool two_sweep = [] { const char* e = getenv("MI_ATTN_TWO_SWEEP"); return e && e[0] == '1'; }();
-    if (two_sweep) return bk == 256 ? launch_attn<256, false>(tmQ, tmK, tmV, a, grid, st) : launch_attn<128, false>(tmQ, tmK, tmV, a, grid, st);
-    return bk == 256 ? launch_attn<256, true>(tmQ, tmK, tmV, a, grid, st) : launch_attn<128, true>(tmQ, tmK, tmV, a, grid, st);
+    launch_k(attn_wg_kernel, dim3(n / kBQ, heads, B), kThreads, kSmemBytes, st, tmQ, tmK, tmV, a);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
 }  // namespace mi

@@ -1,6 +1,6 @@
 // Backward kernels of the TRAINING side of the path (SURVEY.md 8f-2: Imagen.forward / _p_losses, reference
 // minimagen/Imagen.py:512-650, and autograd through Unet.forward).  fp32 on CUDA cores, NHWC like the forward kernels.
-// (Data gradients of tensor-core-shaped convolutions do not come through here: they run on the forward tcgen05 implicit-GEMM
+// (Data gradients of tensor-core-shaped convolutions do not come through here: they run on the forward wgmma implicit-GEMM
 // kernels with flipped / transposed packed weights, see minimagen_b200/autograd.py.)
 //
 //   gemm_f32            C[z] (+)= alpha * op(A[z]) op(B[z]), arbitrary element strides, two-level batch index
@@ -22,6 +22,14 @@
 #include "launch.cuh"
 
 namespace mi {
+
+// SM count of the current device (grid sizing of the split reductions)
+static int num_sms() {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n > 0 ? n : 132;
+}
 
 namespace {
 
@@ -561,7 +569,7 @@ int conv2d_wgrad_f32(const float* dy, const float* x, int B, int Hi, int Wi, int
     const bool flat = Cin < kWgT && KH * KW > 1;
     if (flat) {
         const int tiles = ((Cout + kWgT - 1) / kWgT) * ((Cin * KH * KW + kWgT - 1) / kWgT);
-        long long splits = (16 * 148 + tiles - 1) / tiles;
+        long long splits = (16LL * num_sms() + tiles - 1) / tiles;
         const long long max_splits = (total + 4 * kWgP - 1) / (4 * kWgP);
         if (splits > max_splits) splits = max_splits;
         if (splits < 1) splits = 1;
@@ -575,7 +583,7 @@ int conv2d_wgrad_f32(const float* dy, const float* x, int B, int Hi, int Wi, int
     const int tiles = ((Cout + kWgT - 1) / kWgT) * ((Cin + kWgT - 1) / kWgT);
     // 256-thread blocks with 8 KB of shared memory: ~8 resident per SM -> aim at two full waves of those (the ragged layers that
     // land here -- 3-channel stem / 3-channel output, 15 x 15 taps -- have few (tile, tap) pairs and long pixel loops)
-    long long splits = (16 * 148 + tiles * KH * KW - 1) / (tiles * KH * KW);
+    long long splits = (16LL * num_sms() + tiles * KH * KW - 1) / (tiles * KH * KW);
     const long long max_splits = (total + 4 * kWgP - 1) / (4 * kWgP);
     if (splits > max_splits) splits = max_splits;
     if (splits < 1) splits = 1;
@@ -595,7 +603,7 @@ int gn_silu_bwd(const float* x, const float* dy, const double* sums, int B, int 
     float* A = workspace;                                   // [B][C][2]
     float* gm = workspace + (long long)B * C * 2;           // [B][groups][4]: m1, m2, mean, rstd
     const int blocks_xy = ((C + 31) / 32) * B;
-    int Z = (8 * 148 + blocks_xy - 1) / blocks_xy;          // ~8 blocks per SM over the whole grid
+    int Z = (8 * num_sms() + blocks_xy - 1) / blocks_xy;          // ~8 blocks per SM over the whole grid
     if (Z > HW / 64) Z = HW / 64;
     if (Z < 1) Z = 1;
     if (Z > 1 && cudaMemsetAsync(A, 0, (size_t)B * C * 2 * sizeof(float), st) != cudaSuccess) return -2;
@@ -613,7 +621,7 @@ int ln_rows_bwd(const float* in, const float* dy, long long R, int C, const floa
                 float* dgamma, float* dbeta, cudaStream_t st) {
     if (C < 1 || (size_t)2 * C * sizeof(float) > 48 * 1024) return -1;
     long long blocks = (R + 7) / 8;
-    if (blocks > 2 * 148) blocks = 2 * 148;
+    if (blocks > 2 * num_sms()) blocks = 2 * num_sms();
     launch_k(ln_bwd_kernel, (unsigned)blocks, 256, (size_t)2 * C * sizeof(float), st, in, dy, R, C, gamma, eps, pre_gelu, dx,
              dgamma, dbeta);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;

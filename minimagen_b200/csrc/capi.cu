@@ -49,7 +49,7 @@ int mi_device_ok(void) {
     int dev = 0, major = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return 0;
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-    return major == 10;
+    return major == 9;
 }
 
 int mi_pack_conv_weight_dgrad_f16(const float* w, int c_out, int c_in, int kh, int kw, void* out, void* stream) {
@@ -77,7 +77,7 @@ static int igemm_common(const void* act, int B, int H, int W, int lda, int c_off
     p.act2 = act2; p.lda2 = lda2; p.a_chan_off2 = c_off2; p.Cin1 = c_in1; p.stats = out_stats;
     if (out_stats && (out_sc > 1 || (c_out % 32) != 0)) return fail(-8, "mi_conv2d_igemm_f16: out_stats needs channel-contiguous output and c_out % 32 == 0");
     if (out_stats && ((long long)H * W) % 32 != 0)
-        return fail(-8, "mi_conv2d_igemm_f16: out_stats needs H*W % 32 == 0 (a warp's 32 output rows must belong to one image)");
+        return fail(-8, "mi_conv2d_igemm_f16: out_stats needs H*W % 32 == 0 (a warp's output rows must belong to one image)");
     p.out_f32 = out_f32; p.out_f16 = (__half*)out_f16; p.bias = bias; p.residual = residual;
     p.out_sb = out_sb; p.out_sh = out_sh; p.out_sw = out_sw; p.out_sc = out_sc; p.n_valid = n_valid;
     p.block_n_hint = block_n; p.err_flag = err_flag;
@@ -126,11 +126,6 @@ static int igemm_common(const void* act, int B, int H, int W, int lda, int c_off
     if (out_sc <= 1 && ((out_sw % 4) || (out_sh % 4) || (out_sb % 4)))
         return fail(-8, "mi_conv2d_igemm_f16: channel-contiguous output strides must be multiples of 4 elements");
     if (out_sc > 1 && residual) return fail(-8, "mi_conv2d_igemm_f16: residual needs channel-contiguous output");
-    // kernel selection (measured on B200, profiles/r01_conv_tc_selftest_v9.log): 3x3 layers run fastest on the swapped-operand
-    // halo kernel (needs C_out % 128 == 0, H % 32 == 0), C_out = 128 / 16 layers it cannot take on the pixel-major halo
-    // kernel, everything else on the CTA-pair kernel (all chosen inside conv_tc_launch)
-    p.halo = (mode == 0 && kh == 3 && kw == 3) ? 1 : ((mode == 0 && kh == 15 && kw == 1) ? 3 : 0);   // 3: 15-tap vertical (stem)
-    if (mode >= 2 && mode <= 5 && !getenv("MI_SUBPIX_PAIR")) p.halo = 4;   // sub-pixel phase on the swapped-operand kernel (32 x 8 tiles)
     const int rc = mi::conv_tc_launch(p, S(stream));
     if (rc != 0) return fail(rc, mi::conv_tc_strerror(rc));
     return 0;
@@ -148,7 +143,7 @@ int mi_conv2d_igemm_f16(const void* act, int B, int H, int W, int lda, int c_off
 
 int mi_conv3x3_res1x1_supported(int H, int W, int c_in, int c_out, int x_cin) {
     const bool t16 = W == 16 && H % 16 == 0, t32 = !t16 && H % 32 == 0 && W % 8 == 0;
-    return (t16 || t32) && c_in > 0 && c_in % 64 == 0 && x_cin > 0 && x_cin % 64 == 0 && c_out % 128 == 0;
+    return (t16 || t32) && mi::conv_tc_supported(H, W, c_in, c_out) && x_cin > 0 && x_cin % 64 == 0 && c_out % 128 == 0;
 }
 
 int mi_conv3x3_res1x1_f16(const void* act, int B, int H, int W, int lda, int c_in, const void* act2, int lda2, int c_in1,
@@ -179,9 +174,7 @@ int mi_conv3x3_gn_silu_f16(const float* src0, int c0, const float* src1, int c1,
     p.ss_ld = scale_shift_ld; p.eps = eps; p.wpacked = w; p.Cout = c_out; p.bias = bias; p.residual = residual;
     p.out_f32 = out_f32; p.out_f16 = (__half*)out_f16; p.out_stats = out_stats; p.err_flag = err_flag;
     if (scale_shift && scale_shift_ld < 2 * (c0 + c1)) return fail(-8, "mi_conv3x3_gn_silu_f16: scale_shift_ld < 2*C");
-    // C_out % 256 == 0: the CTA-pair kernel (half the prologue per tensor FLOP); otherwise the single-CTA kernel
-    const bool pair = mi::conv_gn_pair_supported(H, W, c0, c1, c_out, groups) && !getenv("MI_GN_NO_PAIR");
-    const int rc = pair ? mi::conv_gn_pair_launch(p, S(stream)) : mi::conv_gn_launch(p, S(stream));
+    const int rc = mi::conv_gn_launch(p, S(stream));
     if (rc != 0) return fail(rc, rc == -3 ? "mi_conv3x3_gn_silu_f16: unsupported geometry (see mi_conv3x3_gn_supported)"
                                           : mi::conv_tc_strerror(rc));
     return 0;
@@ -262,14 +255,14 @@ long long mi_attention_workspace_bytes(int B, int heads, int kv_head_stride, int
 int mi_attention_fwd(const void* q, long long q_bs, int ldq, const void* k, const void* v, long long kv_bs, int ldkv,
                      int kv_head_stride, const float* null_kv, const uint8_t* key_mask, int B, int heads, int n, int m,
                      void* out, long long o_bs, int ldo, void* workspace, long long workspace_bytes, void* stream) {
-    // tcgen05 path (key masks included) when the shape allows and the caller lends the operand workspace; mma.sync kernel otherwise
-    // (short key sequences -- one 128-key block -- stay on the mma.sync kernel: 19 us vs 33 us at n = 256, m = 59)
-    if (workspace && m >= 128 && mi::attention_tc_supported(n, ldq, ldo, q_bs, key_mask) &&
+    // wgmma path (key masks included) when the shape allows and the caller lends the operand workspace; mma.sync kernel otherwise
+    // (short key sequences -- one 128-key block -- stay on the mma.sync kernel)
+    if (workspace && m >= 128 && mi::attention_tc_supported(n, ldq, ldo, q_bs) &&
         workspace_bytes >= mi::attention_tc_workspace_bytes(B, heads, kv_head_stride, m))
         return check(mi::attention_tc_fwd((const __half*)q, q_bs, ldq, (const __half*)k, (const __half*)v, kv_bs, ldkv,
                                           kv_head_stride, null_kv, key_mask, B, heads, n, m, (__half*)out, o_bs, ldo, workspace,
                                           workspace_bytes, nullptr, S(stream)),
-                     "mi_attention_fwd (tcgen05)");
+                     "mi_attention_fwd (wgmma)");
     return check(mi::attention_fwd((const __half*)q, q_bs, ldq, (const __half*)k, (const __half*)v, kv_bs, ldkv,
                                    kv_head_stride, null_kv, key_mask, B, heads, n, m, (__half*)out, o_bs, ldo, S(stream)),
                  "mi_attention_fwd");

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05 + TMEM), im2col-free.
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma + TMA), im2col-free.
 //
 // Replaces every dense `nn.Conv2d` / `nn.Linear` on the U-Net hot path whose channel counts are multiples of 64
 // (reference call sites: minimagen/layers.py:129 (Block.project 3x3), :415 (res_conv 1x1), :319 (Downsample 4x4 s2),
@@ -10,890 +10,385 @@
 //   * one A tile (128 pixels x 64 channels) for tap (dh, dw) is ONE TMA box load from the 5-D tensor
 //     (C, W, H, P, B) at coordinates (c0, w0 + dw, h0 + dh, p, b0): TMA zero-fills out-of-bounds coordinates, which
 //     IS the convolution's zero padding -- no im2col buffer, no halo handling in the kernel;
-//   * stride-2 convs read a phase-split copy of the input (P = 4 phases) so that every tap is again a unit-stride box;
+//   * stride-2 convs read a phase-split copy of the input (P = 4 phases), or the un-split input with TMA element strides 2,
+//     so that every tap is again one box;
 //   * weights are pre-packed [C_out][taps*C_in] fp16 (K-major), one 2-D TMA box (64 x BLOCK_N) per k-block;
-//   * both operands land in shared memory in the 128-byte-swizzled K-major layout that tcgen05.mma consumes directly;
-//   * accumulators: fp32 in TMEM, double-buffered (2 x BLOCK_N columns) so the epilogue of tile i overlaps the
-//     main loop of tile i+1; persistent CTAs (one per SM) walk the tile list round-robin.
+//   * both operands land in shared memory in the 128-byte-swizzled K-major layout wgmma reads directly;
+//   * a folded 1x1 conv (ResnetBlock.res_conv) appends k-blocks of a second operand x, read at the centre tap;
+//   * persistent CTAs (one per SM) walk the tile list round-robin; the producer runs ahead through the operand ring while
+//     the consumers store the previous tile.
 //
-// Warp roles (256 threads): warp0 = TMA producer (1 lane), warp1 = MMA issuer (1 lane), warp2 = TMEM allocator,
-// warps 4-7 = epilogue (TMEM -> registers -> +bias +residual -> global fp32 and/or fp16).
+// Warp roles (384 threads): warpgroup 0 = producer (one elected lane issues the TMA loads), warpgroups 1 and 2 = consumers,
+// each owning 64 of the 128 pixel rows: wgmma m64nBLOCK_Nk16 with fp32 accumulators in registers, then
+// +bias +residual -> global fp32 and/or fp16 (+ GroupNorm block statistics) straight from the accumulator fragments.
+//
+// Fused GroupNorm variant (Block.forward, minimagen/layers.py:131-145: GroupNorm -> (scale + 1, shift) -> SiLU -> 3x3 conv):
+// the whole producer warpgroup builds the A tile instead of TMA -- it reads the fp32 NHWC source(s) (optionally the virtual
+// concat cat(x, skip * s), Unet.py:445), applies y = SiLU(x * A[b,c] + Bc[b,c]) with per-(image, channel) coefficients folded
+// from the producers' GroupNorm block statistics, affine, FiLM and skip scale, and writes fp16 in the swizzled layout; the
+// normalised tensor never exists in HBM.
 #include "conv_tc.cuh"
 
 #include <cuda_runtime.h>
 #include <mutex>
 #include <stdio.h>
 
-#include "conv_epilogue.cuh"
 #include "kernels.cuh"
-#include "ptx.cuh"
 #include "launch.cuh"
+#include "ptx.cuh"
 #include "sat_half.cuh"
+#include "wgmma.cuh"
 
 namespace mi {
 
 namespace {
 
-constexpr int kNumThreads = 128 + 32 * 8;   // warps 0-3: TMA / MMA / TMEM-alloc / spare, warps 4-11: epilogue
-constexpr uint32_t kABytes = kConvBlockM * kConvBlockK * 2;   // 16 KiB per stage
-constexpr uint32_t kRingBudget = 192 * 1024;                   // shared memory for the operand rings (+ patches + barriers <= 227 KB)
+constexpr int kNumThreads = 384;                               // warpgroup 0: producer, 1-2: consumers
+constexpr uint32_t kABytes = kConvBlockM * kConvBlockK * 2;    // 16 KiB per stage
+constexpr uint32_t kRingBudget = 192 * 1024;                   // operand ring (+ barriers + GN coefficients <= 227 KB)
+constexpr uint32_t kAuxBytes = 512;                            // barriers [0, 256), GroupNorm mean / rstd [256, 512)
+constexpr uint32_t kSmemMax = 227 * 1024;
 
 template <int BLOCK_N>
 struct Cfg {
     static constexpr uint32_t kBBytes = BLOCK_N * kConvBlockK * 2;
     static constexpr uint32_t kStageBytes = kABytes + kBBytes;
-    // fill ~192 KiB with stages
     static constexpr int kStages = (kRingBudget / kStageBytes) > 8 ? 8 : (kRingBudget / kStageBytes);
-    static constexpr uint32_t kTmemCols = (2 * BLOCK_N) < 32 ? 32 : (2 * BLOCK_N);   // powers of two for our BLOCK_Ns
-    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kEpiBytes;
+    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + kAuxBytes;   // + 8 * C_in (GN)
 };
 
-template <int BLOCK_N>
+__device__ __forceinline__ float silu(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
+
+template <int BLOCK_N, bool GN>
 __global__ void __launch_bounds__(kNumThreads, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvTcArgs args) {
+conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmX,
+               const __grid_constant__ CUtensorMap tmX2, const __grid_constant__ ConvTcArgs args,
+               const __grid_constant__ GnPrologueArgs gn) {
     using C = Cfg<BLOCK_N>;
     constexpr int STAGES = C::kStages;
+    static_assert(2 * STAGES * 8 <= 256, "barrier block overlaps the GroupNorm scratch");
 
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024-byte aligned stage bases
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::kStageBytes);
-    uint64_t* full_bar = bars;                    // [STAGES]  TMA -> MMA
-    uint64_t* empty_bar = bars + STAGES;          // [STAGES]  MMA -> TMA
-    uint64_t* tfull_bar = bars + 2 * STAGES;      // [2]       MMA -> epilogue
-    uint64_t* tempty_bar = bars + 2 * STAGES + 2; // [2]       epilogue -> MMA
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-    float* epi_stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256) + (((threadIdx.x >> 5) + 4) & 7) * 32 * kEpiLd;
+    uint64_t* full_bar = bars;                    // [STAGES]  producer -> consumers
+    uint64_t* empty_bar = bars + STAGES;          // [STAGES]  consumers -> producer (one arrival per consumer warpgroup)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     int* err = args.err_flag;
 
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmA2);
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < STAGES; ++i) {
-            ptx::mbar_init(&full_bar[i], 1);
-            ptx::mbar_init(&empty_bar[i], 1);
+        if (!GN) {
+            ptx::prefetch_tensormap(&tmA);
+            ptx::prefetch_tensormap(&tmA2);
         }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&tfull_bar[i], 1);
-            ptx::mbar_init(&tempty_bar[i], 32 * kEpiWarps);
+        for (int i = 0; i < STAGES; ++i) {
+            // GN: the four producer warps' arrivals + the weight load's expect_tx arrival
+            ptx::mbar_init(&full_bar[i], GN ? 5 : 1);
+            ptx::mbar_init(&empty_bar[i], 2);
         }
         ptx::fence_barrier_init();
     }
-    if (warp == 2) {
-        ptx::tmem_alloc(tmem_ptr_smem, C::kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     pdl_wait();      // everything above is independent of the previous kernel's output
 
-    const int num_kb = args.num_taps * args.chunks_per_tap;
+    const int num_tap_kb = args.num_taps * args.chunks_per_tap;
+    const int num_kb = num_tap_kb + args.x_chunks;
     const int tiles_m = args.tiles_w * args.tiles_h * args.tiles_b;
     const int total_tiles = tiles_m * args.tiles_n;
     const int BW = 1 << args.bw_log2, BH = 1 << args.bh_log2;
     const int BB = kConvBlockM >> (args.bw_log2 + args.bh_log2);
 
-    if (warp == 0) {
-        // ===================== TMA producer (warp stays converged, one elected lane issues) =====================
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int nt = tile % args.tiles_n;
-            const int mt = tile / args.tiles_n;
-            const int w0 = (mt % args.tiles_w) * BW;
-            const int h0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
-            const int b0 = (mt / (args.tiles_w * args.tiles_h)) * BB;
-            const int n0 = nt * BLOCK_N;
-            int kb = 0;
-            for (int t = 0; t < args.num_taps; ++t) {
-                const int dh = args.dh[t], dw = args.dw[t], ph = args.ph[t];
-                for (int j = 0; j < args.chunks_per_tap; ++j, ++kb) {
-                    ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 100 + stage);
-                    if (ptx::elect_one()) {
-                        uint8_t* sa = smem + stage * C::kStageBytes;
-                        uint8_t* sb = sa + kABytes;
-                        if ((args.dbg & 1) && (tile != (int)blockIdx.x || kb >= STAGES)) {
-                            ptx::mbar_arrive(&full_bar[stage]);      // DEBUG: no data movement, MMA reuses stale smem
-                        } else {
+    if (wg == 0) {
+        if constexpr (!GN) {
+            // ===================== TMA producer (warp 0 stays converged, one elected lane issues) =====================
+            if (warp == 0) {
+                int stage = 0;
+                uint32_t phase = 0;
+                for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+                    const int nt = tile % args.tiles_n;
+                    const int mt = tile / args.tiles_n;
+                    const int w0 = (mt % args.tiles_w) * BW;
+                    const int h0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
+                    const int b0 = (mt / (args.tiles_w * args.tiles_h)) * BB;
+                    const int n0 = nt * BLOCK_N;
+                    for (int kb = 0; kb < num_kb; ++kb) {
+                        ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 100 + stage);
+                        if (ptx::elect_one()) {
+                            uint8_t* sa = smem + stage * C::kStageBytes;
+                            uint8_t* sb = sa + kABytes;
                             ptx::mbar_arrive_expect_tx(&full_bar[stage], C::kStageBytes);
-                            if (j < args.a_split)
-                                ptx::tma_load_5d(&tmA, &full_bar[stage], sa, args.a_chan_off + j * kConvBlockK, w0 * args.in_stride + dw,
-                                                 h0 * args.in_stride + dh, ph, b0);
-                            else   // second half of a virtual channel concat (skip connection)
-                                ptx::tma_load_5d(&tmA2, &full_bar[stage], sa,
-                                                 args.a_chan_off2 + (j - args.a_split) * kConvBlockK, w0 * args.in_stride + dw,
-                                                 h0 * args.in_stride + dh, ph,
-                                                 b0);
+                            if (kb < num_tap_kb) {
+                                const int t = kb / args.chunks_per_tap, j = kb - t * args.chunks_per_tap;
+                                const int cw = w0 * args.in_stride + args.dw[t], ch = h0 * args.in_stride + args.dh[t];
+                                if (j < args.a_split)
+                                    ptx::tma_load_5d(&tmA, &full_bar[stage], sa, args.a_chan_off + j * kConvBlockK, cw, ch,
+                                                     args.ph[t], b0);
+                                else   // second half of a virtual channel concat (skip connection)
+                                    ptx::tma_load_5d(&tmA2, &full_bar[stage], sa,
+                                                     args.a_chan_off2 + (j - args.a_split) * kConvBlockK, cw, ch, args.ph[t], b0);
+                            } else {   // folded 1x1 conv: k-chunk jx of x at the centre tap
+                                const int jx = kb - num_tap_kb;
+                                if (jx < args.x_split)
+                                    ptx::tma_load_5d(&tmX, &full_bar[stage], sa, args.x_chan_off + jx * kConvBlockK, w0, h0, 0, b0);
+                                else
+                                    ptx::tma_load_5d(&tmX2, &full_bar[stage], sa,
+                                                     args.x_chan_off2 + (jx - args.x_split) * kConvBlockK, w0, h0, 0, b0);
+                            }
                             ptx::tma_load_2d(&tmB, &full_bar[stage], sb, kb * kConvBlockK, n0);
                         }
+                        if (++stage == STAGES) { stage = 0; phase ^= 1; }
                     }
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
+                pdl_trigger();      // last loads issued: the next kernel may be scheduled behind this one's final tile(s)
             }
-        }
-        pdl_trigger();      // last loads issued: the next kernel may be scheduled behind this one's final tile(s)
-    } else if (warp == 1) {
-        // ===================== MMA issuer (warp stays converged, one elected lane issues) =====================
-        constexpr uint32_t idesc = ptx::make_idesc_f16(kConvBlockM, BLOCK_N, 0 /*fp16*/);
-        int stage = 0;
-        uint32_t phase = 0;
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tempty_bar[as], aphase ^ 1, err, 200 + as);
-            ptx::tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BLOCK_N;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                ptx::mbar_wait(&full_bar[stage], phase, err, 300 + stage);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes);
-                    const uint64_t da = ptx::make_kmajor_sw128_desc(sa);
-                    const uint64_t db = ptx::make_kmajor_sw128_desc(sa + kABytes);
-#pragma unroll
-                    for (int k = 0; k < kConvBlockK / 16; ++k) {
-                        // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
-                        // profiling bit 3: odd k-steps accumulate into the OTHER TMEM buffer (two independent chains)
-                        const uint32_t d = ((args.dbg & 8) && (k & 1)) ? tmem_base + (as ^ 1) * BLOCK_N : tmem_d;
-                        ptx::umma_f16(d, da + 2 * k, db + 2 * k, idesc, (kb | (k >> ((args.dbg & 8) ? 1 : 0))) != 0);
-                    }
-                    ptx::umma_commit(&empty_bar[stage]);             // frees the smem slot when these MMAs retire
-                    if (kb == num_kb - 1) ptx::umma_commit(&tfull_bar[as]);   // accumulator complete
-                }
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue =====================
-        const int ew = warp & 3;                 // TMEM lane quarter this warp may access
-        const int c_half = (BLOCK_N >= 64) ? BLOCK_N / 2 : BLOCK_N;   // warps 4-7: first half of the columns, 8-11: second
-        const int c_begin = (BLOCK_N >= 64 && warp >= 8) ? c_half : 0;
-        const int c_end = (BLOCK_N >= 64) ? c_begin + c_half : (warp >= 8 ? 0 : BLOCK_N);
-        const int m = ew * 32 + lane;            // row of the tile == TMEM lane
-        const int bw = m & (BW - 1);
-        const int bh = (m >> args.bw_log2) & (BH - 1);
-        const int bb = m >> (args.bw_log2 + args.bh_log2);
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int nt = tile % args.tiles_n;
-            const int mt = tile / args.tiles_n;
-            const int w = (mt % args.tiles_w) * BW + bw;
-            const int h = ((mt / args.tiles_w) % args.tiles_h) * BH + bh;
-            const int b = (mt / (args.tiles_w * args.tiles_h)) * BB + bb;
-            const int n0 = nt * BLOCK_N;
-            const bool valid = (b < args.B) && (h < args.H) && (w < args.W);
-            const long long pix = (long long)b * args.out_sb + (long long)h * args.out_sh + (long long)w * args.out_sw;
-
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tfull_bar[as], aphase, err, 400 + as);
-            ptx::tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BLOCK_N;
-            if (!(args.dbg & 2)) epilogue_tile<BLOCK_N>(args, taddr, n0, pix, valid, epi_stage, c_begin, c_end, b);   // DEBUG bit 1: skip the epilogue
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tempty_bar[as]);
-        }
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, C::kTmemCols);
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------ 2-CTA variant
-// cta_group::2: a pair of CTAs (one cluster, two SMs of a TPC) computes a 256-pixel x BLOCK_N tile.  Each CTA stages its
-// own 128-pixel A tile and HALF of the weight tile (BLOCK_N/2 rows); one tcgen05.mma issued by the leader CTA consumes
-// both CTAs' shared memory and writes 128 accumulator rows into each CTA's TMEM.  Versus the 1-CTA kernel this halves
-// the weight bytes each SM pulls from L2 and the shared-memory operand traffic per FLOP (see DESIGN.md 4.1).
-template <int BLOCK_N, int KC>
-struct Cfg2 {
-    static constexpr uint32_t kBBytes = (BLOCK_N / 2) * kConvBlockK * 2;       // one 64-channel atom of the half weight tile
-    static constexpr uint32_t kStageBytes = KC * (kABytes + kBBytes);          // KC 64-channel k-chunks per pipeline stage
-    static constexpr int kStages = (kRingBudget / kStageBytes) > 8 ? 8 : (kRingBudget / kStageBytes);
-    static constexpr uint32_t kTmemCols = 2 * BLOCK_N;
-    static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + 256 + kEpiBytes;
-};
-
-template <int BLOCK_N, int KC>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kNumThreads, 1)
-conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvTcArgs args) {
-    using C = Cfg2<BLOCK_N, KC>;
-    constexpr int STAGES = C::kStages;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::kStageBytes);
-    uint64_t* full_bar = bars;                     // used in the leader CTA only
-    uint64_t* empty_bar = bars + STAGES;           // per CTA
-    uint64_t* tfull_bar = bars + 2 * STAGES;       // per CTA
-    uint64_t* tempty_bar = bars + 2 * STAGES + 2;  // used in the leader CTA only
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-    float* epi_stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256) + (((threadIdx.x >> 5) + 4) & 7) * 32 * kEpiLd;
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t rank = ptx::cluster_ctarank();
-    const bool leader = rank == 0;
-    int* err = args.err_flag;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < STAGES; ++i) {
-            ptx::mbar_init(&full_bar[i], 2);      // leader's expect_tx arrive + peer's remote arrive
-            ptx::mbar_init(&empty_bar[i], 1);     // one multicast tcgen05.commit
-        }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(&tfull_bar[i], 1);
-            ptx::mbar_init(&tempty_bar[i], 2 * 32 * kEpiWarps);  // epilogue threads of both CTAs
-        }
-        ptx::fence_barrier_init();
-    }
-    ptx::cluster_sync_all();                      // barrier inits visible cluster-wide before any remote arrive / TMA
-    if (warp == 2) {
-        ptx::tmem_alloc_2sm(tmem_ptr_smem, C::kTmemCols);
-        ptx::tmem_relinquish_2sm();
-    }
-    ptx::tc_fence_before();
-    ptx::cluster_sync_all();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    pdl_wait();      // everything above is independent of the previous kernel's output
-
-    const int num_st = args.num_taps * args.chunks_per_tap / KC;      // pipeline stages (KC k-chunks each) per tile
-    const int tiles_m = args.tiles_w * args.tiles_h * args.tiles_b;
-    const int pairs_m = (tiles_m + 1) >> 1;
-    const int total_pairs = pairs_m * args.tiles_n;
-    const int BW = 1 << args.bw_log2, BH = 1 << args.bh_log2;
-    const int BB = kConvBlockM >> (args.bw_log2 + args.bh_log2);
-    const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs; converged warp, one elected lane issues) =====================
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int pt = cluster_id; pt < total_pairs; pt += num_clusters) {
-            const int s0 = 0, s1 = num_st;
-            const int nt = pt % args.tiles_n;
-            const int mt = 2 * (pt / args.tiles_n) + (int)rank;      // may be == tiles_m (dummy tile: all OOB)
-            const int w0 = (mt % args.tiles_w) * BW;
-            const int h0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
-            const int b0 = (mt / (args.tiles_w * args.tiles_h)) * BB;
-            const int n0 = nt * BLOCK_N + (int)rank * (BLOCK_N / 2);
-            int kb = s0 * KC;
-            int t = kb / args.chunks_per_tap;
-            int j = kb - t * args.chunks_per_tap;
-            for (int s = s0; s < s1; ++s, kb += KC) {
-                const int dh = args.dh[t], dw = args.dw[t], ph = args.ph[t];
-                ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 1100 + stage);
-                if (ptx::elect_one()) {
-                    uint8_t* sa = smem + stage * C::kStageBytes;
-                    uint8_t* sb = sa + KC * kABytes;
-                    if (leader) ptx::mbar_arrive_expect_tx(&full_bar[stage], 2 * C::kStageBytes);
-#pragma unroll
-                    for (int kc = 0; kc < KC; ++kc) {
-                        const int jj = j + kc;
-                        if (jj < args.a_split)
-                            ptx::tma_load_5d_2sm(&tmA, &full_bar[stage], sa + kc * kABytes,
-                                                 args.a_chan_off + jj * kConvBlockK, w0 * args.in_stride + dw,
-                                                 h0 * args.in_stride + dh, ph, b0);
-                        else
-                            ptx::tma_load_5d_2sm(&tmA2, &full_bar[stage], sa + kc * kABytes,
-                                                 args.a_chan_off2 + (jj - args.a_split) * kConvBlockK, w0 * args.in_stride + dw,
-                                                 h0 * args.in_stride + dh,
-                                                 ph, b0);
-                        ptx::tma_load_2d_2sm(&tmB, &full_bar[stage], sb + kc * C::kBBytes, (kb + kc) * kConvBlockK, n0);
-                    }
-                    if (!leader) ptx::mbar_arrive_cluster(&full_bar[stage], 0);
-                }
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                j += KC;
-                if (j >= args.chunks_per_tap) { j = 0; ++t; }
-            }
-        }
-        pdl_trigger();      // last loads issued: the next kernel may be scheduled behind this one's final tile(s)
-    } else if (warp == 1) {
-        if (leader) {
-            // ===================== MMA issuer (leader CTA; converged warp, one elected lane issues) =====================
-            constexpr uint32_t idesc = ptx::make_idesc_f16(256, BLOCK_N, 0);
+        } else {
+            // ===================== GroupNorm / FiLM / SiLU producer: fp32 global -> fp16 swizzled A tile =====================
+            // A tile row m (pixel) occupies bytes [128 m, 128 m + 128); its 16-byte chunk q (channels 8q .. 8q+7) sits at
+            // position q ^ (m & 7) -- the layout TMA's SWIZZLE_128B writes, so the consumers are the same for both producers.
+            float* s_mean = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);   // [32]
+            float* s_rstd = s_mean + 32;                                                        // [32]
+            float* sA = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + kAuxBytes); // A[C] then Bc[C]
+            const int tt = threadIdx.x;                 // 0..127
+            const int lq = tt & 7;                      // channels [8 lq, 8 lq + 8) of the k-chunk
+            const int prow = tt >> 3;                   // rows prow + 16 i, i = 0..7
+            const int C0 = gn.C0, C1 = gn.C1, Ctot = C0 + C1, Cg = Ctot / gn.groups;
+            const int H = args.H, W = args.W;
+            float* sB = sA + Ctot;
             int stage = 0;
             uint32_t phase = 0;
-            int iter = 0;
-            for (int pt = cluster_id; pt < total_pairs; pt += num_clusters, ++iter) {
-                const int s0 = 0, s1 = num_st;
-                const int as = iter & 1;
-                const uint32_t aphase = (iter >> 1) & 1;
-                ptx::mbar_wait(&tempty_bar[as], aphase ^ 1, err, 1200 + as);
-                ptx::tc_fence_after();
-                const uint32_t tmem_d = tmem_base + as * BLOCK_N;
-                for (int s = s0; s < s1; ++s) {
-                    ptx::mbar_wait(&full_bar[stage], phase, err, 1300 + stage);
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one()) {
-                        const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes);
-#pragma unroll
-                        for (int kc = 0; kc < KC; ++kc) {
-                            const uint64_t da = ptx::make_kmajor_sw128_desc(sa + kc * kABytes);
-                            const uint64_t db = ptx::make_kmajor_sw128_desc(sa + KC * kABytes + kc * C::kBBytes);
-#pragma unroll
-                            for (int k = 0; k < kConvBlockK / 16; ++k)
-                                ptx::umma_f16_2sm(tmem_d, da + 2 * k, db + 2 * k, idesc, ((s - s0) | kc | k) != 0);
+            int cur_b = -1;
+            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+                const int nt = tile % args.tiles_n;
+                const int mt = tile / args.tiles_n;
+                const int w0 = (mt % args.tiles_w) * BW;
+                const int h0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
+                const int b = mt / (args.tiles_w * args.tiles_h);      // one image per tile (H * W >= 128)
+                const int n0 = nt * BLOCK_N;
+                if (b != cur_b) {
+                    // coefficient table of image b for all input channels: y = SiLU(x * A[c] + Bc[c]) (the arithmetic of
+                    // gn_apply_silu_kernel); rebuilt only when the image changes
+                    ptx::bar_sync(1, 128);                 // every producer thread has finished reading the previous table
+                    if (tt < gn.groups) {
+                        const int g = tt;
+                        double su = 0.0, sq = 0.0;
+                        const int lo = g * Cg, hi = lo + Cg;
+                        const int lo0 = min(lo, C0), hi0 = min(hi, C0);
+                        for (int e = lo0 / 16; e < hi0 / 16; ++e) {
+                            su += gn.stats0[((long long)b * (C0 / 16) + e) * 2];
+                            sq += gn.stats0[((long long)b * (C0 / 16) + e) * 2 + 1];
                         }
-                        ptx::umma_commit_2sm(&empty_bar[stage], 3);               // frees this stage in BOTH CTAs
-                        if (s + 1 == s1) ptx::umma_commit_2sm(&tfull_bar[as], 3);
+                        const int lo1 = max(lo, C0) - C0, hi1 = max(hi, C0) - C0;
+                        for (int e = lo1 / 16; e < hi1 / 16; ++e) {
+                            su += (double)gn.scale1 * gn.stats1[((long long)b * (C1 / 16) + e) * 2];
+                            sq += (double)gn.scale1 * (double)gn.scale1 * gn.stats1[((long long)b * (C1 / 16) + e) * 2 + 1];
+                        }
+                        const double n = (double)Cg * H * W;
+                        const double mean = su / n;
+                        double var = sq / n - mean * mean;
+                        if (var < 0) var = 0;
+                        s_mean[g] = (float)mean;
+                        s_rstd[g] = (float)(1.0 / sqrt(var + (double)gn.eps));
                     }
+                    ptx::bar_sync(1, 128);
+                    for (int cc = tt; cc < Ctot; cc += 128) {
+                        const int g = cc / Cg;
+                        float a = s_rstd[g] * gn.gamma[cc];
+                        float bb = gn.beta[cc] - s_mean[g] * a;
+                        if (gn.scale_shift) {
+                            const float sc = gn.scale_shift[(long long)b * gn.ss_ld + cc] + 1.0f;
+                            const float shv = gn.scale_shift[(long long)b * gn.ss_ld + Ctot + cc];
+                            a *= sc;
+                            bb = bb * sc + shv;
+                        }
+                        if (cc >= C0) a *= gn.scale1;                     // skip * 2^-1/2 folded into the multiplier
+                        sA[cc] = a;
+                        sB[cc] = bb;
+                    }
+                    cur_b = b;
+                    ptx::bar_sync(1, 128);
+                }
+                const long long img = (long long)b * H * W;
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    const int t = kb / args.chunks_per_tap, j = kb - t * args.chunks_per_tap;
+                    const int dh = args.dh[t], dw = args.dw[t];
+                    const float* cA = sA + j * kConvBlockK + lq * 8;
+                    const float* cB = sB + j * kConvBlockK + lq * 8;
+                    const float4 a0 = *reinterpret_cast<const float4*>(cA), a1 = *reinterpret_cast<const float4*>(cA + 4);
+                    const float4 b0 = *reinterpret_cast<const float4*>(cB), b1 = *reinterpret_cast<const float4*>(cB + 4);
+                    const bool first = j < args.a_split;
+                    const int Cs = first ? C0 : C1;
+                    const float* src = (first ? gn.src0 + (long long)j * kConvBlockK
+                                              : gn.src1 + (long long)(j - args.a_split) * kConvBlockK) + img * Cs + lq * 8;
+
+                    ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 600 + stage);
+                    uint8_t* sa = smem + stage * C::kStageBytes;
+                    if (warp == 0 && ptx::elect_one()) {
+                        ptx::mbar_arrive_expect_tx(&full_bar[stage], C::kBBytes);
+                        ptx::tma_load_2d(&tmB, &full_bar[stage], sa + kABytes, kb * kConvBlockK, n0);
+                    }
+                    float4 x0[8], x1[8];
+                    bool ok[8];
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int m = i * 16 + prow;
+                        const int gw = w0 + (m & (BW - 1)) + dw;
+                        const int gh = h0 + ((m >> args.bw_log2) & (BH - 1)) + dh;
+                        ok[i] = gh >= 0 && gh < H && gw >= 0 && gw < W;
+                        if (ok[i]) {
+                            const float4* s4 = reinterpret_cast<const float4*>(src + ((long long)gh * W + gw) * Cs);
+                            x0[i] = __ldg(s4);
+                            x1[i] = __ldg(s4 + 1);
+                        }
+                    }
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int m = i * 16 + prow;
+                        uint4 o = make_uint4(0u, 0u, 0u, 0u);
+                        if (ok[i]) {
+                            const __half2 h0_ = sat_half2(silu(fmaf(x0[i].x, a0.x, b0.x)), silu(fmaf(x0[i].y, a0.y, b0.y)));
+                            const __half2 h1_ = sat_half2(silu(fmaf(x0[i].z, a0.z, b0.z)), silu(fmaf(x0[i].w, a0.w, b0.w)));
+                            const __half2 h2_ = sat_half2(silu(fmaf(x1[i].x, a1.x, b1.x)), silu(fmaf(x1[i].y, a1.y, b1.y)));
+                            const __half2 h3_ = sat_half2(silu(fmaf(x1[i].z, a1.z, b1.z)), silu(fmaf(x1[i].w, a1.w, b1.w)));
+                            o.x = *reinterpret_cast<const uint32_t*>(&h0_); o.y = *reinterpret_cast<const uint32_t*>(&h1_);
+                            o.z = *reinterpret_cast<const uint32_t*>(&h2_); o.w = *reinterpret_cast<const uint32_t*>(&h3_);
+                        }
+                        *reinterpret_cast<uint4*>(sa + m * 128 + ((lq ^ (m & 7)) << 4)) = o;
+                    }
+                    ptx::fence_proxy_async_smem();        // generic-proxy stores -> visible to wgmma (async proxy)
+                    __syncwarp();
+                    if (lane == 0) ptx::mbar_arrive(&full_bar[stage]);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
+            pdl_trigger();
         }
-    } else if (warp >= 4) {
-        // ===================== epilogue (both CTAs, own 128 rows) =====================
-        const int ew = warp & 3;
-        const int c_half = BLOCK_N / 2;
-        const int c_begin = warp >= 8 ? c_half : 0;
-        const int c_end = c_begin + c_half;
-        const int m = ew * 32 + lane;
-        const int bw = m & (BW - 1);
-        const int bh = (m >> args.bw_log2) & (BH - 1);
-        const int bb = m >> (args.bw_log2 + args.bh_log2);
-        int iter = 0;
-        for (int pt = cluster_id; pt < total_pairs; pt += num_clusters, ++iter) {
-            const int nt = pt % args.tiles_n;
-            const int mt = 2 * (pt / args.tiles_n) + (int)rank;
-            const int w = (mt % args.tiles_w) * BW + bw;
-            const int h = ((mt / args.tiles_w) % args.tiles_h) * BH + bh;
-            const int b = (mt / (args.tiles_w * args.tiles_h)) * BB + bb;
-            const int n0 = nt * BLOCK_N;
-            const bool valid = (mt < tiles_m) && (b < args.B) && (h < args.H) && (w < args.W);
-            const long long pix = (long long)b * args.out_sb + (long long)h * args.out_sh + (long long)w * args.out_sw;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tfull_bar[as], aphase, err, 1400 + as);
-            ptx::tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BLOCK_N;
-            epilogue_tile<BLOCK_N>(args, taddr, n0, pix, valid, epi_stage, c_begin, c_end, b);
-            ptx::tc_fence_before();
-            ptx::mbar_arrive_cluster(&tempty_bar[as], 0);                    // the leader's barrier
+    } else {
+        // ===================== consumers: rows [64 cw, 64 cw + 64) of every tile =====================
+        const int cw = wg - 1;
+        const int wq = warp & 3;                        // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
+        const int cq = 2 * (lane & 3);                  // first of this thread's two columns in every 8-column group
+        float acc[BLOCK_N / 2];
+        int stage = 0;
+        uint32_t phase = 0;
+        // epilogue geometry of this thread's two rows (m, m + 8) of the tile
+        int m_r[2], bw_r[2], bh_r[2], bb_r[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            m_r[r] = cw * 64 + wq * 16 + (lane >> 2) + 8 * r;
+            bw_r[r] = m_r[r] & (BW - 1);
+            bh_r[r] = (m_r[r] >> args.bw_log2) & (BH - 1);
+            bb_r[r] = m_r[r] >> (args.bw_log2 + args.bh_log2);
         }
-    }
+        const int m_warp = cw * 64 + wq * 16;           // the warp's 16 rows belong to one image (stats need H*W % 32 == 0)
+        const int bb_warp = m_warp >> (args.bw_log2 + args.bh_log2);
+        const bool vec = args.out_sc == 1 && ((reinterpret_cast<uintptr_t>(args.out_f32) & 7) == 0) &&
+                         ((reinterpret_cast<uintptr_t>(args.residual) & 7) == 0) &&
+                         ((reinterpret_cast<uintptr_t>(args.out_f16) & 3) == 0);
 
-    ptx::tc_fence_before();
-    ptx::cluster_sync_all();
-    if (warp == 2) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc_2sm(tmem_base, C::kTmemCols);
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------ 3x3 halo variant
-// 3x3 / stride 1 / pad 1 only (92 % of the SR U-Net's FLOPs).  Instead of fetching nine shifted 128-pixel A tiles per
-// 64-channel chunk, ONE (16+2) x (8+2) pixel halo tile is fetched (TMA box 64 x 10 x 18, zero-filled outside the image)
-// and the nine taps are nine tcgen05.mma descriptor windows into it: output tile = 16 rows x 8 columns, so each 8-pixel
-// row segment of a window is exactly one 8 x 128 B swizzle atom, consecutive segments are one halo row (10 x 128 B =
-// 1280 B = the descriptor's stride-byte-offset) apart, and tap (r, s) starts (r*10 + s) * 128 B into the tile.  The
-// 128B swizzle is a function of the shared-memory address bits, so TMA's write pattern and the shifted MMA reads agree.
-// A traffic per chunk drops from 9 x 16 KB to 22.5 KB.
-constexpr int kHaloTH = 16, kHaloTW = 8, kHaloW = kHaloTW + 2, kHaloH = kHaloTH + 2;
-constexpr uint32_t kHaloABytes = kHaloH * kHaloW * 128;                       // 23040
-constexpr uint32_t kHaloAStride = (kHaloABytes + 1023) & ~1023u;              // 23552
-
-// BLOCK_N == 16 (final_conv, C_out = 3 padded to 16): the whole weight matrix (9 taps x <= 4 chunks x 2 KB) stays RESIDENT
-// in shared memory -- it is loaded once per CTA, the B pipeline (18 small TMA round trips per 128-pixel tile, which made
-// this layer latency-bound at 15 % of HBM speed) disappears and the freed barriers/stages deepen the A ring.
-constexpr int kHaloResChunks = 4;
-template <int BLOCK_N>
-struct CfgH {
-    static constexpr bool kBRes = BLOCK_N == 16;
-    static constexpr uint32_t kBBytes = BLOCK_N * kConvBlockK * 2;
-    static constexpr int kAStages = kBRes ? 5 : 3;
-    static constexpr int kBStages = kBRes ? 9 * kHaloResChunks
-        : ((kRingBudget - kAStages * kHaloAStride) / kBBytes > 8 ? 8 : (kRingBudget - kAStages * kHaloAStride) / kBBytes);
-    static constexpr uint32_t kTmemCols = (2 * BLOCK_N) < 32 ? 32 : (2 * BLOCK_N);
-    static constexpr uint32_t kSmemBytes = kAStages * kHaloAStride + kBStages * kBBytes + 1024 + 256 + kEpiBytes;
-};
-
-__device__ __forceinline__ uint64_t make_halo_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((kHaloW * 128u) >> 4) << 32;   // SBO: one halo row between 8-pixel row segments
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-
-template <int BLOCK_N>
-__global__ void __launch_bounds__(kNumThreads, 1)
-conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ ConvTcArgs args) {
-    using C = CfgH<BLOCK_N>;
-    constexpr int NA = C::kAStages, NB = C::kBStages;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* smem_b = smem + NA * kHaloAStride;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + NB * C::kBBytes);
-    uint64_t* fullA = bars;
-    uint64_t* emptyA = bars + NA;
-    constexpr int NBB = C::kBRes ? 1 : NB;          // barriers of the B ring (resident weights: one "loaded" barrier)
-    uint64_t* fullB = bars + 2 * NA;
-    uint64_t* emptyB = bars + 2 * NA + NBB;
-    uint64_t* tfull_bar = bars + 2 * NA + 2 * NBB;
-    static_assert((2 * NA + 2 * NBB + 4) * 8 + 8 <= 256, "barrier block overlaps the epilogue patches");
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    float* epi_stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256) + (((threadIdx.x >> 5) + 4) & 7) * 32 * kEpiLd;
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    int* err = args.err_flag;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < NA; ++i) { ptx::mbar_init(&fullA[i], 1); ptx::mbar_init(&emptyA[i], 1); }
-        for (int i = 0; i < NBB; ++i) { ptx::mbar_init(&fullB[i], 1); ptx::mbar_init(&emptyB[i], 1); }
-        for (int i = 0; i < 2; ++i) { ptx::mbar_init(&tfull_bar[i], 1); ptx::mbar_init(&tempty_bar[i], 32 * kEpiWarps); }
-        ptx::fence_barrier_init();
-    }
-    if (warp == 2) {
-        ptx::tmem_alloc(tmem_ptr_smem, C::kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    pdl_wait();      // everything above is independent of the previous kernel's output
-
-    const int chunks = args.chunks_per_tap;
-    const int tiles_m = args.tiles_w * args.tiles_h * args.tiles_b;
-    const int total_tiles = tiles_m * args.tiles_n;
-    const int Cin = chunks * kConvBlockK;
-
-    if (warp == 0) {
-        // ===================== TMA producer (converged warp, one elected lane issues) =====================
-        int sa = 0, sb = 0;
-        uint32_t pa = 0, pb = 0;
-        if constexpr (C::kBRes) {
-            // resident weights: tile (j, t) at slot j*9 + t, all on one barrier (tiles_n == 1)
-            if (ptx::elect_one()) {
-                ptx::mbar_arrive_expect_tx(&fullB[0], 9 * chunks * C::kBBytes);
-                for (int j = 0; j < chunks; ++j)
-                    for (int t = 0; t < 9; ++t)
-                        ptx::tma_load_2d(&tmB, &fullB[0], smem_b + (j * 9 + t) * C::kBBytes, t * Cin + j * kConvBlockK, 0);
-            }
-        }
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int nt = tile % args.tiles_n;
             const int mt = tile / args.tiles_n;
-            const int w0 = (mt % args.tiles_w) * kHaloTW;
-            const int h0 = ((mt / args.tiles_w) % args.tiles_h) * kHaloTH;
-            const int b0 = mt / (args.tiles_w * args.tiles_h);
             const int n0 = nt * BLOCK_N;
-            for (int j = 0; j < chunks; ++j) {
-                ptx::mbar_wait(&emptyA[sa], pa ^ 1, err, 2100 + sa);
-                if (ptx::elect_one()) {
-                    ptx::mbar_arrive_expect_tx(&fullA[sa], kHaloABytes);
-                    ptx::tma_load_5d(&tmA, &fullA[sa], smem + sa * kHaloAStride, args.a_chan_off + j * kConvBlockK,
-                                     w0 - 1, h0 - 1, 0, b0);
-                }
-                if (++sa == NA) { sa = 0; pa ^= 1; }
-                if constexpr (!C::kBRes) {
-                    for (int t = 0; t < 9; ++t) {
-                        ptx::mbar_wait(&emptyB[sb], pb ^ 1, err, 2200 + sb);
-                        if (ptx::elect_one()) {
-                            ptx::mbar_arrive_expect_tx(&fullB[sb], C::kBBytes);
-                            ptx::tma_load_2d(&tmB, &fullB[sb], smem_b + sb * C::kBBytes, t * Cin + j * kConvBlockK, n0);
+            int prev = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                ptx::mbar_wait(&full_bar[stage], phase, err, 300 + stage);
+                const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes);
+                const uint64_t da = ptx::make_sw128_desc(sa + cw * (64 * 128));
+                const uint64_t db = ptx::make_sw128_desc(sa + kABytes);
+                ptx::wg_fence();
+#pragma unroll
+                for (int k = 0; k < kConvBlockK / 16; ++k)
+                    // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
+                    ptx::Wgmma<BLOCK_N, 0>::run(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+                ptx::wg_commit();
+                ptx::wg_wait<1>();                      // the previous k-block's MMAs have retired: free its stage
+                if (prev >= 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            ptx::wg_wait<0>();
+            ptx::wg_fence_regs(acc);
+            if (prev >= 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[prev]);
+
+            // ---- epilogue: fragment element 4j + 2r + e = row m_r[r], column n0 + 8j + cq + e
+            const int tw0 = (mt % args.tiles_w) * BW;
+            const int th0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
+            const int tb0 = (mt / (args.tiles_w * args.tiles_h)) * BB;
+            bool valid[2];
+            long long pix[2];
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int w = tw0 + bw_r[r], h = th0 + bh_r[r], b = tb0 + bb_r[r];
+                valid[r] = (b < args.B) && (h < args.H) && (w < args.W);
+                pix[r] = (long long)b * args.out_sb + (long long)h * args.out_sh + (long long)w * args.out_sw;
+            }
+            const bool fast = vec && n0 + BLOCK_N <= args.n_valid;
+            float st_s[BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1], st_q[BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1];
+#pragma unroll
+            for (int q = 0; q < BLOCK_N / 16; ++q) { st_s[q] = 0.f; st_q[q] = 0.f; }
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int n = n0 + 8 * j + cq;
+                if (fast) {
+                    float2 bv = make_float2(0.f, 0.f);
+                    if (args.bias) bv = __ldg(reinterpret_cast<const float2*>(args.bias + n));
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        if (!valid[r]) continue;
+                        const long long o = pix[r] + n;
+                        float2 f = make_float2(acc[4 * j + 2 * r] + bv.x, acc[4 * j + 2 * r + 1] + bv.y);
+                        if (args.residual) {
+                            const float2 rv = *reinterpret_cast<const float2*>(args.residual + o);
+                            f.x += rv.x; f.y += rv.y;
                         }
-                        if (++sb == NB) { sb = 0; pb ^= 1; }
+                        st_s[j >> 1] += f.x + f.y;
+                        st_q[j >> 1] += f.x * f.x + f.y * f.y;
+                        if (args.out_f32) *reinterpret_cast<float2*>(args.out_f32 + o) = f;
+                        if (args.out_f16) *reinterpret_cast<__half2*>(args.out_f16 + o) = sat_half2(f.x, f.y);
                     }
-                }
-            }
-        }
-        pdl_trigger();      // last loads issued: the next kernel may be scheduled behind this one's final tile(s)
-    } else if (warp == 1) {
-        // ===================== MMA issuer (converged warp, one elected lane issues) =====================
-        constexpr uint32_t idesc = ptx::make_idesc_f16(kConvBlockM, BLOCK_N, 0);
-        int sa = 0, sb = 0;
-        uint32_t pa = 0, pb = 0;
-        int iter = 0;
-        if constexpr (C::kBRes) ptx::mbar_wait(&fullB[0], 0, err, 2500);     // resident weights have landed
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tempty_bar[as], aphase ^ 1, err, 2300 + as);
-            ptx::tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BLOCK_N;
-            for (int j = 0; j < chunks; ++j) {
-                ptx::mbar_wait(&fullA[sa], pa, err, 2400 + sa);
-                const uint32_t a_base = ptx::smem_u32(smem + sa * kHaloAStride);
-                for (int t = 0; t < 9; ++t) {
-                    if constexpr (C::kBRes) sb = j * 9 + t;
-                    else ptx::mbar_wait(&fullB[sb], pb, err, 2500 + sb);
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one()) {
-                        const uint32_t a_win = a_base + ((t / 3) * kHaloW + (t % 3)) * 128;
-                        const uint64_t da = make_halo_desc(a_win);
-                        const uint64_t db = ptx::make_kmajor_sw128_desc(ptx::smem_u32(smem_b + sb * C::kBBytes));
+                } else {
 #pragma unroll
-                        for (int k = 0; k < kConvBlockK / 16; ++k)
-                            ptx::umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (j | t | k) != 0);
-                        if constexpr (!C::kBRes) ptx::umma_commit(&emptyB[sb]);
-                    }
-                    if constexpr (!C::kBRes) {
-                        if (++sb == NB) { sb = 0; pb ^= 1; }
-                    }
-                }
-                if (ptx::elect_one()) ptx::umma_commit(&emptyA[sa]);
-                if (++sa == NA) { sa = 0; pa ^= 1; }
-            }
-            if (ptx::elect_one()) ptx::umma_commit(&tfull_bar[as]);
-        }
-    } else if (warp >= 4) {
-        const int ew = warp & 3;
-        const int c_half = BLOCK_N / 2;
-        const int c_begin = warp >= 8 ? c_half : 0;
-        const int c_end = c_begin + c_half;
-        const int m = ew * 32 + lane;
-        const int bw = m & (kHaloTW - 1);
-        const int bh = m >> 3;
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int nt = tile % args.tiles_n;
-            const int mt = tile / args.tiles_n;
-            const int w = (mt % args.tiles_w) * kHaloTW + bw;
-            const int h = ((mt / args.tiles_w) % args.tiles_h) * kHaloTH + bh;
-            const int b = mt / (args.tiles_w * args.tiles_h);
-            const int n0 = nt * BLOCK_N;
-            const bool valid = (b < args.B) && (h < args.H) && (w < args.W);
-            const long long pix = (long long)b * args.out_sb + (long long)h * args.out_sh + (long long)w * args.out_sw;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tfull_bar[as], aphase, err, 2600 + as);
-            ptx::tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BLOCK_N;
-            epilogue_tile<BLOCK_N>(args, taddr, n0, pix, valid, epi_stage, c_begin, c_end, b);
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tempty_bar[as]);
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, C::kTmemCols);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------ 3x3 halo, swapped operands
-// For 128-channel outputs the GEMM above is M = 128 pixels x N = 128 channels per instruction, and a tcgen05.mma costs
-// ~100 clk + 0.35 clk per N column on this part (profiles/r01_conv_tc_bottleneck_study.md): N = 128 tops out near 1.0
-// PFLOP/s.  So this variant computes the TRANSPOSED tile  D^T[128 channels][256 pixels] = W[128][K] x Act^T :
-//   * the "A" operand (M = 128 rows) is the 128 x 64 weight tile of one (tap, chunk),
-//   * the "B" operand (N = 256 rows) is a window of a (32+2) x (8+2)-pixel halo tile: 32 row segments of 8 pixels, one
-//     halo row (1280 B) apart -- the same shifted-descriptor trick as conv3x3_halo_kernel, now with N = 256,
-//   * the accumulator holds channels in TMEM lanes and pixels in columns, which is exactly what an NHWC store wants: a
-//     warp-wide tcgen05.ld hands lane c the value of channel c for 32 pixels, so every global access of the epilogue is one
-//     pixel's 32 consecutive channels (128 B) -- no shared-memory transposition at all.
-// The virtual concat (two activation tensors) is supported: chunk j >= a_split comes from the second tensor map.
-// Geometry G32x8: 32 x 8 output pixels from one (34 x 10)-pixel halo tile per chunk (SBO = one halo row).
-// Geometry G16x16 (16-pixel-wide images): a halo row is then 18 pixels, not a whole number of 8-pixel segments, so the
-// tile is fetched three times per chunk -- shifted by dw = -1 / 0 / +1 pixel, 18 rows x exactly 16 pixels each (TMA
-// zero-fills the out-of-image column) -- and tap (dh, dw) reads rows dh.. of the dw copy: 32 segments at the standard
-// 1024-byte stride.  2.5x the activation bytes into shared memory, still less L2 traffic than pixel-major tiles.
-constexpr int kHtPix = 256;                                                   // UMMA N
-// Geometry V15 (the stem, CrossEmbedLayer as a 15-tap vertical conv over the 128-wide unrolled operand): 32 x 8 output
-// pixels from a (32+14) x 8 tile; tap dh is the window that starts dh rows in (segments at the standard 1024-byte stride).
-// Geometry Sub (one sub-pixel phase of "nearest x2 up-sampling + 3x3 conv", ABI modes 2..5): 2 x 2 taps on the LOW-RES tensor; a
-// 32 x 8 tile reads a (32+1) x (8+1) halo tile whose origin is the phase's first tap; tap (r, s) starts (r*9 + s) pixels in,
-// segments one 9-pixel halo row apart; the epilogue writes every second pixel / row of the 2H x 2W output (caller's strides).
-enum { kG32x8 = 0, kG16x16 = 1, kGV15 = 2, kGSub = 4 };
-template <int G>
-struct CfgT {
-    static constexpr bool kW16 = G == kG16x16;
-    static constexpr int kTaps = G == kGV15 ? 15 : (G == kGSub ? 4 : 9);
-    static constexpr int kTH = kW16 ? 16 : 32, kTW = kW16 ? 16 : 8;           // output tile
-    static constexpr int kBoxH = G == kGV15 ? kTH + 14 : (G == kGSub ? kTH + 1 : kTH + 2);
-    static constexpr int kBoxW = G == kG32x8 ? 10 : (kW16 ? 16 : (G == kGSub ? 9 : 8));       // TMA box (pixels)
-    static constexpr uint32_t kHaloBytes = kBoxH * kBoxW * 128;               // 43520 / 36864 / 47104
-    static constexpr uint32_t kHaloStride = (kHaloBytes + 1023) & ~1023u;
-    static constexpr uint32_t kWBytes = 128 * kConvBlockK * 2;                // one (tap, chunk) weight tile
-    static constexpr int kHStages = kW16 ? 3 : 2;
-    static constexpr int kWStages = (kRingBudget - kHStages * kHaloStride) / kWBytes;   // 6 / 5 / 6
-    static constexpr uint32_t kTmemCols = 2 * kHtPix;                         // 512: two accumulator stages
-    static constexpr uint32_t kSmemBytes = kHStages * kHaloStride + kWStages * kWBytes + 1024 + 256;
-};
-
-__device__ __forceinline__ uint64_t make_halo_t_desc(uint32_t smem_addr, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;        // stride between 8-pixel row segments
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-
-template <int G>
-__global__ void __launch_bounds__(kNumThreads, 1)
-conv3x3_halo_t_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                      const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmX,
-                      const __grid_constant__ CUtensorMap tmX2, const __grid_constant__ ConvTcArgs args) {
-    using C = CfgT<G>;
-    constexpr bool kW16 = C::kW16;
-    constexpr int NH = C::kHStages, NW = C::kWStages;
-    constexpr int kLoads = kW16 ? 3 : 1;           // activation tile loads per 64-channel chunk
-    constexpr int kTapsPerLoad = C::kTaps / kLoads;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* smem_w = smem + NH * C::kHaloStride;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_w + NW * C::kWBytes);
-    uint64_t* fullH = bars;
-    uint64_t* emptyH = bars + NH;
-    uint64_t* fullW = bars + 2 * NH;
-    uint64_t* emptyW = bars + 2 * NH + NW;
-    uint64_t* tfull_bar = bars + 2 * NH + 2 * NW;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    static_assert((2 * NH + 2 * NW + 4) * 8 + 8 <= 256, "barrier block too large");
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    int* err = args.err_flag;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tmA);
-        ptx::prefetch_tensormap(&tmB);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < NH; ++i) { ptx::mbar_init(&fullH[i], 1); ptx::mbar_init(&emptyH[i], 1); }
-        for (int i = 0; i < NW; ++i) { ptx::mbar_init(&fullW[i], 1); ptx::mbar_init(&emptyW[i], 1); }
-        for (int i = 0; i < 2; ++i) { ptx::mbar_init(&tfull_bar[i], 1); ptx::mbar_init(&tempty_bar[i], 32 * kEpiWarps); }
-        ptx::fence_barrier_init();
-    }
-    if (warp == 2) {
-        ptx::tmem_alloc(tmem_ptr_smem, C::kTmemCols);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    pdl_wait();      // everything above is independent of the previous kernel's output
-
-    const int chunks = args.chunks_per_tap;
-    const int tiles_m = args.tiles_w * args.tiles_h * args.tiles_b;
-    const int total_tiles = tiles_m * args.tiles_n;
-    const int Cin = chunks * kConvBlockK;
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        int sh = 0, sw = 0;
-        uint32_t ph = 0, pw = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int nt = tile % args.tiles_n;
-            const int mt = tile / args.tiles_n;
-            const int w0 = (mt % args.tiles_w) * C::kTW;
-            const int h0 = ((mt / args.tiles_w) % args.tiles_h) * C::kTH;
-            const int b0 = mt / (args.tiles_w * args.tiles_h);
-            const int n0 = nt * 128;
-            for (int j = 0; j < chunks; ++j) {
-                for (int l = 0; l < kLoads; ++l) {
-                    ptx::mbar_wait(&emptyH[sh], ph ^ 1, err, 3100 + sh);
-                    if (ptx::elect_one()) {
-                        const int wc = kW16 ? w0 + l - 1 : (G == kGV15 ? w0 : (G == kGSub ? w0 + args.dw[0] : w0 - 1));   // G16x16: copy l is shifted by dw = l - 1
-                        const int hc = G == kGV15 ? h0 - 7 : (G == kGSub ? h0 + args.dh[0] : h0 - 1);          // Sub: origin = the phase's first tap
-                        ptx::mbar_arrive_expect_tx(&fullH[sh], C::kHaloBytes);
-                        if (j < args.a_split)
-                            ptx::tma_load_5d(&tmA, &fullH[sh], smem + sh * C::kHaloStride,
-                                             args.a_chan_off + j * kConvBlockK, wc, hc, 0, b0);
-                        else
-                            ptx::tma_load_5d(&tmA2, &fullH[sh], smem + sh * C::kHaloStride,
-                                             args.a_chan_off2 + (j - args.a_split) * kConvBlockK, wc, hc, 0, b0);
-                    }
-                    if (++sh == NH) { sh = 0; ph ^= 1; }
-                    for (int u = 0; u < kTapsPerLoad; ++u) {
-                        const int t = kW16 ? u * 3 + l : u;             // tap index in the packed weights (dh*3 + dw)
-                        ptx::mbar_wait(&emptyW[sw], pw ^ 1, err, 3200 + sw);
-                        if (ptx::elect_one()) {
-                            ptx::mbar_arrive_expect_tx(&fullW[sw], C::kWBytes);
-                            ptx::tma_load_2d(&tmB, &fullW[sw], smem_w + sw * C::kWBytes, t * Cin + j * kConvBlockK, n0);
+                    for (int r = 0; r < 2; ++r) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            if (!valid[r] || n + e >= args.n_valid) continue;
+                            float f = acc[4 * j + 2 * r + e] + (args.bias ? __ldg(args.bias + n + e) : 0.f);
+                            const long long o = pix[r] + (long long)(n + e) * args.out_sc;
+                            if (args.residual && args.out_sc == 1) f += args.residual[o];
+                            st_s[j >> 1] += f;
+                            st_q[j >> 1] += f * f;
+                            if (args.out_f32) args.out_f32[o] = f;
+                            if (args.out_f16) args.out_f16[o] = sat_half(f);
                         }
-                        if (++sw == NW) { sw = 0; pw ^= 1; }
                     }
-                }
-            }
-            if constexpr (G == kG32x8 || G == kG16x16) {
-                // folded 1x1 conv (res_conv): one halo tile (the dw = 0 copy for 16-wide images) + one weight tile per chunk of x
-                for (int jx = 0; jx < args.x_chunks; ++jx) {
-                    ptx::mbar_wait(&emptyH[sh], ph ^ 1, err, 3150 + sh);
-                    if (ptx::elect_one()) {
-                        ptx::mbar_arrive_expect_tx(&fullH[sh], C::kHaloBytes);
-                        if (jx < args.x_split)
-                            ptx::tma_load_5d(&tmX, &fullH[sh], smem + sh * C::kHaloStride, args.x_chan_off + jx * kConvBlockK,
-                                             kW16 ? w0 : w0 - 1, h0 - 1, 0, b0);
-                        else
-                            ptx::tma_load_5d(&tmX2, &fullH[sh], smem + sh * C::kHaloStride,
-                                             args.x_chan_off2 + (jx - args.x_split) * kConvBlockK, kW16 ? w0 : w0 - 1, h0 - 1, 0, b0);
-                    }
-                    if (++sh == NH) { sh = 0; ph ^= 1; }
-                    ptx::mbar_wait(&emptyW[sw], pw ^ 1, err, 3250 + sw);
-                    if (ptx::elect_one()) {
-                        ptx::mbar_arrive_expect_tx(&fullW[sw], C::kWBytes);
-                        ptx::tma_load_2d(&tmB, &fullW[sw], smem_w + sw * C::kWBytes, C::kTaps * Cin + jx * kConvBlockK, n0);
-                    }
-                    if (++sw == NW) { sw = 0; pw ^= 1; }
-                }
-            }
-        }
-        pdl_trigger();      // last loads issued: the next kernel may be scheduled behind this one's final tile(s)
-    } else if (warp == 1) {
-        // ===================== MMA issuer: D^T[128 ch][256 px] += W_tile[128][64] x window^T =====================
-        constexpr uint32_t idesc = ptx::make_idesc_f16(128, kHtPix, 0);
-        int sh = 0, sw = 0;
-        uint32_t ph = 0, pw = 0;
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tempty_bar[as], aphase ^ 1, err, 3300 + as);
-            ptx::tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * kHtPix;
-            for (int j = 0; j < chunks; ++j) {
-                for (int l = 0; l < kLoads; ++l) {
-                    ptx::mbar_wait(&fullH[sh], ph, err, 3400 + sh);
-                    const uint32_t h_base = ptx::smem_u32(smem + sh * C::kHaloStride);
-                    for (int u = 0; u < kTapsPerLoad; ++u) {
-                        ptx::mbar_wait(&fullW[sw], pw, err, 3500 + sw);
-                        ptx::tc_fence_after();
-                        if (ptx::elect_one()) {
-                            const uint64_t da = ptx::make_kmajor_sw128_desc(ptx::smem_u32(smem_w + sw * C::kWBytes));
-                            // G32x8: tap u = dh*3 + dw starts (dh*10 + dw) pixels into the halo tile, segments one halo
-                            // row apart; G16x16: tap (dh = u) of copy dw = l starts dh rows in, segments 1024 B apart
-                            // V15: tap u = dh starts dh rows (8 pixels each) in, segments 1024 B apart
-                            const uint64_t db = kW16 ? make_halo_t_desc(h_base + u * 16 * 128, 1024)
-                                : (G == kGV15 ? make_halo_t_desc(h_base + u * 8 * 128, 1024)
-                                : G == kGSub ? make_halo_t_desc(h_base + ((u >> 1) * C::kBoxW + (u & 1)) * 128, C::kBoxW * 128)
-                                              : make_halo_t_desc(h_base + ((u / 3) * C::kBoxW + (u % 3)) * 128, C::kBoxW * 128));
-#pragma unroll
-                            for (int k = 0; k < kConvBlockK / 16; ++k)
-                                ptx::umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (j | l | u | k) != 0);
-                            ptx::umma_commit(&emptyW[sw]);
-                        }
-                        if (++sw == NW) { sw = 0; pw ^= 1; }
-                    }
-                    if (ptx::elect_one()) ptx::umma_commit(&emptyH[sh]);
-                    if (++sh == NH) { sh = 0; ph ^= 1; }
-                }
-            }
-            if constexpr (G == kG32x8 || G == kG16x16) {
-                for (int jx = 0; jx < args.x_chunks; ++jx) {          // folded 1x1 conv: the centre-tap window of x's halo tile
-                    ptx::mbar_wait(&fullH[sh], ph, err, 3450 + sh);
-                    const uint32_t h_base = ptx::smem_u32(smem + sh * C::kHaloStride);
-                    ptx::mbar_wait(&fullW[sw], pw, err, 3550 + sw);
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one()) {
-                        const uint64_t da = ptx::make_kmajor_sw128_desc(ptx::smem_u32(smem_w + sw * C::kWBytes));
-                        const uint64_t db = kW16 ? make_halo_t_desc(h_base + 16 * 128, 1024)
-                                                 : make_halo_t_desc(h_base + (C::kBoxW + 1) * 128, C::kBoxW * 128);
-#pragma unroll
-                        for (int k = 0; k < kConvBlockK / 16; ++k) ptx::umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, 1);
-                        ptx::umma_commit(&emptyW[sw]);
-                        ptx::umma_commit(&emptyH[sh]);
-                    }
-                    if (++sw == NW) { sw = 0; pw ^= 1; }
-                    if (++sh == NH) { sh = 0; ph ^= 1; }
-                }
-            }
-            if (ptx::elect_one()) ptx::umma_commit(&tfull_bar[as]);
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue: lane = channel, columns = pixels =====================
-        constexpr int kTwLog2 = kW16 ? 4 : 3;
-        const int q = warp & 3;                       // TMEM lane quarter -> channels [32q, 32q + 32) of the tile
-        const int half = warp >= 8 ? 1 : 0;           // pixel columns [128*half, 128*half + 128)
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++iter) {
-            const int nt = tile % args.tiles_n;
-            const int mt = tile / args.tiles_n;
-            const int w0 = (mt % args.tiles_w) * C::kTW;
-            const int h0 = ((mt / args.tiles_w) % args.tiles_h) * C::kTH;
-            const int b = mt / (args.tiles_w * args.tiles_h);
-            const int n = nt * 128 + q * 32 + lane;   // this thread's output channel
-            const float bias_v = args.bias ? __ldg(args.bias + n) : 0.f;
-            const long long base = (long long)b * args.out_sb + (long long)(h0 + half * (C::kTH / 2)) * args.out_sh +
-                                   (long long)w0 * args.out_sw + n;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(&tfull_bar[as], aphase, err, 3600 + as);
-            ptx::tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * kHtPix + half * 128;
-            float st_s = 0.f, st_q = 0.f;
-#pragma unroll 1
-            for (int c = 0; c < 128; c += 32) {       // 32 pixels per step
-                uint32_t v0[16], v1[16];
-                ptx::tmem_ld_x16(taddr + c, v0);
-                ptx::tmem_ld_x16(taddr + c + 16, v1);
-                const long long rowb = base + (long long)(c >> kTwLog2) * args.out_sh;
-                float r[32];
-                if (args.residual) {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i)
-                        r[i] = args.residual[rowb + (long long)(i >> kTwLog2) * args.out_sh +
-                                             (long long)(i & (C::kTW - 1)) * args.out_sw];
-                }
-                ptx::tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float f = __uint_as_float(i < 16 ? v0[i] : v1[i - 16]) + bias_v;
-                    if (args.residual) f += r[i];
-                    st_s += f;
-                    st_q += f * f;
-                    const long long o = rowb + (long long)(i >> kTwLog2) * args.out_sh +
-                                        (long long)(i & (C::kTW - 1)) * args.out_sw;
-                    if (args.out_f32) args.out_f32[o] = f;
-                    if (args.out_f16) args.out_f16[o] = sat_half(f);
                 }
             }
             if (args.stats) {
-                // 16-channel blocks = half warps: lanes 0-15 and 16-31
+                // GroupNorm statistics of the tensor being written, per (image, 16-channel block): the warp's 16 rows x 16
+                // columns of each block reduce over all 32 lanes
+                const int b_img = tb0 + bb_warp;
+                const bool any = __any_sync(0xffffffffu, valid[0] || valid[1]);
 #pragma unroll
-                for (int o = 1; o <= 8; o <<= 1) {
-                    st_s += __shfl_xor_sync(0xffffffffu, st_s, o);
-                    st_q += __shfl_xor_sync(0xffffffffu, st_q, o);
-                }
-                if ((lane & 15) == 0) {
-                    double* dst = args.stats + ((long long)b * args.stats_blocks + (n >> 4)) * 2;
-                    atomicAdd(dst, (double)st_s);
-                    atomicAdd(dst + 1, (double)st_q);
+                for (int q = 0; q < BLOCK_N / 16; ++q) {
+#pragma unroll
+                    for (int o = 1; o <= 16; o <<= 1) {
+                        st_s[q] += __shfl_xor_sync(0xffffffffu, st_s[q], o);
+                        st_q[q] += __shfl_xor_sync(0xffffffffu, st_q[q], o);
+                    }
+                    if (lane == 0 && any) {
+                        double* dst = args.stats + ((long long)b_img * args.stats_blocks + (n0 >> 4) + q) * 2;
+                        atomicAdd(dst, (double)st_s[q]);
+                        atomicAdd(dst + 1, (double)st_q[q]);
+                    }
                 }
             }
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&tempty_bar[as]);
         }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, C::kTmemCols);
     }
 }
 
@@ -922,68 +417,92 @@ int ilog2_exact(int v) {
     return ((1 << l) == v) ? l : -1;
 }
 
-template <int BLOCK_N>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const ConvTcArgs& args,
-           int total_tiles, int num_sms, cudaStream_t stream) {
+int num_sms_of_current_device() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    static int cache[64] = {0};
+    if (dev < 64 && cache[dev] != 0) return cache[dev];
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (dev < 64) cache[dev] = n;
+    return n;
+}
+
+// 128-pixel tile box: BW x BH pixels x BB images
+void tile_geometry(int H, int W, int B, ConvTcArgs& a) {
+    int BW = W >= 128 ? 128 : W;
+    int BH = 128 / BW;
+    if (BH > H) BH = H;
+    const int BB = 128 / (BW * BH);
+    a.bw_log2 = ilog2_exact(BW);
+    a.bh_log2 = ilog2_exact(BH);
+    a.tiles_w = (W + BW - 1) / BW;
+    a.tiles_h = H / BH;
+    a.tiles_b = (B + BB - 1) / BB;
+    a.B = B; a.H = H; a.W = W;
+}
+
+// largest BLOCK_N of {128,64,32,16} dividing C_out that still gives every SM a tile; never shrink below 64 for that.
+// (BLOCK_N = 256 would need 128 accumulator registers per consumer thread and spills at 384 threads per CTA.)
+int pick_block_n(int Cout, int tiles_m, int hint, int num_sms) {
+    const int cands[4] = {128, 64, 32, 16};
+    if (hint < 0) hint = -hint;
+    if (hint > 0 && Cout % hint == 0)
+        for (int i = 0; i < 4; ++i)
+            if (cands[i] == hint) return hint;
+    int block_n = 16;
+    for (int i = 0; i < 4; ++i) {
+        if (Cout % cands[i] != 0) continue;
+        block_n = cands[i];
+        if (tiles_m * (Cout / cands[i]) >= num_sms || cands[i] <= 64) break;
+    }
+    return block_n;
+}
+
+CUresult encode_act(PFN_encodeTiled enc, CUtensorMap* m, const void* ptr, cuuint64_t channels, cuuint64_t ld, int W, int H,
+                    int phases, int B, int in_stride, const ConvTcArgs& a) {
+    // (C, W, H, P, B), fp16, box (64, BW, BH, 1, BB), 128B swizzle, OOB -> zeros.  in_stride == 2 (Downsample read in place):
+    // the tensor is the (2H x 2W) input, the box spans 2*BW x 2*BH pixels and the element strides make TMA keep every second
+    // pixel -> the same 128-pixel tile lands in shared memory
+    const cuuint64_t IS = in_stride;
+    const int BW = 1 << a.bw_log2, BH = 1 << a.bh_log2, BB = kConvBlockM >> (a.bw_log2 + a.bh_log2);
+    cuuint64_t gdim[5] = {channels, (cuuint64_t)W * IS, (cuuint64_t)H * IS, (cuuint64_t)phases, (cuuint64_t)B};
+    cuuint64_t gstr[4] = {ld * 2, (cuuint64_t)W * IS * ld * 2, (cuuint64_t)H * IS * W * IS * ld * 2,
+                          (cuuint64_t)phases * H * IS * W * IS * ld * 2};
+    cuuint32_t box[5] = {kConvBlockK, (cuuint32_t)(BW * IS), (cuuint32_t)(BH * IS), 1, (cuuint32_t)BB};
+    cuuint32_t estr[5] = {1, (cuuint32_t)IS, (cuuint32_t)IS, 1, 1};
+    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(ptr), gdim, gstr, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+CUresult encode_weights(PFN_encodeTiled enc, CUtensorMap* m, const void* ptr, cuuint64_t K, int Cout, int block_n) {
+    cuuint64_t gdim[2] = {K, (cuuint64_t)Cout};
+    cuuint64_t gstr[1] = {K * 2};
+    cuuint32_t box[2] = {kConvBlockK, (cuuint32_t)block_n};
+    cuuint32_t estr[2] = {1, 1};
+    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim, gstr, box, estr,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+template <int BLOCK_N, bool GN>
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const CUtensorMap& tmX,
+           const CUtensorMap& tmX2, const ConvTcArgs& args, const GnPrologueArgs& gn, uint32_t extra_smem,
+           cudaStream_t stream) {
     using C = Cfg<BLOCK_N>;
     static bool attr_set = false;   // per-template-instance; benign race (idempotent call)
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             C::kSmemBytes);
-        if (e != cudaSuccess) return -10;
-        attr_set = true;
-    }
-    const int grid = total_tiles < num_sms ? total_tiles : num_sms;
-    launch_k(conv_tc_kernel<BLOCK_N>, grid, kNumThreads, C::kSmemBytes, stream, tmA, tmA2, tmB, args);
-    return cudaGetLastError() == cudaSuccess ? 0 : -11;
-}
-
-template <int BLOCK_N, int KC>
-int launch2(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const ConvTcArgs& args,
-            int total_pairs, int num_sms, cudaStream_t stream) {
-    using C = Cfg2<BLOCK_N, KC>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(conv_tc2_kernel<BLOCK_N, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes) !=
+        if (cudaFuncSetAttribute(conv_wg_kernel<BLOCK_N, GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) !=
             cudaSuccess)
             return -10;
         attr_set = true;
     }
-    int clusters = num_sms / 2;
-    if (clusters > total_pairs) clusters = total_pairs;
-    launch_k(conv_tc2_kernel<BLOCK_N, KC>, 2 * clusters, kNumThreads, C::kSmemBytes, stream, tmA, tmA2, tmB, args);
-    return cudaGetLastError() == cudaSuccess ? 0 : -11;
-}
-
-template <int BLOCK_N>
-int launch_halo(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvTcArgs& args, int total_tiles, int num_sms,
-                cudaStream_t stream) {
-    using C = CfgH<BLOCK_N>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(conv3x3_halo_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 C::kSmemBytes) != cudaSuccess)
-            return -10;
-        attr_set = true;
-    }
+    const int total_tiles = args.tiles_w * args.tiles_h * args.tiles_b * args.tiles_n;
+    const int num_sms = num_sms_of_current_device();
     const int grid = total_tiles < num_sms ? total_tiles : num_sms;
-    launch_k(conv3x3_halo_kernel<BLOCK_N>, grid, kNumThreads, C::kSmemBytes, stream, tmA, tmB, args);
-    return cudaGetLastError() == cudaSuccess ? 0 : -11;
-}
-
-template <int G>
-int launch_halo_t(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const CUtensorMap& tmX,
-                  const CUtensorMap& tmX2, const ConvTcArgs& args, int total_tiles, int num_sms, cudaStream_t stream) {
-    using C = CfgT<G>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(conv3x3_halo_t_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 C::kSmemBytes) != cudaSuccess)
-            return -10;
-        attr_set = true;
-    }
-    const int grid = total_tiles < num_sms ? total_tiles : num_sms;
-    launch_k(conv3x3_halo_t_kernel<G>, grid, kNumThreads, C::kSmemBytes, stream, tmA, tmA2, tmB, tmX, tmX2, args);
+    launch_k(conv_wg_kernel<BLOCK_N, GN>, grid, kNumThreads, C::kSmemBytes + extra_smem, stream, tmA, tmA2, tmB, tmX, tmX2,
+             args, gn);
     return cudaGetLastError() == cudaSuccess ? 0 : -11;
 }
 
@@ -1002,7 +521,7 @@ const char* conv_tc_strerror(int code) {
         case -6: return "conv_tc: tensor map encode failed (activations)";
         case -7: return "conv_tc: tensor map encode failed (weights)";
         case -8: return "conv_tc: pointer/stride alignment (16 B) violated";
-        case -9: return "conv_tc: folded 1x1 operand needs the swapped-operand 3x3 kernel (C_out % 128, H % 32 / W % 8 or 16x16 tiles)";
+        case -9: return "conv_tc: the folded 1x1 operand needs a stride-1 conv over one phase";
         case -10: return "conv_tc: cudaFuncSetAttribute(max dynamic smem) failed";
         case -11: return "conv_tc: kernel launch failed";
         default: return "conv_tc: unknown error";
@@ -1029,157 +548,10 @@ int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream) {
     PFN_encodeTiled enc = get_encode();
     if (!enc) return -5;
 
-    // ---- 3x3 halo kernel with swapped operands (channels in TMEM lanes): 128-wide channel tiles, H % 32 == 0, W % 8 == 0
-    const bool t16 = p.W == 16 && p.H % 16 == 0;                       // G16x16: one 16 x 16 tile per image (row block)
-    const bool t32 = !t16 && p.H % 32 == 0 && p.W % 8 == 0;            // G32x8
-    const bool v15 = p.halo == 3 && p.num_taps == 15 && t32 && !p.act2;   // 15-tap vertical conv (stem)
-    const bool sub = p.halo == 4 && p.num_taps == 4 && t32 && !p.act2 && !p.x_act;   // one sub-pixel phase of the up-sampling conv
-    if (p.halo && p.halo != 2 && (v15 || sub || (p.halo != 3 && p.halo != 4 && p.num_taps == 9)) && p.phases == 1 && (t16 || t32) &&
-        p.Cout % 128 == 0 && p.out_sc <= 1 && (p.n_valid == 0 || p.n_valid == p.Cout) && p.dbg == 0) {
-        bool canon = true;
-        if (v15) for (int t = 0; t < 15; ++t) canon = canon && p.dh[t] == t - 7 && p.dw[t] == 0 && p.ph[t] == 0;
-        else if (sub) for (int t = 0; t < 4; ++t) canon = canon && p.dh[t] == p.dh[0] + (t >> 1) && p.dw[t] == p.dw[0] + (t & 1) && p.ph[t] == 0;
-        else for (int t = 0; t < 9; ++t) canon = canon && p.dh[t] == t / 3 - 1 && p.dw[t] == t % 3 - 1 && p.ph[t] == 0;
-        if (p.act2 && (p.Cin1 <= 0 || p.Cin1 % kConvBlockK || p.Cin1 >= p.Cin || (p.lda2 % 8) ||
-                       (reinterpret_cast<uintptr_t>(p.act2) & 15)))
-            return -8;
-        if (canon) {
-            ConvTcArgs h{};
-            h.num_taps = p.num_taps; h.chunks_per_tap = p.Cin / kConvBlockK;
-            h.tiles_w = t16 ? 1 : p.W / 8; h.tiles_h = t16 ? p.H / 16 : p.H / 32; h.tiles_b = p.B; h.tiles_n = p.Cout / 128;
-            h.B = p.B; h.H = p.H; h.W = p.W; h.a_chan_off = p.a_chan_off;
-            h.a_split = (p.act2 ? p.Cin1 : p.Cin) / kConvBlockK; h.a_chan_off2 = p.a_chan_off2;
-            h.out_sb = p.out_sb; h.out_sh = p.out_sh; h.out_sw = p.out_sw; h.out_sc = 1; h.n_valid = p.Cout;
-            h.out_f32 = p.out_f32; h.out_f16 = p.out_f16; h.bias = p.bias; h.residual = p.residual; h.err_flag = p.err_flag;
-            h.stats = p.stats; h.stats_blocks = p.Cout / 16;
-            h.dh[0] = p.dh[0]; h.dw[0] = p.dw[0];        // Sub: halo origin relative to the tile (the phase's first tap)
-            int dev = 0, num_sms = 148;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-            CUtensorMap tmA, tmA2, tmB;
-            cuuint32_t box[5] = {kConvBlockK, (cuuint32_t)(t16 ? 16 : (v15 ? 8 : (sub ? 9 : 10))),
-                                 (cuuint32_t)(t16 ? 18 : (v15 ? 46 : (sub ? 33 : 34))), 1, 1};
-            cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-            {
-                cuuint64_t gdim[5] = {(cuuint64_t)p.a_channels, (cuuint64_t)p.W, (cuuint64_t)p.H, 1, (cuuint64_t)p.B};
-                cuuint64_t gstr[4] = {(cuuint64_t)p.lda * 2, (cuuint64_t)p.W * p.lda * 2, (cuuint64_t)p.H * p.W * p.lda * 2,
-                                      (cuuint64_t)p.H * p.W * p.lda * 2};
-                if (enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(p.act), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-                    return -6;
-            }
-            tmA2 = tmA;
-            if (p.act2) {
-                cuuint64_t gdim[5] = {(cuuint64_t)p.lda2, (cuuint64_t)p.W, (cuuint64_t)p.H, 1, (cuuint64_t)p.B};
-                cuuint64_t gstr[4] = {(cuuint64_t)p.lda2 * 2, (cuuint64_t)p.W * p.lda2 * 2, (cuuint64_t)p.H * p.W * p.lda2 * 2,
-                                      (cuuint64_t)p.H * p.W * p.lda2 * 2};
-                if (enc(&tmA2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(p.act2), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-                    return -6;
-            }
-            // folded 1x1 conv over a second operand x (res_conv): same halo geometry, its own tensor map(s)
-            CUtensorMap tmX = tmA, tmX2 = tmA;
-            if (p.x_act) {
-                if (v15 || p.Cx <= 0 || p.Cx % kConvBlockK || (p.x_lda % 8) || (reinterpret_cast<uintptr_t>(p.x_act) & 15)) return -8;
-                if (p.x_act2 && (p.Cx1 <= 0 || p.Cx1 % kConvBlockK || p.Cx1 >= p.Cx || (p.x_lda2 % 8) ||
-                                 (reinterpret_cast<uintptr_t>(p.x_act2) & 15)))
-                    return -8;
-                h.x_chunks = p.Cx / kConvBlockK;
-                h.x_split = (p.x_act2 ? p.Cx1 : p.Cx) / kConvBlockK;
-                h.x_chan_off = p.x_chan_off; h.x_chan_off2 = p.x_chan_off2;
-                for (int which = 0; which < (p.x_act2 ? 2 : 1); ++which) {
-                    const void* ptr = which ? p.x_act2 : p.x_act;
-                    const cuuint64_t ld = which ? p.x_lda2 : p.x_lda;
-                    cuuint64_t gdim[5] = {ld, (cuuint64_t)p.W, (cuuint64_t)p.H, 1, (cuuint64_t)p.B};
-                    cuuint64_t gstr[4] = {ld * 2, (cuuint64_t)p.W * ld * 2, (cuuint64_t)p.H * p.W * ld * 2,
-                                          (cuuint64_t)p.H * p.W * ld * 2};
-                    if (enc(which ? &tmX2 : &tmX, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(ptr), gdim, gstr, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-                        return -6;
-                }
-                if (!p.x_act2) tmX2 = tmX;
-            }
-            const cuuint64_t K = (cuuint64_t)p.num_taps * p.Cin + (p.x_act ? (cuuint64_t)p.Cx : 0);
-            cuuint64_t wdim[2] = {K, (cuuint64_t)p.Cout};
-            cuuint64_t wstr[1] = {K * 2};
-            cuuint32_t wbox[2] = {kConvBlockK, 128};
-            cuuint32_t westr[2] = {1, 1};
-            if (enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(p.wpacked), wdim, wstr, wbox, westr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-                return -7;
-            const int total = h.tiles_w * h.tiles_h * h.tiles_b * h.tiles_n;
-            if (v15) return launch_halo_t<kGV15>(tmA, tmA2, tmB, tmX, tmX2, h, total, num_sms, stream);
-            if (sub) return launch_halo_t<kGSub>(tmA, tmA2, tmB, tmX, tmX2, h, total, num_sms, stream);
-            return t16 ? launch_halo_t<kG16x16>(tmA, tmA2, tmB, tmX, tmX2, h, total, num_sms, stream)
-                       : launch_halo_t<kG32x8>(tmA, tmA2, tmB, tmX, tmX2, h, total, num_sms, stream);
-        }
-    }
-
-    if (p.x_act) return -9;      // the folded 1x1 operand exists only in the swapped-operand 3x3 kernel above
-
-    // ---- 3x3 halo kernel (opt-in via p.halo): needs the canonical 3x3 tap order, H % 16 == 0, W % 8 == 0
-    if (p.halo && !p.act2 && p.num_taps == 9 && p.phases == 1 && p.H % kHaloTH == 0 && p.W % kHaloTW == 0 &&
-        ((p.Cout % 128 == 0 && (p.halo == 2 || p.Cout % 256 != 0)) ||
-         (p.Cout == 16 && p.Cin <= kHaloResChunks * kConvBlockK))) {
-        bool canon = true;
-        for (int t = 0; t < 9; ++t) canon = canon && p.dh[t] == t / 3 - 1 && p.dw[t] == t % 3 - 1 && p.ph[t] == 0;
-        if (canon) {
-            ConvTcArgs h{};
-            h.num_taps = 9; h.chunks_per_tap = p.Cin / kConvBlockK;
-            h.tiles_w = p.W / kHaloTW; h.tiles_h = p.H / kHaloTH; h.tiles_b = p.B;
-            h.B = p.B; h.H = p.H; h.W = p.W; h.a_chan_off = p.a_chan_off;
-            h.out_sb = p.out_sb; h.out_sh = p.out_sh; h.out_sw = p.out_sw;
-            h.out_sc = p.out_sc > 0 ? p.out_sc : 1; h.n_valid = p.n_valid > 0 ? p.n_valid : p.Cout;
-            h.out_f32 = p.out_f32; h.out_f16 = p.out_f16; h.bias = p.bias; h.residual = p.residual; h.err_flag = p.err_flag;
-            h.stats = p.stats; h.stats_blocks = p.Cout / 16;
-            int dev = 0, num_sms = 148;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
-            const int bn = p.Cout == 16 ? 16 : ((p.Cout % 256 == 0 && p.block_n_hint != 128) ? 256 : 128);
-            h.tiles_n = p.Cout / bn;
-            CUtensorMap tmA, tmB;
-            cuuint64_t gdim[5] = {(cuuint64_t)p.a_channels, (cuuint64_t)p.W, (cuuint64_t)p.H, 1, (cuuint64_t)p.B};
-            cuuint64_t gstr[4] = {(cuuint64_t)p.lda * 2, (cuuint64_t)p.W * p.lda * 2, (cuuint64_t)p.H * p.W * p.lda * 2,
-                                  (cuuint64_t)p.H * p.W * p.lda * 2};
-            cuuint32_t box[5] = {kConvBlockK, kHaloW, kHaloH, 1, 1};
-            cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-            if (enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(p.act), gdim, gstr, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-                return -6;
-            const cuuint64_t K = (cuuint64_t)9 * p.Cin;
-            cuuint64_t wdim[2] = {K, (cuuint64_t)p.Cout};
-            cuuint64_t wstr[1] = {K * 2};
-            cuuint32_t wbox[2] = {kConvBlockK, (cuuint32_t)bn};
-            cuuint32_t westr[2] = {1, 1};
-            if (enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(p.wpacked), wdim, wstr, wbox, westr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-                return -7;
-            const int total = h.tiles_w * h.tiles_h * h.tiles_b * h.tiles_n;
-            if (bn == 16) return launch_halo<16>(tmA, tmB, h, total, num_sms, stream);
-            return bn == 256 ? launch_halo<256>(tmA, tmB, h, total, num_sms, stream)
-                             : launch_halo<128>(tmA, tmB, h, total, num_sms, stream);
-        }
-    }
-
     ConvTcArgs a{};
     a.num_taps = p.num_taps;
     a.chunks_per_tap = p.Cin / kConvBlockK;
-    int BW = p.W >= 128 ? 128 : p.W;
-    int BH = 128 / BW;
-    if (BH > p.H) BH = p.H;
-    int BB = 128 / (BW * BH);
-    a.bw_log2 = ilog2_exact(BW);
-    a.bh_log2 = ilog2_exact(BH);
-    a.tiles_w = (p.W + BW - 1) / BW;
-    a.tiles_h = p.H / BH;
-    a.tiles_b = (p.B + BB - 1) / BB;
-    a.B = p.B; a.H = p.H; a.W = p.W;
+    tile_geometry(p.H, p.W, p.B, a);
     a.a_chan_off = p.a_chan_off;
     a.in_stride = p.in_stride == 2 ? 2 : 1;
     a.out_sb = p.out_sb; a.out_sh = p.out_sh; a.out_sw = p.out_sw;
@@ -1187,112 +559,95 @@ int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream) {
     a.n_valid = p.n_valid > 0 ? p.n_valid : p.Cout;
     a.out_f32 = p.out_f32; a.out_f16 = p.out_f16; a.bias = p.bias; a.residual = p.residual;
     a.err_flag = p.err_flag;
-    a.dbg = p.dbg;
     a.stats = p.stats; a.stats_blocks = p.Cout / 16;
     for (int t = 0; t < p.num_taps; ++t) { a.dh[t] = p.dh[t]; a.dw[t] = p.dw[t]; a.ph[t] = p.ph[t]; }
 
-    // BLOCK_N: largest of {256,128,64,32,16} dividing C_out that still yields >= 1 wave of tiles if possible
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static int num_sms_cache[64] = {0};
-    if (dev < 64 && num_sms_cache[dev] == 0)
-        cudaDeviceGetAttribute(&num_sms_cache[dev], cudaDevAttrMultiProcessorCount, dev);
-    const int num_sms = dev < 64 ? num_sms_cache[dev] : 148;
     const int tiles_m = a.tiles_w * a.tiles_h * a.tiles_b;
-    int block_n = 0;
-    const int cands[5] = {256, 128, 64, 32, 16};
-    // CTA pairs (cta_group::2, 256-pixel x block_n tiles) whenever C_out allows and there is work for every pair
-    bool pair = false;
-    if (p.cta_pair != 1 && p.block_n_hint >= 0) {
-        const int pairs_m = (tiles_m + 1) / 2;
-        int want = (p.block_n_hint == 128 || p.block_n_hint == 256) ? p.block_n_hint : (p.Cout % 256 == 0 ? 256 : 128);
-        // 1x1 convs / linears (one tap): the short K loop does not amortise the pair's cluster hand-shakes -- measured
-        // 0.033 ms (1-CTA) vs 0.047 ms (pair) on 16x16 2048->1024 -- so they stay on the 1-CTA kernel
-        if (p.Cout % want == 0 && (p.cta_pair == 2 || (p.num_taps > 1 && pairs_m * (p.Cout / want) >= num_sms / 4))) {
-            pair = true;
-            block_n = want;
-        }
-    }
-    const int hint = p.block_n_hint < 0 ? -p.block_n_hint : p.block_n_hint;
-    if (!pair && hint > 0 && p.Cout % hint == 0) {
-        for (int i = 0; i < 5; ++i)
-            if (cands[i] == hint) block_n = cands[i];
-    }
-    if (block_n == 0) {
-        // largest BLOCK_N dividing C_out that still gives every SM a tile; never shrink below 64 for that reason
-        for (int i = 0; i < 5; ++i) {
-            if (p.Cout % cands[i] != 0) continue;
-            block_n = cands[i];
-            if (tiles_m * (p.Cout / cands[i]) >= num_sms || cands[i] <= 64) break;
-        }
-    }
+    const int block_n = pick_block_n(p.Cout, tiles_m, p.block_n_hint, num_sms_of_current_device());
     a.tiles_n = p.Cout / block_n;
-    const int total_tiles = tiles_m * a.tiles_n;
 
-    // activation map: (C, W, H, P, B), fp16, box (64, BW, BH, 1, BB), 128B swizzle, OOB -> zeros
-    CUtensorMap tmA, tmA2, tmB;
+    CUtensorMap tmA, tmA2, tmB, tmX, tmX2;
     a.a_split = (p.act2 ? p.Cin1 : p.Cin) / kConvBlockK;
     a.a_chan_off2 = p.a_chan_off2;
+    if (encode_act(enc, &tmA, p.act, p.a_channels, p.lda, p.W, p.H, p.phases, p.B, a.in_stride, a) != CUDA_SUCCESS) return -6;
+    tmA2 = tmA;
     if (p.act2) {
         if (p.Cin1 <= 0 || p.Cin1 % kConvBlockK || p.Cin1 >= p.Cin || (p.lda2 % 8) || (reinterpret_cast<uintptr_t>(p.act2) & 15) ||
             a.in_stride != 1)
             return -8;
-        cuuint64_t gdim[5] = {(cuuint64_t)p.lda2, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.phases, (cuuint64_t)p.B};
-        cuuint64_t gstr[4] = {(cuuint64_t)p.lda2 * 2, (cuuint64_t)p.W * p.lda2 * 2, (cuuint64_t)p.H * p.W * p.lda2 * 2,
-                              (cuuint64_t)p.phases * p.H * p.W * p.lda2 * 2};
-        cuuint32_t box[5] = {kConvBlockK, (cuuint32_t)BW, (cuuint32_t)BH, 1, (cuuint32_t)BB};
-        cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-        if (enc(&tmA2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(p.act2), gdim, gstr, box, estr,
-                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return -6;
+        if (encode_act(enc, &tmA2, p.act2, p.lda2, p.lda2, p.W, p.H, p.phases, p.B, 1, a) != CUDA_SUCCESS) return -6;
     }
-    {
-        // in_stride == 2 (Downsample read in place): the tensor is the (2H x 2W) input, the box spans 2*BW x 2*BH pixels
-        // and the element strides make TMA keep every second pixel -> the same 128-pixel tile lands in shared memory
-        const cuuint64_t IS = a.in_stride;
-        cuuint64_t gdim[5] = {(cuuint64_t)p.a_channels, (cuuint64_t)p.W * IS, (cuuint64_t)p.H * IS, (cuuint64_t)p.phases,
-                              (cuuint64_t)p.B};
-        cuuint64_t gstr[4] = {(cuuint64_t)p.lda * 2, (cuuint64_t)p.W * IS * p.lda * 2,
-                              (cuuint64_t)p.H * IS * p.W * IS * p.lda * 2,
-                              (cuuint64_t)p.phases * p.H * IS * p.W * IS * p.lda * 2};
-        cuuint32_t box[5] = {kConvBlockK, (cuuint32_t)(BW * IS), (cuuint32_t)(BH * IS), 1, (cuuint32_t)BB};
-        cuuint32_t estr[5] = {1, (cuuint32_t)IS, (cuuint32_t)IS, 1, 1};
-        CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(p.act), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return -6;
-        if (!p.act2) tmA2 = tmA;
+    // folded 1x1 conv over a second operand x (res_conv): its own tensor map(s), read at the centre tap
+    tmX = tmA; tmX2 = tmA;
+    if (p.x_act) {
+        if (p.phases != 1 || a.in_stride != 1) return -9;
+        if (p.Cx <= 0 || p.Cx % kConvBlockK || (p.x_lda % 8) || (reinterpret_cast<uintptr_t>(p.x_act) & 15)) return -8;
+        if (p.x_act2 && (p.Cx1 <= 0 || p.Cx1 % kConvBlockK || p.Cx1 >= p.Cx || (p.x_lda2 % 8) ||
+                         (reinterpret_cast<uintptr_t>(p.x_act2) & 15)))
+            return -8;
+        a.x_chunks = p.Cx / kConvBlockK;
+        a.x_split = (p.x_act2 ? p.Cx1 : p.Cx) / kConvBlockK;
+        a.x_chan_off = p.x_chan_off; a.x_chan_off2 = p.x_chan_off2;
+        if (encode_act(enc, &tmX, p.x_act, p.x_lda, p.x_lda, p.W, p.H, 1, p.B, 1, a) != CUDA_SUCCESS) return -6;
+        tmX2 = tmX;
+        if (p.x_act2 && encode_act(enc, &tmX2, p.x_act2, p.x_lda2, p.x_lda2, p.W, p.H, 1, p.B, 1, a) != CUDA_SUCCESS) return -6;
     }
-    {
-        const cuuint64_t K = (cuuint64_t)p.num_taps * p.Cin;
-        cuuint64_t gdim[2] = {K, (cuuint64_t)p.Cout};
-        cuuint64_t gstr[1] = {K * 2};
-        cuuint32_t box[2] = {kConvBlockK, (cuuint32_t)(pair ? block_n / 2 : block_n)};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(p.wpacked), gdim, gstr, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return -7;
-    }
+    const cuuint64_t K = (cuuint64_t)p.num_taps * p.Cin + (p.x_act ? (cuuint64_t)p.Cx : 0);
+    if (encode_weights(enc, &tmB, p.wpacked, K, p.Cout, block_n) != CUDA_SUCCESS) return -7;
 
-    if (pair) {
-        const int total_pairs = ((tiles_m + 1) / 2) * a.tiles_n;
-        // two 64-channel k-chunks per pipeline stage (half the barrier round trips) when the channel counts allow
-        const bool kc2 = p.kmerge != 1 && (a.chunks_per_tap % 2 == 0) && (a.a_split % 2 == 0);
-        if (block_n == 256)
-            return kc2 ? launch2<256, 2>(tmA, tmA2, tmB, a, total_pairs, num_sms, stream)
-                       : launch2<256, 1>(tmA, tmA2, tmB, a, total_pairs, num_sms, stream);
-        return kc2 ? launch2<128, 2>(tmA, tmA2, tmB, a, total_pairs, num_sms, stream)
-                   : launch2<128, 1>(tmA, tmA2, tmB, a, total_pairs, num_sms, stream);
-    }
+    const GnPrologueArgs gn{};
     switch (block_n) {
-        case 256: return launch<256>(tmA, tmA2, tmB, a, total_tiles, num_sms, stream);
-        case 128: return launch<128>(tmA, tmA2, tmB, a, total_tiles, num_sms, stream);
-        case 64: return launch<64>(tmA, tmA2, tmB, a, total_tiles, num_sms, stream);
-        case 32: return launch<32>(tmA, tmA2, tmB, a, total_tiles, num_sms, stream);
-        default: return launch<16>(tmA, tmA2, tmB, a, total_tiles, num_sms, stream);
+        case 128: return launch<128, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
+        case 64: return launch<64, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
+        case 32: return launch<32, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
+        default: return launch<16, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
     }
+}
+
+// ------------------------------------------------------------------------------------------------ fused GroupNorm conv
+
+bool conv_gn_supported(int H, int W, int C0, int C1, int Cout, int groups) {
+    const int C = C0 + C1;
+    if (H <= 0 || W <= 0 || H % 32 || W % 8 || C0 <= 0 || C0 % 64 || C1 < 0 || C1 % 64 || Cout <= 0 || Cout % 128) return false;
+    if (!conv_tc_supported(H, W, C, Cout) || H * W < kConvBlockM) return false;   // one image per 128-pixel tile
+    if (groups < 1 || groups > 32 || C % groups) return false;
+    if (Cfg<128>::kSmemBytes + 8u * (uint32_t)C > kSmemMax) return false;        // coefficient table A[C], Bc[C]
+    return (C / groups) % 16 == 0;
+}
+
+int conv_gn_launch(const ConvGnProblem& p, cudaStream_t stream) {
+    if (!conv_gn_supported(p.H, p.W, p.C0, p.C1, p.Cout, p.groups)) return -3;
+    if (p.C1 && (!p.src1 || !p.stats1)) return -8;
+    if (!p.src0 || !p.stats0 || !p.gamma || !p.beta) return -8;
+    if ((reinterpret_cast<uintptr_t>(p.src0) & 15) || (reinterpret_cast<uintptr_t>(p.src1) & 15) ||
+        (reinterpret_cast<uintptr_t>(p.wpacked) & 15))
+        return -8;
+    PFN_encodeTiled enc = get_encode();
+    if (!enc) return -5;
+    const int C = p.C0 + p.C1;
+
+    ConvTcArgs a{};
+    a.num_taps = 9;
+    for (int t = 0; t < 9; ++t) { a.dh[t] = (int8_t)(t / 3 - 1); a.dw[t] = (int8_t)(t % 3 - 1); a.ph[t] = 0; }
+    a.chunks_per_tap = C / kConvBlockK;
+    a.a_split = p.C0 / kConvBlockK;
+    a.in_stride = 1;
+    tile_geometry(p.H, p.W, p.B, a);
+    a.out_sb = (long long)p.H * p.W * p.Cout; a.out_sh = (long long)p.W * p.Cout; a.out_sw = p.Cout; a.out_sc = 1;
+    a.n_valid = p.Cout;
+    a.out_f32 = p.out_f32; a.out_f16 = p.out_f16; a.bias = p.bias; a.residual = p.residual; a.err_flag = p.err_flag;
+    a.stats = p.out_stats; a.stats_blocks = p.Cout / 16;
+    a.tiles_n = p.Cout / 128;
+
+    GnPrologueArgs g{};
+    g.src0 = p.src0; g.src1 = p.src1;
+    g.C0 = p.C0; g.C1 = p.C1; g.groups = p.groups; g.scale1 = p.scale1; g.eps = p.eps;
+    g.stats0 = p.stats0; g.stats1 = p.stats1; g.gamma = p.gamma; g.beta = p.beta;
+    g.scale_shift = p.scale_shift; g.ss_ld = p.ss_ld;
+
+    CUtensorMap tmB;
+    if (encode_weights(enc, &tmB, p.wpacked, (cuuint64_t)9 * C, p.Cout, 128) != CUDA_SUCCESS) return -7;
+    return launch<128, true>(tmB, tmB, tmB, tmB, tmB, a, g, 8u * (uint32_t)C, stream);
 }
 
 }  // namespace mi

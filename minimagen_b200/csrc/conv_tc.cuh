@@ -1,4 +1,4 @@
-// Host/device interface of the tcgen05 implicit-GEMM convolution (see conv_tc.cu).
+// Host/device interface of the wgmma implicit-GEMM convolution (see conv_tc.cu).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -6,7 +6,7 @@
 
 namespace mi {
 
-constexpr int kConvBlockM = 128;   // pixels per tile (UMMA M)
+constexpr int kConvBlockM = 128;   // pixels per tile (two 64-row wgmma warpgroups)
 constexpr int kConvBlockK = 64;    // fp16 channels per k-block (= one 128-byte swizzle row)
 constexpr int kConvMaxTaps = 16;   // 4x4 kernel
 
@@ -29,7 +29,6 @@ struct ConvTcArgs {
     const float* bias;                    // optional, [C_out]
     const float* residual;                // optional, fp32, same strides as the output
     int* err_flag;                        // optional: pipeline-timeout code is written here before trapping
-    int dbg;                              // profiling experiments only (bit 0: no TMA after warm-up, bit 1: no epilogue)
     double* stats;                        // optional [B][C_out/16][2]: (sum, sum of squares) of the output per 16-channel block
     int stats_blocks;                     // C_out / 16
     int8_t dh[kConvMaxTaps], dw[kConvMaxTaps], ph[kConvMaxTaps];
@@ -49,7 +48,7 @@ struct ConvTcProblem {
     int lda2, a_chan_off2, Cin1;
     const void* wpacked;    // fp16 [Cout][num_taps*Cin (+ Cx)]
     int Cout;
-    // optional folded 1x1 conv over a second operand x (swapped-operand 3x3 kernel only): out += W1x1 x, with the 1x1 weights
+    // optional folded 1x1 conv over a second operand x (stride-1 convs): out += W1x1 x, with the 1x1 weights
     // appended to every row of wpacked as Cx extra K columns; x may itself be a virtual concat (x_act2 holds channels >= Cx1)
     const void* x_act; int x_lda, x_chan_off, Cx;
     const void* x_act2; int x_lda2, x_chan_off2, Cx1;
@@ -59,17 +58,12 @@ struct ConvTcProblem {
     long long out_sb, out_sh, out_sw;
     long long out_sc;       // 0 or 1 = contiguous channels
     int n_valid;            // 0 = all C_out channels are stored
-    int block_n_hint;       // 0 = auto; > 0 preferred tile width; < 0: |value| with the 1-CTA kernel forced
-    int cta_pair;           // 0 = auto, 1 = never (1-CTA kernel), 2 = always when C_out % 128 == 0
-    int halo;               // 1 = use a 3x3 halo-tile kernel when the geometry allows (swapped-operand form preferred),
-                            // 2 = only the pixel-major halo kernel, 3 = 15 x 1 vertical taps (stem) on the swapped kernel
-    int kmerge;             // 0 = auto (two k-chunks per stage when possible), 1 = one k-chunk per stage
-    int dbg;                // profiling experiments only
+    int block_n_hint;       // 0 = auto; otherwise the preferred tile width (sign ignored)
     double* stats;          // optional GroupNorm block statistics of the output (pre-zeroed), see ConvTcArgs
     int* err_flag;
 };
 
-// GroupNorm / FiLM / SiLU prologue of the fused Block kernel (conv_gn.cu)
+// GroupNorm / FiLM / SiLU prologue of the fused Block kernel (conv_tc.cu)
 struct GnPrologueArgs {
     const float* src0;            // fp32 NHWC [B][H][W][C0]
     const float* src1;            // fp32 NHWC [B][H][W][C1] or null
@@ -98,9 +92,6 @@ struct ConvGnProblem {
 
 bool conv_gn_supported(int H, int W, int C0, int C1, int Cout, int groups);
 int conv_gn_launch(const ConvGnProblem& p, cudaStream_t stream);
-// CTA-pair form (conv_gn_pair.cu): C_out % 256 == 0, two CTAs share one prologue per 256-channel x 256-pixel tile
-bool conv_gn_pair_supported(int H, int W, int C0, int C1, int Cout, int groups);
-int conv_gn_pair_launch(const ConvGnProblem& p, cudaStream_t stream);
 
 bool conv_tc_supported(int H, int W, int Cin, int Cout);
 int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream);

@@ -47,12 +47,13 @@ int attention_fwd(const __half* q, long long q_bs, int ldq, const __half* k, con
                   int kv_hs, const float* null_kv, const uint8_t* mask, int B, int heads, int n, int m, __half* out,
                   long long o_bs, int ldo, cudaStream_t st);
 
-// attention_tc.cu: tcgen05 / TMEM path (no mask, n % 128 == 0, contiguous q); workspace = padded K and transposed V
-bool attention_tc_supported(int n, int ldq, int ldo, long long q_bs, const void* mask);
+// attention_tc.cu: wgmma path (n % 128 == 0, batch-contiguous q, key masks included); workspace = padded K, transposed V and
+// key-validity bits
+bool attention_tc_supported(int n, int ldq, int ldo, long long q_bs);
 long long attention_tc_workspace_bytes(int B, int heads, int kv_hs, int m);
 int attention_tc_fwd(const __half* q, long long q_bs, int ldq, const __half* k, const __half* v, long long kv_bs, int ldkv,
-                     int kv_hs, const float* null_kv, const uint8_t* key_mask, int B, int heads, int n, int m, __half* out, long long o_bs, int ldo,
-                     void* workspace, long long workspace_bytes, int* err_flag, cudaStream_t st);
+                     int kv_hs, const float* null_kv, const uint8_t* key_mask, int B, int heads, int n, int m, __half* out,
+                     long long o_bs, int ldo, void* workspace, long long workspace_bytes, int* err_flag, cudaStream_t st);
 
 // conv_tc.cu: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda link dependency)
 typedef CUresult (*PFN_tmaEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -87,7 +88,7 @@ int conv2d_dgrad_f32(const float* dy, int B, int Ho, int Wo, int Cout, const flo
                      int pad, float* dx, int Hi, int Wi, cudaStream_t st);
 int conv2d_wgrad_f32(const float* dy, const float* x, int B, int Hi, int Wi, int Cin, int Ho, int Wo, int Cout, int KH,
                      int KW, int stride, int pad, float* dw, cudaStream_t st);
-// wgrad_tc.cu: weight gradient of stride-1 'same' convs on tcgen05 (MN-major operands, contraction over pixels)
+// wgrad_tc.cu: weight gradient of stride-1 'same' convs on wgmma (MN-major operands, contraction over pixels)
 bool conv_wgrad_tc_supported(int H, int W, int Cin, int Cout, int kh, int kw, int stride);
 long long conv_wgrad_tc_workspace_bytes(int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride);
 int conv_wgrad_tc(const __half* dy, const __half* x, int B, int H, int W, int Cin, int Cout, int kh, int kw, int stride,

@@ -1,6 +1,6 @@
 // Kernel launch helper: every kernel of the library goes through launch_k so that programmatic dependent launch (PDL)
 // can be switched on for the whole step.  With PDL the next kernel's CTAs are scheduled, and run their prologue
-// (barrier init, TMEM allocation, tensor-map prefetch, coefficient set-up), while the tail of the previous kernel is
+// (barrier init, tensor-map prefetch, coefficient set-up), while the tail of the previous kernel is
 // still draining; every kernel executes pdl_wait() before its first global-memory access, so ordering is unchanged.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and matrix descriptors.
 // Everything the tensor-core kernels need and nothing else.  No CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -55,9 +55,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* e
     }
 }
 
-// One lane of a fully converged warp (elect.sync).  Issuing TMA / tcgen05 instructions under this predicate -- instead of
-// under `lane == 0` -- lets the compiler keep their operands in uniform registers; with a plain lane test it wraps every
-// UTCHMMA / UTMALDG in an ELECT + R2UR.BROADCAST + BRA.U.ANY loop, which made the MMA issue rate the bottleneck.
+// One lane of a fully converged warp (elect.sync).  Issuing TMA instructions under this predicate -- instead of under
+// `lane == 0` -- lets the compiler keep their operands in uniform registers.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n .reg .pred p;\n elect.sync _|p, 0xffffffff;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(pred));
@@ -96,198 +95,32 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar,
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {   // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {   // whole warp
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {   // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem]; one thread issues for the CTA.  kind::f16 covers fp16 and bf16 operands.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// The same with the A operand read from TENSOR MEMORY (lane = row of A, two 16-bit K elements per 32-bit column, so one
-// K = 16 step spans 8 columns): no shared-memory A fetch, the instruction runs at the N/2-clock floor.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp receives lane (base_lane + t), columns [col, col+16).
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 32 lanes x 16 consecutive 32-bit columns, registers -> TMEM (the warp's own lane quarter); complete after tmem_st_wait()
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-          "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle, rows of 64 x 16-bit elements:
-//   start address >>4 in bits [0,14); LBO (unused for swizzled K-major) bits [16,30);
-//   SBO = 1024 B (8 rows x 128 B) >>4 in bits [32,46); version=1 in bits [46,48); layout SWIZZLE_128B=2 in bits [61,64).
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
+// Shared-memory matrix descriptor, 128-byte swizzle (sm_90 layout: start >>4 in bits [0,14), LBO >>4 in [16,30), SBO >>4 in
+// [32,46), layout SWIZZLE_128B = 1 in bits [62,64)).  K-major: rows of 64 x 16-bit elements, SBO = 1024 B between 8-row groups,
+// LBO unused.  MN-major: LBO = distance between 64-element MN blocks, SBO = 1024 B between 8-row K groups.
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t lbo_bytes = 16) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= static_cast<uint64_t>(1024u >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
-// Instruction descriptor for kind::f16: fp16 (fmt 0) or bf16 (fmt 1) A/B, fp32 accumulate, both K-major, M x N tile.
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t ab_fmt = 0) {
-    return (1u << 4) | (ab_fmt << 7) | (ab_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-}  // namespace ptx
-}  // namespace mi
-
-// ------------------------------------------------------------------------------------------------ 2-CTA (cta_group::2)
-namespace mi {
-namespace ptx {
-
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address -> even (leader) CTA
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same smem offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 remAddr32;\n\t"
-        "mapa.shared::cluster.u32 remAddr32, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [remAddr32];\n\t"
-        "}"
-        ::"r"(smem_u32(bar)), "r"(cta)
-        : "memory");
-}
-// cluster-scope release / acquire forms: a CTA hands generic-proxy shared-memory writes (made visible to the async proxy by
-// fence.proxy.async) to a tcgen05.mma.cta_group::2 issued by the OTHER CTA of the pair
-__device__ __forceinline__ void mbar_arrive_release_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 remAddr32;\n\t"
-        "mapa.shared::cluster.u32 remAddr32, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remAddr32];\n\t"
-        "}"
-        ::"r"(smem_u32(bar)), "r"(cta)
-        : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_acquire_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_acquire_cluster(uint64_t* bar, uint32_t parity, int* err, int code) {
-    if (mbar_try_wait_acquire_cluster(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try_wait_acquire_cluster(bar, parity)) {
-        if (clock64() - t0 > 4000000000LL) {
-            if (err) { atomicExch(err, code); __threadfence_system(); }
-            __trap();
-        }
-    }
-}
-// TMA loads issued by either CTA of a pair; completion bytes are signalled on the LEADER CTA's barrier
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-        "[%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_2sm(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1, int c2,
-                                                int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-        "%5, %6, %7}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1),
-        "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {   // one warp in EACH CTA of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs, 256 rows] (+)= [A_cta0; A_cta1] * [B_cta0; B_cta1]^T ; issued by one thread of the leader CTA
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive (once all prior MMAs retire) on the barrier at this smem offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(smem_u32(bar)), "h"(cta_mask)
-        : "memory");
+// named barrier over `count` threads (a subset of the CTA)
+__device__ __forceinline__ void bar_sync(int id, int count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 }  // namespace ptx

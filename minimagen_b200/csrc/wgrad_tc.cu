@@ -4,30 +4,30 @@
 //     dW[co][ci][r][s] = sum over output pixels p = (b, h, w) of  dY[p][co] * X[b][stride*h + r - pad][stride*w + s - pad][ci]
 //
 // = for every tap one GEMM  dW_t[C_out][C_in] = dY^T[C_out][P] x X_t[P][C_in]  whose CONTRACTION runs over the pixels.  dY and X
-// are NHWC fp16 (channels contiguous), i.e. both operands are "MN-major" for tcgen05.mma: the kernel loads (8 x 8 pixels) x 64
+// are NHWC fp16 (channels contiguous), i.e. both operands are "MN-major" for wgmma: the kernel loads (8 x 8 pixels) x 64
 // channel boxes with TMA (128B swizzle: one pixel = one 128-byte row, 8 rows = one 1024-byte atom), the tap's shift is applied to
 // X's box coordinates (TMA zero-fills outside the image = the conv's zero padding; for stride 2 the box spans 16 x 16 input pixels
-// and TMA element strides keep every second one), and the instruction descriptor marks A and
-// B as MN-major (bits 15 / 16); the matrix descriptors step through K in 8-row atoms (SBO = 1024 B) and through the 64-channel
-// blocks of M / N with LBO = one box (8 KB).  fp32 accumulation in TMEM over this CTA's pixel range; the pixel axis is split over
-// gridDim.y CTAs per (co tile, ci tile, tap); every CTA stores its partial tile to the workspace [split][tap][C_out][C_in]
-// (64 contiguous bytes per thread) and wgrad_reduce_kernel sums the splits into the OIHW result.  (The first version added the
-// partial tiles to dW with fp32 atomics: 128 scattered REDs per thread, 36 bytes apart for a 3x3 -- that epilogue, not the
-// MMAs, was the kernel's time.)
+// and TMA element strides keep every second one), and the wgmma transpose flags mark A and B as MN-major; the matrix
+// descriptors step through K in 8-row atoms (SBO = 1024 B) and through the 64-channel blocks of N with LBO = one box (8 KB).
+// fp32 accumulation in registers over this CTA's pixel range; the pixel axis is split over gridDim.y CTAs per (co tile, ci tile,
+// tap); every CTA stores its partial tile to the workspace [split][tap][C_out][C_in] and wgrad_reduce_kernel sums the splits
+// into the OIHW result.
 //
-// Warp roles (256 threads): 0 TMA producer, 1 MMA issuer, 2 TMEM allocator, 4-7 epilogue (lane = output channel).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one elected lane), warpgroups 1 and 2 = consumers, each owning 64 of
+// the 128 output channels of the tile.
 #include <cuda_runtime.h>
 
 #include "conv_tc.cuh"
 #include "kernels.cuh"
 #include "launch.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace mi {
 
 namespace {
 
-constexpr int kWgThreads = 256;
+constexpr int kWgThreads = 384;
 constexpr int kPx = 64;                                   // pixels per pipeline stage: one 8 x 8 box
 constexpr uint32_t kBoxBytes = kPx * 128;                 // 64 pixels x 64 channels fp16 = 8 KiB
 constexpr int kMaxStages = 6;
@@ -42,51 +42,28 @@ struct WgradArgs {
     int* err;
 };
 
-// kind::f16, fp32 accumulate, A and B MN-major
-__host__ __device__ constexpr uint32_t make_idesc_mn(uint32_t M, uint32_t N) {
-    return (1u << 4) | (1u << 15) | (1u << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// MN-major operand, 128B swizzle: LBO = distance between 64-element MN blocks, SBO = distance between 8-row K groups
-__device__ __forceinline__ uint64_t make_mn_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>(1024u >> 4) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-
+template <int NB>
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmX,
                      const __grid_constant__ WgradArgs a) {
+    constexpr int N = NB * 64;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int NB = a.n_blocks;
-    const uint32_t stage_bytes = (2 + NB) * kBoxBytes;           // dY: two 64-channel blocks (M = 128); X: NB blocks
+    constexpr uint32_t stage_bytes = (2 + NB) * kBoxBytes;       // dY: two 64-channel blocks (M = 128); X: NB blocks
     const int STAGES = a.stages;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * stage_bytes);
     uint64_t* full_bar = bars;
     uint64_t* empty_bar = bars + kMaxStages;
-    uint64_t* tfull_bar = bars + 2 * kMaxStages;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     int* err = a.err;
-    if (warp == 0 && lane == 0) { ptx::prefetch_tensormap(&tmY); ptx::prefetch_tensormap(&tmX); }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < STAGES; ++i) { ptx::mbar_init(&full_bar[i], 1); ptx::mbar_init(&empty_bar[i], 1); }
-        ptx::mbar_init(tfull_bar, 1);
+    if (threadIdx.x == 0) {
+        ptx::prefetch_tensormap(&tmY);
+        ptx::prefetch_tensormap(&tmX);
+        for (int i = 0; i < STAGES; ++i) { ptx::mbar_init(&full_bar[i], 1); ptx::mbar_init(&empty_bar[i], 2); }
         ptx::fence_barrier_init();
     }
-    if (warp == 2) {
-        ptx::tmem_alloc(tmem_ptr_smem, 128);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     pdl_wait();
 
     // this CTA's problem: (co tile, ci tile, tap) and a range of 8 x 8 pixel boxes
@@ -99,75 +76,65 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_const
     long long p1 = p0 + a.px_tiles_per_cta;
     if (p1 > a.total_px_tiles) p1 = a.total_px_tiles;
     const int n_steps = (int)(p1 > p0 ? p1 - p0 : 0);
-    const int N = NB * 64;
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int i = 0; i < n_steps; ++i) {
-            const long long pt = p0 + i;
-            const int tw = (int)(pt % a.tiles_w);
-            const int th = (int)((pt / a.tiles_w) % a.tiles_h);
-            const int b = (int)(pt / ((long long)a.tiles_w * a.tiles_h));
-            ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 7100 + stage);
-            if (ptx::elect_one()) {
-                uint8_t* s = smem + stage * stage_bytes;
-                ptx::mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
-                ptx::tma_load_5d(&tmY, &full_bar[stage], s, co_t * 128, tw * 8, th * 8, 0, b);
-                ptx::tma_load_5d(&tmY, &full_bar[stage], s + kBoxBytes, co_t * 128 + 64, tw * 8, th * 8, 0, b);
-                for (int nb = 0; nb < NB; ++nb)
-                    ptx::tma_load_5d(&tmX, &full_bar[stage], s + (2 + nb) * kBoxBytes, ci_t * N + nb * 64, tw * 8 * a.stride + dw_,
-                                     th * 8 * a.stride + dh, 0, b);
+    if (wg == 0) {
+        if (warp == 0) {
+            // ===================== TMA producer =====================
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int i = 0; i < n_steps; ++i) {
+                const long long pt = p0 + i;
+                const int tw = (int)(pt % a.tiles_w);
+                const int th = (int)((pt / a.tiles_w) % a.tiles_h);
+                const int b = (int)(pt / ((long long)a.tiles_w * a.tiles_h));
+                ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 7100 + stage);
+                if (ptx::elect_one()) {
+                    uint8_t* s = smem + stage * stage_bytes;
+                    ptx::mbar_arrive_expect_tx(&full_bar[stage], stage_bytes);
+                    ptx::tma_load_5d(&tmY, &full_bar[stage], s, co_t * 128, tw * 8, th * 8, 0, b);
+                    ptx::tma_load_5d(&tmY, &full_bar[stage], s + kBoxBytes, co_t * 128 + 64, tw * 8, th * 8, 0, b);
+                    for (int nb = 0; nb < NB; ++nb)
+                        ptx::tma_load_5d(&tmX, &full_bar[stage], s + (2 + nb) * kBoxBytes, ci_t * N + nb * 64,
+                                         tw * 8 * a.stride + dw_, th * 8 * a.stride + dh, 0, b);
+                }
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            pdl_trigger();
         }
-        pdl_trigger();
-    } else if (warp == 1) {
-        // ===================== MMA issuer: D[128 co][N ci] += dY^T (MN-major A) x X (MN-major B), K = 64 pixels per stage =====================
-        const uint32_t idesc = make_idesc_mn(128, (uint32_t)N);
-        int stage = 0;
+    } else if (n_steps > 0) {
+        // ===================== consumers: D[64 co][N ci] += dY^T (MN-major A) x X (MN-major B), K = 64 pixels per stage ==========
+        const int cw = wg - 1;
+        float acc[N / 2];
+        int stage = 0, prev = -1;
         uint32_t phase = 0;
         for (int i = 0; i < n_steps; ++i) {
             ptx::mbar_wait(&full_bar[stage], phase, err, 7200 + stage);
-            ptx::tc_fence_after();
-            if (ptx::elect_one()) {
-                const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
-                const uint64_t da = make_mn_desc(sa, kBoxBytes);
-                const uint64_t db = make_mn_desc(sa + 2 * kBoxBytes, kBoxBytes);
+            const uint32_t sa = ptx::smem_u32(smem + stage * stage_bytes);
+            const uint64_t da = ptx::make_sw128_desc(sa + cw * kBoxBytes, kBoxBytes);
+            const uint64_t db = ptx::make_sw128_desc(sa + 2 * kBoxBytes, kBoxBytes);
+            ptx::wg_fence();
 #pragma unroll
-                for (int k = 0; k < kPx / 16; ++k)      // 16 pixels = two 8-row atoms = 2048 B further along K
-                    ptx::umma_f16(tmem_base, da + (uint64_t)(k * 128), db + (uint64_t)(k * 128), idesc, (i | k) != 0);
-                ptx::umma_commit(&empty_bar[stage]);
-                if (i + 1 == n_steps) ptx::umma_commit(tfull_bar);
-            }
+            for (int k = 0; k < kPx / 16; ++k)      // 16 pixels = two 8-row atoms = 2048 B further along K
+                ptx::Wgmma<N, 1>::run(acc, da + (uint64_t)(k * 128), db + (uint64_t)(k * 128), (i | k) != 0);
+            ptx::wg_commit();
+            ptx::wg_wait<1>();
+            if (prev >= 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[prev]);
+            prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-    } else if (warp >= 4 && n_steps > 0) {
-        // ===================== epilogue: lane = output channel, columns = input channels -> this split's partial tile ==========
-        const int q = warp & 3;
-        const int co = co_t * 128 + q * 32 + lane;
-        ptx::mbar_wait(tfull_bar, 0, err, 7300);
-        ptx::tc_fence_after();
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+        ptx::wg_wait<0>();
+        ptx::wg_fence_regs(acc);
+        // ---- this split's partial tile: fragment element 4j + 2r + e = co row 16 wq + lane/4 + 8r, ci column 8j + 2(lane%4) + e
+        const int wq = warp & 3;
         const int taps = a.kh * a.kw;
-        float* dst = a.ws + (((long long)blockIdx.y * taps + tap) * a.Cout + co) * a.Cin + ci_t * N;
-#pragma unroll 1
-        for (int c = 0; c < N; c += 16) {
-            uint32_t v[16];
-            ptx::tmem_ld_x16(taddr + c, v);
-            ptx::tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < 16; i += 4)
-                *reinterpret_cast<uint4*>(dst + c + i) = make_uint4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+        for (int r = 0; r < 2; ++r) {
+            const int co = co_t * 128 + cw * 64 + wq * 16 + (lane >> 2) + 8 * r;
+            float* dst = a.ws + (((long long)blockIdx.y * taps + tap) * a.Cout + co) * a.Cin + ci_t * N + 2 * (lane & 3);
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j)
+                *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]);
         }
-        ptx::tc_fence_before();
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, 128);
     }
 }
 
@@ -193,7 +160,7 @@ WgradPlan wgrad_plan(int B, int H, int W, int Cin, int Cout, int kh, int kw) {
     p.tiles_co = Cout / 128; p.tiles_ci = Cin / (p.n_blocks * 64);
     p.total_px_tiles = (long long)B * (W / 8) * (H / 8);
     p.groups = p.tiles_co * p.tiles_ci * kh * kw;
-    int dev = 0, num_sms = 148;
+    int dev = 0, num_sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
     long long splits = (2LL * num_sms + p.groups - 1) / p.groups;            // about two CTAs per SM over the whole grid
@@ -259,11 +226,14 @@ int conv_wgrad_tc(const __half* dy, const __half* x, int B, int H, int W, int Ci
     }
     static bool attr_set = false;
     if (!attr_set) {
-        if (cudaFuncSetAttribute(conv_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -2;
+        if (cudaFuncSetAttribute(conv_wgrad_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess ||
+            cudaFuncSetAttribute(conv_wgrad_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
+            return -2;
         attr_set = true;
     }
     dim3 grid(groups, (unsigned)splits);
-    launch_k(conv_wgrad_tc_kernel, grid, kWgThreads, smem, stream, tmY, tmX, a);
+    if (a.n_blocks == 2) launch_k(conv_wgrad_tc_kernel<2>, grid, kWgThreads, smem, stream, tmY, tmX, a);
+    else launch_k(conv_wgrad_tc_kernel<1>, grid, kWgThreads, smem, stream, tmY, tmX, a);
     const long long cc = (long long)Cout * Cin, total = cc * kh * kw;
     launch_k(wgrad_reduce_kernel, dim3((unsigned)((total + 255) / 256)), 256, 0, stream, (const float*)workspace, (int)splits, kh * kw, cc, dw);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;

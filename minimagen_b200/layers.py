@@ -1,8 +1,8 @@
-"""Building blocks of the U-Net, B200-native.
+"""Building blocks of the U-Net, H100-native.
 
 Every class keeps the NAME, constructor signature, sub-module attribute names and parameter shapes of its counterpart
 in the reference's `minimagen/layers.py` (so `state_dict()` keys are identical -- the checkpoint ABI), but none of the
-reference's torch forward code: each module lowers itself onto the sm_100a kernels through `run(...)`, which works on
+reference's torch forward code: each module lowers itself onto the sm_90a kernels through `run(...)`, which works on
 NHWC fp32 activations `[B, H, W, C]` and makes C-ABI calls via `minimagen_b200.ops`.
 
 `forward(...)` keeps the reference's NCHW (or `[b, n, c]` for attention) calling convention for stand-alone use and
@@ -31,10 +31,9 @@ GN_INPUT_F32 = True
 
 # Block.forward as ONE kernel (GroupNorm/FiLM/SiLU as the conv's prologue: mi_conv3x3_gn_silu_f16) where the geometry allows
 # (3x3, H % 32 == 0, W % 8 == 0, channels % 64, C_out % 128, fp32 sources with epilogue block statistics)
-# 'pair' : layers with C_out % 256 == 0 on the CTA-pair kernel (conv_gn_pair.cu: two CTAs share one prologue per 256-channel
-#          tile -- half the prologue work per tensor FLOP);
-# True   : 'pair' plus the C_out == 128 layers on the single-CTA kernel (one channel tile per pixel tile);
-# 'all'  : wherever supported; False: never.   Measurements: profiles/r02_fused_gn_study.md.
+# 'pair' : only the layers with C_out % 256 == 0 (the name is historical: every mode runs the same fused kernel, conv_tc.cu);
+# True   : 'pair' plus the C_out == 128 layers;
+# 'all'  : wherever supported; False: never.
 FUSE_GN_CONV = {"0": False, "1": True, "pair": "pair", "all": "all"}.get(os.environ.get("MI_FUSE_GN_CONV", "0"), False)
 # a ResnetBlock tail can either fold res_conv into block2's conv (FOLD_RES_CONV) or run block2 on the fused kernel; which wins
 FUSE_OVER_FOLD = os.environ.get("MI_FUSE_OVER_FOLD", "1") == "1"
@@ -50,7 +49,7 @@ def fuse_block_ok(c_out):
 
 
 # ResnetBlock tail  block2.project(h) + res_conv(x)  as ONE launch (mi_conv3x3_res1x1_f16: the 1x1 conv rides the 3x3 conv's
-# accumulator as extra K chunks) where block2's conv runs on the swapped-operand 3x3 kernel
+# accumulator as extra K chunks) where the geometry allows (mi_conv3x3_res1x1_supported)
 FOLD_RES_CONV = os.environ.get("MI_FOLD_RES_CONV", "1") == "1"
 
 # nearest-x2 upsample + 3x3 conv as four 2x2 sub-pixel convs on the low-res tensor (4/9 of the FLOPs, no upsampled copy)
@@ -178,7 +177,7 @@ def _srcs(x, prefer_f16):
 def _no_grad_check(*tensors):
     if torch.is_grad_enabled() and any(exists(t) and t.requires_grad for t in tensors):
         raise NotImplementedError(
-            "minimagen_b200 implements the inference (sampling) hot path only; autograd through the sm_100a kernels "
+            "minimagen_b200 implements the inference (sampling) hot path only; autograd through the sm_90a kernels "
             "(training, SURVEY.md 8f-2) is not built yet. Call under torch.no_grad().")
 
 
@@ -349,7 +348,7 @@ class TokenView(nn.Module):
 
 # ------------------------------------------------------------------------------------------------ convolutions
 class Conv2d(nn.Conv2d):
-    """nn.Conv2d parameter container (same keys / shapes) lowered onto the tcgen05 implicit GEMM
+    """nn.Conv2d parameter container (same keys / shapes) lowered onto the wgmma implicit GEMM
     (mi_conv2d_igemm_f16) or, for non-tensor-core shapes, the direct fp32 kernel (mi_conv2d_direct_f32).
 
     Supported geometries = the ones the reference U-Net uses: k x k stride 1 'same' padding (k odd), and the

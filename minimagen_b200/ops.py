@@ -27,8 +27,8 @@ def _chk_out(t, dtype, name):
 
 
 class NativeOps:
-    name = "native-sm100a"
-    attention_tc = True      # tcgen05 attention core where the shape allows (mi_attention_fwd workspace)
+    name = "native-sm90a"
+    attention_tc = True      # wgmma attention core where the shape allows (mi_attention_fwd workspace)
 
     def set_launch_mode(self, pdl):
         """Programmatic dependent launch for every kernel of the library (mi_set_launch_mode)."""
@@ -191,8 +191,8 @@ class NativeOps:
         _chk(null_kv, F32, "null_kv"); _chk(mask, U8, "mask")
         ws = None
         if self.attention_tc and n % 128 == 0 and m >= 128:
-            # operand workspace of the tcgen05 kernel (null-prepended padded K, transposed V); per call, so it is safe under
-            # CUDA-graph capture and concurrent streams
+            # operand workspace of the wgmma kernel (null-prepended padded K, transposed V, key-validity bits); per call, so
+            # it is safe under CUDA-graph capture and concurrent streams
             nbytes = int(N.load().mi_attention_workspace_bytes(B, heads, kv_hs, m))
             ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
         N.call("mi_attention_fwd", N.ptr(q), q_bs, ldq, N.ptr(k), N.ptr(v), kv_bs, ldkv, kv_hs, N.ptr(null_kv),

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- generates tests/golden/*.pt by running the UNMODIFIED reference (oracle/reference.py)
 on the CPU in this container.  Re-run with:  python oracle/make_golden.py
-The fixtures pin (a) oracle/restatement.py and (b) the CUDA path on the GPU box, where /root/reference is absent.
+The fixtures pin (a) oracle/restatement.py and (b) the CUDA path on machines where the reference tree is absent.
 """
 import os
 import sys
@@ -208,12 +208,77 @@ def train_case():
                     cond_drop_prob=0.15), os.path.join(OUT, "train_tiny.pt"))
 
 
+LIVE_CFGS = [
+    (dict(dim=32, dim_mults=(1, 2), attend_at_middle=True, text_embed_dim=768), 32, False),
+    (dict(dim=32, dim_mults=(1, 2), lowres_cond=True, memory_efficient=True, num_resnet_blocks=(1, 2),
+          layer_attns=(False, True), layer_cross_attns=(False, True)), 32, True),
+]
+
+
+RESIZE_CASES = [(64, 256, "reflect", None), (16, 64, "reflect", (0., 1.)), (128, 64, "reflect", (-1., 1.)),
+                (24, 36, "constant", None), (32, 128, "edge", None)]
+
+
+def resize_sample(n):
+    return torch.randperm(n, generator=torch.Generator().manual_seed(n))[:4096]
+
+
+def live_inputs(cfg, s, lowres):
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(2, 3, s, s, generator=g)
+    te = torch.randn(2, 20, cfg.get("text_embed_dim", 512), generator=g)
+    tm = torch.ones(2, 20, dtype=torch.bool)
+    tm[1, 5:] = False
+    kw = dict(text_embeds=te, text_mask=tm)
+    if lowres:
+        kw.update(lowres_cond_img=torch.randn(2, 3, s, s, generator=g), lowres_noise_times=torch.tensor([200, 3]))
+    return x, torch.tensor([999, 0]), kw
+
+
+def live_case():
+    """The reference's public signatures / class defaults, and its U-Net outputs on two small configurations whose weights
+    are the project's own seeded initialisation (regenerated by the test, so only outputs are stored)."""
+    import inspect
+    import minimagen.Unet as RU
+    import minimagen.Imagen as RI
+    import minimagen.diffusion_model as RD
+    from minimagen_b200.Unet import Unet as MyUnet
+
+    def params(f):
+        return [(p.name, int(p.kind), repr(p.default)) for p in inspect.signature(f).parameters.values()]
+    sig = {"Unet.__init__": params(RU.Unet.__init__), "Imagen.__init__": params(RI.Imagen.__init__),
+           "GaussianDiffusion.__init__": params(RD.GaussianDiffusion.__init__), "Unet.forward": params(RU.Unet.forward),
+           "Imagen.sample": params(RI.Imagen.sample)}
+    defaults = {cls: getattr(RU, cls).defaults for cls in ("Base", "Super", "BaseTest", "SuperTest")}
+    outs = []
+    for cfg, s, lowres in LIVE_CFGS:
+        torch.manual_seed(0)
+        sd = MyUnet(**cfg).state_dict()
+        r = RU.Unet(**cfg).eval()
+        r.load_state_dict(sd)
+        x, t, kw = live_inputs(cfg, s, lowres)
+        with torch.no_grad():
+            outs.append([r(x, t, cond_drop_prob=cdp, **kw) for cdp in (0., 1.)])
+    # helpers.resize_image_to on the resize_right stand-in: a fixed sample of 4096 output values per case
+    import minimagen.helpers as RH
+    resize = {}
+    for n_in, n_out, pad, clamp in RESIZE_CASES:
+        x = torch.rand(2, 3, n_in, n_in, generator=torch.Generator().manual_seed(n_in)) * 2 - 0.5
+        want = RH.resize_image_to(x, n_out, clamp_range=clamp, pad_mode=pad)
+        idx = resize_sample(want.numel())
+        resize[(n_in, n_out, pad, clamp)] = (tuple(want.shape), want.reshape(-1)[idx].clone())
+    torch.save(dict(signatures=sig, defaults=defaults, outputs=outs, resize=resize), os.path.join(OUT, "reference_live.pt"))
+
+
 if __name__ == "__main__":
     reference.load()
     os.makedirs(OUT, exist_ok=True)
     from minimagen.Unet import BaseTest, SuperTest
     if len(sys.argv) > 1 and sys.argv[1] == "train":
         train_case()
+        sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == "live":
+        live_case()
         sys.exit(0)
     unet_case("unet_tiny_base", dict(BaseTest.defaults), 64, False)
     unet_case("unet_tiny_sr", dict(SuperTest.defaults, lowres_cond=True), 64, True)

@@ -237,9 +237,9 @@ def test_groupnorm_block_statistics_from_conv_epilogue(native):
     (2, 32, 16, 128, 256, 128, True, True),          # GroupNorm groups (48 channels) straddle the two sources
     (1, 32, 32, 512, 512, 512, True, True),          # deep K (16 chunks), 4 channel tiles
     (5, 64, 32, 128, 0, 128, True, False),           # two chunks, many tiles per image
-    (2, 64, 32, 256, 0, 256, True, True),            # CTA-pair kernel (C_out % 256 == 0), several pair tiles per image
-    (3, 32, 8, 128, 128, 512, False, True),          # pair kernel, two 256-channel tiles, concat
-    (1, 32, 32, 512, 512, 1024, True, True),         # pair kernel, deep K
+    (2, 64, 32, 256, 0, 256, True, True),            # C_out % 256 == 0, several tiles per image
+    (3, 32, 8, 128, 128, 512, False, True),          # four 128-channel tiles, concat
+    (1, 32, 32, 512, 512, 1024, True, True),         # eight channel tiles, deep K
 ])
 def test_fused_groupnorm_conv(native, B, H, W, C0, C1, Cout, res, ss):
     """mi_conv3x3_gn_silu_f16 == mi_gn_apply_silu (block statistics) followed by mi_conv2d_igemm_f16"""
@@ -305,13 +305,14 @@ def test_conv_igemm_two_sources(native):
         assert rel_l2(o_n, o_e) < 2e-5
 
 
-@pytest.mark.parametrize("B,H,W,C0,C1,Cout", [(2, 32, 32, 128, 0, 128),     # swapped halo kernel, 32 x 8 tiles
-                                               (1, 64, 16, 64, 0, 256),      # 16-wide images: three shifted tile copies
-                                               (2, 32, 32, 64, 64, 128),     # two TMA sources, 32 x 8 tiles
-                                               (3, 16, 16, 128, 64, 128)])   # two TMA sources, 16 x 16 tiles
+@pytest.mark.parametrize("B,H,W,C0,C1,Cout", [(2, 32, 32, 128, 0, 128),     # one source, 4 x 32-pixel tiles
+                                               (1, 64, 16, 64, 0, 256),      # 16-wide images, two channel tiles
+                                               (2, 32, 32, 64, 64, 128),     # two TMA sources
+                                               (3, 16, 16, 128, 64, 128)])   # two TMA sources, 16 x 16 images
 def test_conv3x3_swapped_halo_paths(native, B, H, W, C0, C1, Cout):
-    """3x3 convs with C_out % 128 == 0 run on the swapped-operand halo kernels (channels in TMEM lanes): bias, residual,
-    both output copies and the epilogue GroupNorm statistics, single and two-source inputs"""
+    """3x3 convs with C_out % 128 == 0, one or two TMA sources: bias, residual, both output copies and the epilogue
+    GroupNorm statistics.  (The name is kept from when these shapes selected separate halo kernels; every case now runs on
+    the one implicit-GEMM kernel of csrc/conv_tc.cu.)"""
     Cin = C0 + C1
     a0 = _rand(B, 1, H, W, C0, seed=90).to(F16)
     a1 = _rand(B, 1, H, W, C1, seed=91).to(F16) if C1 else None
@@ -336,7 +337,7 @@ def test_conv3x3_swapped_halo_paths(native, B, H, W, C0, C1, Cout):
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 16, 16, 64, 128), (1, 32, 32, 128, 256), (2, 8, 8, 64, 64),
-                                           (3, 64, 16, 128, 128), (2, 32, 8, 64, 128), (1, 64, 64, 256, 128)])   # last three: swapped-operand Sub geometry
+                                           (3, 64, 16, 128, 128), (2, 32, 8, 64, 128), (1, 64, 64, 256, 128)])   # last three: C_out % 128 == 0 grids
 def test_conv_igemm_subpixel_upsample_phases(native, B, H, W, Cin, Cout):
     """modes 2..5: the four 2x2 sub-pixel phases of 'nearest x2 upsample + 3x3 conv' on the low-res tensor, written
     interleaved into the 2H x 2W output; vs the emulation and vs the literal upsample + conv"""
@@ -469,7 +470,7 @@ def test_resize_separable(native, n_in, n_out, pad, clamp):
                                                          (3, 8, 128, 59, False, False),      # one padded key block
                                                          (2, 4, 384, 127, True, False),      # m + 1 == 128 exactly
                                                          (1, 2, 4096, 4096, True, False),    # base U-Net 64x64 tokens
-                                                         (2, 8, 512, 300, False, True),      # key mask inside the two-tile tcgen05 kernel
+                                                         (2, 8, 512, 300, False, True),      # key mask, two query tiles
                                                          (2, 4, 384, 700, True, True),       # ... and inside the one-tile kernel (n % 256 != 0)
                                                          (1, 8, 256, 2000, True, True)])     # ... over many key blocks
 def test_attention(native, B, heads, n, m, shared, use_mask):
@@ -496,9 +497,9 @@ def test_attention(native, B, heads, n, m, shared, use_mask):
 @pytest.mark.parametrize("B,heads,n,m,shared,ramp", [(1, 8, 1024, 1280, True, "up"), (2, 4, 256, 600, False, "up"),
                                                      (1, 8, 1024, 1280, True, "down"), (2, 4, 128, 1500, True, "rows")])
 def test_attention_single_sweep_rescales(native, B, heads, n, m, shared, ramp):
-    """The tcgen05 attention kernel makes ONE sweep over the keys against a lazily raised reference maximum
-    (csrc/attention_tc.cu): key norms that grow along the sequence ("up") force a rescale of the TMEM accumulator in almost
-    every key block, shrinking ones ("down") none after the first, "rows" makes only some query rows of a CTA move."""
+    """Online softmax over long key sequences: key norms that grow along the sequence ("up") force a rescale of the
+    running accumulator in almost every key block, shrinking ones ("down") none after the first, "rows" makes only some
+    query rows of a CTA move."""
     inner = heads * 64
     g = torch.Generator().manual_seed(91)
     q = torch.randn(B * n, inner, generator=g) * 0.5

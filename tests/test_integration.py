@@ -1,41 +1,11 @@
-"""Boundary proof through the REFERENCE's own callers (SURVEY.md 8b / 8f-3): INTEGRATION.md's snippet run verbatim, and a
-Training Directory round trip through the reference's `generate.load_minimagen` after `install_as_minimagen()`.
-Needs /root/reference (build container only); runs in a subprocess because it re-binds sys.modules['minimagen*']."""
-import json
+"""`install_as_minimagen()` without the reference on the path; runs in a subprocess because it re-binds
+sys.modules['minimagen*']."""
 import os
 import subprocess
 import sys
 
-import pytest
-
-from oracle import reference
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _run(mode):
-    env = dict(os.environ)
-    shims = os.path.join(ROOT, "oracle", "shims")
-    env["PYTHONPATH"] = os.pathsep.join([ROOT, os.path.join(ROOT, "tests"), reference.REFERENCE_ROOT, shims,
-                                         env.get("PYTHONPATH", "")])
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "_integration_script.py"), mode], env=env,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
-@pytest.mark.skipif(not reference.available(), reason="reference checkout not present")
-def test_reference_generate_loads_b200_classes_from_training_directory():
-    res = _run("emu")
-    assert res["generate_file"].startswith(reference.REFERENCE_ROOT)          # the reference's own generate.py ran
-    assert res["generate_uses_b200_classes"] and res["training_uses_b200_unet"]
-    assert res["loaded_type"] == "minimagen_b200.Imagen.Imagen"
-    assert res["unet_types"] == ["minimagen_b200.Unet"]
-    assert res["weights_equal"] and res["sample_equal"] and res["sample_finite"]
-    assert res["sample_shape"] == [2, 3, 32, 32]
-    # the reference's training loop (training.MinimagenTrain) trained the B200 classes and wrote loadable checkpoints
-    assert res["train_weights_changed"] and res["trained_loaded_type"] == "minimagen_b200.Imagen"
-    assert res["train_files"] == ["unet_0_state_20260101_000000.pth", "unet_1_state_20260101_000000.pth"]
 
 
 def test_install_as_minimagen_without_reference_is_alias_only():

@@ -1,7 +1,7 @@
 """Micro-benchmarks of the non-GEMM kernels at the cfg-3 (SR 64->256, dim 128, batch 32) shapes.  GPU only.
 
 Diagnostics for kernel tuning, not a bench value: CUDA events around `reps` back-to-back launches, rotating over enough
-buffer sets that the working set exceeds the 126 MB L2 ("cold") or re-using one set ("warm").
+buffer sets that the working set exceeds the 50 MB L2 ("cold") or re-using one set ("warm").
 Usage: python tools/bench_ops.py [gn ln linear quantile attn cast final stem]
 """
 import os
@@ -14,7 +14,18 @@ from minimagen_b200 import _native, ops as ops_mod   # noqa: E402
 
 F16, F32, F64 = torch.float16, torch.float32, torch.float64
 dev = torch.device("cuda", 0)
-HBM = 6486.5   # GB/s, MEASURED_PEAKS.json
+
+def _hbm_gbs():
+    """HBM bandwidth of the roofline: MEASURED_PEAKS.json when present, else the H100 SXM data sheet (3.35 TB/s)."""
+    import json
+    try:
+        return float(json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
+                                                  "MEASURED_PEAKS.json")))["hbm_gbs"])
+    except Exception:
+        return 3350.0
+
+
+HBM = _hbm_gbs()   # GB/s
 
 
 def timeit(fn_list, reps=20):
@@ -120,7 +131,7 @@ def bench_attn(ops):
             ops.attention_tc = tc
             f = lambda: ops.attention(q, n * inner, inner, *args, null_kv, None, B, heads, n, m, out, n * inner, inner)
             ms = timeit([f], reps=5)
-            res.append(f"{'tcgen05' if tc else 'mma.sync'} {ms * 1e3:9.1f} us ({fl / ms / 1e9:6.1f} TFLOP/s)")
+            res.append(f"{'wgmma' if tc else 'mma.sync'} {ms * 1e3:9.1f} us ({fl / ms / 1e9:6.1f} TFLOP/s)")
         ops.attention_tc = True
         print(f"attention B={B} n={n} m={m} {'multi-query' if shared else 'per-head kv'}:  " + "   ".join(res), flush=True)
 

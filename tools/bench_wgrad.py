@@ -1,4 +1,4 @@
-"""Micro-benchmark: conv weight gradient, tcgen05 kernel (csrc/wgrad_tc.cu) vs the fp32 CUDA-core kernel (csrc/backward.cu)."""
+"""Micro-benchmark: conv weight gradient, wgmma kernel (csrc/wgrad_tc.cu) vs the fp32 CUDA-core kernel (csrc/backward.cu)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
