@@ -246,6 +246,9 @@ int mi_step_epilogue(const float* x_t, const float* eps_cond, const float* eps_n
 /* t[b] <- max(t[b] - 1, 0): the next iteration's timestep of Imagen._p_sample_loop (Imagen.py:398-415 walks the list of
  * diffusion_model.py:81-87), advanced on the device so that a captured step can be replayed back to back */
 int mi_step_advance_t(long long* t, int B, void* stream);
+/* t[b] <- next_t[t[b]]: the next iteration's timestep on a respaced sampling grid tau_S > ... > tau_1 = 0 (next_t [T] holds
+ * next_t[tau_i] = tau_{i-1}, next_t[0] = 0).  A t[b] outside [0, T) becomes 0.  No host work: capturable in a CUDA graph. */
+int mi_step_advance_t_table(long long* t, const long long* next_t, int T, int B, void* stream);
 /* clamp_(-1,1) and (x+1)*0.5 (Imagen.py:418-419) */
 int mi_step_finalize(const float* x, long long n, int unnormalize, float* out, void* stream);
 /* GaussianDiffusion.q_sample (diffusion_model.py:127-147) followed by v*post_scale + post_shift */

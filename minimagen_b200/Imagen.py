@@ -7,11 +7,13 @@ x0 prediction, EXACT per-image dynamic-threshold quantile (radix select), poster
 (both U-Net passes + epilogue) is optionally replayed from a CUDA graph so the ~10^3 kernel launches per step cost
 nothing on the host.
 
-Two additions that the reference does not have (both optional, defaults reproduce the reference):
+Three additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
-    its shard, ONE NCCL all-gather assembles the finished images (`sample(..., distributed=True)`).
+    its shard, ONE NCCL all-gather assembles the finished images (`sample(..., distributed=True)`);
+  * fewer-step DDIM sampling (`sample(..., sampling_timesteps=S, ddim_eta=eta)`): S steps over a respaced grid through
+    the same step kernels, with per-loop coefficient tables (GaussianDiffusion.sampling_schedule).
 """
 from contextlib import contextmanager
 from typing import Callable, List, Literal, Tuple, Union
@@ -21,7 +23,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from .Unet import Unet
-from .diffusion_model import GaussianDiffusion
+from .diffusion_model import GaussianDiffusion, SamplingSchedule
 from .helpers import (cast_tuple, default, eval_decorator, exists, identity, maybe, module_device,
                       normalize_neg_one_to_one, null_context, resize_image_to, unnormalize_zero_to_one)
 from . import _native as N
@@ -43,18 +45,26 @@ def quantile_rank(n: int, q: float):
 class _StepGraph:
     """One captured denoising step (U-Net pass(es) + step epilogue) over STATIC buffers:
          x      [B, C, s, s]  the image, updated IN PLACE by every replay (x_t -> x_{t-1});
-         t      [B] int64     the timestep, decremented (floor 0) at the end of every replay;
+         t      [B] int64     the timestep, decremented (floor 0) at the end of every replay -- or, in a respaced graph,
+                              moved to the next grid point through the static `sched.next_t` table;
          noise  [B, C, s, s]  the step's Gaussian draw: drawn INSIDE the graph (graph-safe Philox) unless the caller
                               injects noise, in which case it is copied here before each replay;
-         cond   static copies of text_embeds / text_mask / lowres_cond_img / lowres_noise_times (`set_cond` refreshes them).
-    A whole sampling loop is then `set x, t; replay() * T` -- no per-step host-side tensor ops."""
+         cond   static copies of text_embeds / text_mask / lowres_cond_img / lowres_noise_times (`set_cond` refreshes them);
+         sched  respaced graphs only: static [T] copies of a SamplingSchedule's c1 / c2 / sigma / next_t tables
+                (`set_schedule` refreshes them, so one captured graph serves every step count and eta).
+    A whole sampling loop is then `set x, t; replay() * T` (or `* S` on a respaced grid) -- no per-step host-side tensor ops."""
 
     def __init__(self):
         self.graph = None
         self.x = self.t = self.noise = None
         self.cond = {}
+        self.sched = None
         self.inject_noise = False
         self.unet = None
+
+    def set_schedule(self, sched):
+        for name in ('c1', 'c2', 'sigma', 'next_t'):
+            getattr(self.sched, name).copy_(getattr(sched, name))
 
     def set_cond(self, **tensors):
         for k, v in tensors.items():
@@ -224,17 +234,18 @@ class Imagen(nn.Module):
                 noise_scheduler.posterior_log_variance_clipped.gather(-1, t).reshape(shp))
 
     def _step(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-              cond_scale, model_output=None, out=None):
+              cond_scale, model_output=None, out=None, schedule=None):
         """x_{t-1} = posterior_mean(x_t, clamp-thresholded x0(x_t, eps)) + [t != 0] * sigma_t * noise.
-        `out` may be `x` itself (the captured step updates the image in place)."""
+        `out` may be `x` itself (the captured step updates the image in place).  `schedule` (a SamplingSchedule) replaces
+        the posterior coefficients and sigma by its DDIM tables: the step then goes to the next point of its grid."""
         with N.device_of(x):
             return self._step_impl(unet, x, t, noise, noise_scheduler=noise_scheduler, text_embeds=text_embeds,
                                    text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                                    lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
-                                   model_output=model_output, out=out)
+                                   model_output=model_output, out=out, schedule=schedule)
 
     def _step_impl(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                   lowres_noise_times, cond_scale, model_output=None, out=None):
+                   lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None):
         assert not (cond_scale != 1. and not self.can_classifier_guidance), \
             'imagen was not trained with conditional dropout, and thus one cannot use classifier free guidance ' \
             '(cond_scale anything other than 1)'
@@ -265,8 +276,10 @@ class Imagen(nn.Module):
             out = torch.empty_like(x)
         # ONE kernel: CFG combine + x0 + exact dynamic-threshold quantile + clamp/divide + posterior mean + noise
         # (mi_step_epilogue; images too large for its register-resident select take the three-kernel form inside the ABI)
+        c1, c2, sigma = ((sch.posterior_mean_coef1, sch.posterior_mean_coef2, sch.sigma) if schedule is None else
+                         (schedule.c1, schedule.c2, schedule.sigma))
         ops.step_epilogue(x, eps, eps_null, cond_scale, t, sch.sqrt_recip_alphas_cumprod, sch.sqrt_recipm1_alphas_cumprod,
-                          sch.posterior_mean_coef1, sch.posterior_mean_coef2, sch.sigma, noise, B, n, lo, hi, w, 1.0, out)
+                          c1, c2, sigma, noise, B, n, lo, hi, w, 1.0, out)
         return out
 
     @torch.no_grad()
@@ -281,13 +294,13 @@ class Imagen(nn.Module):
 
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-                   cond_scale):
+                   cond_scale, respaced=False):
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         p0 = next(unet.parameters())
         return (id(unet), tuple(shape), float(cond_scale), bool(self.cfg_batched), exists(self.noise_fn),
                 noise_scheduler.num_timesteps, sig(text_embeds), sig(text_mask), sig(lowres_cond_img),
                 sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
-                self.dynamic_thresholding_percentile)
+                self.dynamic_thresholding_percentile, bool(respaced))
 
     def clear_graphs(self):
         """Drop the captured step graphs (and the activation memory their pools hold)."""
@@ -297,12 +310,14 @@ class Imagen(nn.Module):
         self.max_cached_graphs = 4
 
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                    lowres_noise_times, cond_scale):
+                    lowres_noise_times, cond_scale, respaced=False):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
-        every later sampling loop of the same signature; the conditioning tensors are refreshed in its static buffers."""
+        every later sampling loop of the same signature; the conditioning tensors are refreshed in its static buffers.
+        `respaced`: the step reads its coefficients from static schedule tables (`_StepGraph.set_schedule`) and walks t
+        through next_t; neither the step count nor eta is part of the signature."""
         device = self.device
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                              lowres_noise_times, cond_scale)
+                              lowres_noise_times, cond_scale, respaced)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times)
         g = self._graphs.get(key)
@@ -322,12 +337,22 @@ class Imagen(nn.Module):
                   **{k: g.cond.get(k) for k in cond})
         g.refresh_static()
         ops = get_ops()
+        T = noise_scheduler.num_timesteps
+        if respaced:
+            # placeholder contents (the DDPM walk); every sampling loop installs its own tables with set_schedule
+            g.sched = SamplingSchedule(grid=(), c1=noise_scheduler.posterior_mean_coef1.clone(),
+                                       c2=noise_scheduler.posterior_mean_coef2.clone(),
+                                       sigma=noise_scheduler.sigma.clone(),
+                                       next_t=(torch.arange(T, device=device) - 1).clamp(min=0))
 
         def body():
             if not g.inject_noise:
                 g.noise.normal_()                       # the reference's randn_like(x) (Imagen.py:361), graph-safe Philox
-            self._step(unet, g.x, g.t, g.noise, out=g.x, **kw)
-            ops.step_advance_t(g.t, shape[0])           # t <- max(t - 1, 0): the next loop iteration's timestep
+            self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, **kw)
+            if respaced:
+                ops.step_advance_t_table(g.t, g.sched.next_t, T, shape[0])   # t <- next grid point
+            else:
+                ops.step_advance_t(g.t, shape[0])       # t <- max(t - 1, 0): the next loop iteration's timestep
 
         # warm-up on a side stream (packs weights, sizes the caching allocator), then capture
         side = torch.cuda.Stream(device=device)
@@ -344,10 +369,12 @@ class Imagen(nn.Module):
 
     @torch.no_grad()
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
-                       lowres_noise_times=None, cond_scale=1., max_steps=None, out=None):
+                       lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
-        reference) receives the finished images (e.g. this rank's slot of the all-gather buffer)."""
+        reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
+        reference; a SamplingSchedule from `noise_scheduler.sampling_schedule`) walks its respaced grid with DDIM steps
+        instead of every timestep.  One 'step' draw is taken per iteration, labelled with the iteration's timestep."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -355,7 +382,12 @@ class Imagen(nn.Module):
             if exists(lowres_cond_img):
                 lowres_cond_img = lowres_cond_img.to(F32).contiguous()
             batch = shape[0]
-            timesteps = noise_scheduler._get_sampling_timesteps(batch, device=device)
+            if exists(schedule):
+                grid = list(schedule.grid)
+                timesteps = [torch.full((batch,), t, device=device, dtype=torch.long) for t in grid]
+            else:
+                timesteps = noise_scheduler._get_sampling_timesteps(batch, device=device)
+                grid = [noise_scheduler.num_timesteps - 1 - i for i in range(len(timesteps))]
             if exists(max_steps):
                 timesteps = timesteps[:max_steps]
             img = self._noise('init', shape, -1, device)
@@ -363,18 +395,20 @@ class Imagen(nn.Module):
             kw = dict(noise_scheduler=noise_scheduler, text_embeds=text_embeds, text_mask=text_mask,
                       lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale)
             if self.use_cuda_graph and img.is_cuda and len(timesteps) > 2:
-                g = self._step_graph(unet, tuple(shape), **kw)
+                g = self._step_graph(unet, tuple(shape), respaced=exists(schedule), **kw)
+                if exists(schedule):
+                    g.set_schedule(schedule)
                 g.x.copy_(img)
                 g.t.copy_(timesteps[0])
                 for i in range(len(timesteps)):
                     if g.inject_noise:
-                        g.noise.copy_(self._noise('step', shape, noise_scheduler.num_timesteps - 1 - i, device))
-                    g.replay()                              # x <- x_{t-1} in place, t <- t - 1
+                        g.noise.copy_(self._noise('step', shape, grid[i], device))
+                    g.replay()                              # x <- x_{t-1} in place, t <- t - 1 (or the next grid point)
                 img = g.x
             else:
                 for i, times in enumerate(timesteps):
-                    noise = self._noise('step', shape, noise_scheduler.num_timesteps - 1 - i, device)
-                    img = self._step(unet, img, times, noise, **kw)
+                    noise = self._noise('step', shape, grid[i], device)
+                    img = self._step(unet, img, times, noise, schedule=schedule, **kw)
 
             if out is None:
                 out = torch.empty(tuple(shape), dtype=F32, device=device)
@@ -385,21 +419,42 @@ class Imagen(nn.Module):
     @eval_decorator
     def sample(self, texts: List[str] = None, text_masks=None, text_embeds=None, cond_scale: float = 1.,
                lowres_sample_noise_level: float = None, return_pil_images: bool = False, device=None,
-               distributed: bool = False):
+               distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0.):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
-        all-gather returns the full batch on every rank."""
+        all-gather returns the full batch on every rank.
+        `sampling_timesteps` (None, an int, or one entry per U-Net, each None or an int S with 2 <= S <= that stage's
+        timesteps) samples a stage with S DDIM steps over round(linspace(0, T-1, S)) instead of all T DDPM steps;
+        `ddim_eta` in [0, 1] scales their noise (0: deterministic given x_T; 1 at S = T: the DDPM sampler).  None (the
+        default) runs the DDPM loop."""
+        steps = self._sampling_steps(sampling_timesteps, ddim_eta)
         device = torch.device(default(device, self.device))
         self._reset_unets_all_one_device(device=device)
         if self._temp.device != device:
             self.to(device)
         with N.device_of(self._temp):
             return self._sample_impl(texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level,
-                                     return_pil_images, device, distributed)
+                                     return_pil_images, device, distributed, steps, ddim_eta)
+
+    def _sampling_steps(self, sampling_timesteps, ddim_eta):
+        """Per-U-Net step counts (None = the DDPM loop), validated."""
+        assert 0. <= ddim_eta <= 1., f'ddim_eta must be between 0 and 1, got {ddim_eta}'
+        n = len(self.unets)
+        if not isinstance(sampling_timesteps, (list, tuple)):
+            steps = (sampling_timesteps,) * n
+        else:
+            steps = tuple(sampling_timesteps)
+            assert len(steps) == n, \
+                f'sampling_timesteps must have one entry per unet ({n}), got {len(steps)}'
+        for s, sch in zip(steps, self.noise_schedulers):
+            if s is not None:
+                assert 2 <= s <= sch.num_timesteps, \
+                    f'sampling timesteps must be between 2 and the unet\'s {sch.num_timesteps} timesteps, got {s}'
+        return steps
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
-                     device, distributed):
+                     device, distributed, steps=None, ddim_eta=0.):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -428,9 +483,10 @@ class Imagen(nn.Module):
         img = None
         gathered = None
         n_stages = len(self.unets)
-        for unet_number, unet, channel, image_size, noise_scheduler in zip(
+        steps = default(steps, (None,) * n_stages)
+        for unet_number, unet, channel, image_size, noise_scheduler, n_steps in zip(
                 range(1, n_stages + 1), self.unets, self.sample_channels, self.image_sizes,
-                self.noise_schedulers):
+                self.noise_schedulers, steps):
             with self._one_unet_in_gpu(unet=unet):
                 lowres_cond_img = lowres_noise_times = None
                 if unet.lowres_cond:
@@ -450,10 +506,11 @@ class Imagen(nn.Module):
                     # the last stage finalises straight into this rank's slot of the all-gather buffer (no staging copy)
                     gathered = torch.empty((world * batch_size, *shape[1:]), dtype=F32, device=device)
                     slot = gathered[rank * batch_size:(rank + 1) * batch_size]
+                schedule = None if n_steps is None else noise_scheduler.sampling_schedule(n_steps, ddim_eta, device)
                 img = self._p_sample_loop(unet, shape, text_embeds=text_embeds, text_mask=text_masks,
                                           cond_scale=cond_scale, lowres_cond_img=lowres_cond_img,
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
-                                          out=slot)
+                                          out=slot, schedule=schedule)
 
         outputs = img
         if gathered is not None:

@@ -53,6 +53,7 @@ SIGNATURES = {
     "mi_step_epilogue_workspace_floats": [_I, _I],
     "mi_step_epilogue": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P, _P, _P, _P],
     "mi_step_advance_t": [_P, _I, _P],
+    "mi_step_advance_t_table": [_P, _P, _I, _I, _P],
     "mi_step_finalize": [_P, _L, _I, _P, _P],
     "mi_q_sample": [_P, _P, _P, _P, _P, _I, _I, _F, _F, _P, _P],
     # training side (backward)

@@ -293,6 +293,9 @@ int mi_step_epilogue(const float* x_t, const float* eps_cond, const float* eps_n
 int mi_step_advance_t(long long* t, int B, void* stream) {
     return check(mi::step_advance_t(t, B, S(stream)), "mi_step_advance_t");
 }
+int mi_step_advance_t_table(long long* t, const long long* next_t, int T, int B, void* stream) {
+    return check(mi::step_advance_t_table(t, next_t, T, B, S(stream)), "mi_step_advance_t_table");
+}
 int mi_step_finalize(const float* x, long long n, int unnormalize, float* out, void* stream) {
     return check(mi::step_finalize(x, n, unnormalize, out, S(stream)), "mi_step_finalize");
 }

@@ -422,6 +422,18 @@ __global__ void advance_t_kernel(long long* t, int B) {
     if (i < B) t[i] = t[i] > 0 ? t[i] - 1 : 0;
 }
 
+// t <- next_t[t]: the same walk over a respaced grid tau_S > ... > tau_1 = 0 (next_t[tau_i] = tau_{i-1}, next_t[0] = 0), so a
+// captured step replays any number of sampling steps.  A t outside [0, T) goes to 0 instead of indexing past the table.
+__global__ void advance_t_table_kernel(long long* t, const long long* __restrict__ next_t, int T, int B) {
+    pdl_wait();
+    pdl_trigger();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < B) {
+        const long long tb = t[i];
+        t[i] = (tb >= 0 && tb < T) ? next_t[tb] : 0;
+    }
+}
+
 // img.clamp_(-1, 1); (img + 1) * 0.5      (Imagen.py:418-419, helpers.py:183)
 __global__ void finalize_kernel(const float* __restrict__ x, long long n, int unnormalize, float* __restrict__ out) {
     pdl_wait();
@@ -505,6 +517,13 @@ int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null
 
 int step_advance_t(long long* t, int B, cudaStream_t st) {
     launch_k(advance_t_kernel, (B + 127) / 128, 128, 0, st, t, B);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+int step_advance_t_table(long long* t, const long long* next_t, int T, int B, cudaStream_t st) {
+    if (T <= 0 || B < 0) return -1;
+    if (B == 0) return 0;
+    launch_k(advance_t_table_kernel, (B + 127) / 128, 128, 0, st, t, next_t, T, B);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -8,11 +8,28 @@ per-timestep noise scale the fused step kernel gathers (reference computes it ev
 The tensor methods are kept for API parity (they are one-line broadcasts of table lookups); the sampling loop does
 NOT go through them -- it uses the fused step kernels (minimagen_b200/csrc/step.cu).
 """
+from typing import NamedTuple, Tuple
+
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from .helpers import default, extract, log
+
+
+def _betas_fp64(timesteps):
+    scale = 1000 / timesteps
+    return torch.linspace(scale * 0.0001, scale * 0.02, timesteps, dtype=torch.float64)
+
+
+class SamplingSchedule(NamedTuple):
+    """A respaced (DDIM) sampling walk, see `GaussianDiffusion.sampling_schedule`.  The tables are indexed by the step's
+    own timestep t and feed the fused step epilogue in place of posterior_mean_coef1 / posterior_mean_coef2 / sigma."""
+    grid: Tuple[int, ...]        # descending timesteps tau_S = T-1 > ... > tau_1 = 0 (host side)
+    c1: torch.Tensor             # [T] fp32: coefficient of the clamped x0
+    c2: torch.Tensor             # [T] fp32: coefficient of x_t
+    sigma: torch.Tensor          # [T] fp32: scale of the step's noise (exactly 0 for eta = 0 and at t = 0)
+    next_t: torch.Tensor         # [T] int64: next_t[tau_i] = tau_{i-1}, next_t[0] = 0
 
 
 class GaussianDiffusion(nn.Module):
@@ -22,8 +39,7 @@ class GaussianDiffusion(nn.Module):
         assert not timesteps < 20, f'timsteps must be at least 20'
         self.num_timesteps = timesteps
 
-        scale = 1000 / timesteps
-        betas = torch.linspace(scale * 0.0001, scale * 0.02, timesteps, dtype=torch.float64)
+        betas = _betas_fp64(timesteps)
         alphas = 1. - betas
         acp = torch.cumprod(alphas, axis=0)
         acp_prev = F.pad(acp[:-1], (1, 0), value=1.)
@@ -46,6 +62,50 @@ class GaussianDiffusion(nn.Module):
         reg('posterior_mean_coef2', (1. - acp_prev) * torch.sqrt(alphas) / (1. - acp))
         # what `(0.5 * model_log_variance).exp()` (Imagen.py:370) evaluates to on the fp32 table, op by op in fp32
         reg('sigma', (0.5 * self.posterior_log_variance_clipped).exp())
+        self._schedules = {}
+
+    # ---- respaced sampling (no reference counterpart)
+    def sampling_schedule(self, steps: int, eta: float, device) -> SamplingSchedule:
+        """DDIM (Song et al. 2021, eq. 12) over the grid tau = round(linspace(0, T-1, steps)), walked from T-1 down to 0.
+        With a_t = alphas_cumprod[t] and a_prev = alphas_cumprod[prev] (1 at the last step):
+            sigma^2 = eta^2 (1 - a_prev) / (1 - a_t) (1 - a_t / a_prev),   d = sqrt(max(1 - a_prev - sigma^2, 0)),
+            x_prev  = sqrt(a_prev) x0 + d eps' + sigma z,                  eps' = (x_t - sqrt(a_t) x0) / sqrt(1 - a_t),
+        which is x_prev = c1 x0 + c2 x_t + sigma z with c1 = sqrt(a_prev) - d sqrt(a_t) / sqrt(1 - a_t), c2 = d / sqrt(1 - a_t):
+        the form of the DDPM posterior step, so the same step kernels run it.  The tables are computed in fp64 and cast to
+        fp32; sigma is exp(0.5 * fp32(log sigma^2)) like `self.sigma`.  At steps = T, eta = 1 they equal
+        posterior_mean_coef1 / posterior_mean_coef2 (and sigma for t >= 1): the DDPM sampler.  Cached per (steps, eta, device)."""
+        T = self.num_timesteps
+        steps, eta = int(steps), float(eta)
+        assert 2 <= steps <= T, f'sampling timesteps must be between 2 and {T} (the number of training timesteps)'
+        assert 0. <= eta <= 1., f'ddim_eta must be in [0, 1], got {eta}'
+        device = torch.device(device)
+        key = (steps, eta, str(device))
+        sched = self._schedules.get(key)
+        if sched is not None:
+            return sched
+        grid_up = torch.linspace(0, T - 1, steps, dtype=torch.float64).round().long()
+        assert bool((grid_up[1:] > grid_up[:-1]).all()) and grid_up[0] == 0 and grid_up[-1] == T - 1
+        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        a_t = acp[grid_up]
+        a_prev = torch.cat((torch.ones(1, dtype=torch.float64), acp[grid_up[:-1]]))
+        sig2 = eta ** 2 * (1. - a_prev) / (1. - a_t) * (1. - a_t / a_prev)
+        d = (1. - a_prev - sig2).clamp(min=0.).sqrt()
+        c1 = a_prev.sqrt() - d * a_t.sqrt() / (1. - a_t).sqrt()
+        c2 = d / (1. - a_t).sqrt()
+        pos = sig2 > 0
+        sigma = torch.zeros(steps, dtype=torch.float32)
+        sigma[pos] = (0.5 * sig2[pos].log().to(torch.float32)).exp()
+
+        def table(v, dtype):
+            out = torch.zeros(T, dtype=dtype)
+            out[grid_up] = v.to(dtype)
+            return out.to(device)
+        next_t = torch.cat((torch.zeros(1, dtype=torch.long), grid_up[:-1]))
+        sched = SamplingSchedule(grid=tuple(grid_up.flip(0).tolist()), c1=table(c1, torch.float32),
+                                 c2=table(c2, torch.float32), sigma=table(sigma, torch.float32),
+                                 next_t=table(next_t, torch.long))
+        self._schedules[key] = sched
+        return sched
 
     # ---- integer timestep generators (diffusion_model.py:68-87)
     def _get_times(self, batch_size, noise_level, *, device):

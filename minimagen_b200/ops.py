@@ -242,6 +242,13 @@ class NativeOps:
         _chk(t, I64, "t")
         N.call("mi_step_advance_t", N.ptr(t), B, N.stream())
 
+    def step_advance_t_table(self, t, next_t, T, B):
+        """t <- next_t[t] (a t outside [0, T) becomes 0): the walk over a respaced sampling grid."""
+        _chk(t, I64, "t"); _chk(next_t, I64, "next_t")
+        if next_t.numel() < T:
+            raise ValueError(f"next_t: expected at least {T} entries, got {next_t.numel()}")
+        N.call("mi_step_advance_t_table", N.ptr(t), N.ptr(next_t), int(T), int(B), N.stream())
+
     def step_finalize(self, x, n, unnormalize, out):
         _chk(x, F32, "x"); _chk(out, F32, "out")
         N.call("mi_step_finalize", N.ptr(x), n, int(unnormalize), N.ptr(out), N.stream())
