@@ -21,6 +21,8 @@
 // Warp roles (384 threads): warpgroup 0 = producer (one elected lane issues the TMA loads), warpgroups 1 and 2 = consumers,
 // each owning 64 of the 128 pixel rows: wgmma m64nBLOCK_Nk16 with fp32 accumulators in registers, then
 // +bias +residual -> global fp32 and/or fp16 (+ GroupNorm block statistics) straight from the accumulator fragments.
+// In the TMA kernel the producer warpgroup gives its registers to the consumers (setmaxnreg 40 / 232): that is what lets
+// a consumer hold the 128 accumulators of a 256-wide tile.
 //
 // Fused GroupNorm variant (Block.forward, minimagen/layers.py:131-145: GroupNorm -> (scale + 1, shift) -> SiLU -> 3x3 conv):
 // the whole producer warpgroup builds the A tile instead of TMA -- it reads the fp32 NHWC source(s) (optionally the virtual
@@ -48,6 +50,10 @@ constexpr uint32_t kABytes = kConvBlockM * kConvBlockK * 2;    // 16 KiB per sta
 constexpr uint32_t kRingBudget = 192 * 1024;                   // operand ring (+ barriers + GN coefficients <= 227 KB)
 constexpr uint32_t kAuxBytes = 512;                            // barriers [0, 256), GroupNorm mean / rstd [256, 512)
 constexpr uint32_t kSmemMax = 227 * 1024;
+// register split of the TMA kernel: 128 * 40 + 256 * 232 <= 64K registers per SM
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file overcommitted");
 
 template <int BLOCK_N>
 struct Cfg {
@@ -107,6 +113,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (wg == 0) {
         if constexpr (!GN) {
             // ===================== TMA producer (warp 0 stays converged, one elected lane issues) =====================
+            ptx::setmaxnreg_dec<kProducerRegs>();
             if (warp == 0) {
                 int stage = 0;
                 uint32_t phase = 0;
@@ -270,6 +277,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
     } else {
         // ===================== consumers: rows [64 cw, 64 cw + 64) of every tile =====================
+        if constexpr (!GN) ptx::setmaxnreg_inc<kConsumerRegs>();
         const int cw = wg - 1;
         const int wq = warp & 3;                        // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
         const int cq = 2 * (lane & 3);                  // first of this thread's two columns in every 8-column group
@@ -442,16 +450,17 @@ void tile_geometry(int H, int W, int B, ConvTcArgs& a) {
     a.B = B; a.H = H; a.W = W;
 }
 
-// largest BLOCK_N of {128,64,32,16} dividing C_out that still gives every SM a tile; never shrink below 64 for that.
-// (BLOCK_N = 256 would need 128 accumulator registers per consumer thread and spills at 384 threads per CTA.)
+// Largest BLOCK_N of {256,128,64,32,16} dividing C_out that still gives every SM a tile; never shrink below 64 for that.
+// A 256-wide tile moves 25 % fewer operand bytes per FLOP than a 128-wide one; its 128 accumulators per consumer thread
+// fit because of the setmaxnreg split (only the TMA kernel has it: the fused GroupNorm kernel stays 128 wide).
 int pick_block_n(int Cout, int tiles_m, int hint, int num_sms) {
-    const int cands[4] = {128, 64, 32, 16};
+    const int cands[5] = {256, 128, 64, 32, 16};
     if (hint < 0) hint = -hint;
     if (hint > 0 && Cout % hint == 0)
-        for (int i = 0; i < 4; ++i)
+        for (int i = 0; i < 5; ++i)
             if (cands[i] == hint) return hint;
     int block_n = 16;
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < 5; ++i) {
         if (Cout % cands[i] != 0) continue;
         block_n = cands[i];
         if (tiles_m * (Cout / cands[i]) >= num_sms || cands[i] <= 64) break;
@@ -597,6 +606,7 @@ int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream) {
 
     const GnPrologueArgs gn{};
     switch (block_n) {
+        case 256: return launch<256, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
         case 128: return launch<128, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
         case 64: return launch<64, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
         case 32: return launch<32, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);

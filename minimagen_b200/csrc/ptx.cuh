@@ -1,4 +1,5 @@
-// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and matrix descriptors.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and matrix descriptors,
+// setmaxnreg.
 // Everything the tensor-core kernels need and nothing else.  No CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -122,6 +123,13 @@ __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t
 __device__ __forceinline__ void bar_sync(int id, int count) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+
+// Per-warpgroup register budget (all four warps of the warpgroup execute it): a warpgroup that needs few registers
+// releases them with dec, one that needs more claims them with inc (which waits until the registers are free).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 }  // namespace ptx
 }  // namespace mi

@@ -1,8 +1,9 @@
-"""Micro-benchmarks of the non-GEMM kernels at the cfg-3 (SR 64->256, dim 128, batch 32) shapes.  GPU only.
+"""Micro-benchmarks of single kernels at the cfg-3 (SR 64->256, dim 128, batch 32) shapes.  GPU only.
 
 Diagnostics for kernel tuning, not a bench value: CUDA events around `reps` back-to-back launches, rotating over enough
 buffer sets that the working set exceeds the 50 MB L2 ("cold") or re-using one set ("warm").
 Usage: python tools/bench_ops.py [gn ln linear quantile attn cast final stem]
+       python tools/bench_ops.py conv [block_n ...]   (implicit-GEMM convs; block_n 0 = the library's choice)
 """
 import os
 import sys
@@ -173,10 +174,75 @@ def bench_stem(ops):
     report("stem_unroll 6ch -> 128-wide f16, 256x256 b32", ms, ms, B * H * H * (6 * 4 + 128 * 2))
 
 
+# cfg-3 conv shape classes at b=32: (label, H=W, C_in of source 0, C_in of source 1 (virtual concat), C_out, kernel)
+CONV_SHAPES = [("3x3 1024->1024 @16", 16, 1024, 0, 1024, 3), ("3x3 2048->1024 @16 concat", 16, 1024, 1024, 1024, 3),
+               ("3x3 512->512 @32", 32, 512, 0, 512, 3), ("3x3 1024->512 @32", 32, 1024, 0, 512, 3),
+               ("3x3 256->256 @64", 64, 256, 0, 256, 3), ("3x3 512->256 @64", 64, 512, 0, 256, 3),
+               ("3x3 128->128 @256", 256, 128, 0, 128, 3), ("3x3 128->128 @128", 128, 128, 0, 128, 3),
+               ("3x3 256->128 @128", 128, 256, 0, 128, 3), ("1x1 1024->512 @32", 32, 1024, 0, 512, 1)]
+
+
+def conv_auto_block_n(c_out, tiles_m, num_sms):
+    """The tile width conv_tc.cu's pick_block_n selects without a hint (C_out % 64 == 0 here)."""
+    for bn in (256, 128):
+        if c_out % bn == 0 and tiles_m * (c_out // bn) >= num_sms:
+            return bn
+    return 64
+
+
+def conv_operand_bytes(tiles_m, c_out, k_blocks, block_n):
+    """L2 -> SM operand bytes of one launch: per tile and k-block one TMA stage, a 128x64 A box and a block_n x 64 B box."""
+    return tiles_m * (c_out // block_n) * k_blocks * (128 * 64 * 2 + block_n * 64 * 2)
+
+
+def bench_conv(ops, hints=(0,)):
+    """Usage: bench_ops.py conv [block_n ...] -- 0 = the library's own choice (default)."""
+    B = 32
+    num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    rows = [(lbl, H, c0, c1, co, k, False) for (lbl, H, c0, c1, co, k) in CONV_SHAPES]
+    rows.append(("3x3 512->512 @32 + res 1x1 1024 concat", 32, 512, 0, 512, 3, True))
+    for (lbl, H, c0, c1, c_out, k, res) in rows:
+        c_in = c0 + c1
+        act = torch.randn(B, H, H, c0, device=dev).to(F16)
+        act2 = torch.randn(B, H, H, c1, device=dev).to(F16) if c1 else None
+        out = torch.empty(B, H, H, c_out, device=dev, dtype=F16)
+        stats = torch.zeros(B, c_out // 16, 2, device=dev, dtype=F64)
+        bias = torch.randn(c_out, device=dev)
+        tiles_m = B * H * H // 128
+        k_blocks = k * k * c_in // 64
+        flop = 2.0 * B * H * H * c_out * k * k * c_in
+        if res:
+            x = torch.randn(B, H, H, 512, device=dev).to(F16)
+            x2 = torch.randn(B, H, H, 512, device=dev).to(F16)
+            wp = torch.randn(c_out, 9 * c_in + 1024, device=dev).to(F16) * 0.01
+            k_blocks += 1024 // 64
+            flop += 2.0 * B * H * H * c_out * 1024
+        else:
+            wp = torch.randn(c_out, k * k * c_in, device=dev).to(F16) * 0.01
+        res_line = []
+        for hint in ((0,) if res else hints):        # the folded res_conv takes no hint
+            if res:
+                f = lambda: ops.conv_res1x1(act, B, H, H, c_in, c_in, None, 0, 0, x, 512, 1024, x2, 512, 512, wp, c_out,
+                                            bias, None, None, out, stats)
+            else:
+                f = lambda hint=hint: ops.conv_igemm(act, B, H, H, c0, 0, c_in, wp, c_out, k, k, 0, bias, None, None, out,
+                                                     (H * H * c_out, H * c_out, c_out), block_n=hint, act2=act2, lda2=c1,
+                                                     c_in1=c0 if c1 else 0, out_stats=stats)
+            ms = timeit([f], reps=20)
+            bn = hint if hint and c_out % hint == 0 else conv_auto_block_n(c_out, tiles_m, num_sms)
+            nbytes = conv_operand_bytes(tiles_m, c_out, k_blocks, bn)
+            res_line.append(f"n{bn:<3d} {ms * 1e3:8.1f} us {flop / ms / 1e9:6.1f} TFLOP/s L2->SM {nbytes / ms / 1e9:5.2f} TB/s")
+        print(f"conv {lbl:40s} " + "  |  ".join(res_line), flush=True)
+
+
 def main():
     _native.load()
     ops = ops_mod.get_ops()
     which = sys.argv[1:] or ["gn", "ln", "linear", "quantile", "attn", "cast", "final", "stem"]
+    if which[0] == "conv":           # conv [block_n ...]
+        with torch.no_grad():
+            bench_conv(ops, tuple(int(h) for h in which[1:]) or (0,))
+        return
     table = {"gn": bench_gn, "ln": bench_ln, "linear": bench_linear, "quantile": bench_quantile, "attn": bench_attn,
              "cast": bench_cast, "final": bench_final, "stem": bench_stem}
     with torch.no_grad():
