@@ -251,6 +251,23 @@ int mi_step_advance_t(long long* t, int B, void* stream);
 int mi_step_advance_t_table(long long* t, const long long* next_t, int T, int B, void* stream);
 /* clamp_(-1,1) and (x+1)*0.5 (Imagen.py:418-419) */
 int mi_step_finalize(const float* x, long long n, int unnormalize, float* out, void* stream);
+/* RePaint inpainting (Imagen.sample(..., inpaint_images=, inpaint_masks=)).  x, k, z_*: [B, C, hw] fp32; m: [B, hw] fp32,
+ * broadcast over the C channels, a pixel is known where m >= 0.5; t, r: [B] int64 on the device; tables [T] fp32.
+ * mi_inpaint_prologue, in place on x, per image b with t = t[b]:
+ *   if r[b] > 0:   x <- ra[t] * x + rb[t] * z_renoise                      (re-noise from the next grid point back to t)
+ *   where known:   x <- sqrt_alphas_cumprod[t] * k + sqrt_one_minus_alphas_cumprod[t] * z_known
+ * rounded op by op (no fused multiply-add); the paste is a select, so an image with r[b] = 0 and no known pixel is left
+ * bitwise unchanged.  z_renoise is only read for images with r[b] > 0.  An image whose t is outside [0, T) is untouched.
+ * mi_inpaint_advance, the loop counter: if 0 < t[b] < T and r[b] + 1 < R[0], r[b] += 1; otherwise r[b] = 0 and t[b] moves
+ * to next_t[t[b]] (0 for a t outside [0, T)).  R is a device int64, so a captured graph serves every R.
+ * mi_inpaint_finalize: out = mi_step_finalize(where(m >= 0.5, k, x)).  All three capturable in a CUDA graph. */
+int mi_inpaint_prologue(float* x, const long long* t, const long long* r, const float* ra, const float* rb,
+                        const float* sqrt_alphas_cumprod, const float* sqrt_one_minus_alphas_cumprod, const float* k,
+                        const float* m, const float* z_renoise, const float* z_known, int T, int B, int C, int hw,
+                        void* stream);
+int mi_inpaint_advance(long long* t, long long* r, const long long* next_t, const long long* R, int T, int B, void* stream);
+int mi_inpaint_finalize(const float* x, const float* k, const float* m, int B, int C, int hw, int unnormalize, float* out,
+                        void* stream);
 /* GaussianDiffusion.q_sample (diffusion_model.py:127-147) followed by v*post_scale + post_shift */
 int mi_q_sample(const float* x0, const float* noise, const long long* t, const float* sqrt_alphas_cumprod,
                 const float* sqrt_one_minus_alphas_cumprod, int B, int n, float post_scale, float post_shift,

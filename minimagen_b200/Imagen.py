@@ -7,13 +7,21 @@ x0 prediction, EXACT per-image dynamic-threshold quantile (radix select), poster
 (both U-Net passes + epilogue) is optionally replayed from a CUDA graph so the ~10^3 kernel launches per step cost
 nothing on the host.
 
-Three additions that the reference does not have (all optional, defaults reproduce the reference):
+Four additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
     its shard, ONE NCCL all-gather assembles the finished images (`sample(..., distributed=True)`);
   * fewer-step DDIM sampling (`sample(..., sampling_timesteps=S, ddim_eta=eta)`): S steps over a respaced grid through
-    the same step kernels, with per-loop coefficient tables (GaussianDiffusion.sampling_schedule).
+    the same step kernels, with per-loop coefficient tables (GaussianDiffusion.sampling_schedule);
+  * inpainting with RePaint resampling (`sample(..., inpaint_images=, inpaint_masks=, inpaint_resample_times=R)`): at every
+    grid point t > 0 the step runs R times.  Each run after the first starts by re-noising x from the next grid point
+    back to t; then every run pastes in the known region, noised to t (Lugmayr et al. 2022, jump length 1).
+
+`noise_fn` kinds: 'init' (x_T, step -1), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
+augmentation noise, labelled with the U-Net number).  Inpainting labels the draws of iteration r at grid point t with
+t * R + r (at R = 1 that is t) and takes them in this order: 'renoise' (the re-noising draw, r > 0 only), 'inpaint' (the
+noise of the pasted known region), 'step'.
 """
 from contextlib import contextmanager
 from typing import Callable, List, Literal, Tuple, Union
@@ -51,20 +59,31 @@ class _StepGraph:
                               injects noise, in which case it is copied here before each replay;
          cond   static copies of text_embeds / text_mask / lowres_cond_img / lowres_noise_times (`set_cond` refreshes them);
          sched  respaced graphs only: static [T] copies of a SamplingSchedule's c1 / c2 / sigma / next_t tables
-                (`set_schedule` refreshes them, so one captured graph serves every step count and eta).
-    A whole sampling loop is then `set x, t; replay() * T` (or `* S` on a respaced grid) -- no per-step host-side tensor ops."""
+                (`set_schedule` refreshes them, so one captured graph serves every step count and eta);
+         inp    inpainting graphs only (always respaced): static k [B, C, s, s] (normalised known image), m [B, s*s]
+                (mask, known where >= 0.5), the RePaint counter r [B] and its limit R [1] (int64), the re-noising tables
+                ra / rb [T] and the draws z_renoise / z_known (`set_inpaint` refreshes them, so one graph serves any
+                mask, image and R).
+    A whole sampling loop is then `set x, t; replay() * T` (or `* S` on a respaced grid, `* ((S-1) R + 1)` when
+    inpainting) -- no per-step host-side tensor ops."""
 
     def __init__(self):
         self.graph = None
         self.x = self.t = self.noise = None
         self.cond = {}
         self.sched = None
+        self.inp = None
         self.inject_noise = False
         self.unet = None
 
     def set_schedule(self, sched):
         for name in ('c1', 'c2', 'sigma', 'next_t'):
             getattr(self.sched, name).copy_(getattr(sched, name))
+
+    def set_inpaint(self, k, m, R, ra, rb):
+        for name, v in (('k', k), ('m', m), ('ra', ra), ('rb', rb)):
+            self.inp[name].copy_(v)
+        self.inp['R'].fill_(int(R))
 
     def set_cond(self, **tensors):
         for k, v in tensors.items():
@@ -294,13 +313,14 @@ class Imagen(nn.Module):
 
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-                   cond_scale, respaced=False):
+                   cond_scale, respaced=False, inpaint=False):
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         p0 = next(unet.parameters())
-        return (id(unet), tuple(shape), float(cond_scale), bool(self.cfg_batched), exists(self.noise_fn),
-                noise_scheduler.num_timesteps, sig(text_embeds), sig(text_mask), sig(lowres_cond_img),
-                sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
-                self.dynamic_thresholding_percentile, bool(respaced))
+        key = (id(unet), tuple(shape), float(cond_scale), bool(self.cfg_batched), exists(self.noise_fn),
+               noise_scheduler.num_timesteps, sig(text_embeds), sig(text_mask), sig(lowres_cond_img),
+               sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
+               self.dynamic_thresholding_percentile, bool(respaced))
+        return key + ('inpaint',) if inpaint else key
 
     def clear_graphs(self):
         """Drop the captured step graphs (and the activation memory their pools hold)."""
@@ -310,14 +330,17 @@ class Imagen(nn.Module):
         self.max_cached_graphs = 4
 
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                    lowres_noise_times, cond_scale, respaced=False):
+                    lowres_noise_times, cond_scale, respaced=False, inpaint=False):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
         every later sampling loop of the same signature; the conditioning tensors are refreshed in its static buffers.
         `respaced`: the step reads its coefficients from static schedule tables (`_StepGraph.set_schedule`) and walks t
-        through next_t; neither the step count nor eta is part of the signature."""
+        through next_t; neither the step count nor eta is part of the signature.
+        `inpaint` (implies `respaced`): one RePaint iteration -- draws, mi_inpaint_prologue, the step, mi_inpaint_advance --
+        over the static buffers of `_StepGraph.set_inpaint`; neither the mask, the image nor R is part of the signature."""
         device = self.device
+        respaced = respaced or inpaint
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                              lowres_noise_times, cond_scale, respaced)
+                              lowres_noise_times, cond_scale, respaced, inpaint)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times)
         g = self._graphs.get(key)
@@ -344,12 +367,33 @@ class Imagen(nn.Module):
                                        c2=noise_scheduler.posterior_mean_coef2.clone(),
                                        sigma=noise_scheduler.sigma.clone(),
                                        next_t=(torch.arange(T, device=device) - 1).clamp(min=0))
+        p = None
+        if inpaint:
+            B, C, hw = shape[0], shape[1], shape[2] * shape[3]
+            # placeholder contents (nothing known, R = 1); every sampling loop installs its own with set_inpaint
+            g.inp = p = dict(k=torch.zeros(shape, dtype=F32, device=device),
+                             m=torch.zeros((B, hw), dtype=F32, device=device),
+                             r=torch.zeros((B,), dtype=torch.long, device=device),
+                             R=torch.ones((1,), dtype=torch.long, device=device),
+                             ra=torch.ones((T,), dtype=F32, device=device),
+                             rb=torch.zeros((T,), dtype=F32, device=device),
+                             z_renoise=torch.zeros(shape, dtype=F32, device=device),
+                             z_known=torch.zeros(shape, dtype=F32, device=device))
 
         def body():
             if not g.inject_noise:
+                if inpaint:
+                    p['z_renoise'].normal_()            # drawn every iteration, read only where r > 0
+                    p['z_known'].normal_()
                 g.noise.normal_()                       # the reference's randn_like(x) (Imagen.py:361), graph-safe Philox
+            if inpaint:
+                ops.inpaint_prologue(g.x, g.t, p['r'], p['ra'], p['rb'], noise_scheduler.sqrt_alphas_cumprod,
+                                     noise_scheduler.sqrt_one_minus_alphas_cumprod, p['k'], p['m'], p['z_renoise'],
+                                     p['z_known'], T, B, C, hw)
             self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, **kw)
-            if respaced:
+            if inpaint:
+                ops.inpaint_advance(g.t, p['r'], g.sched.next_t, p['R'], T, B)   # next repeat, or next grid point
+            elif respaced:
                 ops.step_advance_t_table(g.t, g.sched.next_t, T, shape[0])   # t <- next grid point
             else:
                 ops.step_advance_t(g.t, shape[0])       # t <- max(t - 1, 0): the next loop iteration's timestep
@@ -369,12 +413,15 @@ class Imagen(nn.Module):
 
     @torch.no_grad()
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
-                       lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None):
+                       lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
         reference; a SamplingSchedule from `noise_scheduler.sampling_schedule`) walks its respaced grid with DDIM steps
-        instead of every timestep.  One 'step' draw is taken per iteration, labelled with the iteration's timestep."""
+        instead of every timestep.  One 'step' draw is taken per iteration, labelled with the iteration's timestep.
+        `inpaint` (not in the reference): (k, m, R) -- the normalised known image [B, C, s, s] fp32, the mask [B, s*s] fp32
+        (known where >= 0.5) and the resample count R >= 1 -- runs the RePaint loop of `_repaint` and pastes k into the
+        known region of the finished images."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -394,6 +441,15 @@ class Imagen(nn.Module):
 
             kw = dict(noise_scheduler=noise_scheduler, text_embeds=text_embeds, text_mask=text_mask,
                       lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale)
+            if exists(inpaint):
+                k, m, R = inpaint
+                img = self._repaint(unet, shape, img, grid, schedule, k, m, R, max_steps, kw)
+                if out is None:
+                    out = torch.empty(tuple(shape), dtype=F32, device=device)
+                # where(m, k, x), clamp_(-1,1), (x+1)/2
+                ops.inpaint_finalize(img.contiguous(), k, m, shape[0], shape[1], shape[2] * shape[3],
+                                     int(self.auto_normalize_img), out)
+                return out
             if self.use_cuda_graph and img.is_cuda and len(timesteps) > 2:
                 g = self._step_graph(unet, tuple(shape), respaced=exists(schedule), **kw)
                 if exists(schedule):
@@ -415,11 +471,61 @@ class Imagen(nn.Module):
             ops.step_finalize(img.contiguous(), img.numel(), int(self.auto_normalize_img), out)   # clamp_(-1,1); (x+1)/2
             return out
 
+    def _repaint(self, unet, shape, img, grid, schedule, k, m, R, max_steps, kw):
+        """The RePaint iterations of one stage from x_T = `img` over `grid` (t', below, is the next grid point after t).  At
+        each grid point t the iterations r = 0 .. reps-1 (reps = R for t > 0, 1 at t = 0) each run
+            r > 0:  x <- sqrt(a_t / a_t') x + sqrt(1 - a_t / a_t') z_renoise       (back from t' to t)
+                    x <- where(m, sqrt(a_t) k + sqrt(1 - a_t) z_known, x)          (the known region, noised to t)
+                    x <- step(x, t)                                                (DDPM or DDIM, to t')
+        i.e. (S - 1) R + 1 U-Net evaluations for S grid points; `max_steps` counts iterations.  Returns x before the final
+        paste."""
+        device = self.device
+        ops = get_ops()
+        sch = kw['noise_scheduler']
+        T = sch.num_timesteps
+        B, C, hw = shape[0], shape[1], shape[2] * shape[3]
+        _, ra, rb = sch.inpaint_tables(schedule, device)    # the graph walks t through its schedule's next_t
+        plan = [(t, r) for t in grid for r in range(R if t > 0 else 1)]
+        if exists(max_steps):
+            plan = plan[:max_steps]
+
+        def draw(kind, t, r):
+            return self._noise(kind, shape, t * R + r, device)
+
+        if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
+            g = self._step_graph(unet, tuple(shape), inpaint=True, **kw)
+            g.set_schedule(schedule if exists(schedule) else sch.ddpm_schedule(device))
+            g.set_inpaint(k, m, R, ra, rb)
+            p = g.inp
+            g.x.copy_(img)
+            g.t.fill_(plan[0][0])
+            p['r'].zero_()
+            for t, r in plan:
+                if g.inject_noise:
+                    if r > 0:
+                        p['z_renoise'].copy_(draw('renoise', t, r))
+                    p['z_known'].copy_(draw('inpaint', t, r))
+                    g.noise.copy_(draw('step', t, r))
+                g.replay()                              # prologue + step in place; then (t, r) <- the next iteration
+            return g.x
+        img = img.clone()                               # the prologue works in place; x_T may be the caller's draw
+        for t, r in plan:
+            times = torch.full((B,), t, device=device, dtype=torch.long)
+            reps = torch.full((B,), r, device=device, dtype=torch.long)
+            z_renoise = draw('renoise', t, r) if r > 0 else None
+            z_known = draw('inpaint', t, r)
+            # at r = 0 the re-noising draw is not read: z_known stands in for the pointer
+            ops.inpaint_prologue(img, times, reps, ra, rb, sch.sqrt_alphas_cumprod, sch.sqrt_one_minus_alphas_cumprod,
+                                 k, m, z_renoise if r > 0 else z_known, z_known, T, B, C, hw)
+            img = self._step(unet, img, times, draw('step', t, r), schedule=schedule, **kw)
+        return img
+
     @torch.no_grad()
     @eval_decorator
     def sample(self, texts: List[str] = None, text_masks=None, text_embeds=None, cond_scale: float = 1.,
                lowres_sample_noise_level: float = None, return_pil_images: bool = False, device=None,
-               distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0.):
+               distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0., inpaint_images=None,
+               inpaint_masks=None, inpaint_resample_times: int = 5):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -427,15 +533,26 @@ class Imagen(nn.Module):
         `sampling_timesteps` (None, an int, or one entry per U-Net, each None or an int S with 2 <= S <= that stage's
         timesteps) samples a stage with S DDIM steps over round(linspace(0, T-1, S)) instead of all T DDPM steps;
         `ddim_eta` in [0, 1] scales their noise (0: deterministic given x_T; 1 at S = T: the DDPM sampler).  None (the
-        default) runs the DDPM loop."""
+        default) runs the DDPM loop.
+        `inpaint_images` (b, channels, s, s) float in `input_image_range` and `inpaint_masks` (b, s, s) bool, given
+        together (b: the full batch of the text conditioning), inpaint: True marks a pixel kept from `inpaint_images`,
+        False one the model generates.  Every stage resizes both to its size (known where the resized mask >= 0.5) and
+        runs RePaint with `inpaint_resample_times` (an int R >= 1) iterations per grid point t > 0, on the DDPM or the
+        DDIM walk, and pastes the known pixels into its output (module docstring)."""
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
+        assert exists(inpaint_images) == exists(inpaint_masks), \
+            'inpaint_images and inpaint_masks must be given together'
+        assert isinstance(inpaint_resample_times, int) and not isinstance(inpaint_resample_times, bool) \
+            and inpaint_resample_times >= 1, \
+            f'inpaint_resample_times must be an int >= 1, got {inpaint_resample_times!r}'
         device = torch.device(default(device, self.device))
         self._reset_unets_all_one_device(device=device)
         if self._temp.device != device:
             self.to(device)
+        inpaint = (inpaint_images, inpaint_masks, inpaint_resample_times) if exists(inpaint_images) else None
         with N.device_of(self._temp):
             return self._sample_impl(texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level,
-                                     return_pil_images, device, distributed, steps, ddim_eta)
+                                     return_pil_images, device, distributed, steps, ddim_eta, inpaint)
 
     def _sampling_steps(self, sampling_timesteps, ddim_eta):
         """Per-U-Net step counts (None = the DDPM loop), validated."""
@@ -454,7 +571,7 @@ class Imagen(nn.Module):
         return steps
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
-                     device, distributed, steps=None, ddim_eta=0.):
+                     device, distributed, steps=None, ddim_eta=0., inpaint=None):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -462,6 +579,21 @@ class Imagen(nn.Module):
         assert exists(text_embeds), 'text or text encodings must be passed into Imagen'
         assert not (exists(text_embeds) and text_embeds.shape[-1] != self.text_embed_dim), \
             f'invalid text embedding dimension being passed in (should be {self.text_embed_dim})'
+        inpaint_images = inpaint_masks = None
+        if exists(inpaint):
+            inpaint_images, inpaint_masks, resample_times = inpaint
+            b = text_embeds.shape[0]
+            assert torch.is_tensor(inpaint_images) and inpaint_images.is_floating_point(), \
+                'inpaint_images must be a float tensor'
+            assert inpaint_images.dim() == 4 and tuple(inpaint_images.shape[:2]) == (b, self.channels) and \
+                inpaint_images.shape[2] == inpaint_images.shape[3], \
+                f'inpaint_images must be (b, channels, s, s) = ({b}, {self.channels}, s, s), got ' \
+                f'{tuple(inpaint_images.shape)}'
+            s = inpaint_images.shape[-1]
+            assert torch.is_tensor(inpaint_masks) and inpaint_masks.dtype == torch.bool, \
+                'inpaint_masks must be a bool tensor'
+            assert tuple(inpaint_masks.shape) == (b, s, s), \
+                f'inpaint_masks must be (b, s, s) = ({b}, {s}, {s}), got {tuple(inpaint_masks.shape)}'
 
         world, rank = 1, 0
         if distributed:
@@ -473,8 +605,14 @@ class Imagen(nn.Module):
             per = full_b // world
             text_embeds = text_embeds[rank * per:(rank + 1) * per]
             text_masks = text_masks[rank * per:(rank + 1) * per] if exists(text_masks) else None
+            if exists(inpaint):
+                inpaint_images = inpaint_images[rank * per:(rank + 1) * per]
+                inpaint_masks = inpaint_masks[rank * per:(rank + 1) * per]
 
         batch_size = text_embeds.shape[0]
+        if exists(inpaint):
+            inpaint_images = inpaint_images.to(device=device, dtype=F32).contiguous()
+            inpaint_masks = inpaint_masks.to(device=device, dtype=F32)[:, None].contiguous()
         text_embeds = text_embeds.to(device=device, dtype=F32).contiguous()
         text_masks = text_masks.to(device).contiguous() if exists(text_masks) else None
         lowres_sample_noise_level = default(lowres_sample_noise_level, self.lowres_sample_noise_level)
@@ -507,10 +645,17 @@ class Imagen(nn.Module):
                     gathered = torch.empty((world * batch_size, *shape[1:]), dtype=F32, device=device)
                     slot = gathered[rank * batch_size:(rank + 1) * batch_size]
                 schedule = None if n_steps is None else noise_scheduler.sampling_schedule(n_steps, ddim_eta, device)
+                stage_inpaint = None
+                if exists(inpaint):
+                    # this stage's known image (normalised) and mask; unchanged when already at the stage's size
+                    k = resize_image_to(inpaint_images, image_size, clamp_range=self.input_image_range)
+                    m = resize_image_to(inpaint_masks, image_size, clamp_range=self.input_image_range)
+                    stage_inpaint = (self.normalize_img(k).contiguous(), m.reshape(batch_size, -1).contiguous(),
+                                     resample_times)
                 img = self._p_sample_loop(unet, shape, text_embeds=text_embeds, text_mask=text_masks,
                                           cond_scale=cond_scale, lowres_cond_img=lowres_cond_img,
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
-                                          out=slot, schedule=schedule)
+                                          out=slot, schedule=schedule, inpaint=stage_inpaint)
 
         outputs = img
         if gathered is not None:

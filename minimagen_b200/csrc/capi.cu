@@ -299,6 +299,21 @@ int mi_step_advance_t_table(long long* t, const long long* next_t, int T, int B,
 int mi_step_finalize(const float* x, long long n, int unnormalize, float* out, void* stream) {
     return check(mi::step_finalize(x, n, unnormalize, out, S(stream)), "mi_step_finalize");
 }
+int mi_inpaint_prologue(float* x, const long long* t, const long long* r, const float* ra, const float* rb,
+                        const float* sqrt_alphas_cumprod, const float* sqrt_one_minus_alphas_cumprod, const float* k,
+                        const float* m, const float* z_renoise, const float* z_known, int T, int B, int C, int hw,
+                        void* stream) {
+    return check(mi::inpaint_prologue(x, t, r, ra, rb, sqrt_alphas_cumprod, sqrt_one_minus_alphas_cumprod, k, m, z_renoise,
+                                      z_known, T, B, C, hw, S(stream)), "mi_inpaint_prologue");
+}
+int mi_inpaint_advance(long long* t, long long* r, const long long* next_t, const long long* R, int T, int B,
+                       void* stream) {
+    return check(mi::inpaint_advance(t, r, next_t, R, T, B, S(stream)), "mi_inpaint_advance");
+}
+int mi_inpaint_finalize(const float* x, const float* k, const float* m, int B, int C, int hw, int unnormalize, float* out,
+                        void* stream) {
+    return check(mi::inpaint_finalize(x, k, m, B, C, hw, unnormalize, out, S(stream)), "mi_inpaint_finalize");
+}
 int mi_q_sample(const float* x0, const float* noise, const long long* t, const float* tab_a, const float* tab_b, int B,
                 int n, float post_scale, float post_shift, float* out, void* stream) {
     return check(mi::q_sample(x0, noise, t, tab_a, tab_b, B, n, post_scale, post_shift, out, S(stream)), "mi_q_sample");

@@ -77,6 +77,13 @@ int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null
 int step_advance_t(long long* t, int B, cudaStream_t st);
 int step_advance_t_table(long long* t, const long long* next_t, int T, int B, cudaStream_t st);
 int step_finalize(const float* x, long long n, int unnormalize, float* out, cudaStream_t st);
+int inpaint_prologue(float* x, const long long* t, const long long* r, const float* ra, const float* rb,
+                     const float* sqrt_acp, const float* sqrt_1m_acp, const float* k, const float* m,
+                     const float* z_renoise, const float* z_known, int T, int B, int C, int hw, cudaStream_t st);
+int inpaint_advance(long long* t, long long* r, const long long* next_t, const long long* R, int T, int B,
+                    cudaStream_t st);
+int inpaint_finalize(const float* x, const float* k, const float* m, int B, int C, int hw, int unnormalize, float* out,
+                     cudaStream_t st);
 int q_sample(const float* x0, const float* noise, const long long* t, const float* tab_a, const float* tab_b, int B,
              int n_per_img, float post_scale, float post_shift, float* out, cudaStream_t st);
 

@@ -463,7 +463,100 @@ __global__ void q_sample_kernel(const float* __restrict__ x0, const float* __res
     out[idx] = v;
 }
 
+// RePaint inpainting, one iteration's prologue, in place on x [B, C, hw] (m, k broadcast over C; m: [B, hw]):
+//   r[b] > 0:  x <- ra[t] x + rb[t] z_renoise                          (re-noise from the next grid point back to t)
+//   m >= 0.5:  x <- sqrt_acp[t] k + sqrt_1m_acp[t] z_known             (paste the known region, noised to t)
+// Same op order as a torch restatement (explicit _rn, no contraction).  The paste is a select, so where m < 0.5 and
+// r[b] = 0 x is left bitwise unchanged.  z_renoise is only read where r[b] > 0; a t outside [0, T) leaves the image alone.
+__global__ void inpaint_prologue_kernel(float* __restrict__ x, const long long* __restrict__ t,
+                                        const long long* __restrict__ r, const float* __restrict__ ra,
+                                        const float* __restrict__ rb, const float* __restrict__ sqrt_acp,
+                                        const float* __restrict__ sqrt_1m_acp, const float* __restrict__ k,
+                                        const float* __restrict__ m, const float* __restrict__ z_renoise,
+                                        const float* __restrict__ z_known, int T, int C, int hw) {
+    pdl_wait();
+    pdl_trigger();
+    const int b = blockIdx.y;
+    const long long n_per_img = (long long)C * hw;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_per_img) return;
+    const long long tb = t[b];
+    if (tb < 0 || tb >= T) return;
+    const long long idx = (long long)b * n_per_img + i;
+    float v = x[idx];
+    if (r[b] > 0) v = __fadd_rn(__fmul_rn(ra[tb], v), __fmul_rn(rb[tb], z_renoise[idx]));
+    if (m[(long long)b * hw + i % hw] >= 0.5f)
+        v = __fadd_rn(__fmul_rn(sqrt_acp[tb], k[idx]), __fmul_rn(sqrt_1m_acp[tb], z_known[idx]));
+    x[idx] = v;
+}
+
+// The RePaint loop counter: r <- r + 1 while r + 1 < R at a grid point 0 < t < T; otherwise r <- 0 and t moves to the next
+// grid point (next_t[t]; a t outside [0, T) goes to 0).  R is read from the device so a captured graph serves every R.
+__global__ void inpaint_advance_kernel(long long* t, long long* r, const long long* __restrict__ next_t,
+                                       const long long* __restrict__ R, int T, int B) {
+    pdl_wait();
+    pdl_trigger();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B) return;
+    const long long tb = t[i], rr = r[i];
+    if (tb > 0 && tb < T && rr + 1 < R[0]) {
+        r[i] = rr + 1;
+    } else {
+        r[i] = 0;
+        t[i] = (tb >= 0 && tb < T) ? next_t[tb] : 0;
+    }
+}
+
+// finalize(where(m >= 0.5, k, x)): the last paste of the known region fused with clamp_(-1, 1) and (v + 1) * 0.5
+__global__ void inpaint_finalize_kernel(const float* __restrict__ x, const float* __restrict__ k,
+                                        const float* __restrict__ m, int C, int hw, int unnormalize,
+                                        float* __restrict__ out) {
+    pdl_wait();
+    pdl_trigger();
+    const int b = blockIdx.y;
+    const long long n_per_img = (long long)C * hw;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_per_img) return;
+    const long long idx = (long long)b * n_per_img + i;
+    float v = m[(long long)b * hw + i % hw] >= 0.5f ? k[idx] : x[idx];
+    v = fminf(fmaxf(v, -1.f), 1.f);
+    if (unnormalize) v = __fmul_rn(__fadd_rn(v, 1.f), 0.5f);
+    out[idx] = v;
+}
+
 }  // namespace
+
+int inpaint_prologue(float* x, const long long* t, const long long* r, const float* ra, const float* rb,
+                     const float* sqrt_acp, const float* sqrt_1m_acp, const float* k, const float* m,
+                     const float* z_renoise, const float* z_known, int T, int B, int C, int hw, cudaStream_t st) {
+    if (T <= 0 || B < 0 || C <= 0 || hw <= 0) return -1;
+    if (B == 0) return 0;
+    const long long n = (long long)C * hw;
+    if ((n + 255) / 256 > 0x7fffffffLL || B > 65535) return -1;
+    dim3 grid((unsigned)((n + 255) / 256), B);
+    launch_k(inpaint_prologue_kernel, grid, 256, 0, st, x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known,
+             T, C, hw);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+int inpaint_advance(long long* t, long long* r, const long long* next_t, const long long* R, int T, int B,
+                    cudaStream_t st) {
+    if (T <= 0 || B < 0) return -1;
+    if (B == 0) return 0;
+    launch_k(inpaint_advance_kernel, (B + 127) / 128, 128, 0, st, t, r, next_t, R, T, B);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+int inpaint_finalize(const float* x, const float* k, const float* m, int B, int C, int hw, int unnormalize, float* out,
+                     cudaStream_t st) {
+    if (B < 0 || C <= 0 || hw <= 0) return -1;
+    if (B == 0) return 0;
+    const long long n = (long long)C * hw;
+    if ((n + 255) / 256 > 0x7fffffffLL || B > 65535) return -1;
+    dim3 grid((unsigned)((n + 255) / 256), B);
+    launch_k(inpaint_finalize_kernel, grid, 256, 0, st, x, k, m, C, hw, unnormalize, out);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
 
 int step_x0(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const long long* t,
             const float* tab_recip, const float* tab_recipm1, int B, int n_per_img, float* x0, cudaStream_t st) {

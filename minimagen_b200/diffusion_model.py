@@ -107,6 +107,47 @@ class GaussianDiffusion(nn.Module):
         self._schedules[key] = sched
         return sched
 
+    def ddpm_schedule(self, device) -> SamplingSchedule:
+        """The DDPM walk T-1, ..., 0 as a SamplingSchedule: the posterior tables and next_t[t] = max(t - 1, 0).  A graph that
+        reads its coefficients from schedule tables runs the DDPM sampler with these installed.  Cached per device."""
+        device = torch.device(device)
+        key = ('ddpm', str(device))
+        sched = self._schedules.get(key)
+        if sched is None:
+            T = self.num_timesteps
+            sched = SamplingSchedule(grid=tuple(range(T - 1, -1, -1)),
+                                     c1=self.posterior_mean_coef1.to(device).clone(),
+                                     c2=self.posterior_mean_coef2.to(device).clone(),
+                                     sigma=self.sigma.to(device).clone(),
+                                     next_t=(torch.arange(T, device=device) - 1).clamp(min=0))
+            self._schedules[key] = sched
+        return sched
+
+    def inpaint_tables(self, schedule, device):
+        """Re-noising tables of RePaint inpainting (no reference counterpart) for the walk of `schedule` (a SamplingSchedule,
+        or None for the DDPM walk): (next_t [T] int64, ra [T] fp32, rb [T] fp32) with
+            ra[t] = sqrt(a_t / a_next),   rb[t] = sqrt(1 - a_t / a_next),   a = alphas_cumprod, next = next_t[t],
+        so that ra[t] x_next + rb[t] z takes a sample at the next grid point back to t.  Computed in fp64, cast to fp32;
+        ra = 1, rb = 0 at t = 0 and at timesteps off the grid.  For DDPM, ra[t] = sqrt(1 - beta_t).  Cached per walk."""
+        device = torch.device(device)
+        walk = self.ddpm_schedule(device) if schedule is None else schedule
+        key = ('inpaint', walk.grid, str(device))
+        tabs = self._schedules.get(key)
+        if tabs is not None:
+            return tabs
+        T = self.num_timesteps
+        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        on = torch.tensor([t for t in walk.grid if t > 0], dtype=torch.long)
+        nxt = walk.next_t.cpu()[on]
+        ratio = acp[on] / acp[nxt]
+        ra = torch.ones(T, dtype=torch.float64)
+        rb = torch.zeros(T, dtype=torch.float64)
+        ra[on] = ratio.sqrt()
+        rb[on] = (1. - ratio).sqrt()
+        tabs = (walk.next_t, ra.to(torch.float32).to(device), rb.to(torch.float32).to(device))
+        self._schedules[key] = tabs
+        return tabs
+
     # ---- integer timestep generators (diffusion_model.py:68-87)
     def _get_times(self, batch_size, noise_level, *, device):
         return torch.full((batch_size,), int(self.num_timesteps * noise_level), device=device, dtype=torch.long)

@@ -253,6 +253,39 @@ class NativeOps:
         _chk(x, F32, "x"); _chk(out, F32, "out")
         N.call("mi_step_finalize", N.ptr(x), n, int(unnormalize), N.ptr(out), N.stream())
 
+    def inpaint_prologue(self, x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
+        """RePaint prologue in place on x [B, C, hw]: re-noise where r > 0 (ra, rb), then paste the known region
+        (m [B, hw] >= 0.5) as sqrt_acp[t] k + sqrt_1m_acp[t] z_known.  z_renoise is only read where r > 0."""
+        for nm, tt in (("x", x), ("ra", ra), ("rb", rb), ("sqrt_acp", sqrt_acp), ("sqrt_1m_acp", sqrt_1m_acp), ("k", k),
+                       ("m", m), ("z_renoise", z_renoise), ("z_known", z_known)):
+            _chk(tt, F32, nm)
+        _chk(t, I64, "t"); _chk(r, I64, "r")
+        for nm, tab in (("ra", ra), ("rb", rb), ("sqrt_acp", sqrt_acp), ("sqrt_1m_acp", sqrt_1m_acp)):
+            if tab.numel() < T:
+                raise ValueError(f"{nm}: expected at least {T} entries, got {tab.numel()}")
+        for nm, tt in (("x", x), ("k", k), ("z_renoise", z_renoise), ("z_known", z_known)):
+            if tt.numel() != B * C * hw:
+                raise ValueError(f"{nm}: expected {B * C * hw} values, got {tt.numel()}")
+        if m.numel() != B * hw:
+            raise ValueError(f"m: expected {B * hw} values, got {m.numel()}")
+        N.call("mi_inpaint_prologue", N.ptr(x), N.ptr(t), N.ptr(r), N.ptr(ra), N.ptr(rb), N.ptr(sqrt_acp),
+               N.ptr(sqrt_1m_acp), N.ptr(k), N.ptr(m), N.ptr(z_renoise), N.ptr(z_known), int(T), int(B), int(C), int(hw),
+               N.stream())
+
+    def inpaint_advance(self, t, r, next_t, R, T, B):
+        """r <- r + 1 while r + 1 < R[0] at 0 < t < T, else r <- 0 and t <- next_t[t] (0 outside [0, T))."""
+        _chk(t, I64, "t"); _chk(r, I64, "r"); _chk(next_t, I64, "next_t"); _chk(R, I64, "R")
+        if next_t.numel() < T:
+            raise ValueError(f"next_t: expected at least {T} entries, got {next_t.numel()}")
+        N.call("mi_inpaint_advance", N.ptr(t), N.ptr(r), N.ptr(next_t), N.ptr(R), int(T), int(B), N.stream())
+
+    def inpaint_finalize(self, x, k, m, B, C, hw, unnormalize, out):
+        """out = clamp(where(m >= 0.5, k, x), -1, 1), then (v + 1) / 2 if unnormalize."""
+        for nm, tt in (("x", x), ("k", k), ("m", m), ("out", out)):
+            _chk(tt, F32, nm)
+        N.call("mi_inpaint_finalize", N.ptr(x), N.ptr(k), N.ptr(m), int(B), int(C), int(hw), int(unnormalize), N.ptr(out),
+               N.stream())
+
     def q_sample(self, x0, noise, t, tab_a, tab_b, B, n, post_scale, post_shift, out):
         _chk(x0, F32, "x0"); _chk(noise, F32, "noise"); _chk(t, I64, "t"); _chk(out, F32, "out")
         N.call("mi_q_sample", N.ptr(x0), N.ptr(noise), N.ptr(t), N.ptr(tab_a), N.ptr(tab_b), B, n, float(post_scale),
