@@ -5,7 +5,8 @@ Same class surface as the reference's `Imagen` (constructor `Imagen.py:27-42`, `
 asserts and messages.  The reverse-diffusion step is executed by the fused step kernels (csrc/step.cu): CFG combine,
 x0 prediction, EXACT per-image dynamic-threshold quantile (radix select), posterior mean and noise add; the whole step
 (both U-Net passes + epilogue) is optionally replayed from a CUDA graph so the ~10^3 kernel launches per step cost
-nothing on the host.
+nothing on the host.  Sampling captures two graph flavours: text-only (one graph serves the DDPM walk and every DDIM
+step count and eta) and inpainting.
 
 Four additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
@@ -31,7 +32,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from .Unet import Unet
-from .diffusion_model import GaussianDiffusion, SamplingSchedule
+from .diffusion_model import GaussianDiffusion
 from .helpers import (cast_tuple, default, eval_decorator, exists, identity, maybe, module_device,
                       normalize_neg_one_to_one, null_context, resize_image_to, unnormalize_zero_to_one)
 from . import _native as N
@@ -53,19 +54,19 @@ def quantile_rank(n: int, q: float):
 class _StepGraph:
     """One captured denoising step (U-Net pass(es) + step epilogue) over STATIC buffers:
          x      [B, C, s, s]  the image, updated IN PLACE by every replay (x_t -> x_{t-1});
-         t      [B] int64     the timestep, decremented (floor 0) at the end of every replay -- or, in a respaced graph,
-                              moved to the next grid point through the static `sched.next_t` table;
+         t      [B] int64     the timestep, moved to the next grid point through the static `sched.next_t` table at the
+                              end of every replay;
          noise  [B, C, s, s]  the step's Gaussian draw: drawn INSIDE the graph (graph-safe Philox) unless the caller
                               injects noise, in which case it is copied here before each replay;
          cond   static copies of text_embeds / text_mask / lowres_cond_img / lowres_noise_times (`set_cond` refreshes them);
-         sched  respaced graphs only: static [T] copies of a SamplingSchedule's c1 / c2 / sigma / next_t tables
-                (`set_schedule` refreshes them, so one captured graph serves every step count and eta);
-         inp    inpainting graphs only (always respaced): static k [B, C, s, s] (normalised known image), m [B, s*s]
-                (mask, known where >= 0.5), the RePaint counter r [B] and its limit R [1] (int64), the re-noising tables
-                ra / rb [T] and the draws z_renoise / z_known (`set_inpaint` refreshes them, so one graph serves any
-                mask, image and R).
-    A whole sampling loop is then `set x, t; replay() * T` (or `* S` on a respaced grid, `* ((S-1) R + 1)` when
-    inpainting) -- no per-step host-side tensor ops."""
+         sched  static [T] copies of a SamplingSchedule's c1 / c2 / sigma / next_t tables (`set_schedule` installs a walk's,
+                so one captured graph serves the DDPM walk and every DDIM step count and eta);
+         inp    inpainting graphs only: static k [B, C, s, s] (normalised known image), m [B, s*s] (mask, known where
+                >= 0.5), the RePaint counter r [B] and its limit R [1] (int64), the re-noising tables ra / rb [T] and the
+                draws z_renoise / z_known (`set_inpaint` refreshes them, so one graph serves any mask, image and R).
+    Two flavours: text-only (the step, then mi_step_advance_t_table) and inpainting (draws, mi_inpaint_prologue, the step,
+    mi_inpaint_advance).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
+    for DDPM; `* ((S-1) R + 1)` when inpainting) -- no per-step host-side tensor ops."""
 
     def __init__(self):
         self.graph = None
@@ -313,13 +314,13 @@ class Imagen(nn.Module):
 
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-                   cond_scale, respaced=False, inpaint=False):
+                   cond_scale, inpaint=False):
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         p0 = next(unet.parameters())
         key = (id(unet), tuple(shape), float(cond_scale), bool(self.cfg_batched), exists(self.noise_fn),
                noise_scheduler.num_timesteps, sig(text_embeds), sig(text_mask), sig(lowres_cond_img),
                sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
-               self.dynamic_thresholding_percentile, bool(respaced))
+               self.dynamic_thresholding_percentile)
         return key + ('inpaint',) if inpaint else key
 
     def clear_graphs(self):
@@ -330,85 +331,88 @@ class Imagen(nn.Module):
         self.max_cached_graphs = 4
 
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                    lowres_noise_times, cond_scale, respaced=False, inpaint=False):
+                    lowres_noise_times, cond_scale, schedule=None, inpaint=None):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
-        every later sampling loop of the same signature; the conditioning tensors are refreshed in its static buffers.
-        `respaced`: the step reads its coefficients from static schedule tables (`_StepGraph.set_schedule`) and walks t
-        through next_t; neither the step count nor eta is part of the signature.
-        `inpaint` (implies `respaced`): one RePaint iteration -- draws, mi_inpaint_prologue, the step, mi_inpaint_advance --
-        over the static buffers of `_StepGraph.set_inpaint`; neither the mask, the image nor R is part of the signature."""
+        every later sampling loop of the same signature.  Every lookup refreshes the conditioning tensors in its static
+        buffers and installs the walk `schedule` (a SamplingSchedule; None: the DDPM walk) in its static tables: the step
+        reads its coefficients from them and walks t through next_t, so neither the step count nor eta is part of the
+        signature.
+        `inpaint` ((k, m, R) as in `_p_sample_loop`): the inpainting flavour -- one RePaint iteration, draws,
+        mi_inpaint_prologue, the step, mi_inpaint_advance -- with k, m, R and the walk's re-noising tables installed by
+        `_StepGraph.set_inpaint`; neither the mask, the image nor R is part of the signature."""
         device = self.device
-        respaced = respaced or inpaint
+        schedule = default(schedule, lambda: noise_scheduler.ddpm_schedule(device))
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                              lowres_noise_times, cond_scale, respaced, inpaint)
+                              lowres_noise_times, cond_scale, exists(inpaint))
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times)
         g = self._graphs.get(key)
         if g is not None:
             g.set_cond(**cond)
-            return g
-        if len(self._graphs) >= self.max_cached_graphs:
-            self._graphs.pop(next(iter(self._graphs))).release()
-        g = _StepGraph()
-        g.unet = unet
-        g.inject_noise = exists(self.noise_fn)
-        g.x = torch.zeros(shape, dtype=F32, device=device)
-        g.noise = torch.zeros(shape, dtype=F32, device=device)
-        g.t = torch.zeros((shape[0],), dtype=torch.long, device=device)
-        g.cond = {k: v.clone() for k, v in cond.items() if v is not None}
-        kw = dict(noise_scheduler=noise_scheduler, cond_scale=cond_scale,
-                  **{k: g.cond.get(k) for k in cond})
-        g.refresh_static()
-        ops = get_ops()
-        T = noise_scheduler.num_timesteps
-        if respaced:
-            # placeholder contents (the DDPM walk); every sampling loop installs its own tables with set_schedule
-            g.sched = SamplingSchedule(grid=(), c1=noise_scheduler.posterior_mean_coef1.clone(),
-                                       c2=noise_scheduler.posterior_mean_coef2.clone(),
-                                       sigma=noise_scheduler.sigma.clone(),
-                                       next_t=(torch.arange(T, device=device) - 1).clamp(min=0))
-        p = None
-        if inpaint:
+        else:
+            if len(self._graphs) >= self.max_cached_graphs:
+                self._graphs.pop(next(iter(self._graphs))).release()
+            g = _StepGraph()
+            g.unet = unet
+            g.inject_noise = exists(self.noise_fn)
+            g.x = torch.zeros(shape, dtype=F32, device=device)
+            g.noise = torch.zeros(shape, dtype=F32, device=device)
+            g.t = torch.zeros((shape[0],), dtype=torch.long, device=device)
+            g.cond = {k: v.clone() for k, v in cond.items() if v is not None}
+            kw = dict(noise_scheduler=noise_scheduler, cond_scale=cond_scale,
+                      **{k: g.cond.get(k) for k in cond})
+            g.refresh_static()
+            ops = get_ops()
+            T = noise_scheduler.num_timesteps
             B, C, hw = shape[0], shape[1], shape[2] * shape[3]
-            # placeholder contents (nothing known, R = 1); every sampling loop installs its own with set_inpaint
-            g.inp = p = dict(k=torch.zeros(shape, dtype=F32, device=device),
-                             m=torch.zeros((B, hw), dtype=F32, device=device),
-                             r=torch.zeros((B,), dtype=torch.long, device=device),
-                             R=torch.ones((1,), dtype=torch.long, device=device),
-                             ra=torch.ones((T,), dtype=F32, device=device),
-                             rb=torch.zeros((T,), dtype=F32, device=device),
-                             z_renoise=torch.zeros(shape, dtype=F32, device=device),
-                             z_known=torch.zeros(shape, dtype=F32, device=device))
+            ddpm = noise_scheduler.ddpm_schedule(device)
+            # static copies (the grid stays with the caller); set_schedule installs the requested walk below
+            g.sched = ddpm._replace(grid=(), c1=ddpm.c1.clone(), c2=ddpm.c2.clone(), sigma=ddpm.sigma.clone(),
+                                    next_t=ddpm.next_t.clone())
+            p = None
+            if exists(inpaint):
+                # placeholder contents (nothing known, R = 1); set_inpaint installs the caller's below
+                g.inp = p = dict(k=torch.zeros(shape, dtype=F32, device=device),
+                                 m=torch.zeros((B, hw), dtype=F32, device=device),
+                                 r=torch.zeros((B,), dtype=torch.long, device=device),
+                                 R=torch.ones((1,), dtype=torch.long, device=device),
+                                 ra=torch.ones((T,), dtype=F32, device=device),
+                                 rb=torch.zeros((T,), dtype=F32, device=device),
+                                 z_renoise=torch.zeros(shape, dtype=F32, device=device),
+                                 z_known=torch.zeros(shape, dtype=F32, device=device))
 
-        def body():
-            if not g.inject_noise:
-                if inpaint:
-                    p['z_renoise'].normal_()            # drawn every iteration, read only where r > 0
-                    p['z_known'].normal_()
-                g.noise.normal_()                       # the reference's randn_like(x) (Imagen.py:361), graph-safe Philox
-            if inpaint:
-                ops.inpaint_prologue(g.x, g.t, p['r'], p['ra'], p['rb'], noise_scheduler.sqrt_alphas_cumprod,
-                                     noise_scheduler.sqrt_one_minus_alphas_cumprod, p['k'], p['m'], p['z_renoise'],
-                                     p['z_known'], T, B, C, hw)
-            self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, **kw)
-            if inpaint:
-                ops.inpaint_advance(g.t, p['r'], g.sched.next_t, p['R'], T, B)   # next repeat, or next grid point
-            elif respaced:
-                ops.step_advance_t_table(g.t, g.sched.next_t, T, shape[0])   # t <- next grid point
-            else:
-                ops.step_advance_t(g.t, shape[0])       # t <- max(t - 1, 0): the next loop iteration's timestep
+            def body():
+                if not g.inject_noise:
+                    if exists(p):
+                        p['z_renoise'].normal_()        # drawn every iteration, read only where r > 0
+                        p['z_known'].normal_()
+                    g.noise.normal_()                   # the reference's randn_like(x) (Imagen.py:361), graph-safe Philox
+                if exists(p):
+                    ops.inpaint_prologue(g.x, g.t, p['r'], p['ra'], p['rb'], noise_scheduler.sqrt_alphas_cumprod,
+                                         noise_scheduler.sqrt_one_minus_alphas_cumprod, p['k'], p['m'], p['z_renoise'],
+                                         p['z_known'], T, B, C, hw)
+                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, **kw)
+                if exists(p):
+                    ops.inpaint_advance(g.t, p['r'], g.sched.next_t, p['R'], T, B)   # next repeat, or next grid point
+                else:
+                    ops.step_advance_t_table(g.t, g.sched.next_t, T, B)              # t <- next grid point
 
-        # warm-up on a side stream (packs weights, sizes the caching allocator), then capture
-        side = torch.cuda.Stream(device=device)
-        side.wait_stream(torch.cuda.current_stream(device))
-        with torch.cuda.stream(side):
-            body()
-        torch.cuda.current_stream(device).wait_stream(side)
-        torch.cuda.synchronize(device)
-        g.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g.graph):
-            body()
-        self._graphs[key] = g
+            # warm-up on a side stream (packs weights, sizes the caching allocator), then capture
+            side = torch.cuda.Stream(device=device)
+            side.wait_stream(torch.cuda.current_stream(device))
+            with torch.cuda.stream(side):
+                body()
+            torch.cuda.current_stream(device).wait_stream(side)
+            torch.cuda.synchronize(device)
+            g.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g.graph):
+                body()
+            self._graphs[key] = g
+        g.set_schedule(schedule)
+        if exists(inpaint):
+            k, m, R = inpaint
+            _, ra, rb = noise_scheduler.inpaint_tables(schedule, device)
+            g.set_inpaint(k, m, R, ra, rb)
         return g
 
     @torch.no_grad()
@@ -418,107 +422,74 @@ class Imagen(nn.Module):
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
         reference; a SamplingSchedule from `noise_scheduler.sampling_schedule`) walks its respaced grid with DDIM steps
-        instead of every timestep.  One 'step' draw is taken per iteration, labelled with the iteration's timestep.
+        instead of every timestep.
         `inpaint` (not in the reference): (k, m, R) -- the normalised known image [B, C, s, s] fp32, the mask [B, s*s] fp32
-        (known where >= 0.5) and the resample count R >= 1 -- runs the RePaint loop of `_repaint` and pastes k into the
-        known region of the finished images."""
+        (known where >= 0.5) and the resample count R >= 1 -- runs RePaint and pastes k into the known region of the
+        finished images.  With t' the next grid point after t, the iterations r = 0 .. reps-1 at grid point t (reps = R for
+        t > 0, 1 at t = 0) each run
+            r > 0:  x <- sqrt(a_t / a_t') x + sqrt(1 - a_t / a_t') z_renoise       (back from t' to t)
+                    x <- where(m, sqrt(a_t) k + sqrt(1 - a_t) z_known, x)          (the known region, noised to t)
+                    x <- step(x, t)                                                (DDPM or DDIM, to t')
+        i.e. (S - 1) R + 1 U-Net evaluations for S grid points.  Without `inpaint` an iteration is the step alone (R = 1).
+        `max_steps` counts iterations.  The draws of each iteration are those of the module docstring."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
             lowres_cond_img = maybe(self.normalize_img)(lowres_cond_img)
             if exists(lowres_cond_img):
                 lowres_cond_img = lowres_cond_img.to(F32).contiguous()
-            batch = shape[0]
-            if exists(schedule):
-                grid = list(schedule.grid)
-                timesteps = [torch.full((batch,), t, device=device, dtype=torch.long) for t in grid]
-            else:
-                timesteps = noise_scheduler._get_sampling_timesteps(batch, device=device)
-                grid = [noise_scheduler.num_timesteps - 1 - i for i in range(len(timesteps))]
+            sch = noise_scheduler
+            walk = default(schedule, lambda: sch.ddpm_schedule(device))
+            k, m, R = default(inpaint, (None, None, 1))
+            plan = [(t, r) for t in walk.grid for r in range(R if t > 0 else 1)]
             if exists(max_steps):
-                timesteps = timesteps[:max_steps]
+                plan = plan[:max_steps]
+            if exists(inpaint):
+                draws = [([('renoise', t * R + r)] if r > 0 else []) + [('inpaint', t * R + r), ('step', t * R + r)]
+                         for t, r in plan]
+            else:
+                draws = [[('step', t)] for t, _ in plan]
+            B, C, hw = shape[0], shape[1], shape[2] * shape[3]
             img = self._noise('init', shape, -1, device)
 
             kw = dict(noise_scheduler=noise_scheduler, text_embeds=text_embeds, text_mask=text_mask,
                       lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale)
-            if exists(inpaint):
-                k, m, R = inpaint
-                img = self._repaint(unet, shape, img, grid, schedule, k, m, R, max_steps, kw)
-                if out is None:
-                    out = torch.empty(tuple(shape), dtype=F32, device=device)
-                # where(m, k, x), clamp_(-1,1), (x+1)/2
-                ops.inpaint_finalize(img.contiguous(), k, m, shape[0], shape[1], shape[2] * shape[3],
-                                     int(self.auto_normalize_img), out)
-                return out
-            if self.use_cuda_graph and img.is_cuda and len(timesteps) > 2:
-                g = self._step_graph(unet, tuple(shape), respaced=exists(schedule), **kw)
-                if exists(schedule):
-                    g.set_schedule(schedule)
+            if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
+                g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, **kw)
+                static = dict(step=g.noise)
+                if exists(inpaint):
+                    static.update(renoise=g.inp['z_renoise'], inpaint=g.inp['z_known'])
+                    g.inp['r'].zero_()
                 g.x.copy_(img)
-                g.t.copy_(timesteps[0])
-                for i in range(len(timesteps)):
+                g.t.fill_(plan[0][0])
+                for iteration in draws:
                     if g.inject_noise:
-                        g.noise.copy_(self._noise('step', shape, grid[i], device))
-                    g.replay()                              # x <- x_{t-1} in place, t <- t - 1 (or the next grid point)
+                        for kind, label in iteration:
+                            static[kind].copy_(self._noise(kind, shape, label, device))
+                    g.replay()                  # [prologue +] step in place; then t (and r) <- the next iteration's
                 img = g.x
             else:
-                for i, times in enumerate(timesteps):
-                    noise = self._noise('step', shape, grid[i], device)
-                    img = self._step(unet, img, times, noise, schedule=schedule, **kw)
+                if exists(inpaint):
+                    _, ra, rb = sch.inpaint_tables(walk, device)
+                    img = img.clone()           # the prologue works in place; x_T may be the caller's draw
+                for (t, r), iteration in zip(plan, draws):
+                    z = {kind: self._noise(kind, shape, label, device) for kind, label in iteration}
+                    times = torch.full((B,), t, device=device, dtype=torch.long)
+                    if exists(inpaint):
+                        reps = torch.full((B,), r, device=device, dtype=torch.long)
+                        # at r = 0 the re-noising draw is not read: the 'inpaint' draw stands in for the pointer
+                        ops.inpaint_prologue(img, times, reps, ra, rb, sch.sqrt_alphas_cumprod,
+                                             sch.sqrt_one_minus_alphas_cumprod, k, m, z.get('renoise', z['inpaint']),
+                                             z['inpaint'], sch.num_timesteps, B, C, hw)
+                    img = self._step(unet, img, times, z['step'], schedule=walk, **kw)
 
             if out is None:
                 out = torch.empty(tuple(shape), dtype=F32, device=device)
-            ops.step_finalize(img.contiguous(), img.numel(), int(self.auto_normalize_img), out)   # clamp_(-1,1); (x+1)/2
+            if exists(inpaint):         # where(m, k, x), clamp_(-1,1), (x+1)/2
+                ops.inpaint_finalize(img.contiguous(), k, m, B, C, hw, int(self.auto_normalize_img), out)
+            else:                       # clamp_(-1,1); (x+1)/2
+                ops.step_finalize(img.contiguous(), img.numel(), int(self.auto_normalize_img), out)
             return out
-
-    def _repaint(self, unet, shape, img, grid, schedule, k, m, R, max_steps, kw):
-        """The RePaint iterations of one stage from x_T = `img` over `grid` (t', below, is the next grid point after t).  At
-        each grid point t the iterations r = 0 .. reps-1 (reps = R for t > 0, 1 at t = 0) each run
-            r > 0:  x <- sqrt(a_t / a_t') x + sqrt(1 - a_t / a_t') z_renoise       (back from t' to t)
-                    x <- where(m, sqrt(a_t) k + sqrt(1 - a_t) z_known, x)          (the known region, noised to t)
-                    x <- step(x, t)                                                (DDPM or DDIM, to t')
-        i.e. (S - 1) R + 1 U-Net evaluations for S grid points; `max_steps` counts iterations.  Returns x before the final
-        paste."""
-        device = self.device
-        ops = get_ops()
-        sch = kw['noise_scheduler']
-        T = sch.num_timesteps
-        B, C, hw = shape[0], shape[1], shape[2] * shape[3]
-        _, ra, rb = sch.inpaint_tables(schedule, device)    # the graph walks t through its schedule's next_t
-        plan = [(t, r) for t in grid for r in range(R if t > 0 else 1)]
-        if exists(max_steps):
-            plan = plan[:max_steps]
-
-        def draw(kind, t, r):
-            return self._noise(kind, shape, t * R + r, device)
-
-        if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
-            g = self._step_graph(unet, tuple(shape), inpaint=True, **kw)
-            g.set_schedule(schedule if exists(schedule) else sch.ddpm_schedule(device))
-            g.set_inpaint(k, m, R, ra, rb)
-            p = g.inp
-            g.x.copy_(img)
-            g.t.fill_(plan[0][0])
-            p['r'].zero_()
-            for t, r in plan:
-                if g.inject_noise:
-                    if r > 0:
-                        p['z_renoise'].copy_(draw('renoise', t, r))
-                    p['z_known'].copy_(draw('inpaint', t, r))
-                    g.noise.copy_(draw('step', t, r))
-                g.replay()                              # prologue + step in place; then (t, r) <- the next iteration
-            return g.x
-        img = img.clone()                               # the prologue works in place; x_T may be the caller's draw
-        for t, r in plan:
-            times = torch.full((B,), t, device=device, dtype=torch.long)
-            reps = torch.full((B,), r, device=device, dtype=torch.long)
-            z_renoise = draw('renoise', t, r) if r > 0 else None
-            z_known = draw('inpaint', t, r)
-            # at r = 0 the re-noising draw is not read: z_known stands in for the pointer
-            ops.inpaint_prologue(img, times, reps, ra, rb, sch.sqrt_alphas_cumprod, sch.sqrt_one_minus_alphas_cumprod,
-                                 k, m, z_renoise if r > 0 else z_known, z_known, T, B, C, hw)
-            img = self._step(unet, img, times, draw('step', t, r), schedule=schedule, **kw)
-        return img
 
     @torch.no_grad()
     @eval_decorator

@@ -1,6 +1,6 @@
 """Fewer-step DDIM sampling on the GPU: the timestep-table kernel (mi_step_advance_t_table), the respaced loop through the
 captured step graph and eagerly, against the DDPM path (S = T, eta = 1), the paper-form CPU restatement and the
-reference's cascade golden."""
+reference's cascade golden; one captured graph serving DDPM and DDIM loops in turn."""
 import pytest
 import torch
 
@@ -106,6 +106,25 @@ def test_respaced_graph_reused_across_steps_and_eta(native):
     want = _loop(ref, g, ref.noise_schedulers[0].sampling_schedule(10, 0.5, "cuda"), False, max_steps=4)
     assert len(im._graphs) == 1 and rel_l2(out, want) <= 1e-5
     assert im.noise_fn.calls == [("init", -1), ("step", 999), ("step", 888), ("step", 777), ("step", 666)]
+
+
+def test_one_graph_serves_ddpm_and_ddim(native):
+    """DDPM, then DDIM (S = 8, eta = 0.5), then DDPM again on one Imagen run through one captured graph; each loop equals
+    its own eager run, and the last DDPM loop equals the first (the DDIM tables were replaced)."""
+    g = load_golden("sample_loop.pt")
+    im = _tiny_imagen(g, 25, "cuda")
+    ref = _tiny_imagen(g, 25, "cuda")
+    outs = []
+    for S in (None, 8, None):
+        im.noise_fn, ref.noise_fn = _bank(11), _bank(11)
+        out = _loop(im, g, None if S is None else im.noise_schedulers[0].sampling_schedule(S, 0.5, "cuda"), True)
+        want = _loop(ref, g, None if S is None else ref.noise_schedulers[0].sampling_schedule(S, 0.5, "cuda"), False)
+        err = rel_l2(out, want)
+        print(f"S={S}: graph vs eager {err:.3e}")
+        assert err <= 1e-5
+        outs.append(out)
+    assert len(im._graphs) == 1
+    assert rel_l2(outs[2], outs[0]) <= 1e-5
 
 
 def test_cascade_full_steps_vs_reference_golden(native):

@@ -158,13 +158,46 @@ def test_max_steps_counts_iterations(emu_inp):
                                  ("step", 69)]
 
 
-def test_graph_key_flag():
+def test_graph_key_ignores_the_walk():
+    """DDPM and DDIM lookups of one signature hit the same cached text-only graph, which installs the walk it is given on
+    every hit; the inpainting graph has its own key.  Graphs stand in for captured ones in the cache (no GPU needed)."""
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 25)
-    args = (im.unets[0], SHAPE, im.noise_schedulers[0], g["text_embeds"], g["text_mask"], None, None, 3.)
-    plain = im._graph_key(*args, True)
-    assert im._graph_key(*args, True, False) == plain
-    assert im._graph_key(*args, True, True) == plain + ("inpaint",)
+    sch = im.noise_schedulers[0]
+    args = (im.unets[0], SHAPE, sch, g["text_embeds"], g["text_mask"], None, None, 3.)
+    assert im._graph_key(*args, inpaint=True) == im._graph_key(*args) + ("inpaint",)
+
+    class Cached:
+        def __init__(self):
+            self.walks, self.inpaints = [], []
+
+        def set_cond(self, **cond):
+            pass
+
+        def set_schedule(self, sched):
+            self.walks.append(sched)
+
+        def set_inpaint(self, *args):
+            self.inpaints.append(args)
+
+    text, inp = Cached(), Cached()
+    im._graphs = {im._graph_key(*args): text, im._graph_key(*args, inpaint=True): inp}
+    kw = dict(noise_scheduler=sch, text_embeds=g["text_embeds"], text_mask=g["text_mask"], lowres_cond_img=None,
+              lowres_noise_times=None, cond_scale=3.)
+    ddim = sch.sampling_schedule(8, 0.5, "cpu")
+    assert im._step_graph(im.unets[0], SHAPE, **kw) is text
+    assert im._step_graph(im.unets[0], SHAPE, schedule=ddim, **kw) is text
+    assert im._step_graph(im.unets[0], SHAPE, **kw) is text
+    ddpm = sch.ddpm_schedule("cpu")
+    assert len(text.walks) == 3 and all(w is want for w, want in zip(text.walks, (ddpm, ddim, ddpm)))
+    assert not text.inpaints
+    img, mask = known_and_mask(0)
+    k, m = (img * 2 - 1).contiguous(), mask.float().reshape(2, -1)
+    assert im._step_graph(im.unets[0], SHAPE, schedule=ddim, inpaint=(k, m, 3), **kw) is inp
+    _, ra, rb = sch.inpaint_tables(ddim, "cpu")
+    assert len(inp.walks) == 1 and inp.walks[0] is ddim and len(inp.inpaints) == 1
+    assert all(a is b for a, b in zip(inp.inpaints[0], (k, m, 3, ra, rb)))
+    assert len(im._graphs) == 2
 
 
 # ------------------------------------------------------------------------------------------------ argument checks

@@ -68,15 +68,12 @@ def main():
     known = torch.rand(shape, generator=gen, device=dev) * 2 - 1                      # normalised known image
     mask = (torch.rand((B, shape[2] * shape[3]), generator=gen, device=dev) < 0.5).float()
     sched = sch.sampling_schedule(S, args.eta, dev)
-    _, ra, rb = sch.inpaint_tables(sched, dev)
     n_iter = {"inpaint": (S - 1) * R + 1, "respaced": S}
 
     with torch.no_grad():
-        graphs = {"inpaint": im._step_graph(u, shape, noise_scheduler=sch, cond_scale=1.0, inpaint=True, **ckw),
-                  "respaced": im._step_graph(u, shape, noise_scheduler=sch, cond_scale=1.0, respaced=True, **ckw)}
-        for g in graphs.values():
-            g.set_schedule(sched)
-        graphs["inpaint"].set_inpaint(known, mask, R, ra, rb)
+        kw = dict(noise_scheduler=sch, cond_scale=1.0, schedule=sched, **ckw)
+        graphs = {"inpaint": im._step_graph(u, shape, inpaint=(known, mask, R), **kw),
+                  "respaced": im._step_graph(u, shape, **kw)}
 
         def loop(name):
             """One whole loop from x_T at t = T-1; returns ms."""
