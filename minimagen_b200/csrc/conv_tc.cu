@@ -18,11 +18,15 @@
 //   * persistent CTAs (one per SM) walk the tile list round-robin; the producer runs ahead through the operand ring while
 //     the consumers store the previous tile.
 //
-// Warp roles (384 threads): warpgroup 0 = producer (one elected lane issues the TMA loads), warpgroups 1 and 2 = consumers,
-// each owning 64 of the 128 pixel rows: wgmma m64nBLOCK_Nk16 with fp32 accumulators in registers, then
-// +bias +residual -> global fp32 and/or fp16 (+ GroupNorm block statistics) straight from the accumulator fragments.
+// Warp roles (384 threads): warpgroup 0 = producer (one elected lane issues the TMA loads), warpgroups 1 and 2 = consumers:
+// wgmma m64nBLOCK_Nk16 with fp32 accumulators in registers, then +bias +residual -> global fp32 and/or fp16 (+ GroupNorm
+// block statistics) straight from the accumulator fragments.  The consumers share the tiles in one of two schedules:
+//   * cooperative (BLOCK_N = 256, and the fused GroupNorm kernel): both consumers work on every tile, each owning 64 of
+//     the 128 pixel rows.  Their epilogue leaves the tensor cores idle, which long-K tiles amortise;
+//   * ping-pong (TMA kernel, BLOCK_N <= 128): consumer c owns the CTA's tiles c, c + 2, c + 4, ... whole (two wgmma per
+//     k16 step, rows 0-63 and 64-127), so one consumer's epilogue runs under the other's mainloop.
 // In the TMA kernel the producer warpgroup gives its registers to the consumers (setmaxnreg 40 / 232): that is what lets
-// a consumer hold the 128 accumulators of a 256-wide tile.
+// a consumer hold 128 accumulators, of a 256-wide cooperative tile or of a 128-wide ping-pong one.
 //
 // Fused GroupNorm variant (Block.forward, minimagen/layers.py:131-145: GroupNorm -> (scale + 1, shift) -> SiLU -> 3x3 conv):
 // the whole producer warpgroup builds the A tile instead of TMA -- it reads the fp32 NHWC source(s) (optionally the virtual
@@ -54,6 +58,13 @@ constexpr uint32_t kSmemMax = 227 * 1024;
 constexpr int kProducerRegs = 40;
 constexpr int kConsumerRegs = 232;
 static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file overcommitted");
+// ping-pong turn-taking: named barrier kTurnBar + c releases consumer c into its next mainloop (id 1 is the GroupNorm
+// producer's)
+constexpr int kTurnBar = 2;
+// statistics reduction of the ping-pong tiles: named barrier kStatBar + c syncs consumer c's four warps around the scratch
+// that follows the aux block, [2 consumers][4 warps][BLOCK_N / 16 blocks][sum, sum of squares] doubles
+constexpr int kStatBar = 4;
+constexpr uint32_t stat_scratch_bytes(int block_n) { return 2 * 4 * (block_n / 16 > 0 ? block_n / 16 : 1) * 2 * 8; }
 
 template <int BLOCK_N>
 struct Cfg {
@@ -74,13 +85,15 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     using C = Cfg<BLOCK_N>;
     constexpr int STAGES = C::kStages;
     static_assert(2 * STAGES * 8 <= 256, "barrier block overlaps the GroupNorm scratch");
+    constexpr bool PP = !GN && BLOCK_N <= 128;    // ping-pong schedule (else cooperative)
+    constexpr int HALVES = PP ? 2 : 1;            // 64-row halves of a tile one consumer computes
 
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024-byte aligned stage bases
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::kStageBytes);
     uint64_t* full_bar = bars;                    // [STAGES]  producer -> consumers
-    uint64_t* empty_bar = bars + STAGES;          // [STAGES]  consumers -> producer (one arrival per consumer warpgroup)
+    uint64_t* empty_bar = bars + STAGES;          // [STAGES]  consumers -> producer (one arrival per consuming warpgroup)
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -96,7 +109,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int i = 0; i < STAGES; ++i) {
             // GN: the four producer warps' arrivals + the weight load's expect_tx arrival
             ptx::mbar_init(&full_bar[i], GN ? 5 : 1);
-            ptx::mbar_init(&empty_bar[i], 2);
+            ptx::mbar_init(&empty_bar[i], PP ? 1 : 2);
         }
         ptx::fence_barrier_init();
     }
@@ -276,125 +289,179 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             pdl_trigger();
         }
     } else {
-        // ===================== consumers: rows [64 cw, 64 cw + 64) of every tile =====================
+        // ===================== consumers: rows [64 cw, 64 cw + 64) of every tile (cooperative), or every row of the
+        // ===================== CTA's tiles cw, cw + 2, ... (ping-pong)
         if constexpr (!GN) ptx::setmaxnreg_inc<kConsumerRegs>();
         const int cw = wg - 1;
-        const int wq = warp & 3;                        // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
+        const int wq = warp & 3;                        // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of a half
         const int cq = 2 * (lane & 3);                  // first of this thread's two columns in every 8-column group
-        float acc[BLOCK_N / 2];
+        float acc[HALVES][BLOCK_N / 2];
         int stage = 0;
         uint32_t phase = 0;
-        // epilogue geometry of this thread's two rows (m, m + 8) of the tile
-        int m_r[2], bw_r[2], bh_r[2], bb_r[2];
+        // moves the ring position n k-blocks on: in ping-pong, past the other consumer's tile
+        auto skip = [&](int n) {
+            stage += n % STAGES;
+            phase ^= (uint32_t)(n / STAGES) & 1u;
+            if (stage >= STAGES) { stage -= STAGES; phase ^= 1; }
+        };
+        if (PP) skip(cw * num_kb);
+        // epilogue geometry of this thread's rows (m, m + 8) in each of its 64-row halves: row 2 h + r
+        int bw_r[2 * HALVES], bh_r[2 * HALVES], bb_r[2 * HALVES], bb_warp[HALVES];
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            m_r[r] = cw * 64 + wq * 16 + (lane >> 2) + 8 * r;
-            bw_r[r] = m_r[r] & (BW - 1);
-            bh_r[r] = (m_r[r] >> args.bw_log2) & (BH - 1);
-            bb_r[r] = m_r[r] >> (args.bw_log2 + args.bh_log2);
+        for (int h = 0; h < HALVES; ++h) {
+            const int m_warp = (PP ? h : cw) * 64 + wq * 16;   // the warp's 16 rows belong to one image (stats need
+            bb_warp[h] = m_warp >> (args.bw_log2 + args.bh_log2);   // H*W % 32 == 0); the two halves may not
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int m = m_warp + (lane >> 2) + 8 * r;
+                bw_r[2 * h + r] = m & (BW - 1);
+                bh_r[2 * h + r] = (m >> args.bw_log2) & (BH - 1);
+                bb_r[2 * h + r] = m >> (args.bw_log2 + args.bh_log2);
+            }
         }
-        const int m_warp = cw * 64 + wq * 16;           // the warp's 16 rows belong to one image (stats need H*W % 32 == 0)
-        const int bb_warp = m_warp >> (args.bw_log2 + args.bh_log2);
+        // ping-pong, one image per tile: the statistics of a tile's rows are summed over the warpgroup in shared memory.
+        // Cooperative tiles keep per-warp atomics: the two extra warpgroup barriers per tile cost cfg 3 0.3-0.6 ms per
+        // step there (64.1-64.3 vs 63.6-63.8 ms on an H100 SXM at 700 W)
+        constexpr int NQ = BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1;
+        const bool tile_stats = PP && args.stats != nullptr && BB == 1;
+        double* st_red = reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(bars) + kAuxBytes);   // [2][4][NQ][2]
         const bool vec = args.out_sc == 1 && ((reinterpret_cast<uintptr_t>(args.out_f32) & 7) == 0) &&
                          ((reinterpret_cast<uintptr_t>(args.residual) & 7) == 0) &&
                          ((reinterpret_cast<uintptr_t>(args.out_f16) & 3) == 0);
 
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        for (int tile = blockIdx.x + (PP ? cw : 0) * gridDim.x; tile < total_tiles; tile += (PP ? 2 : 1) * gridDim.x) {
             const int nt = tile % args.tiles_n;
             const int mt = tile / args.tiles_n;
             const int n0 = nt * BLOCK_N;
+            // Ping-pong turn: start this tile's mainloop only once the other consumer has waited on every k-block of the
+            // CTA's previous tile.  Every k-block before this tile then has been loaded, so each full_bar this mainloop
+            // waits on is at most one phase behind the one it waits for, and the parity wait cannot succeed on a phase
+            // two fills old (the previous tile's operands): skip() jumps a whole tile of ring slots, so without the turn
+            // a slot's previous fill could still be pending, in the other consumer's tile.  The turns also keep the two
+            // mainloops from sharing the tensor cores; the epilogues overlap the other mainloop.
+            if (PP && tile != (int)blockIdx.x) ptx::bar_sync(kTurnBar + cw, 256);
             int prev = -1;
             for (int kb = 0; kb < num_kb; ++kb) {
                 ptx::mbar_wait(&full_bar[stage], phase, err, 300 + stage);
                 const uint32_t sa = ptx::smem_u32(smem + stage * C::kStageBytes);
-                const uint64_t da = ptx::make_sw128_desc(sa + cw * (64 * 128));
                 const uint64_t db = ptx::make_sw128_desc(sa + kABytes);
                 ptx::wg_fence();
 #pragma unroll
                 for (int k = 0; k < kConvBlockK / 16; ++k)
-                    // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
-                    ptx::Wgmma<BLOCK_N, 0>::run(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+#pragma unroll
+                    for (int h = 0; h < HALVES; ++h) {
+                        const uint64_t da = ptx::make_sw128_desc(sa + (PP ? h : cw) * (64 * 128));
+                        // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
+                        ptx::Wgmma<BLOCK_N, 0>::run(acc[h], da + 2 * k, db + 2 * k, (kb | k) != 0);
+                    }
                 ptx::wg_commit();
                 ptx::wg_wait<1>();                      // the previous k-block's MMAs have retired: free its stage
                 if (prev >= 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[prev]);
                 prev = stage;
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
+            // the other consumer's turn, if the CTA has a next tile (so every arrival meets a bar_sync)
+            if (PP && tile + (int)gridDim.x < total_tiles) ptx::bar_arrive(kTurnBar + (cw ^ 1), 256);
+            if (PP) skip(num_kb);
             ptx::wg_wait<0>();
-            ptx::wg_fence_regs(acc);
+#pragma unroll
+            for (int h = 0; h < HALVES; ++h) ptx::wg_fence_regs(acc[h]);
             if (prev >= 0 && (threadIdx.x & 127) == 0) ptx::mbar_arrive(&empty_bar[prev]);
 
-            // ---- epilogue: fragment element 4j + 2r + e = row m_r[r], column n0 + 8j + cq + e
+            // ---- epilogue: fragment element 4j + 2r + e of half h = row (h, r), column n0 + 8j + cq + e
             const int tw0 = (mt % args.tiles_w) * BW;
             const int th0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
             const int tb0 = (mt / (args.tiles_w * args.tiles_h)) * BB;
-            bool valid[2];
-            long long pix[2];
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const int w = tw0 + bw_r[r], h = th0 + bh_r[r], b = tb0 + bb_r[r];
-                valid[r] = (b < args.B) && (h < args.H) && (w < args.W);
-                pix[r] = (long long)b * args.out_sb + (long long)h * args.out_sh + (long long)w * args.out_sw;
-            }
             const bool fast = vec && n0 + BLOCK_N <= args.n_valid;
-            float st_s[BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1], st_q[BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1];
 #pragma unroll
-            for (int q = 0; q < BLOCK_N / 16; ++q) { st_s[q] = 0.f; st_q[q] = 0.f; }
+            for (int hf = 0; hf < HALVES; ++hf) {
+                bool valid[2];
+                long long pix[2];
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) {
-                const int n = n0 + 8 * j + cq;
-                if (fast) {
-                    float2 bv = make_float2(0.f, 0.f);
-                    if (args.bias) bv = __ldg(reinterpret_cast<const float2*>(args.bias + n));
+                for (int r = 0; r < 2; ++r) {
+                    const int w = tw0 + bw_r[2 * hf + r], h = th0 + bh_r[2 * hf + r], b = tb0 + bb_r[2 * hf + r];
+                    valid[r] = (b < args.B) && (h < args.H) && (w < args.W);
+                    pix[r] = (long long)b * args.out_sb + (long long)h * args.out_sh + (long long)w * args.out_sw;
+                }
+                const float* a = acc[hf];
+                float st_s[BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1], st_q[BLOCK_N / 16 > 0 ? BLOCK_N / 16 : 1];
 #pragma unroll
-                    for (int r = 0; r < 2; ++r) {
-                        if (!valid[r]) continue;
-                        const long long o = pix[r] + n;
-                        float2 f = make_float2(acc[4 * j + 2 * r] + bv.x, acc[4 * j + 2 * r + 1] + bv.y);
-                        if (args.residual) {
-                            const float2 rv = *reinterpret_cast<const float2*>(args.residual + o);
-                            f.x += rv.x; f.y += rv.y;
+                for (int q = 0; q < BLOCK_N / 16; ++q) { st_s[q] = 0.f; st_q[q] = 0.f; }
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    const int n = n0 + 8 * j + cq;
+                    if (fast) {
+                        float2 bv = make_float2(0.f, 0.f);
+                        if (args.bias) bv = __ldg(reinterpret_cast<const float2*>(args.bias + n));
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            if (!valid[r]) continue;
+                            const long long o = pix[r] + n;
+                            float2 f = make_float2(a[4 * j + 2 * r] + bv.x, a[4 * j + 2 * r + 1] + bv.y);
+                            if (args.residual) {
+                                const float2 rv = *reinterpret_cast<const float2*>(args.residual + o);
+                                f.x += rv.x; f.y += rv.y;
+                            }
+                            st_s[j >> 1] += f.x + f.y;
+                            st_q[j >> 1] += f.x * f.x + f.y * f.y;
+                            if (args.out_f32) *reinterpret_cast<float2*>(args.out_f32 + o) = f;
+                            if (args.out_f16) *reinterpret_cast<__half2*>(args.out_f16 + o) = sat_half2(f.x, f.y);
                         }
-                        st_s[j >> 1] += f.x + f.y;
-                        st_q[j >> 1] += f.x * f.x + f.y * f.y;
-                        if (args.out_f32) *reinterpret_cast<float2*>(args.out_f32 + o) = f;
-                        if (args.out_f16) *reinterpret_cast<__half2*>(args.out_f16 + o) = sat_half2(f.x, f.y);
+                    } else {
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                if (!valid[r] || n + e >= args.n_valid) continue;
+                                float f = a[4 * j + 2 * r + e] + (args.bias ? __ldg(args.bias + n + e) : 0.f);
+                                const long long o = pix[r] + (long long)(n + e) * args.out_sc;
+                                if (args.residual && args.out_sc == 1) f += args.residual[o];
+                                st_s[j >> 1] += f;
+                                st_q[j >> 1] += f * f;
+                                if (args.out_f32) args.out_f32[o] = f;
+                                if (args.out_f16) args.out_f16[o] = sat_half(f);
+                            }
+                        }
                     }
-                } else {
+                }
+                if (args.stats) {
+                    // GroupNorm statistics of the tensor being written, per (image, 16-channel block): the warp's 16 rows
+                    // x 16 columns of each block reduce over all 32 lanes
+                    const int b_img = tb0 + bb_warp[hf];
+                    const bool any = __any_sync(0xffffffffu, valid[0] || valid[1]);
 #pragma unroll
-                    for (int r = 0; r < 2; ++r) {
+                    for (int q = 0; q < BLOCK_N / 16; ++q) {
 #pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            if (!valid[r] || n + e >= args.n_valid) continue;
-                            float f = acc[4 * j + 2 * r + e] + (args.bias ? __ldg(args.bias + n + e) : 0.f);
-                            const long long o = pix[r] + (long long)(n + e) * args.out_sc;
-                            if (args.residual && args.out_sc == 1) f += args.residual[o];
-                            st_s[j >> 1] += f;
-                            st_q[j >> 1] += f * f;
-                            if (args.out_f32) args.out_f32[o] = f;
-                            if (args.out_f16) args.out_f16[o] = sat_half(f);
+                        for (int o = 1; o <= 16; o <<= 1) {
+                            st_s[q] += __shfl_xor_sync(0xffffffffu, st_s[q], o);
+                            st_q[q] += __shfl_xor_sync(0xffffffffu, st_q[q], o);
+                        }
+                        if (lane == 0 && tile_stats) {
+                            double* r = st_red + ((cw * 4 + wq) * NQ + q) * 2;
+                            r[0] = (hf == 0 ? 0.0 : r[0]) + (double)st_s[q];
+                            r[1] = (hf == 0 ? 0.0 : r[1]) + (double)st_q[q];
+                        } else if (lane == 0 && any) {
+                            double* dst = args.stats + ((long long)b_img * args.stats_blocks + (n0 >> 4) + q) * 2;
+                            atomicAdd(dst, (double)st_s[q]);
+                            atomicAdd(dst + 1, (double)st_q[q]);
                         }
                     }
                 }
             }
-            if (args.stats) {
-                // GroupNorm statistics of the tensor being written, per (image, 16-channel block): the warp's 16 rows x 16
-                // columns of each block reduce over all 32 lanes
-                const int b_img = tb0 + bb_warp;
-                const bool any = __any_sync(0xffffffffu, valid[0] || valid[1]);
+            if (tile_stats) {
+                // one atomic pair per (consumer warpgroup, tile, 16-channel block) instead of one per warp and half: every
+                // CTA works on the same image at once, and the per-warp atomics queued on its few addresses
+                ptx::bar_sync(kStatBar + cw, 128);
+                if (wq == 0 && lane < NQ) {
+                    const double* r = st_red + (cw * 4 * NQ + lane) * 2;
+                    double s = r[0], sq = r[1];
 #pragma unroll
-                for (int q = 0; q < BLOCK_N / 16; ++q) {
-#pragma unroll
-                    for (int o = 1; o <= 16; o <<= 1) {
-                        st_s[q] += __shfl_xor_sync(0xffffffffu, st_s[q], o);
-                        st_q[q] += __shfl_xor_sync(0xffffffffu, st_q[q], o);
-                    }
-                    if (lane == 0 && any) {
-                        double* dst = args.stats + ((long long)b_img * args.stats_blocks + (n0 >> 4) + q) * 2;
-                        atomicAdd(dst, (double)st_s[q]);
-                        atomicAdd(dst + 1, (double)st_q[q]);
-                    }
+                    for (int w = 1; w < 4; ++w) { s += r[w * NQ * 2]; sq += r[w * NQ * 2 + 1]; }
+                    double* dst = args.stats + ((long long)tb0 * args.stats_blocks + (n0 >> 4) + lane) * 2;
+                    atomicAdd(dst, s);
+                    atomicAdd(dst + 1, sq);
                 }
+                ptx::bar_sync(kStatBar + cw, 128);     // the scratch is read before the next tile writes it
             }
         }
     }
@@ -453,6 +520,9 @@ void tile_geometry(int H, int W, int B, ConvTcArgs& a) {
 // Largest BLOCK_N of {256,128,64,32,16} dividing C_out that still gives every SM a tile; never shrink below 64 for that.
 // A 256-wide tile moves 25 % fewer operand bytes per FLOP than a 128-wide one; its 128 accumulators per consumer thread
 // fit because of the setmaxnreg split (only the TMA kernel has it: the fused GroupNorm kernel stays 128 wide).
+// The width also picks the schedule: 256 is cooperative, <= 128 ping-pong.  Taking the 128-wide ping-pong tile for
+// C_out % 256 == 0 at <= 36 k-blocks per tile won 0-7 % per launch at 3x3 -> 256 on 64x64 (tools/bench_ops.py conv, b = 32,
+// H100 SXM at a 400 W power limit) but lost 0.2-0.3 ms per cfg-3 step (85.7-85.9 vs 85.4-85.7 ms), so it is not used.
 int pick_block_n(int Cout, int tiles_m, int hint, int num_sms) {
     const int cands[5] = {256, 128, 64, 32, 16};
     if (hint < 0) hint = -hint;
@@ -510,8 +580,8 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& t
     const int total_tiles = args.tiles_w * args.tiles_h * args.tiles_b * args.tiles_n;
     const int num_sms = num_sms_of_current_device();
     const int grid = total_tiles < num_sms ? total_tiles : num_sms;
-    launch_k(conv_wg_kernel<BLOCK_N, GN>, grid, kNumThreads, C::kSmemBytes + extra_smem, stream, tmA, tmA2, tmB, tmX, tmX2,
-             args, gn);
+    const uint32_t smem = C::kSmemBytes + (!GN && BLOCK_N <= 128 ? stat_scratch_bytes(BLOCK_N) : 0u) + extra_smem;
+    launch_k(conv_wg_kernel<BLOCK_N, GN>, grid, kNumThreads, smem, stream, tmA, tmA2, tmB, tmX, tmX2, args, gn);
     return cudaGetLastError() == cudaSuccess ? 0 : -11;
 }
 

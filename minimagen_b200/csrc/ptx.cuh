@@ -123,6 +123,10 @@ __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t
 __device__ __forceinline__ void bar_sync(int id, int count) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// counts this warp's threads towards named barrier `id` without waiting for it (the producer side of bar_sync)
+__device__ __forceinline__ void bar_arrive(int id, int count) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // Per-warpgroup register budget (all four warps of the warpgroup execute it): a warpgroup that needs few registers
 // releases them with dec, one that needs more claims them with inc (which waits until the registers are free).

@@ -3,7 +3,8 @@
 Diagnostics for kernel tuning, not a bench value: CUDA events around `reps` back-to-back launches, rotating over enough
 buffer sets that the working set exceeds the 50 MB L2 ("cold") or re-using one set ("warm").
 Usage: python tools/bench_ops.py [gn ln linear quantile attn cast final stem]
-       python tools/bench_ops.py conv [block_n ...]   (implicit-GEMM convs; block_n 0 = the library's choice)
+       python tools/bench_ops.py conv [block_n ...]   (implicit-GEMM convs; block_n 0 = the library's choice; ends with
+                                                       the k-block sweep and its per-tile cost fit)
 """
 import os
 import sys
@@ -190,6 +191,11 @@ def conv_auto_block_n(c_out, tiles_m, num_sms):
     return 64
 
 
+# k-block sweep: 3x3 convs at b=32 whose k-blocks per tile (9 C_in / 64) run from 9 to 72, at the two cfg-3 geometries
+# of the short-K layers; per-tile time against k-blocks fits a line whose intercept is the cost paid once per tile
+SWEEP_SHAPES = [(128, 128, (64, 128, 256, 512)), (64, 256, (64, 128, 256, 512))]   # (H = W, C_out, C_in sweep)
+
+
 def conv_operand_bytes(tiles_m, c_out, k_blocks, block_n):
     """L2 -> SM operand bytes of one launch: per tile and k-block one TMA stage, a 128x64 A box and a block_n x 64 B box."""
     return tiles_m * (c_out // block_n) * k_blocks * (128 * 64 * 2 + block_n * 64 * 2)
@@ -233,6 +239,46 @@ def bench_conv(ops, hints=(0,)):
             nbytes = conv_operand_bytes(tiles_m, c_out, k_blocks, bn)
             res_line.append(f"n{bn:<3d} {ms * 1e3:8.1f} us {flop / ms / 1e9:6.1f} TFLOP/s L2->SM {nbytes / ms / 1e9:5.2f} TB/s")
         print(f"conv {lbl:40s} " + "  |  ".join(res_line), flush=True)
+    bench_conv_sweep(ops, hints, num_sms)
+
+
+def bench_conv_sweep(ops, hints, num_sms):
+    """Per-tile cost against k-blocks per tile, with the fp16 + statistics epilogue most convs write ("f16") and with what
+    ResnetBlock.block2 writes ("block2": bias, fp32 residual in, fp32 + fp16 out, statistics).  us/tile is the launch time
+    over its tiles per SM; the fit per (shape, epilogue, width) is  us/tile = F + c * k-blocks."""
+    import numpy as np
+    B = 32
+    for (H, c_out, c_ins) in SWEEP_SHAPES:
+        tiles_m = B * H * H // 128
+        for epi in ("f16", "block2"):
+            pts = {}
+            for c_in in c_ins:
+                act = torch.randn(B, H, H, c_in, device=dev).to(F16)
+                wp = (torch.randn(c_out, 9 * c_in, device=dev) * 0.01).to(F16)
+                bias = torch.randn(c_out, device=dev)
+                out16 = torch.empty(B, H, H, c_out, device=dev, dtype=F16)
+                stats = torch.zeros(B, c_out // 16, 2, device=dev, dtype=F64)
+                res = torch.randn(B, H, H, c_out, device=dev) if epi == "block2" else None
+                out32 = torch.empty(B, H, H, c_out, device=dev) if epi == "block2" else None
+                k_blocks = 9 * c_in // 64
+                line = []
+                for hint in hints:
+                    bn = hint if hint and c_out % hint == 0 else conv_auto_block_n(c_out, tiles_m, num_sms)
+                    f = lambda hint=hint: ops.conv_igemm(act, B, H, H, c_in, 0, c_in, wp, c_out, 3, 3, 0, bias, res, out32,
+                                                         out16, (H * H * c_out, H * c_out, c_out), block_n=hint,
+                                                         out_stats=stats)
+                    ms = timeit([f], reps=20)
+                    per_tile = ms * 1e3 / (tiles_m * (c_out // bn) / num_sms)
+                    pts.setdefault((hint, bn), []).append((k_blocks, per_tile))
+                    line.append(f"n{bn:<3d} {ms * 1e3:8.1f} us {per_tile:6.2f} us/tile "
+                                f"{2.0 * B * H * H * c_out * 9 * c_in / ms / 1e9:6.1f} TFLOP/s")
+                print(f"conv sweep 3x3 {c_in:4d}->{c_out} @{H} {epi:6s} kb={k_blocks:3d} " + "  |  ".join(line), flush=True)
+            for (hint, bn), p in sorted(pts.items()):
+                kb, us = np.array(p).T
+                c, F = np.polyfit(kb, us, 1)
+                print(f"conv sweep fit C_out={c_out} @{H} {epi:6s} n{bn:<3d}{'' if hint else ' (auto)'}: F = {F:5.2f} us/tile, "
+                      f"{c:5.3f} us per k-block",
+                      flush=True)
 
 
 def main():
