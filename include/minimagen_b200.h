@@ -245,6 +245,18 @@ int mi_step_epilogue(const float* x_t, const float* eps_cond, const float* eps_n
                      const float* posterior_mean_coef1, const float* posterior_mean_coef2, const float* sigma,
                      const float* noise, int B, int n, int rank_lo, int rank_hi, float weight, float min_s, float* out,
                      float* s_out, float* x0_workspace, void* stream);
+/* The multistep form of mi_step_epilogue (DPM-Solver++(2M), Imagen.sample(..., sampler='dpmpp_2m')): with xs the clamped
+ * and divided x0 and h = x0_hist [B][n] (the previous step's xs), per element
+ *   out = ((c1[t] * xs + c2[t] * x_t) + c3[t] * h) + sigma[t] * noise       rounded op by op (no fused multiply-add),
+ * where the c3[t] * h term is skipped (not multiplied) for images with c3[t] == 0, so a stale or NaN history cannot leak
+ * into a first-order step, and an all-zero c3 gives mi_step_epilogue's bits.  Then xs is written to x0_hist in place.
+ * `out` may be `x_t`; x0_hist must not alias any other argument.  Same workspace rule as mi_step_epilogue. */
+int mi_step_epilogue_multistep(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                               const long long* t, const float* sqrt_recip_alphas_cumprod,
+                               const float* sqrt_recipm1_alphas_cumprod, const float* c1, const float* c2,
+                               const float* sigma, const float* c3, const float* noise, float* x0_hist, int B, int n,
+                               int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
+                               float* x0_workspace, void* stream);
 /* t[b] <- max(t[b] - 1, 0): the next iteration's timestep of Imagen._p_sample_loop (Imagen.py:398-415 walks the list of
  * diffusion_model.py:81-87), advanced on the device so that a captured step can be replayed back to back */
 int mi_step_advance_t(long long* t, int B, void* stream);

@@ -5,10 +5,10 @@ Same class surface as the reference's `Imagen` (constructor `Imagen.py:27-42`, `
 asserts and messages.  The reverse-diffusion step is executed by the fused step kernels (csrc/step.cu): CFG combine,
 x0 prediction, EXACT per-image dynamic-threshold quantile (radix select), posterior mean and noise add; the whole step
 (both U-Net passes + epilogue) is optionally replayed from a CUDA graph so the ~10^3 kernel launches per step cost
-nothing on the host.  Sampling captures two graph flavours: text-only (one graph serves the DDPM walk and every DDIM
-step count and eta) and inpainting.
+nothing on the host.  Sampling captures three graph flavours: text-only (one graph serves the DDPM walk and every DDIM
+step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).
 
-Four additions that the reference does not have (all optional, defaults reproduce the reference):
+Five additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -17,12 +17,16 @@ Four additions that the reference does not have (all optional, defaults reproduc
     the same step kernels, with per-loop coefficient tables (GaussianDiffusion.sampling_schedule);
   * inpainting with RePaint resampling (`sample(..., inpaint_images=, inpaint_masks=, inpaint_resample_times=R)`): at every
     grid point t > 0 the step runs R times.  Each run after the first starts by re-noising x from the next grid point
-    back to t; then every run pastes in the known region, noised to t (Lugmayr et al. 2022, jump length 1).
+    back to t; then every run pastes in the known region, noised to t (Lugmayr et al. 2022, jump length 1);
+  * DPM-Solver++(2M) sampling (`sample(..., sampling_timesteps=S, sampler='dpmpp_2m')`, Lu et al. 2022): a second-order
+    multistep solver on the thresholded x0 over S points uniform in log-SNR.  Its step is DDIM's table form plus the
+    previous step's clamped x0 times a third table c3 (mi_step_epilogue_multistep), still one U-Net evaluation per point.
 
 `noise_fn` kinds: 'init' (x_T, step -1), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
 augmentation noise, labelled with the U-Net number).  Inpainting labels the draws of iteration r at grid point t with
 t * R + r (at R = 1 that is t) and takes them in this order: 'renoise' (the re-noising draw, r > 0 only), 'inpaint' (the
-noise of the pasted known region), 'step'.
+noise of the pasted known region), 'step'.  DPM-Solver++(2M) takes the 'step' draws of DDIM with eta = 0 (one per grid
+point, multiplied by a zero sigma).
 """
 from contextlib import contextmanager
 from typing import Callable, List, Literal, Tuple, Union
@@ -64,8 +68,10 @@ class _StepGraph:
          inp    inpainting graphs only: static k [B, C, s, s] (normalised known image), m [B, s*s] (mask, known where
                 >= 0.5), the RePaint counter r [B] and its limit R [1] (int64), the re-noising tables ra / rb [T] and the
                 draws z_renoise / z_known (`set_inpaint` refreshes them, so one graph serves any mask, image and R).
-    Two flavours: text-only (the step, then mi_step_advance_t_table) and inpainting (draws, mi_inpaint_prologue, the step,
-    mi_inpaint_advance).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
+         hist   multistep graphs only: [B, C, s, s], the previous step's clamped x0 (zeroed at the start of every loop); the
+                sched copy then also has c3 [T].
+    Three flavours: text-only (the step, then mi_step_advance_t_table), inpainting (draws, mi_inpaint_prologue, the step,
+    mi_inpaint_advance) and multistep (the draw, mi_step_epilogue_multistep's step, mi_step_advance_t_table).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
     for DDPM; `* ((S-1) R + 1)` when inpainting) -- no per-step host-side tensor ops."""
 
     def __init__(self):
@@ -73,12 +79,13 @@ class _StepGraph:
         self.x = self.t = self.noise = None
         self.cond = {}
         self.sched = None
+        self.hist = None
         self.inp = None
         self.inject_noise = False
         self.unet = None
 
     def set_schedule(self, sched):
-        for name in ('c1', 'c2', 'sigma', 'next_t'):
+        for name in ('c1', 'c2', 'sigma', 'next_t') + (('c3',) if self.sched.c3 is not None else ()):
             getattr(self.sched, name).copy_(getattr(sched, name))
 
     def set_inpaint(self, k, m, R, ra, rb):
@@ -254,18 +261,20 @@ class Imagen(nn.Module):
                 noise_scheduler.posterior_log_variance_clipped.gather(-1, t).reshape(shp))
 
     def _step(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-              cond_scale, model_output=None, out=None, schedule=None):
+              cond_scale, model_output=None, out=None, schedule=None, hist=None):
         """x_{t-1} = posterior_mean(x_t, clamp-thresholded x0(x_t, eps)) + [t != 0] * sigma_t * noise.
         `out` may be `x` itself (the captured step updates the image in place).  `schedule` (a SamplingSchedule) replaces
-        the posterior coefficients and sigma by its DDIM tables: the step then goes to the next point of its grid."""
+        the posterior coefficients and sigma by its DDIM tables: the step then goes to the next point of its grid.  A
+        multistep schedule (one with c3, DPM-Solver++(2M)) also adds c3[t] * hist, the previous step's clamped x0, and then
+        stores this step's clamped x0 in `hist` ([B, C, s, s] fp32, zeros before the first step)."""
         with N.device_of(x):
             return self._step_impl(unet, x, t, noise, noise_scheduler=noise_scheduler, text_embeds=text_embeds,
                                    text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                                    lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
-                                   model_output=model_output, out=out, schedule=schedule)
+                                   model_output=model_output, out=out, schedule=schedule, hist=hist)
 
     def _step_impl(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                   lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None):
+                   lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None, hist=None):
         assert not (cond_scale != 1. and not self.can_classifier_guidance), \
             'imagen was not trained with conditional dropout, and thus one cannot use classifier free guidance ' \
             '(cond_scale anything other than 1)'
@@ -298,8 +307,14 @@ class Imagen(nn.Module):
         # (mi_step_epilogue; images too large for its register-resident select take the three-kernel form inside the ABI)
         c1, c2, sigma = ((sch.posterior_mean_coef1, sch.posterior_mean_coef2, sch.sigma) if schedule is None else
                          (schedule.c1, schedule.c2, schedule.sigma))
-        ops.step_epilogue(x, eps, eps_null, cond_scale, t, sch.sqrt_recip_alphas_cumprod, sch.sqrt_recipm1_alphas_cumprod,
-                          c1, c2, sigma, noise, B, n, lo, hi, w, 1.0, out)
+        if exists(schedule) and exists(schedule.c3):
+            assert exists(hist), 'a multistep schedule needs the x0 history (hist=)'
+            ops.step_epilogue_multistep(x, eps, eps_null, cond_scale, t, sch.sqrt_recip_alphas_cumprod,
+                                        sch.sqrt_recipm1_alphas_cumprod, c1, c2, sigma, schedule.c3, noise, hist, B, n,
+                                        lo, hi, w, 1.0, out)
+        else:
+            ops.step_epilogue(x, eps, eps_null, cond_scale, t, sch.sqrt_recip_alphas_cumprod,
+                              sch.sqrt_recipm1_alphas_cumprod, c1, c2, sigma, noise, B, n, lo, hi, w, 1.0, out)
         return out
 
     @torch.no_grad()
@@ -314,14 +329,16 @@ class Imagen(nn.Module):
 
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-                   cond_scale, inpaint=False):
+                   cond_scale, inpaint=False, multistep=False):
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         p0 = next(unet.parameters())
         key = (id(unet), tuple(shape), float(cond_scale), bool(self.cfg_batched), exists(self.noise_fn),
                noise_scheduler.num_timesteps, sig(text_embeds), sig(text_mask), sig(lowres_cond_img),
                sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
                self.dynamic_thresholding_percentile)
-        return key + ('inpaint',) if inpaint else key
+        if inpaint:
+            return key + ('inpaint',)
+        return key + ('multistep',) if multistep else key
 
     def clear_graphs(self):
         """Drop the captured step graphs (and the activation memory their pools hold)."""
@@ -339,11 +356,15 @@ class Imagen(nn.Module):
         signature.
         `inpaint` ((k, m, R) as in `_p_sample_loop`): the inpainting flavour -- one RePaint iteration, draws,
         mi_inpaint_prologue, the step, mi_inpaint_advance -- with k, m, R and the walk's re-noising tables installed by
-        `_StepGraph.set_inpaint`; neither the mask, the image nor R is part of the signature."""
+        `_StepGraph.set_inpaint`; neither the mask, the image nor R is part of the signature.
+        A multistep `schedule` (with c3) selects the multistep flavour, keyed apart from the other two: static c1 / c2 / c3 /
+        sigma / next_t tables and the x0 history `hist`, stepped by mi_step_epilogue_multistep."""
         device = self.device
         schedule = default(schedule, lambda: noise_scheduler.ddpm_schedule(device))
+        multistep = exists(schedule.c3)
+        assert not (multistep and exists(inpaint)), 'a multistep schedule cannot be combined with inpainting'
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                              lowres_noise_times, cond_scale, exists(inpaint))
+                              lowres_noise_times, cond_scale, exists(inpaint), multistep)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times)
         g = self._graphs.get(key)
@@ -368,7 +389,10 @@ class Imagen(nn.Module):
             ddpm = noise_scheduler.ddpm_schedule(device)
             # static copies (the grid stays with the caller); set_schedule installs the requested walk below
             g.sched = ddpm._replace(grid=(), c1=ddpm.c1.clone(), c2=ddpm.c2.clone(), sigma=ddpm.sigma.clone(),
-                                    next_t=ddpm.next_t.clone())
+                                    next_t=ddpm.next_t.clone(),
+                                    c3=torch.zeros((T,), dtype=F32, device=device) if multistep else None)
+            if multistep:
+                g.hist = torch.zeros(shape, dtype=F32, device=device)     # the previous step's clamped x0
             p = None
             if exists(inpaint):
                 # placeholder contents (nothing known, R = 1); set_inpaint installs the caller's below
@@ -391,7 +415,7 @@ class Imagen(nn.Module):
                     ops.inpaint_prologue(g.x, g.t, p['r'], p['ra'], p['rb'], noise_scheduler.sqrt_alphas_cumprod,
                                          noise_scheduler.sqrt_one_minus_alphas_cumprod, p['k'], p['m'], p['z_renoise'],
                                          p['z_known'], T, B, C, hw)
-                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, **kw)
+                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, hist=g.hist, **kw)
                 if exists(p):
                     ops.inpaint_advance(g.t, p['r'], g.sched.next_t, p['R'], T, B)   # next repeat, or next grid point
                 else:
@@ -431,7 +455,10 @@ class Imagen(nn.Module):
                     x <- where(m, sqrt(a_t) k + sqrt(1 - a_t) z_known, x)          (the known region, noised to t)
                     x <- step(x, t)                                                (DDPM or DDIM, to t')
         i.e. (S - 1) R + 1 U-Net evaluations for S grid points.  Without `inpaint` an iteration is the step alone (R = 1).
-        `max_steps` counts iterations.  The draws of each iteration are those of the module docstring."""
+        `max_steps` counts iterations.  The draws of each iteration are those of the module docstring.
+        A multistep `schedule` (from `noise_scheduler.dpm_solver_schedule`, DPM-Solver++(2M)) carries the previous step's
+        clamped x0 from step to step in a history buffer, zeroed at the start of the loop; it cannot be combined with
+        `inpaint` (RePaint's re-noising would break the history)."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -440,6 +467,8 @@ class Imagen(nn.Module):
                 lowres_cond_img = lowres_cond_img.to(F32).contiguous()
             sch = noise_scheduler
             walk = default(schedule, lambda: sch.ddpm_schedule(device))
+            multistep = exists(walk.c3)
+            assert not (multistep and exists(inpaint)), 'a multistep schedule cannot be combined with inpainting'
             k, m, R = default(inpaint, (None, None, 1))
             plan = [(t, r) for t in walk.grid for r in range(R if t > 0 else 1)]
             if exists(max_steps):
@@ -460,6 +489,8 @@ class Imagen(nn.Module):
                 if exists(inpaint):
                     static.update(renoise=g.inp['z_renoise'], inpaint=g.inp['z_known'])
                     g.inp['r'].zero_()
+                if multistep:
+                    g.hist.zero_()
                 g.x.copy_(img)
                 g.t.fill_(plan[0][0])
                 for iteration in draws:
@@ -472,6 +503,7 @@ class Imagen(nn.Module):
                 if exists(inpaint):
                     _, ra, rb = sch.inpaint_tables(walk, device)
                     img = img.clone()           # the prologue works in place; x_T may be the caller's draw
+                hist = torch.zeros(tuple(shape), dtype=F32, device=device) if multistep else None
                 for (t, r), iteration in zip(plan, draws):
                     z = {kind: self._noise(kind, shape, label, device) for kind, label in iteration}
                     times = torch.full((B,), t, device=device, dtype=torch.long)
@@ -481,7 +513,7 @@ class Imagen(nn.Module):
                         ops.inpaint_prologue(img, times, reps, ra, rb, sch.sqrt_alphas_cumprod,
                                              sch.sqrt_one_minus_alphas_cumprod, k, m, z.get('renoise', z['inpaint']),
                                              z['inpaint'], sch.num_timesteps, B, C, hw)
-                    img = self._step(unet, img, times, z['step'], schedule=walk, **kw)
+                    img = self._step(unet, img, times, z['step'], schedule=walk, hist=hist, **kw)
 
             if out is None:
                 out = torch.empty(tuple(shape), dtype=F32, device=device)
@@ -496,7 +528,7 @@ class Imagen(nn.Module):
     def sample(self, texts: List[str] = None, text_masks=None, text_embeds=None, cond_scale: float = 1.,
                lowres_sample_noise_level: float = None, return_pil_images: bool = False, device=None,
                distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0., inpaint_images=None,
-               inpaint_masks=None, inpaint_resample_times: int = 5):
+               inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim'):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -509,8 +541,18 @@ class Imagen(nn.Module):
         together (b: the full batch of the text conditioning), inpaint: True marks a pixel kept from `inpaint_images`,
         False one the model generates.  Every stage resizes both to its size (known where the resized mask >= 0.5) and
         runs RePaint with `inpaint_resample_times` (an int R >= 1) iterations per grid point t > 0, on the DDPM or the
-        DDIM walk, and pastes the known pixels into its output (module docstring)."""
+        DDIM walk, and pastes the known pixels into its output (module docstring).
+        `sampler` picks the walk of the stages with a `sampling_timesteps` entry: 'ddim' (the default, above) or
+        'dpmpp_2m', DPM-Solver++(2M) over S points uniform in log-SNR (GaussianDiffusion.dpm_solver_schedule): a
+        deterministic second-order multistep solver of the probability-flow ODE, still S U-Net evaluations (2S with
+        unbatched guidance), that needs sampling_timesteps, ddim_eta = 0 and no inpainting.  Stages whose entry is None
+        keep the DDPM loop."""
+        assert sampler in ('ddim', 'dpmpp_2m'), f"sampler must be 'ddim' or 'dpmpp_2m', got {sampler!r}"
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
+        if sampler == 'dpmpp_2m':
+            assert any(s is not None for s in steps), "sampler='dpmpp_2m' needs sampling_timesteps"
+            assert ddim_eta == 0., f"sampler='dpmpp_2m' is deterministic: ddim_eta must be 0, got {ddim_eta}"
+            assert not exists(inpaint_images), "sampler='dpmpp_2m' cannot be combined with inpainting"
         assert exists(inpaint_images) == exists(inpaint_masks), \
             'inpaint_images and inpaint_masks must be given together'
         assert isinstance(inpaint_resample_times, int) and not isinstance(inpaint_resample_times, bool) \
@@ -523,7 +565,7 @@ class Imagen(nn.Module):
         inpaint = (inpaint_images, inpaint_masks, inpaint_resample_times) if exists(inpaint_images) else None
         with N.device_of(self._temp):
             return self._sample_impl(texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level,
-                                     return_pil_images, device, distributed, steps, ddim_eta, inpaint)
+                                     return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler)
 
     def _sampling_steps(self, sampling_timesteps, ddim_eta):
         """Per-U-Net step counts (None = the DDPM loop), validated."""
@@ -542,7 +584,7 @@ class Imagen(nn.Module):
         return steps
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
-                     device, distributed, steps=None, ddim_eta=0., inpaint=None):
+                     device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim'):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -615,7 +657,10 @@ class Imagen(nn.Module):
                     # the last stage finalises straight into this rank's slot of the all-gather buffer (no staging copy)
                     gathered = torch.empty((world * batch_size, *shape[1:]), dtype=F32, device=device)
                     slot = gathered[rank * batch_size:(rank + 1) * batch_size]
-                schedule = None if n_steps is None else noise_scheduler.sampling_schedule(n_steps, ddim_eta, device)
+                schedule = None
+                if n_steps is not None:
+                    schedule = (noise_scheduler.dpm_solver_schedule(n_steps, device) if sampler == 'dpmpp_2m' else
+                                noise_scheduler.sampling_schedule(n_steps, ddim_eta, device))
                 stage_inpaint = None
                 if exists(inpaint):
                     # this stage's known image (normalised) and mask; unchanged when already at the stage's size

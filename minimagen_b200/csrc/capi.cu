@@ -290,6 +290,16 @@ int mi_step_epilogue(const float* x_t, const float* eps_cond, const float* eps_n
                                    rank_hi, weight, min_s, out, s_out, x0_workspace, S(stream)),
                  "mi_step_epilogue");
 }
+int mi_step_epilogue_multistep(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                               const long long* t, const float* tab_a, const float* tab_b, const float* c1,
+                               const float* c2, const float* sigma, const float* c3, const float* noise, float* x0_hist,
+                               int B, int n, int rank_lo, int rank_hi, float weight, float min_s, float* out,
+                               float* s_out, float* x0_workspace, void* stream) {
+    return check(mi::step_epilogue_multistep(x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, c3,
+                                             noise, x0_hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out,
+                                             x0_workspace, S(stream)),
+                 "mi_step_epilogue_multistep");
+}
 int mi_step_advance_t(long long* t, int B, void* stream) {
     return check(mi::step_advance_t(t, B, S(stream)), "mi_step_advance_t");
 }

@@ -241,11 +241,15 @@ quantile_cluster_kernel(const float* __restrict__ x0, int n, int rank_lo, int ra
     }
 }
 
+// kHist (the multistep form, mi_step_epilogue_multistep): mean += c3[t] * x0_hist, skipped where c3[t] == 0, then the
+// clamped x0 replaces x0_hist.  The extra arguments come last so that the kHist = false instance is the plain kernel.
+template <bool kHist>
 __global__ void __launch_bounds__(256)
 posterior_kernel(const float* __restrict__ x0, const float* x_t, const float* __restrict__ noise,
                  const float* __restrict__ s, const long long* __restrict__ t, const float* __restrict__ tab_c1,
                  const float* __restrict__ tab_c2, const float* __restrict__ tab_sigma, int n_per_img,
-                 float* out) {   // out may alias x_t (same index read before written by the same thread)
+                 float* out,     // out may alias x_t (same index read before written by the same thread)
+                 const float* __restrict__ tab_c3, float* __restrict__ x0_hist) {
     pdl_wait();
     pdl_trigger();
     const int b = blockIdx.y;
@@ -259,7 +263,12 @@ posterior_kernel(const float* __restrict__ x0, const float* x_t, const float* __
     float xs = x0[idx];
     xs = fminf(fmaxf(xs, -sb), sb);
     xs = __fdiv_rn(xs, sb);
-    const float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[idx]));
+    float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[idx]));
+    if constexpr (kHist) {
+        const float c3 = tab_c3[tb];
+        if (c3 != 0.f) mean = __fadd_rn(mean, __fmul_rn(c3, x0_hist[idx]));
+        x0_hist[idx] = xs;
+    }
     out[idx] = __fadd_rn(mean, __fmul_rn(sig, noise[idx]));
 }
 
@@ -274,13 +283,16 @@ posterior_kernel(const float* __restrict__ x0, const float* x_t, const float* __
 // Versus the three-kernel form the x0 tensor never exists in memory (one write + two reads of the image less) and two
 // launches disappear from the step.  `out` may alias `x_t` (in-place update of the sampling state): every element is
 // read and written by the same thread.  Arithmetic is op-for-op that of x0_kernel / posterior_kernel (bit-identical).
+// kHist: the multistep form, as posterior_kernel<true>; the history is only touched in the final register loop.
+template <bool kHist>
 __global__ void __cluster_dims__(kSelCluster, 1, 1) __launch_bounds__(kSelThreads)
 step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
                      float cond_scale, const long long* __restrict__ t, const float* __restrict__ tab_recip,
                      const float* __restrict__ tab_recipm1, const float* __restrict__ tab_c1,
                      const float* __restrict__ tab_c2, const float* __restrict__ tab_sigma,
                      const float* __restrict__ noise, int n, int rank_lo, int rank_hi, float weight, float min_s,
-                     float* out, float* __restrict__ s_out) {
+                     float* out, float* __restrict__ s_out, const float* __restrict__ tab_c3,
+                     float* __restrict__ x0_hist) {
     pdl_wait();
     pdl_trigger();
     namespace cg = cooperative_groups;
@@ -315,14 +327,23 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
         x0v[j] = v;
     }
     uint32_t prefix = 0, maskbits = 0, k = (uint32_t)rank_lo;
+    // kHist reads each pass's mask through shared memory.  With the mask a compile-time constant of the unrolled passes,
+    // ptxas precomputes the next pass's masked keys and keeps them alongside x0v: at 64 registers that spills (36 bytes
+    // in this instance).  Written by thread 0 after the barrier that ends the pass's reads.
+    __shared__ uint32_t sh_maskbits;
+    if constexpr (kHist) {
+        if (tid == 0) sh_maskbits = 0;
+    }
     for (int pass = 0; pass < 4; ++pass) {
         const int shift = 24 - 8 * pass;
         if (tid < 256) hist[tid] = 0;
         __syncthreads();
+        uint32_t mb = maskbits;
+        if constexpr (kHist) mb = sh_maskbits;
 #pragma unroll
         for (int j = 0; j < kSelPerThread; ++j) {
             const uint32_t key = absbits(x0v[j]);
-            const bool live = (tid + j * kSelThreads < cnt) && ((key & maskbits) == prefix);
+            const bool live = (tid + j * kSelThreads < cnt) && ((key & mb) == prefix);
             const unsigned bin = live ? ((key >> shift) & 0xFF) : 256u;
             const unsigned peers = __match_any_sync(0xffffffffu, bin);
             if (live && lane == (__ffs(peers) - 1)) atomicAdd(&hist[bin], __popc(peers));
@@ -362,6 +383,9 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
         prefix = sh_prefix;
         k = sh_k;
         maskbits |= 0xFFu << shift;
+        if constexpr (kHist) {
+            if (tid == 0) sh_maskbits = maskbits;
+        }
         cluster.sync();
     }
     const uint32_t v_lo = prefix;
@@ -401,6 +425,24 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
 
     const float c1 = tab_c1[tb], c2 = tab_c2[tb];
     const float sig = (tb == 0) ? 0.f : tab_sigma[tb];
+    if constexpr (kHist) {
+        const float c3 = tab_c3[tb];
+        if (c3 != 0.f) {
+#pragma unroll
+            for (int j = 0; j < kSelPerThread; ++j) {
+                const int i = tid + j * kSelThreads;
+                if (i < cnt) {
+                    float xs = fminf(fmaxf(x0v[j], -sb), sb);
+                    xs = __fdiv_rn(xs, sb);
+                    float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[base + i]));
+                    mean = __fadd_rn(mean, __fmul_rn(c3, x0_hist[base + i]));
+                    x0_hist[base + i] = xs;
+                    out[base + i] = __fadd_rn(mean, __fmul_rn(sig, noise[base + i]));
+                }
+            }
+            return;
+        }
+    }
 #pragma unroll
     for (int j = 0; j < kSelPerThread; ++j) {
         const int i = tid + j * kSelThreads;
@@ -408,6 +450,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
             float xs = fminf(fmaxf(x0v[j], -sb), sb);
             xs = __fdiv_rn(xs, sb);
             const float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[base + i]));
+            if constexpr (kHist) x0_hist[base + i] = xs;
             out[base + i] = __fadd_rn(mean, __fmul_rn(sig, noise[base + i]));
         }
     }
@@ -576,27 +619,38 @@ int step_quantile(const float* x0, int B, int n_per_img, int rank_lo, int rank_h
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
+template <bool kHist>
+static int step_posterior_impl(const float* x0, const float* x_t, const float* noise, const float* s,
+                               const long long* t, const float* tab_c1, const float* tab_c2, const float* tab_sigma,
+                               const float* tab_c3, int B, int n_per_img, float* out, float* x0_hist, cudaStream_t st) {
+    dim3 grid((n_per_img + 255) / 256, B);
+    launch_k(posterior_kernel<kHist>, grid, 256, 0, st, x0, x_t, noise, s, t, tab_c1, tab_c2, tab_sigma, n_per_img, out,
+             tab_c3, x0_hist);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
 int step_posterior(const float* x0, const float* x_t, const float* noise, const float* s, const long long* t,
                    const float* tab_c1, const float* tab_c2, const float* tab_sigma, int B, int n_per_img, float* out,
                    cudaStream_t st) {
-    dim3 grid((n_per_img + 255) / 256, B);
-    launch_k(posterior_kernel, grid, 256, 0, st, x0, x_t, noise, s, t, tab_c1, tab_c2, tab_sigma, n_per_img, out);
-    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+    return step_posterior_impl<false>(x0, x_t, noise, s, t, tab_c1, tab_c2, tab_sigma, nullptr, B, n_per_img, out,
+                                      nullptr, st);
 }
 
 bool step_epilogue_fused_ok(int n_per_img) {
     return (n_per_img + kSelCluster - 1) / kSelCluster <= kSelThreads * kSelPerThread;
 }
 
-int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const long long* t,
-                  const float* tab_recip, const float* tab_recipm1, const float* tab_c1, const float* tab_c2,
-                  const float* tab_sigma, const float* noise, int B, int n_per_img, int rank_lo, int rank_hi,
-                  float weight, float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st) {
+template <bool kHist>
+static int step_epilogue_impl(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                              const long long* t, const float* tab_recip, const float* tab_recipm1, const float* tab_c1,
+                              const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
+                              float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight,
+                              float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st) {
     if (rank_lo < 0 || rank_hi < rank_lo || rank_hi >= n_per_img) return -1;
     if (step_epilogue_fused_ok(n_per_img)) {
-        launch_k(step_epilogue_kernel, B * kSelCluster, kSelThreads, 0, st, x_t, eps_cond, eps_null, cond_scale, t,
-                 tab_recip, tab_recipm1, tab_c1, tab_c2, tab_sigma, noise, n_per_img, rank_lo, rank_hi, weight, min_s, out,
-                 s_out);
+        launch_k(step_epilogue_kernel<kHist>, B * kSelCluster, kSelThreads, 0, st, x_t, eps_cond, eps_null, cond_scale,
+                 t, tab_recip, tab_recipm1, tab_c1, tab_c2, tab_sigma, noise, n_per_img, rank_lo, rank_hi, weight, min_s,
+                 out, s_out, tab_c3, x0_hist);
         return cudaGetLastError() == cudaSuccess ? 0 : -2;
     }
     // images beyond the register-resident select (> 196 608 values, e.g. 3 x 1024 x 1024): x0 through the caller's scratch
@@ -605,7 +659,28 @@ int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null
     if (rc) return rc;
     rc = step_quantile(x0_ws, B, n_per_img, rank_lo, rank_hi, weight, min_s, s_out, st);
     if (rc) return rc;
-    return step_posterior(x0_ws, x_t, noise, s_out, t, tab_c1, tab_c2, tab_sigma, B, n_per_img, out, st);
+    return step_posterior_impl<kHist>(x0_ws, x_t, noise, s_out, t, tab_c1, tab_c2, tab_sigma, tab_c3, B, n_per_img, out,
+                                      x0_hist, st);
+}
+
+int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const long long* t,
+                  const float* tab_recip, const float* tab_recipm1, const float* tab_c1, const float* tab_c2,
+                  const float* tab_sigma, const float* noise, int B, int n_per_img, int rank_lo, int rank_hi,
+                  float weight, float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st) {
+    return step_epilogue_impl<false>(x_t, eps_cond, eps_null, cond_scale, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
+                                     tab_sigma, nullptr, noise, nullptr, B, n_per_img, rank_lo, rank_hi, weight, min_s,
+                                     out, s_out, x0_ws, st);
+}
+
+int step_epilogue_multistep(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                            const long long* t, const float* tab_recip, const float* tab_recipm1, const float* tab_c1,
+                            const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
+                            float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
+                            float* out, float* s_out, float* x0_ws, cudaStream_t st) {
+    if (!tab_c3 || !x0_hist) return -1;
+    return step_epilogue_impl<true>(x_t, eps_cond, eps_null, cond_scale, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
+                                    tab_sigma, tab_c3, noise, x0_hist, B, n_per_img, rank_lo, rank_hi, weight, min_s,
+                                    out, s_out, x0_ws, st);
 }
 
 int step_advance_t(long long* t, int B, cudaStream_t st) {

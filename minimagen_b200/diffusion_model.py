@@ -8,7 +8,7 @@ per-timestep noise scale the fused step kernel gathers (reference computes it ev
 The tensor methods are kept for API parity (they are one-line broadcasts of table lookups); the sampling loop does
 NOT go through them -- it uses the fused step kernels (minimagen_b200/csrc/step.cu).
 """
-from typing import NamedTuple, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -24,12 +24,14 @@ def _betas_fp64(timesteps):
 
 class SamplingSchedule(NamedTuple):
     """A respaced (DDIM) sampling walk, see `GaussianDiffusion.sampling_schedule`.  The tables are indexed by the step's
-    own timestep t and feed the fused step epilogue in place of posterior_mean_coef1 / posterior_mean_coef2 / sigma."""
+    own timestep t and feed the fused step epilogue in place of posterior_mean_coef1 / posterior_mean_coef2 / sigma.
+    A multistep walk (`GaussianDiffusion.dpm_solver_schedule`) also has c3 and runs on mi_step_epilogue_multistep."""
     grid: Tuple[int, ...]        # descending timesteps tau_S = T-1 > ... > tau_1 = 0 (host side)
     c1: torch.Tensor             # [T] fp32: coefficient of the clamped x0
     c2: torch.Tensor             # [T] fp32: coefficient of x_t
     sigma: torch.Tensor          # [T] fp32: scale of the step's noise (exactly 0 for eta = 0 and at t = 0)
     next_t: torch.Tensor         # [T] int64: next_t[tau_i] = tau_{i-1}, next_t[0] = 0
+    c3: Optional[torch.Tensor] = None   # [T] fp32: coefficient of the previous step's clamped x0 (multistep walks only)
 
 
 class GaussianDiffusion(nn.Module):
@@ -104,6 +106,65 @@ class GaussianDiffusion(nn.Module):
         sched = SamplingSchedule(grid=tuple(grid_up.flip(0).tolist()), c1=table(c1, torch.float32),
                                  c2=table(c2, torch.float32), sigma=table(sigma, torch.float32),
                                  next_t=table(next_t, torch.long))
+        self._schedules[key] = sched
+        return sched
+
+    def dpm_solver_schedule(self, steps: int, device) -> SamplingSchedule:
+        """DPM-Solver++(2M) (Lu et al. 2022, Algorithm 2, data prediction) as schedule tables, over a grid uniform in
+        log-SNR lambda_t = 0.5 (log a_t - log(1 - a_t)), a = alphas_cumprod.  Grid, ascending: u_0 = 0; for j >= 1, u_j is the
+        t whose lambda_t is nearest to linspace(lambda_0, lambda_{T-1}, steps)[j], clamped into [u_{j-1} + 1, T - steps + j]
+        (so exactly `steps` distinct points, the last one T-1).  The walk t_0 = T-1, ..., t_{S-1} = 0 is u reversed; with
+        a_k = a(t_k), h_k = lambda(t_{k+1}) - lambda(t_k) and phi_k = sqrt(a_{k+1}) - sqrt(1 - a_{k+1}) sqrt(a_k) / sqrt(1 - a_k)
+        (DDIM's c1 at eta = 0, = alpha_{k+1} (1 - e^{-h_k})), step k updates
+            x <- c1 x0_k + c2 x + c3 x0_{k-1},   c2 = sqrt(1 - a_{k+1}) / sqrt(1 - a_k),
+            k = 0:              c1 = phi_0, c3 = 0                                     (first order)
+            0 < k < S-1:        c1 = phi_k (1 + 1 / (2 r_k)), c3 = -phi_k / (2 r_k),  r_k = h_{k-1} / h_k
+            k = S-1 (t = 0):    c1 = 1, c2 = c3 = 0                                    (x = x0, as DDIM)
+        with x0 the thresholded data prediction.  sigma = 0.  phi and c2 use sampling_schedule's fp64 expressions, so at
+        steps = 2 the tables are those of sampling_schedule(2, 0.).  Computed in fp64, cast to fp32; cached per
+        (steps, device)."""
+        T = self.num_timesteps
+        steps = int(steps)
+        assert 2 <= steps <= T, f'sampling timesteps must be between 2 and {T} (the number of training timesteps)'
+        device = torch.device(device)
+        key = ('dpmpp_2m', steps, str(device))
+        sched = self._schedules.get(key)
+        if sched is not None:
+            return sched
+        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        lam = 0.5 * (acp.log() - (1. - acp).log())
+        # at T = 20 the last beta is 1, so lambda_{T-1} = -inf: the targets then end at lambda_{T-2}, and the last point is
+        # still T-1 (for a finite lambda_{T-1} the rule above gives T-1 anyway)
+        end = float(lam[T - 1]) if torch.isfinite(lam[T - 1]) else float(lam[T - 2])
+        target = torch.linspace(float(lam[0]), end, steps, dtype=torch.float64)
+        grid_up = [0]
+        for j in range(1, steps - 1):
+            nearest = int((lam - target[j]).abs().argmin())
+            grid_up.append(min(max(nearest, grid_up[-1] + 1), T - steps + j))
+        grid_up.append(T - 1)
+        grid_up = torch.tensor(grid_up, dtype=torch.long)
+        assert bool((grid_up[1:] > grid_up[:-1]).all()) and grid_up[-1] == T - 1
+        walk = grid_up.flip(0)                                    # t_0 = T-1, ..., t_{S-1} = 0
+        a = acp[walk]
+        a_next = torch.cat((a[1:], torch.ones(1, dtype=torch.float64)))
+        d = (1. - a_next).clamp(min=0.).sqrt()
+        phi = a_next.sqrt() - d * a.sqrt() / (1. - a).sqrt()
+        c2 = d / (1. - a).sqrt()
+        c1, c3 = phi.clone(), torch.zeros(steps, dtype=torch.float64)
+        h = lam[walk[1:]] - lam[walk[:-1]]                        # h_k, k = 0 .. S-2
+        if steps > 2:
+            r = h[:-1] / h[1:]                                    # r_k, k = 1 .. S-2
+            c1[1:-1] = phi[1:-1] * (1. + 1. / (2. * r))
+            c3[1:-1] = -phi[1:-1] / (2. * r)
+
+        def table(v, dtype):
+            out = torch.zeros(T, dtype=dtype)
+            out[grid_up] = v.flip(0).to(dtype)
+            return out.to(device)
+        next_t = torch.cat((walk[1:], torch.zeros(1, dtype=torch.long)))
+        sched = SamplingSchedule(grid=tuple(walk.tolist()), c1=table(c1, torch.float32), c2=table(c2, torch.float32),
+                                 sigma=torch.zeros(T, dtype=torch.float32, device=device),
+                                 next_t=table(next_t, torch.long), c3=table(c3, torch.float32))
         self._schedules[key] = sched
         return sched
 

@@ -238,6 +238,29 @@ class NativeOps:
                N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(noise), B, n, int(rank_lo), int(rank_hi),
                float(weight), float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
 
+    def step_epilogue_multistep(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist,
+                                B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """step_epilogue plus c3[t] * hist in the mean (skipped where c3[t] == 0); then hist <- the clamped x0.
+        `out` may be `x_t`; `hist` [B, n] must not alias the other tensors."""
+        for nm, tt in (("x_t", x_t), ("eps_cond", eps_cond), ("eps_null", eps_null), ("tab_a", tab_a), ("tab_b", tab_b),
+                       ("c1", c1), ("c2", c2), ("sigma", sigma), ("c3", c3), ("noise", noise), ("hist", hist),
+                       ("out", out), ("s_out", s_out)):
+            _chk(tt, F32, nm)
+        _chk(t, I64, "t")
+        if c3 is None or hist is None:
+            raise ValueError("step_epilogue_multistep: c3 and hist are required")
+        if hist.numel() != B * n:
+            raise ValueError(f"hist: expected {B * n} values, got {hist.numel()}")
+        ws = None
+        nws = int(N.load().mi_step_epilogue_workspace_floats(B, n))
+        if nws:
+            ws = torch.empty(nws, dtype=F32, device=x_t.device)
+            if s_out is None:
+                s_out = torch.empty(B, dtype=F32, device=x_t.device)
+        N.call("mi_step_epilogue_multistep", N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), float(cond_scale), N.ptr(t),
+               N.ptr(tab_a), N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(c3), N.ptr(noise), N.ptr(hist), B, n,
+               int(rank_lo), int(rank_hi), float(weight), float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
+
     def step_advance_t(self, t, B):
         _chk(t, I64, "t")
         N.call("mi_step_advance_t", N.ptr(t), B, N.stream())
