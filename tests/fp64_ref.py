@@ -1,0 +1,353 @@
+"""TEST INFRASTRUCTURE ONLY: float64 references of the token-side kernels with elementwise error bounds.
+
+Every reference takes the operands exactly as the kernel reads them (fp16-rounded where the kernel reads fp16, the null
+key/value included), computes in float64 on the operands' device, and returns (reference, bound): |kernel - reference| <=
+bound must hold for EVERY element.  A bound is derived from the kernel's own rounding steps (the derivation is in each
+docstring) and has the general form
+
+    c * n * u * twin + u_out * |ref|,        c <= 4,
+
+with n the accumulation length (it may follow the kernel's documented summation structure), u the unit roundoff of the
+accumulation (U32) or of an fp16 operand (U16), and `twin` the same expression evaluated on absolute values.  The
+constants are fixed here and not tuned per test.  tests/test_error_bounds.py shows on the CPU that the torch emulation of
+the kernels' contract passes every bound and that planted defects fail it.
+"""
+import math
+
+import torch
+
+U16 = 2.0 ** -11            # unit roundoff of fp16
+U32 = 2.0 ** -24            # unit roundoff of fp32
+ETA32 = 2.0 ** -147         # four fp32 subnormal spacings: absolute error of a few roundings in the underflow range
+HALF_MAX = 65504.0
+F64 = torch.float64
+
+
+def _d(t):
+    return None if t is None else t.detach().to(F64)
+
+
+def _abs(t):
+    return 0.0 if t is None else t.abs()
+
+
+def check(out, ref, bound, what, sentinel=None):
+    """Assert that `out` is finite, that |out - ref| <= bound elementwise and that the sentinel elements of the output
+    buffer (bool mask of `out`'s shape, True = must still be NaN) were not written.  Prints -- and on failure reports --
+    the worst element and its ratio |out - ref| / bound.  Returns that ratio."""
+    o = out.detach().to(F64)
+    ref = ref.to(o.device, F64).expand(o.shape)
+    bound = torch.as_tensor(bound, dtype=F64, device=o.device).expand(o.shape)
+    live = torch.ones(o.shape, dtype=torch.bool, device=o.device)
+    if sentinel is not None:
+        sentinel = sentinel.to(o.device)
+        touched = int((~torch.isnan(o[sentinel])).sum())
+        assert touched == 0, f"{what}: {touched} sentinel elements were overwritten"
+        live = ~sentinel
+    bad = live & ~torch.isfinite(o)
+    assert not bad.any(), f"{what}: {int(bad.sum())} non-finite elements, first at {tuple(bad.nonzero()[0].tolist())}"
+    err = torch.where(live, (o - ref).abs(), torch.zeros((), dtype=F64, device=o.device))
+    ratio = err / bound.clamp(min=1e-300)
+    worst = int(ratio.reshape(-1).argmax())
+    idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(worst), o.shape))
+    r = float(ratio.reshape(-1)[worst])
+    msg = (f"{what}: worst |err|/bound = {r:.3g} at {idx} (out {float(o[idx]):.9g}, ref {float(ref[idx]):.9g}, "
+           f"bound {float(bound[idx]):.3g})")
+    print(msg)
+    assert r <= 1.0, msg
+    return r
+
+
+def check_rel_l2(out, ref, limit, what):
+    """Assert ||out - ref|| / ||ref|| < limit over the whole tensor.  The elementwise bounds are worst cases: at long
+    accumulations they leave room for a small error that is the same in every element (fp16 operands in an fp32 GEMM, a
+    1e-4 relative scale error, a 1 % error over a whole attention output with zero-mean values), which rounding noise
+    never produces.  This aggregate check sees such an error; it uses the limits the op tests have always used.  Prints
+    and returns the value."""
+    o = out.detach().to(F64)
+    ref = ref.to(o.device, F64)
+    r = float((o - ref).norm() / ref.norm().clamp(min=1e-300))
+    msg = f"{what}: rel-L2 = {r:.3g} (limit {limit:.3g})"
+    print(msg)
+    assert r < limit, msg
+    return r
+
+
+def half_out(ref, bound):
+    """Reference and bound of an fp16 output whose fp32 value (before rounding) has reference `ref` and bound `bound`.
+    The kernels convert with saturation (csrc/sat_half.cuh: beyond +-65504 -> +-65504), so the reference is clamped to
+    +-65504 and then rounded.  Clamping is 1-Lipschitz and each of the two roundings (kernel value, reference) is off by
+    at most U16 relative or, among subnormals, 2^-25 absolute:
+        |fp16(clamp(y)) - fp16(clamp(r))| <= (1 + U16) bound + 2 U16 |clamp(r)| + 2^-24."""
+    rc = ref.clamp(-HALF_MAX, HALF_MAX)
+    return rc.to(torch.float16).to(F64), (1 + U16) * bound + 2 * U16 * rc.abs() + 2.0 ** -24
+
+
+def _gelu(x):
+    return 0.5 * x * (1.0 + torch.erf(x * (0.5 ** 0.5)))
+
+
+def _silu(x):
+    return x * torch.sigmoid(x)
+
+
+# ---------------------------------------------------------------------------------------------- attention
+def attention_views(q, q_bs, ldq, k, v, kv_bs, ldkv, kv_hs, B, heads, n, m):
+    """The [B, h, n, 64] query and [B, hk, m, 64] key / value views that mi_attention_fwd reads (hk = 1: kv_hs == 0)."""
+    hk = heads if kv_hs else 1
+    qv = q.as_strided((B, heads, n, 64), (q_bs, 64, ldq, 1), q.storage_offset())
+    kv = k.as_strided((B, hk, m, 64), (kv_bs, kv_hs, ldkv, 1), k.storage_offset())
+    vv = v.as_strided((B, hk, m, 64), (kv_bs, kv_hs, ldkv, 1), v.storage_offset())
+    return qv, kv, vv
+
+
+def attention_ref(q, k, v, null_kv, mask=None, p16=True, out16=True):
+    """softmax([null_k, k] q^T) [null_v, v] per (batch, head, query row) -- mi_attention_fwd and AttentionFn.forward.
+
+    q [B, h, n, 64]; k, v [B, hk, m, 64] with hk = h or 1 (multi-query); null_kv [2, 64]; mask [B, m] (nonzero = key
+    takes part; the null key always does).  Pass the values the kernel reads: fp16-rounded q / k / v / null_kv for the
+    fused kernels, the fp32 values for AttentionFn.  Keys that are masked out get probability 0 in the reference, as in
+    both kernels (-FLT_MAX scores underflow exp to exactly 0).
+
+    Bound, per element, with A = sum_j p_j |v_j| over the unmasked keys, L = m + 1 keys and
+    ds = 64 U32 max_j sum_d |q_d k_jd| the row's fp32 score error (64-term fp32 dot products):
+        2 (U16 |o| + (U16 + 4 ds + (L + 8) U32) A)
+      * U16 A      : P is rounded to fp16 before the P V product (p16; 0 for the fp32 path);
+      * 4 ds A     : a score error ds moves exp(s - max) by e^ds and the row sum l by as much: p_j / l off by <= 2 ds
+                     relative, and sum_j dp_j |v_j - o| <= 2 ds 2 A;
+      * (L+8) U32 A: fp32 exp (a few ulp), the L-term sums of l and of P V, the final division;
+      * U16 |o|    : fp16 output rounding (out16; U32 |o| for an fp32 output);
+    doubled for second-order terms.  Chunked per image so that the float64 scores of one image only are live."""
+    B, h, n, D = q.shape
+    m, hk = k.shape[2], k.shape[1]
+    L = m + 1
+    nk = null_kv.detach().to(F64, copy=True).to(q.device)
+    o = torch.empty((B, h, n, D), dtype=F64, device=q.device)
+    bound = torch.empty_like(o)
+    up, uo = (U16 if p16 else 0.0), (U16 if out16 else U32)
+    for b in range(B):
+        kk = torch.cat((nk[0].expand(hk, 1, D), _d(k[b])), dim=1)
+        vv = torch.cat((nk[1].expand(hk, 1, D), _d(v[b])), dim=1)
+        qb = _d(q[b])
+        s = qb @ kk.transpose(-1, -2)                                   # [h, n, L]
+        qk = qb.abs() @ kk.abs().transpose(-1, -2)
+        if mask is not None:
+            valid = torch.cat((torch.ones(1, dtype=torch.bool, device=q.device), mask[b].to(q.device) != 0))
+            s = s.masked_fill(~valid, -math.inf)
+            qk = qk.masked_fill(~valid, 0.0)
+        p = torch.softmax(s, dim=-1)
+        o[b] = p @ vv
+        A = p @ vv.abs()
+        ds = 64 * U32 * qk.amax(dim=-1, keepdim=True)
+        bound[b] = 2 * (uo * o[b].abs() + (up + 4 * ds + (L + 8) * U32) * A)
+    return o, bound
+
+
+def attention_fn_ref(q, k, v, null_kv, heads, do):
+    """AttentionFn (minimagen_b200/autograd.py) forward and backward in float64 autograd: q [B, n, h*64], k / v
+    [B, m, hk*64], null_kv [2, 64], upstream gradient do [B, n, h*64].  Returns {name: (reference, bound)} for
+    o, dq, dk, dv, dnull.
+
+    The fp32 chain is S = q K^T (64-term fma GEMM), P = softmax(S), o = P V (L terms); dP = dO V^T (64 terms),
+    dS = P (dP - sum P dP) (L terms), dq = dS K (L terms), dK = dS^T q and dV = P^T dO (n terms), the multi-query head sum
+    (h terms) and the null key's batch sum (B h terms).  To first order every rounding adds at most U32 times the
+    magnitude of its operands, and every intermediate is dominated by the chain evaluated on absolute values (`twin`:
+    |dP| <= |dO| |V|^T, |dS| <= P (|dP| + sum P |dP|), ...).  The score error ds (see attention_ref) moves P by <= 4 ds
+    relative.  So each gradient is bounded by 2 N U32 twin with N = n + L + 64 + h + B h + 16 + 4 max(ds) / U32; the
+    output uses attention_ref's bound for fp32 P and an fp32 result."""
+    B, n, inner = q.shape
+    m, D = k.shape[1], 64
+    hk = k.shape[2] // D
+    L = m + 1
+    q_, k_, v_, nk_ = (_d(t).requires_grad_(True) for t in (q, k, v, null_kv))
+    with torch.enable_grad():
+        qh = q_.reshape(B, n, heads, D).permute(0, 2, 1, 3)
+        kh = torch.cat((nk_[0].expand(B, hk, 1, D), k_.reshape(B, m, hk, D).permute(0, 2, 1, 3)), dim=2)
+        vh = torch.cat((nk_[1].expand(B, hk, 1, D), v_.reshape(B, m, hk, D).permute(0, 2, 1, 3)), dim=2)
+        p = torch.softmax(qh @ kh.transpose(-1, -2), dim=-1)                           # [B, h, n, L]
+        o = (p @ vh).permute(0, 2, 1, 3).reshape(B, n, inner)
+        grads = torch.autograd.grad(o, (q_, k_, v_, nk_), _d(do))
+    o = o.detach()
+    p = p.detach()
+    qa, ka, va, doa = qh.detach().abs(), kh.detach().abs(), vh.detach().abs(), _d(do).reshape(B, n, heads, D).permute(0, 2, 1, 3).abs()
+    ds = 64 * U32 * (qa @ ka.transpose(-1, -2)).amax()
+    # forward
+    A = (p @ va).permute(0, 2, 1, 3).reshape(B, n, inner)
+    bo = 2 * (U32 * o.abs() + (4 * ds + (L + 8) * U32) * A)
+    # backward twins
+    dPt = doa @ va.transpose(-1, -2)
+    dSt = p * (dPt + (p * dPt).sum(dim=-1, keepdim=True))
+    dqt = (dSt @ ka).permute(0, 2, 1, 3).reshape(B, n, inner)
+    dkt = dSt.transpose(-1, -2) @ qa                                                   # [B, h, L, D]
+    dvt = p.transpose(-1, -2) @ doa
+    if hk == 1:
+        dkt, dvt = dkt.sum(dim=1, keepdim=True), dvt.sum(dim=1, keepdim=True)
+    dnt = torch.stack((dkt[:, :, 0].sum(dim=(0, 1)), dvt[:, :, 0].sum(dim=(0, 1))))
+    dkt = dkt[:, :, 1:].permute(0, 2, 1, 3).reshape(B, m, hk * D)
+    dvt = dvt[:, :, 1:].permute(0, 2, 1, 3).reshape(B, m, hk * D)
+    N = n + L + 64 + heads + B * heads + 16 + 4 * float(ds) / U32
+    out = {"o": (o, bo)}
+    for name, g, t in zip(("dq", "dk", "dv", "dnull"), grads, (dqt, dkt, dvt, dnt)):
+        out[name] = (g.detach(), 2 * N * U32 * t)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------- LayerNorm
+def ln_ref(x, gamma, beta, eps, pre_gelu, residual):
+    """mi_ln_rows: y = (v - mean) rstd gamma + beta + residual over the last dim, v = gelu_erf(x) if pre_gelu else x,
+    rstd = 1 / sqrt(mean((v - mean)^2) + eps).  Reference y and the bound of the fp32 output (half_out for the fp16 one).
+
+    The fp32 mean (a C-term sum) is off by <= C U32 max|v|, the centred value v_c - mean by that plus U32 |v_c - mean|,
+    the variance (C positive terms) and rsqrtf by <= (C + 4) U32 relative.  Scaled by |gamma_c| rstd this is the
+    cancellation term
+        |gamma_c| rstd (C + 16) U32 (max_row |v| + |v_c - mean|),
+    which also holds for near-constant rows (variance << eps), where rstd ~ eps^-1/2 magnifies the mean's error.  The
+    fp32 GELU (erff, a few ulp) is off by <= 4 U32 (|v| + |x|) absolute (1 + erf cancels for negative x); an input error
+    of at most G per element moves y_c by <= |gamma_c| rstd (2 + |xhat_c|) G.  The affine epilogue adds at most
+    4 U32 (|gamma_c xhat_c| + |beta_c| + |residual_c|).  Bound = 2 x the first two terms + the third."""
+    x64 = _d(x)
+    C = x64.shape[-1]
+    v = _gelu(x64) if pre_gelu else x64
+    mu = v.mean(dim=-1, keepdim=True)
+    dv = v - mu
+    rstd = 1.0 / torch.sqrt((dv * dv).mean(dim=-1, keepdim=True) + eps)
+    xh = dv * rstd
+    g = _d(gamma)
+    y = xh * g
+    if beta is not None:
+        y = y + _d(beta)
+    if residual is not None:
+        y = y + _d(residual)
+    canc = (C + 16) * U32 * (v.abs().amax(dim=-1, keepdim=True) + dv.abs())
+    if pre_gelu:
+        canc = canc + (2 + xh.abs()) * 4 * U32 * (v.abs() + x64.abs()).amax(dim=-1, keepdim=True)
+    bound = 2 * g.abs() * rstd * canc + 4 * U32 * ((g * xh).abs() + _abs(_d(beta)) + _abs(_d(residual)))
+    return y, bound
+
+
+def ln_bwd_acc_len(R, sms):
+    """Summation length behind one dgamma / dbeta element of ln_bwd_kernel (csrc/backward.cu): min(ceil(R / 8), 2 sms)
+    blocks of 8 warps stride over the rows; each block accumulates its rows into shared memory, then adds the block's
+    partial to the global accumulator (that already holds the caller's value)."""
+    blocks = min(-(-R // 8), 2 * sms)
+    return -(-R // (8 * blocks)) * 8 + blocks + 1
+
+
+def ln_bwd_ref(x, dy, gamma, eps, pre_gelu, dgamma0, dbeta0, acc_len):
+    """mi_ln_rows_bwd (LayerNorm without beta, optional exact-erf GELU in front): dx, and dgamma / dbeta accumulated
+    onto dgamma0 / dbeta0.  Returns ((dx, bound), (dgamma, bound), (dbeta, bound)).
+
+    With xhat = (v - mean) rstd, g = gamma dy: dx = rstd (g - mean(g) - xhat mean(g xhat)) [* gelu'(x)].  xhat_c is off
+    by <= (C + 16) U32 e_c with e_c = rstd (max_row |v| + |v_c - mean|) (see ln_ref; e_c >= |xhat_c|), the two C-term
+    means by C U32 times their absolute twins, so
+        |d dx_c| <= 4 (C + 16) U32 rstd (|g_c| + mean|g| + e_c mean(|g| e))  (* |gelu'(x_c)|)
+    plus, with GELU, 8 U32 |inner_c| for the fp32 gelu' (inner = dx / gelu') and 4 U32 (|v| + |x|) of GELU error in e.
+    dgamma_c = dgamma0_c + sum_rows dy xhat: acc_len roundings (ln_bwd_acc_len) and the xhat errors:
+        2 (acc_len + C + 16) U32 (sum_rows |dy_c| e_c + |dgamma0_c|);  dbeta likewise with sum_rows |dy_c|."""
+    x64, d = _d(x), _d(dy)
+    C = x64.shape[-1]
+    with torch.enable_grad():
+        x_ = x64.clone().requires_grad_(True)
+        g_ = _d(gamma).clone().requires_grad_(True)
+        v_ = _gelu(x_) if pre_gelu else x_
+        y = torch.nn.functional.layer_norm(v_, (C,), None, None, eps) * g_
+        gx, gg = torch.autograd.grad(y, (x_, g_), d)
+    v = _gelu(x64) if pre_gelu else x64
+    mu = v.mean(dim=-1, keepdim=True)
+    rstd = 1.0 / torch.sqrt(((v - mu) ** 2).mean(dim=-1, keepdim=True) + eps)
+    vmax = v.abs().amax(dim=-1, keepdim=True)
+    if pre_gelu:
+        vmax = vmax + 4 * (v.abs() + x64.abs()).amax(dim=-1, keepdim=True)
+    e = rstd * (vmax + (v - mu).abs())
+    ga = (_d(gamma) * d).abs()
+    twin = ga + ga.mean(dim=-1, keepdim=True) + e * (ga * e).mean(dim=-1, keepdim=True)
+    bdx = 4 * (C + 16) * U32 * rstd * twin
+    if pre_gelu:       # dx = gelu'(x) inner; the fp32 gelu' (erff, expf) is off by <= 8 U32 absolute
+        xh = (v - mu) * rstd
+        g = _d(gamma) * d
+        inner = rstd * (g - g.mean(dim=-1, keepdim=True) - xh * (g * xh).mean(dim=-1, keepdim=True))
+        gp = 0.5 * (1 + torch.erf(x64 * 0.5 ** 0.5)) + x64 * torch.exp(-0.5 * x64 * x64) / math.sqrt(2 * math.pi)
+        bdx = bdx * (gp.abs() + 8 * U32) + 8 * U32 * inner.abs()
+    dg = gg + _d(dgamma0)
+    db = d.sum(dim=0) + _d(dbeta0)
+    bdg = 2 * (acc_len + C + 16) * U32 * ((d.abs() * e).sum(dim=0) + _d(dgamma0).abs())
+    bdb = 2 * acc_len * U32 * (d.abs().sum(dim=0) + _d(dbeta0).abs())
+    return (gx, bdx), (dg, bdg), (db, bdb)
+
+
+# ---------------------------------------------------------------------------------------------- fp32 linear / GEMM
+def linear_ref(x, w, bias, in_act, out_act, addend, out_scale):
+    """mi_linear_f32: y = s * act_out(act_in(x) W^T + bias + addend), act = SiLU when the flag is 1.  Bound of the fp32
+    output (half_out for the fp16 one).
+
+    The K-term fp32 dot product (any order) and the two adds are off by <= (K + 2) U32 twin, twin = |act_in(x)| |W|^T +
+    |bias| + |addend|; the fp32 SiLU of the input (x / (1 + expf(-x)), a few ulp) adds <= 4 U32 twin; SiLU at the output
+    has slope <= 1.1 and rounds by <= 4 U32 |y|; the scale rounds once:
+        |s| 2 (K + 8) U32 twin (x 1.1 with out_act) + 4 U32 |y|."""
+    x64, w64 = _d(x), _d(w)
+    K = x64.shape[-1]
+    xa = _silu(x64) if in_act else x64
+    pre = xa @ w64.t()
+    twin = xa.abs() @ w64.abs().t()
+    if bias is not None:
+        pre, twin = pre + _d(bias), twin + _d(bias).abs()
+    if addend is not None:
+        pre, twin = pre + _d(addend), twin + _d(addend).abs()
+    e = 2 * (K + 8) * U32 * twin
+    y = pre
+    if out_act:
+        y, e = _silu(pre), 1.1 * e
+    y = y * out_scale
+    return y, abs(out_scale) * e + 4 * U32 * y.abs()
+
+
+def gemm_ref(A, B, C0, alpha, accumulate):
+    """mi_gemm_f32: C = alpha A B (+ C0), batched over leading dims.  The kernel accumulates K fused multiply-adds in
+    fp32, scales once and adds once:  2 (K + 2) U32 (|alpha| |A| |B| + |C0|)."""
+    A64, B64 = _d(A), _d(B)
+    K = A64.shape[-1]
+    r = alpha * (A64 @ B64)
+    twin = abs(alpha) * (A64.abs() @ B64.abs())
+    if accumulate:
+        r, twin = r + _d(C0), twin + _d(C0).abs()
+    return r, 2 * (K + 2) * U32 * twin
+
+
+def colsum_acc_len(M):
+    """Summation length behind one column of colsum_kernel (csrc/backward.cu): min(ceil(M / 1024), 512) row splits of
+    rpb rows; a thread sums every 8th row of its split, 8 partials are added, then one atomicAdd per split onto out."""
+    splits = min(-(-M // 1024), 512)
+    rpb = -(-M // splits)
+    return -(-rpb // 8) + 8 + splits + 1
+
+
+def colsum_ref(x, out0, acc_len):
+    """mi_colsum_f32: out = sum_rows x (+ out0):  2 acc_len U32 (sum_rows |x| + |out0|)."""
+    x64 = _d(x)
+    s, twin = x64.sum(dim=0), x64.abs().sum(dim=0)
+    if out0 is not None:
+        s, twin = s + _d(out0), twin + _d(out0).abs()
+    return s, 2 * acc_len * U32 * twin
+
+
+# ---------------------------------------------------------------------------------------------- softmax rows
+def softmax_ref(s):
+    """mi_softmax_rows: p = exp(s - max) / sum.  The fp32 difference s - max rounds by U32 |s - max| (an exponent error:
+    relative error of the same size in p), expf is good to a few ulp, the sum of L positive terms to L U32 relative,
+    the reciprocal and the product to an ulp each; probabilities below 2^-126 are subnormal, where expf and the product
+    round to absolute steps of 2^-149:  2 p ((L + 8) U32 + U32 |s - max|) + ETA32."""
+    s64 = _d(s)
+    L = s64.shape[-1]
+    p = torch.softmax(s64, dim=-1)
+    return p, 2 * p * ((L + 8) * U32 + U32 * (s64 - s64.amax(dim=-1, keepdim=True)).abs()) + ETA32
+
+
+def softmax_bwd_ref(P, dP):
+    """mi_softmax_rows_bwd: dS = P (dP - sum_j P_j dP_j) with the kernel's own (fp32) P.  The dot product is an L-term
+    fma sum, the difference and the product round once (the product by up to 2^-149 absolute among subnormals):
+        2 (L + 4) U32 P (|dP| + sum_j |P_j dP_j|) + ETA32."""
+    P64, d64 = _d(P), _d(dP)
+    L = P64.shape[-1]
+    dot = (P64 * d64).sum(dim=-1, keepdim=True)
+    twin = P64 * (d64.abs() + (P64 * d64).abs().sum(dim=-1, keepdim=True))
+    return P64 * (d64 - dot), 2 * (L + 4) * U32 * twin + ETA32

@@ -160,7 +160,7 @@ def test_conv_direct(native, case):
     assert rel_l2(o_n, o_e) < 1e-5
 
 
-# ---------------------------------------------------------------------------------------------- GroupNorm / casts / LN
+# ---------------------------------------------------------------------------------------------- GroupNorm / casts
 @pytest.mark.parametrize("B,HW,C0,C1,groups", [(2, 256, 128, 0, 8), (2, 1024, 256, 128, 8), (3, 100, 8, 0, 8),
                                                (2, 64, 16, 8, 8), (1, 4096, 2048, 0, 8), (2, 256, 32, 0, 8)])
 @pytest.mark.parametrize("f16", [True, False])
@@ -378,38 +378,7 @@ def test_cast_act(native, mode, f16, in16):
     assert torch.equal(o_n.cpu(), o_e)
 
 
-@pytest.mark.parametrize("R,C,pre_gelu,res,beta", [(100, 16, 0, True, True), (513, 1024, 1, False, False),
-                                                   (64, 2048, 0, True, False), (7, 8, 0, False, True),
-                                                   (520, 128, 0, False, True)])
-def test_ln_rows(native, R, C, pre_gelu, res, beta):
-    x = _rand(R, C, seed=18) * 3 + 1
-    gamma = _rand(C, seed=19)
-    bt = _rand(C, seed=20) if beta else None
-    r = _rand(R, C, seed=21) if res else None
-    o_e, o16_e = torch.zeros(R, C), torch.zeros(R, C, dtype=F16)
-    EMU.ln_rows(x, R, C, gamma, bt, 1e-5, pre_gelu, r, o_e, o16_e)
-    o_n, o16_n = torch.zeros(R, C, device="cuda"), torch.zeros(R, C, dtype=F16, device="cuda")
-    native.ln_rows(x.cuda(), R, C, gamma.cuda(), _cu(bt), 1e-5, pre_gelu, _cu(r), o_n, o16_n)
-    assert rel_l2(o_n, o_e) < 3e-6
-    assert rel_l2(o16_n, o_e) < 1e-3
-
-
 # ---------------------------------------------------------------------------------------------- conditioning
-@pytest.mark.parametrize("M,K,N,in_act,out_act,add", [(2, 8, 32, 0, 1, False), (32, 1024, 2048, 1, 0, False),
-                                                      (32, 512, 512, 0, 0, True), (516, 8, 1024, 0, 0, False),
-                                                      (9, 768, 128, 0, 0, False)])
-def test_linear_f32(native, M, K, N, in_act, out_act, add):
-    x, w, b = _rand(M, K, seed=22), _rand(N, K, seed=23, scale=K ** -0.5), _rand(N, seed=24)
-    a = _rand(M, N, seed=25) if add else None
-    o_e = torch.zeros(M, N)
-    EMU.linear_f32(x, M, K, w, b, N, in_act, out_act, a, o_e, None, 0.125)
-    o_n = torch.zeros(M, N, device="cuda")
-    o16 = torch.zeros(M, N, dtype=F16, device="cuda")
-    native.linear_f32(x.cuda(), M, K, w.cuda(), b.cuda(), N, in_act, out_act, _cu(a), o_n, o16, 0.125)
-    assert rel_l2(o_n, o_e) < 2e-6
-    assert rel_l2(o16, o_e) < 1e-3
-
-
 def test_posemb_and_text_tokens(native):
     t = torch.tensor([0, 1, 17, 500, 999])
     for dim in (8, 128, 256):
@@ -461,67 +430,6 @@ def test_resize_separable(native, n_in, n_out, pad, clamp):
     o_n = torch.zeros(2, 3, ho, ho, device="cuda")
     native.resize_separable(x.cuda(), 6, n_in, n_in, o_n, ho, ho, iy.cuda(), wy.cuda(), iy.cuda(), wy.cuda(), clamp=clamp)
     assert (o_n.cpu() - o_e).abs().max().item() < 2e-6
-
-
-# ---------------------------------------------------------------------------------------------- attention
-@pytest.mark.parametrize("B,heads,n,m,shared,use_mask", [(2, 8, 256, 260, False, False), (2, 8, 64, 258, False, True),
-                                                         (1, 8, 1024, 1024, True, False), (2, 8, 256, 256, True, True),
-                                                         (1, 2, 100, 37, False, True),
-                                                         (3, 8, 128, 59, False, False),      # one padded key block
-                                                         (2, 4, 384, 127, True, False),      # m + 1 == 128 exactly
-                                                         (1, 2, 4096, 4096, True, False),    # base U-Net 64x64 tokens
-                                                         (2, 8, 512, 300, False, True),      # key mask, two query tiles
-                                                         (2, 4, 384, 700, True, True),       # ... and inside the one-tile kernel (n % 256 != 0)
-                                                         (1, 8, 256, 2000, True, True)])     # ... over many key blocks
-def test_attention(native, B, heads, n, m, shared, use_mask):
-    inner = heads * 64
-    q = (_rand(B * n, inner, seed=34) * 0.125).to(F16)
-    ldkv = 128 if shared else 2 * inner
-    kv = _rand(B * m, ldkv, seed=35).to(F16)
-    null_kv = _rand(2, 64, seed=36)
-    mask = None
-    if use_mask:
-        mask = (torch.rand(B, m, generator=torch.Generator().manual_seed(1)) > 0.3).to(torch.uint8)
-    v_off = 64 if shared else inner
-    args = (n * inner, inner)
-    o_e = torch.zeros(B * n, inner, dtype=F16)
-    EMU.attention(q, n * inner, inner, kv, kv[:, v_off:], m * ldkv, ldkv, 0 if shared else 64, null_kv, mask, B, heads,
-                  n, m, o_e, *args)
-    qn, kvn = q.cuda(), kv.cuda()
-    o_n = torch.zeros(B * n, inner, dtype=F16, device="cuda")
-    native.attention(qn, n * inner, inner, kvn, kvn[:, v_off:], m * ldkv, ldkv, 0 if shared else 64, null_kv.cuda(),
-                     _cu(mask), B, heads, n, m, o_n, *args)
-    assert rel_l2(o_n, o_e) < 2e-3           # fp16 P / fp16 output rounding
-
-
-@pytest.mark.parametrize("B,heads,n,m,shared,ramp", [(1, 8, 1024, 1280, True, "up"), (2, 4, 256, 600, False, "up"),
-                                                     (1, 8, 1024, 1280, True, "down"), (2, 4, 128, 1500, True, "rows")])
-def test_attention_single_sweep_rescales(native, B, heads, n, m, shared, ramp):
-    """Online softmax over long key sequences: key norms that grow along the sequence ("up") force a rescale of the
-    running accumulator in almost every key block, shrinking ones ("down") none after the first, "rows" makes only some
-    query rows of a CTA move."""
-    inner = heads * 64
-    g = torch.Generator().manual_seed(91)
-    q = torch.randn(B * n, inner, generator=g) * 0.5
-    if ramp == "rows":
-        q[::7] *= 4.0
-    ldkv = 128 if shared else 2 * inner
-    kv = torch.randn(B * m, ldkv, generator=g)
-    t = torch.linspace(0, 1, m).repeat(B)[:, None]
-    scale = {"up": 1 + 5 * t, "down": 6 - 5 * t, "rows": 1 + 3 * t}[ramp]
-    v_off = 64 if shared else inner
-    kv[:, :v_off] *= scale
-    q, kv = q.to(F16), kv.to(F16)
-    null_kv = _rand(2, 64, seed=36)
-    o_e = torch.zeros(B * n, inner, dtype=F16)
-    EMU.attention(q, n * inner, inner, kv, kv[:, v_off:], m * ldkv, ldkv, 0 if shared else 64, null_kv, None, B, heads, n, m, o_e,
-                  n * inner, inner)
-    qn, kvn = q.cuda(), kv.cuda()
-    o_n = torch.zeros(B * n, inner, dtype=F16, device="cuda")
-    native.attention(qn, n * inner, inner, kvn, kvn[:, v_off:], m * ldkv, ldkv, 0 if shared else 64, null_kv.cuda(), None, B,
-                     heads, n, m, o_n, n * inner, inner)
-    assert torch.isfinite(o_n).all()
-    assert rel_l2(o_n, o_e) < 2e-3
 
 
 # ---------------------------------------------------------------------------------------------- DDPM step
