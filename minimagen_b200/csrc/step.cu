@@ -8,6 +8,10 @@
 //                                                                  (Imagen.py:323, diffusion_model.py:118-125, Imagen.py:361-370)
 // The per-image schedule gathers (helpers.extract) happen inside the kernels from the fp32 tables.
 // Products and sums are kept un-fused (__fmul_rn/__fadd_rn) so that the arithmetic matches torch's op-by-op rounding.
+// Steps 1 and 3 are written once (guided_x0, posterior_elem) and shared by the three-kernel form and the fused kernel.
+// The select of step 2 exists twice, and each is the other's test reference: quantile_kernel (one CTA per image, keys
+// streamed from global memory, any n) and the one inside step_epilogue_kernel (an 8-CTA cluster per image, keys held in
+// registers, n <= 196 608).  Both end in step_threshold.
 #include <cuda_runtime.h>
 #include <float.h>
 #include <stdint.h>
@@ -21,6 +25,43 @@ namespace mi {
 
 namespace {
 
+// Step 1 at element idx: eps = null + (cond - null) * w when eps_null is given, then x0 = a[t] * x_t - b[t] * eps.
+__device__ __forceinline__ float guided_x0(const float* x_t, const float* eps_cond, const float* eps_null,
+                                           float cond_scale, float a, float b, long long idx) {
+    float e = eps_cond[idx];
+    if (eps_null) {
+        const float nl = eps_null[idx];
+        e = __fadd_rn(nl, __fmul_rn(__fsub_rn(e, nl), cond_scale));
+    }
+    return __fsub_rn(__fmul_rn(a, x_t[idx]), __fmul_rn(b, e));
+}
+
+// The threshold from the two selected order statistics (bit patterns of |x0|): at::lerp in its vectorised CPU form,
+// base + coeff * (end - start) with weight < 0.5 ? (start, w) : (end, w - 1), then s.clamp_(min=min_s).
+__device__ __forceinline__ float step_threshold(uint32_t v_lo, uint32_t v_hi, float weight, float min_s) {
+    const float lo = __uint_as_float(v_lo), hi = __uint_as_float(v_hi);
+    const float diff = __fsub_rn(hi, lo);
+    const float s = (weight < 0.5f) ? fmaf(weight, diff, lo) : fmaf(__fsub_rn(weight, 1.0f), diff, hi);
+    return fmaxf(s, min_s);
+}
+
+// Step 3 at element idx: xs = clamp(x0, -s, s) / s, mean = c1 * xs + c2 * x_t, and out = mean + sig * noise.
+// kHist (the multistep form): mean += c3 * x0_hist, skipped where c3 == 0, and xs replaces x0_hist.
+// `out` may alias `x_t`: x_t[idx] is read before out[idx] is written.
+template <bool kHist>
+__device__ __forceinline__ void posterior_elem(float x0, float s, float c1, float c2, float c3, float sig,
+                                               const float* x_t, const float* __restrict__ noise,
+                                               float* __restrict__ x0_hist, float* out, long long idx) {
+    float xs = fminf(fmaxf(x0, -s), s);
+    xs = __fdiv_rn(xs, s);
+    float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[idx]));
+    if constexpr (kHist) {
+        if (c3 != 0.f) mean = __fadd_rn(mean, __fmul_rn(c3, x0_hist[idx]));
+        x0_hist[idx] = xs;
+    }
+    out[idx] = __fadd_rn(mean, __fmul_rn(sig, noise[idx]));
+}
+
 __global__ void __launch_bounds__(256)
 x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
           float cond_scale, const long long* __restrict__ t, const float* __restrict__ tab_recip,
@@ -32,13 +73,7 @@ x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, con
     if (i >= n_per_img) return;
     const long long idx = (long long)b * n_per_img + i;
     const long long tb = t[b];
-    const float a = tab_recip[tb], bb = tab_recipm1[tb];
-    float e = eps_cond[idx];
-    if (eps_null) {
-        const float nl = eps_null[idx];
-        e = __fadd_rn(nl, __fmul_rn(__fsub_rn(e, nl), cond_scale));
-    }
-    x0[idx] = __fsub_rn(__fmul_rn(a, x_t[idx]), __fmul_rn(bb, e));
+    x0[idx] = guided_x0(x_t, eps_cond, eps_null, cond_scale, tab_recip[tb], tab_recipm1[tb], idx);
 }
 
 // One CTA per image.  Exact k-th order statistics of |x| by 4 x 8-bit radix passes over the float bit patterns.
@@ -114,135 +149,11 @@ quantile_kernel(const float* __restrict__ x0, int n, int rank_lo, int rank_hi, f
         v_hi = sh_min[0];
         if (v_hi == 0xFFFFFFFFu) v_hi = v_lo;   // cannot happen for rank_hi < n
     }
-    if (tid == 0) {
-        const float lo = __uint_as_float(v_lo), hi = __uint_as_float(v_hi);
-        // at::lerp (vectorised CPU form): base + coeff * (end - start), weight < 0.5 ? (start, w) : (end, w - 1)
-        const float diff = __fsub_rn(hi, lo);
-        const float s = (weight < 0.5f) ? fmaf(weight, diff, lo) : fmaf(__fsub_rn(weight, 1.0f), diff, hi);
-        s_out[blockIdx.x] = fmaxf(s, min_s);   // s.clamp_(min=1.)
-    }
+    if (tid == 0) s_out[blockIdx.x] = step_threshold(v_lo, v_hi, weight, min_s);
 }
 
-// Cluster variant: 8 CTAs (one thread-block cluster) per image, every CTA keeps its n/8 keys in REGISTERS, so the image
-// is read from memory once instead of four to five times by a single SM; the per-pass 256-bin histograms are summed
-// across the cluster through distributed shared memory.  Same radix select, same result bits.
-constexpr int kSelCluster = 8, kSelPerThread = 24;
-
-__global__ void __cluster_dims__(kSelCluster, 1, 1) __launch_bounds__(kSelThreads)
-quantile_cluster_kernel(const float* __restrict__ x0, int n, int rank_lo, int rank_hi, float weight, float min_s,
-                        float* __restrict__ s_out) {
-    pdl_wait();
-    pdl_trigger();
-    namespace cg = cooperative_groups;
-    cg::cluster_group cluster = cg::this_cluster();
-    __shared__ unsigned hist[256];       // this CTA's histogram of the current pass (read remotely by the peers)
-    __shared__ unsigned ghist[256];      // cluster-wide histogram
-    __shared__ uint32_t sh_prefix, sh_k, sh_eq, sh_cta_min;
-    __shared__ uint32_t sh_min[32];
-    const int img = blockIdx.x / kSelCluster;
-    const unsigned rank = cluster.block_rank();
-    const int tid = threadIdx.x, lane = tid & 31;
-    const int chunk = (n + kSelCluster - 1) / kSelCluster;
-    const int beg = rank * chunk;
-    const int cnt = max(0, min(chunk, n - beg));
-    const float* x = x0 + (long long)img * n + beg;
-
-    uint32_t keys[kSelPerThread];
-#pragma unroll
-    for (int j = 0; j < kSelPerThread; ++j) {
-        const int i = tid + j * kSelThreads;
-        keys[j] = i < cnt ? absbits(x[i]) : 0xFFFFFFFFu;          // sentinel: never matches a prefix of a finite |x|
-    }
-    uint32_t prefix = 0, maskbits = 0, k = (uint32_t)rank_lo;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 24 - 8 * pass;
-        if (tid < 256) hist[tid] = 0;
-        __syncthreads();
-#pragma unroll
-        for (int j = 0; j < kSelPerThread; ++j) {
-            const bool live = (tid + j * kSelThreads < cnt) && ((keys[j] & maskbits) == prefix);
-            const unsigned bin = live ? ((keys[j] >> shift) & 0xFF) : 256u;
-            const unsigned peers = __match_any_sync(0xffffffffu, bin);
-            if (live && lane == (__ffs(peers) - 1)) atomicAdd(&hist[bin], __popc(peers));
-        }
-        cluster.sync();                                            // every CTA's histogram is complete
-        if (tid < 256) {
-            unsigned t = 0;
-#pragma unroll
-            for (int r = 0; r < kSelCluster; ++r) t += *cluster.map_shared_rank(&hist[tid], r);
-            ghist[tid] = t;
-        }
-        __syncthreads();
-        if (tid < 32) {
-            // digit select: lane owns bins [8*lane, 8*lane+8); warp scan of the lane totals, then a scan inside one lane
-            unsigned loc[8], tot = 0;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) { loc[e] = ghist[8 * lane + e]; tot += loc[e]; }
-            unsigned incl = tot;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += v;
-            }
-            const unsigned excl = incl - tot;
-            const bool mine = k >= excl && k < incl;               // exactly one lane (k < total count)
-            if (mine) {
-                unsigned cum = excl;
-                int d = 0;
-                for (; d < 8; ++d) {
-                    if (k < cum + loc[d]) break;
-                    cum += loc[d];
-                }
-                sh_prefix = prefix | ((uint32_t)(8 * lane + d) << shift);
-                sh_k = k - cum;
-                sh_eq = loc[d];
-            }
-        }
-        __syncthreads();
-        prefix = sh_prefix;
-        k = sh_k;
-        maskbits |= 0xFFu << shift;
-        cluster.sync();                                            // peers are done reading hist before it is re-zeroed
-    }
-    const uint32_t v_lo = prefix;
-    uint32_t v_hi = v_lo;
-    if (rank_hi > rank_lo && k + 1 >= sh_eq) {                      // uniform over the cluster (same k, same sh_eq)
-        uint32_t mn = 0xFFFFFFFFu;
-#pragma unroll
-        for (int j = 0; j < kSelPerThread; ++j)
-            if ((tid + j * kSelThreads < cnt) && keys[j] > v_lo && keys[j] < mn) mn = keys[j];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-        if (lane == 0) sh_min[tid >> 5] = mn;
-        __syncthreads();
-        if (tid < 32) {
-            mn = sh_min[tid];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-            if (tid == 0) sh_cta_min = mn;
-        }
-        cluster.sync();
-        if (rank == 0 && tid == 0) {
-            uint32_t m = 0xFFFFFFFFu;
-            for (int r = 0; r < kSelCluster; ++r) m = min(m, *cluster.map_shared_rank(&sh_cta_min, r));
-            sh_min[0] = m;
-        }
-        cluster.sync();                                            // peers keep their smem alive until rank 0 has read it
-        if (rank == 0 && tid == 0) {
-            v_hi = sh_min[0];
-            if (v_hi == 0xFFFFFFFFu) v_hi = v_lo;
-        }
-    }
-    if (rank == 0 && tid == 0) {
-        const float lo = __uint_as_float(v_lo), hi = __uint_as_float(v_hi);
-        const float diff = __fsub_rn(hi, lo);
-        const float s = (weight < 0.5f) ? fmaf(weight, diff, lo) : fmaf(__fsub_rn(weight, 1.0f), diff, hi);
-        s_out[img] = fmaxf(s, min_s);
-    }
-}
-
-// kHist (the multistep form, mi_step_epilogue_multistep): mean += c3[t] * x0_hist, skipped where c3[t] == 0, then the
-// clamped x0 replaces x0_hist.  The extra arguments come last so that the kHist = false instance is the plain kernel.
+// kHist: the multistep form (mi_step_epilogue_multistep) of posterior_elem.  The extra arguments come last so that the
+// kHist = false instance is the plain kernel.
 template <bool kHist>
 __global__ void __launch_bounds__(256)
 posterior_kernel(const float* __restrict__ x0, const float* x_t, const float* __restrict__ noise,
@@ -260,30 +171,24 @@ posterior_kernel(const float* __restrict__ x0, const float* x_t, const float* __
     const float sb = s[b];
     const float c1 = tab_c1[tb], c2 = tab_c2[tb];
     const float sig = (tb == 0) ? 0.f : tab_sigma[tb];   // nonzero_mask * exp(0.5 * log_var)
-    float xs = x0[idx];
-    xs = fminf(fmaxf(xs, -sb), sb);
-    xs = __fdiv_rn(xs, sb);
-    float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[idx]));
-    if constexpr (kHist) {
-        const float c3 = tab_c3[tb];
-        if (c3 != 0.f) mean = __fadd_rn(mean, __fmul_rn(c3, x0_hist[idx]));
-        x0_hist[idx] = xs;
-    }
-    out[idx] = __fadd_rn(mean, __fmul_rn(sig, noise[idx]));
+    const float c3 = kHist ? tab_c3[tb] : 0.f;
+    posterior_elem<kHist>(x0[idx], sb, c1, c2, c3, sig, x_t, noise, x0_hist, out, idx);
 }
 
 
 // ------------------------------------------------------------------------------------------------ fused step epilogue
 // The whole of Imagen._p_sample after the U-Net as ONE kernel (SURVEY 8b `mi_step_epilogue`): an 8-CTA cluster per image
-//   1. computes x0 = a[t] * x_t - b[t] * (null + (cond - null) * w) for its n/8 elements and KEEPS them in registers,
-//   2. runs the exact radix select of quantile_cluster_kernel on their |.| bit patterns (histograms summed over the cluster
-//      through distributed shared memory; every CTA derives the same (v_lo, v_hi) and therefore the same threshold s),
-//   3. clamps / divides the register-resident x0, forms the posterior mean with x_t (re-read, L2-hot) and adds
-//      sigma[t] * noise.
-// Versus the three-kernel form the x0 tensor never exists in memory (one write + two reads of the image less) and two
-// launches disappear from the step.  `out` may alias `x_t` (in-place update of the sampling state): every element is
-// read and written by the same thread.  Arithmetic is op-for-op that of x0_kernel / posterior_kernel (bit-identical).
+//   1. computes guided_x0 for its n/8 elements and KEEPS them in registers (kSelPerThread per thread),
+//   2. runs the exact radix select on their |.| bit patterns: the passes of quantile_kernel, with each CTA's 256-bin
+//      histogram summed over the cluster through distributed shared memory; every CTA derives the same (v_lo, v_hi)
+//      and therefore the same threshold s,
+//   3. applies posterior_elem to the register-resident x0, re-reading x_t (L2-hot) and the noise.
+// The image is read from memory once instead of once per radix pass, the x0 tensor never exists in memory (one write +
+// two reads of the image less than the three-kernel form) and two launches disappear from the step.  `out` may alias
+// `x_t` (in-place update of the sampling state): every element is read and written by the same thread.
 // kHist: the multistep form, as posterior_kernel<true>; the history is only touched in the final register loop.
+constexpr int kSelCluster = 8, kSelPerThread = 24;
+
 template <bool kHist>
 __global__ void __cluster_dims__(kSelCluster, 1, 1) __launch_bounds__(kSelThreads)
 step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
@@ -297,9 +202,9 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
     pdl_trigger();
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
-    __shared__ unsigned hist[256];
-    __shared__ unsigned ghist[256];
-    __shared__ uint32_t sh_prefix, sh_k, sh_eq, sh_cta_min;
+    __shared__ unsigned hist[256];       // this CTA's histogram of the current pass (read remotely by the peers)
+    __shared__ unsigned ghist[256];      // cluster-wide histogram
+    __shared__ uint32_t sh_prefix, sh_k, sh_eq, sh_cta_min, sh_maskbits;
     __shared__ uint32_t sh_min[32];
     const int img = blockIdx.x / kSelCluster;
     const unsigned rank = cluster.block_rank();
@@ -315,40 +220,27 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
 #pragma unroll
     for (int j = 0; j < kSelPerThread; ++j) {
         const int i = tid + j * kSelThreads;
-        float v = 0.f;
-        if (i < cnt) {
-            float e = eps_cond[base + i];
-            if (eps_null) {
-                const float nl = eps_null[base + i];
-                e = __fadd_rn(nl, __fmul_rn(__fsub_rn(e, nl), cond_scale));
-            }
-            v = __fsub_rn(__fmul_rn(ca, x_t[base + i]), __fmul_rn(cb, e));
-        }
-        x0v[j] = v;
+        x0v[j] = i < cnt ? guided_x0(x_t, eps_cond, eps_null, cond_scale, ca, cb, base + i) : 0.f;
     }
-    uint32_t prefix = 0, maskbits = 0, k = (uint32_t)rank_lo;
-    // kHist reads each pass's mask through shared memory.  With the mask a compile-time constant of the unrolled passes,
-    // ptxas precomputes the next pass's masked keys and keeps them alongside x0v: at 64 registers that spills (36 bytes
-    // in this instance).  Written by thread 0 after the barrier that ends the pass's reads.
-    __shared__ uint32_t sh_maskbits;
-    if constexpr (kHist) {
-        if (tid == 0) sh_maskbits = 0;
-    }
+    // Each pass reads its mask from shared memory.  With the mask a compile-time constant of the unrolled passes, ptxas
+    // precomputes the next pass's masked keys next to x0v, and at 64 registers that spills.  Thread 0 updates it after
+    // the barrier that ends the pass's reads.
+    uint32_t prefix = 0, k = (uint32_t)rank_lo;
+    if (tid == 0) sh_maskbits = 0;
     for (int pass = 0; pass < 4; ++pass) {
         const int shift = 24 - 8 * pass;
         if (tid < 256) hist[tid] = 0;
         __syncthreads();
-        uint32_t mb = maskbits;
-        if constexpr (kHist) mb = sh_maskbits;
+        const uint32_t maskbits = sh_maskbits;
 #pragma unroll
         for (int j = 0; j < kSelPerThread; ++j) {
             const uint32_t key = absbits(x0v[j]);
-            const bool live = (tid + j * kSelThreads < cnt) && ((key & mb) == prefix);
+            const bool live = (tid + j * kSelThreads < cnt) && ((key & maskbits) == prefix);
             const unsigned bin = live ? ((key >> shift) & 0xFF) : 256u;
             const unsigned peers = __match_any_sync(0xffffffffu, bin);
             if (live && lane == (__ffs(peers) - 1)) atomicAdd(&hist[bin], __popc(peers));
         }
-        cluster.sync();
+        cluster.sync();                                            // every CTA's histogram is complete
         if (tid < 256) {
             unsigned tt = 0;
 #pragma unroll
@@ -357,6 +249,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
         }
         __syncthreads();
         if (tid < 32) {
+            // digit select: lane owns bins [8*lane, 8*lane+8); warp scan of the lane totals, then a scan inside one lane
             unsigned loc[8], tot = 0;
 #pragma unroll
             for (int e = 0; e < 8; ++e) { loc[e] = ghist[8 * lane + e]; tot += loc[e]; }
@@ -367,7 +260,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
                 if (lane >= o) incl += v;
             }
             const unsigned excl = incl - tot;
-            if (k >= excl && k < incl) {
+            if (k >= excl && k < incl) {                           // exactly one lane (k < total count)
                 unsigned cum = excl;
                 int d = 0;
                 for (; d < 8; ++d) {
@@ -382,15 +275,12 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
         __syncthreads();
         prefix = sh_prefix;
         k = sh_k;
-        maskbits |= 0xFFu << shift;
-        if constexpr (kHist) {
-            if (tid == 0) sh_maskbits = maskbits;
-        }
-        cluster.sync();
+        if (tid == 0) sh_maskbits = maskbits | (0xFFu << shift);
+        cluster.sync();                                            // peers are done reading hist before it is re-zeroed
     }
     const uint32_t v_lo = prefix;
     uint32_t v_hi = v_lo;
-    if (rank_hi > rank_lo && k + 1 >= sh_eq) {                      // uniform over the cluster
+    if (rank_hi > rank_lo && k + 1 >= sh_eq) {                      // uniform over the cluster (same k, same sh_eq)
         uint32_t mn = 0xFFFFFFFFu;
 #pragma unroll
         for (int j = 0; j < kSelPerThread; ++j) {
@@ -417,42 +307,16 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
         v_hi = sh_min[0];
         if (v_hi == 0xFFFFFFFFu) v_hi = v_lo;
     }
-    const float lo = __uint_as_float(v_lo), hi = __uint_as_float(v_hi);
-    const float diff = __fsub_rn(hi, lo);
-    float sb = (weight < 0.5f) ? fmaf(weight, diff, lo) : fmaf(__fsub_rn(weight, 1.0f), diff, hi);
-    sb = fmaxf(sb, min_s);
+    const float sb = step_threshold(v_lo, v_hi, weight, min_s);
     if (s_out && rank == 0 && tid == 0) s_out[img] = sb;
 
     const float c1 = tab_c1[tb], c2 = tab_c2[tb];
     const float sig = (tb == 0) ? 0.f : tab_sigma[tb];
-    if constexpr (kHist) {
-        const float c3 = tab_c3[tb];
-        if (c3 != 0.f) {
-#pragma unroll
-            for (int j = 0; j < kSelPerThread; ++j) {
-                const int i = tid + j * kSelThreads;
-                if (i < cnt) {
-                    float xs = fminf(fmaxf(x0v[j], -sb), sb);
-                    xs = __fdiv_rn(xs, sb);
-                    float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[base + i]));
-                    mean = __fadd_rn(mean, __fmul_rn(c3, x0_hist[base + i]));
-                    x0_hist[base + i] = xs;
-                    out[base + i] = __fadd_rn(mean, __fmul_rn(sig, noise[base + i]));
-                }
-            }
-            return;
-        }
-    }
+    const float c3 = kHist ? tab_c3[tb] : 0.f;
 #pragma unroll
     for (int j = 0; j < kSelPerThread; ++j) {
         const int i = tid + j * kSelThreads;
-        if (i < cnt) {
-            float xs = fminf(fmaxf(x0v[j], -sb), sb);
-            xs = __fdiv_rn(xs, sb);
-            const float mean = __fadd_rn(__fmul_rn(c1, xs), __fmul_rn(c2, x_t[base + i]));
-            if constexpr (kHist) x0_hist[base + i] = xs;
-            out[base + i] = __fadd_rn(mean, __fmul_rn(sig, noise[base + i]));
-        }
+        if (i < cnt) posterior_elem<kHist>(x0v[j], sb, c1, c2, c3, sig, x_t, noise, x0_hist, out, base + i);
     }
 }
 
@@ -611,11 +475,7 @@ int step_x0(const float* x_t, const float* eps_cond, const float* eps_null, floa
 int step_quantile(const float* x0, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
                   float* s_out, cudaStream_t st) {
     if (rank_lo < 0 || rank_hi < rank_lo || rank_hi >= n_per_img) return -1;
-    if ((n_per_img + kSelCluster - 1) / kSelCluster <= kSelThreads * kSelPerThread)
-        launch_k(quantile_cluster_kernel, B * kSelCluster, kSelThreads, 0, st, x0, n_per_img, rank_lo, rank_hi, weight, min_s,
-                                                                        s_out);
-    else
-        launch_k(quantile_kernel, B, kSelThreads, 0, st, x0, n_per_img, rank_lo, rank_hi, weight, min_s, s_out);
+    launch_k(quantile_kernel, B, kSelThreads, 0, st, x0, n_per_img, rank_lo, rank_hi, weight, min_s, s_out);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -2,7 +2,7 @@
 
 Diagnostics for kernel tuning, not a bench value: CUDA events around `reps` back-to-back launches, rotating over enough
 buffer sets that the working set exceeds the 50 MB L2 ("cold") or re-using one set ("warm").
-Usage: python tools/bench_ops.py [gn ln linear quantile attn cast final stem]
+Usage: python tools/bench_ops.py [gn ln linear step attn cast final stem]
        python tools/bench_ops.py conv [block_n ...]   (implicit-GEMM convs; block_n 0 = the library's choice; ends with
                                                        the k-block sweep and its per-tile cost fit)
 """
@@ -102,15 +102,25 @@ def bench_linear(ops):
         report(f"linear_f32 M={M} K={K} N={Nn}", timeit(fns), timeit(fns[:1]), nbytes)
 
 
-def bench_quantile(ops):
+def bench_step(ops):
+    """The two selects sampling runs: the fused step epilogue at the cfg-3 step (cond_scale 1: no eps_null), and the
+    single-CTA step_quantile of the three-kernel form that 3 x 1024 x 1024 images (cfg 5, batch 2) fall back to."""
+    from minimagen_b200.Imagen import quantile_rank
     B, n = 32, 3 * 256 * 256
+    x, eps, noise, out = (torch.randn(B, n, device=dev) for _ in range(4))
+    t = torch.randint(0, 1000, (B,), device=dev)
+    tab_a, tab_b, c1, c2, sigma = (torch.rand(1000, device=dev) for _ in range(5))
+    lo, hi, w = quantile_rank(n, 0.9)
+    f = lambda: ops.step_epilogue(x, eps, None, 1.0, t, tab_a, tab_b, c1, c2, sigma, noise, B, n, lo, hi, w, 1.0, out)
+    ms = timeit([f], reps=500)                                              # ~150 us a launch: a window of tens of ms
+    report(f"step_epilogue B={B} n={n}", ms, ms, B * n * 4 * 4)          # x_t, eps, noise in; out
+    B, n = 2, 3 * 1024 * 1024
     x = torch.randn(B, n, device=dev)
     s = torch.empty(B, device=dev)
-    pos = 0.95 * (n - 1)
-    lo = int(pos)
-    f = lambda: ops.step_quantile(x, B, n, lo, lo + 1, pos - lo, 1.0, s)
+    lo, hi, w = quantile_rank(n, 0.9)
+    f = lambda: ops.step_quantile(x, B, n, lo, hi, w, 1.0, s)
     ms = timeit([f])
-    report("step_quantile B=32 n=196608", ms, ms, B * n * 4)
+    report(f"step_quantile B={B} n={n}", ms, ms, B * n * 4)
 
 
 def bench_attn(ops):
@@ -284,12 +294,12 @@ def bench_conv_sweep(ops, hints, num_sms):
 def main():
     _native.load()
     ops = ops_mod.get_ops()
-    which = sys.argv[1:] or ["gn", "ln", "linear", "quantile", "attn", "cast", "final", "stem"]
+    which = sys.argv[1:] or ["gn", "ln", "linear", "step", "attn", "cast", "final", "stem"]
     if which[0] == "conv":           # conv [block_n ...]
         with torch.no_grad():
             bench_conv(ops, tuple(int(h) for h in which[1:]) or (0,))
         return
-    table = {"gn": bench_gn, "ln": bench_ln, "linear": bench_linear, "quantile": bench_quantile, "attn": bench_attn,
+    table = {"gn": bench_gn, "ln": bench_ln, "linear": bench_linear, "step": bench_step, "attn": bench_attn,
              "cast": bench_cast, "final": bench_final, "stem": bench_stem}
     with torch.no_grad():
         for w in which:
