@@ -466,4 +466,5 @@ class EmuOps:
 
     def upsample2x_bwd(self, dy, B, H, W, C, dx):
         self._log("upsample2x_bwd")
-        dx.reshape(B, H, W, C).copy_(dy.reshape(B, H, 2, W, 2, C).sum(dim=(2, 4)))
+        q = dy.reshape(B, H, 2, W, 2, C)
+        dx.reshape(B, H, W, C).copy_((q[:, :, 0, :, 0] + q[:, :, 0, :, 1]) + (q[:, :, 1, :, 0] + q[:, :, 1, :, 1]))

@@ -1,4 +1,5 @@
-"""TEST INFRASTRUCTURE ONLY: float64 references of the token-side kernels with elementwise error bounds.
+"""TEST INFRASTRUCTURE ONLY: float64 references of the token-side kernels and of the image-side training kernels
+(GroupNorm/SiLU backward, convolution weight and data gradients, upsample backward) with elementwise error bounds.
 
 Every reference takes the operands exactly as the kernel reads them (fp16-rounded where the kernel reads fp16, the null
 key/value included), computes in float64 on the operands' device, and returns (reference, bound): |kernel - reference| <=
@@ -351,3 +352,188 @@ def softmax_bwd_ref(P, dP):
     dot = (P64 * d64).sum(dim=-1, keepdim=True)
     twin = P64 * (d64.abs() + (P64 * d64).abs().sum(dim=-1, keepdim=True))
     return P64 * (d64 - dot), 2 * (L + 4) * U32 * twin + ETA32
+
+
+# ---------------------------------------------------------------------------------------------- GroupNorm/FiLM/SiLU backward
+def gn_bwd_splits(B, HW, C, sms):
+    """Pixel splits Z of gn_bwd_sums_kernel (csrc/backward.cu, gn_silu_bwd): about 8 blocks per SM over the (C/32, B, Z)
+    grid, at most one split per 64 pixels."""
+    blocks_xy = -(-C // 32) * B
+    return max(min(-(-8 * sms // blocks_xy), HW // 64), 1)
+
+
+def gn_bwd_acc_len(B, HW, C, sms):
+    """Summation length behind one pixel sum A[b][c] of gn_bwd_sums_kernel: a thread sums every 8th pixel of its chunk
+    (chunk = ceil(HW / Z)), the 8 partials are added, then one atomicAdd per split onto the zeroed A."""
+    Z = gn_bwd_splits(B, HW, C, sms)
+    return -(-(-(-HW // Z)) // 8) + 8 + Z
+
+
+def gn_silu_bwd_ref(x, dy, gamma, beta, ss, groups, eps, dgamma0, dbeta0, acc_len):
+    """mi_gn_silu_bwd: the gradients of y = SiLU(v), v = (xhat gamma + beta) (scale + 1) + shift, xhat the GroupNorm of x
+    over (pixels, Cg = C / groups channels) per image.  x, dy [B, HW, C] fp32; ss [B, 2C] = [scale | shift] (a strided view
+    is fine) or None.  Returns ((dx, bound), (dgamma, bound), (dbeta, bound), (dscale, bound), (dshift, bound)); dgamma /
+    dbeta accumulate onto dgamma0 / dbeta0.
+
+    With sc = scale + 1, dv = dy silu'(v), A1 = sum_p dv, A2 = sum_p dv xhat (per image and channel), N = Cg HW:
+        dgamma = dgamma0 + sum_b sc A2,  dbeta = dbeta0 + sum_b sc A1,  dscale = gamma A2 + beta A1,  dshift = A1,
+        m1 = sum_{c in g} gamma sc A1 / N,  m2 = sum_{c in g} gamma sc A2 / N,  dx = rstd (gamma sc dv - m1 - xhat m2).
+    Kernel rounding, first order:
+      * xhat: the fp32 mean (off by U32 |mean|), the difference, the fp32 rstd and the product give
+            |d xhat| <= 3 U32 e,   e = rstd (|mean| + |x - mean|):  the cancellation term, e / |xhat| grows with |mean| / std
+            (and with rstd ~ eps^-1/2 on a near-constant group);
+      * v: xhat's error and four roundings (sc = ss + 1 included):  |d v| <= 3 U32 |gamma sc| e + 4 U32 V,
+            V = |gamma sc xhat| + |beta sc| + |shift|;
+      * dv: silu' has slope <= 0.5; the fp32 silu' (expf, a division, 1 - sigmoid times v) is off by <= 8 U32 (1 + |v|);
+            the product rounds once:  Ddv = U32 |dy| (10 (1 + V) + 2 |gamma sc| e);
+      * A1 / A2: acc_len roundings (gn_bwd_acc_len) of the pixel sums plus the summed input errors:
+            dA1 = acc_len U32 T1 + sum_p Ddv,  dA2 = acc_len U32 T2 + sum_p (Ddv |xhat| + 3 U32 |dv| e),
+            T1 = sum_p |dv|,  T2 = sum_p |dv xhat|;
+      * dgamma / dbeta: B atomics onto the caller's value and the product sc A:  (B + 2) U32 (sum_b |sc| T + |d0|);
+      * m1 / m2: a Cg-term shared-memory sum, the products gamma sc A and the multiply by 1 / N:  (Cg + 4) U32 M1t plus
+            sum_c |gamma sc| dA / N, with M1t = sum_{c in g} |gamma sc| T1 / N (M2t likewise with T2);
+      * dx: rstd (|gamma sc| Ddv + dm1 + |xhat| dm2 + 3 U32 e M2t + 8 U32 (|gamma sc dv| + M1t + |xhat| M2t)) -- the
+            errors of the three terms, the difference, the products and rstd's rounding;
+    every bound doubled for second-order terms."""
+    x64, d = _d(x), _d(dy)
+    B, HW, C = x64.shape
+    Cg = C // groups
+    N = Cg * HW
+    dev = x64.device
+    xg = x64.reshape(B, HW, groups, Cg)
+    mu = xg.mean(dim=(1, 3))                                                       # [B, G]
+    rstd = 1.0 / torch.sqrt(((xg - mu[:, None, :, None]) ** 2).mean(dim=(1, 3)) + eps)
+    mu_c = mu.repeat_interleave(Cg, dim=1)[:, None, :]                             # [B, 1, C]
+    rs_c = rstd.repeat_interleave(Cg, dim=1)[:, None, :]
+    g64, b64 = _d(gamma).to(dev), _d(beta).to(dev)
+    if ss is not None:
+        s64 = _d(ss).to(dev)
+        sc, sh = s64[:, :C] + 1.0, s64[:, C:2 * C]
+    else:
+        sc, sh = torch.ones(B, C, dtype=F64, device=dev), torch.zeros(B, C, dtype=F64, device=dev)
+    xh = (x64 - mu_c) * rs_c
+    v = (xh * g64 + b64) * sc[:, None] + sh[:, None]
+    sg = torch.sigmoid(v)
+    dv = d * (sg * (1 + v * (1 - sg)))
+    del sg
+    A1, A2 = dv.sum(dim=1), (dv * xh).sum(dim=1)                                   # [B, C]
+    gs = (g64 * sc).abs()
+    grp = lambda t: t.reshape(B, groups, Cg).sum(dim=2).repeat_interleave(Cg, dim=1)     # group sum, spread over channels
+    m1, m2 = grp(g64 * sc * A1) / N, grp(g64 * sc * A2) / N
+    dx = rs_c * (g64 * sc[:, None] * dv - m1[:, None] - xh * m2[:, None])
+    # bounds
+    e = rs_c * (mu_c.abs() + (x64 - mu_c).abs())
+    ax = xh.abs()
+    del xh, v
+    gs_ = gs[:, None]
+    V = gs_ * ax + (b64 * sc).abs()[:, None] + sh.abs()[:, None]
+    Ddv = U32 * d.abs() * (10 * (1 + V) + 2 * gs_ * e)
+    del V
+    adv = dv.abs()
+    T1, T2 = adv.sum(dim=1), (adv * ax).sum(dim=1)
+    dA1 = acc_len * U32 * T1 + Ddv.sum(dim=1)
+    dA2 = acc_len * U32 * T2 + (Ddv * ax + 3 * U32 * adv * e).sum(dim=1)
+    M1t, M2t = grp(gs * T1) / N, grp(gs * T2) / N
+    dm1 = grp(gs * dA1) / N + (Cg + 4) * U32 * M1t
+    dm2 = grp(gs * dA2) / N + (Cg + 4) * U32 * M2t
+    M1t, M2t, dm1, dm2 = M1t[:, None], M2t[:, None], dm1[:, None], dm2[:, None]
+    bdx = 2 * rs_c * (gs_ * Ddv + dm1 + ax * dm2 + 3 * U32 * e * M2t + 8 * U32 * (gs_ * adv + M1t + ax * M2t))
+    dg0, db0 = _d(dgamma0).to(dev), _d(dbeta0).to(dev)
+    dg = dg0 + (sc * A2).sum(dim=0)
+    db = db0 + (sc * A1).sum(dim=0)
+    bdg = 2 * ((sc.abs() * dA2).sum(dim=0) + (B + 2) * U32 * ((sc.abs() * T2).sum(dim=0) + dg0.abs()))
+    bdb = 2 * ((sc.abs() * dA1).sum(dim=0) + (B + 2) * U32 * ((sc.abs() * T1).sum(dim=0) + db0.abs()))
+    dscale = g64 * A2 + b64 * A1
+    bds = 2 * (g64.abs() * dA2 + b64.abs() * dA1 + 2 * U32 * (g64.abs() * T2 + b64.abs() * T1))
+    return (dx, bdx), (dg, bdg), (db, bdb), (dscale, bds), (A1, 2 * dA1)
+
+
+# ---------------------------------------------------------------------------------------------- convolution gradients
+def wgrad_f32_plan(B, Ho, Wo, Cin, Cout, kh, kw, sms):
+    """(pixels per block, pixel splits) of conv_wgrad_kernel (csrc/backward.cu, conv2d_wgrad_f32): the flat variant
+    (C_in < 32 and more than one tap) tiles (C_out, C_in x taps) by 32 x 32, the tiled one (C_out, C_in) per tap; both aim
+    at 16 blocks per SM, with at least 128 pixels per split, rounded to 32-pixel stages."""
+    total = B * Ho * Wo
+    taps = kh * kw
+    flat = Cin < 32 and taps > 1
+    tiles = -(-Cout // 32) * -(-(Cin * taps if flat else Cin) // 32)
+    work = tiles if flat else tiles * taps
+    splits = min(-(-16 * sms // work), -(-total // 128))
+    splits = min(max(splits, 1), 65535)
+    ppb = -(-(-(-total // splits)) // 32) * 32
+    return ppb, -(-total // ppb)
+
+
+def wgrad_f32_acc_len(B, Ho, Wo, Cin, Cout, kh, kw, sms):
+    """Summation length behind one dW element of conv2d_wgrad_f32: an fma per pixel of the block's range, then one atomicAdd
+    per split onto the zeroed dW."""
+    ppb, splits = wgrad_f32_plan(B, Ho, Wo, Cin, Cout, kh, kw, sms)
+    return ppb + splits
+
+
+def wgrad_tc_plan(B, Ho, Wo, Cin, Cout, k, sms):
+    """(8 x 8 pixel boxes per CTA, splits) of conv_wgrad_tc (csrc/wgrad_tc.cu, wgrad_plan): about two CTAs per SM over
+    (C_out / 128) x (C_in / N) x taps tile groups, N = 128 when C_in % 128 == 0 else 64."""
+    nb = 2 if Cin % 128 == 0 else 1
+    total = B * (Ho // 8) * (Wo // 8)
+    groups = (Cout // 128) * (Cin // (nb * 64)) * k * k
+    splits = min(max(-(-2 * sms // groups), 1), total, 65535)
+    per = -(-total // splits)
+    return per, -(-total // per)
+
+
+def wgrad_tc_acc_len(B, Ho, Wo, Cin, Cout, k, sms):
+    """Summation length behind one dW element of conv_wgrad_tc: 64 pixels per box in the CTA's wgmma accumulators, then
+    wgrad_reduce_kernel's sum over the splits."""
+    per, splits = wgrad_tc_plan(B, Ho, Wo, Cin, Cout, k, sms)
+    return 64 * per + splits
+
+
+def _nchw(t):
+    return _d(t).permute(0, 3, 1, 2)
+
+
+def conv_wgrad_ref(dy, x, stride, pad, kh, kw, acc_len):
+    """dW[co][ci][r][s] = sum over output pixels (b, h, w) of dy[b, h, w, co] x[b, stride h + r - pad, stride w + s - pad, ci]
+    (zero outside the image): conv2d_wgrad_f32 and mi_conv2d_wgrad_f16.  dy [B, Ho, Wo, C_out] and x [B, Hi, Wi, C_in] NHWC
+    as the kernel reads them (fp16 for the tensor-core kernel).  Returns (dW OIHW, bound).
+
+    Bound 3 acc_len U32 twin, twin = the same sum over |dy| |x|; acc_len from wgrad_f32_acc_len / wgrad_tc_acc_len.  The fp32
+    kernel is an fma chain per split plus one atomicAdd per split: acc_len roundings of a partial sum dominated by twin, so
+    2 acc_len U32 twin.  On the tensor cores the products of fp16 operands are exact in fp32, but a wgmma k-group adds 16
+    products to the accumulator by aligning them to the largest exponent and truncating, not rounding to nearest: each of
+    the 17 terms loses less than one unit of 2^-23 relative to the group's largest term, and the normalised sum is
+    truncated once more.  That is <= 17 x 2 U32 x (|accumulator| + sum |products|) <= 34 U32 twin per 16 products,
+    2.125 U32 twin per product; the fp32 split reduction adds U32 twin per split.  Hence c = 3 for both kernels."""
+    g = torch.nn.grad.conv2d_weight
+    Co, Ci = dy.shape[-1], x.shape[-1]
+    shape = (Co, Ci, kh, kw)
+    ref = g(_nchw(x), shape, _nchw(dy), stride=stride, padding=pad)
+    twin = g(_nchw(x).abs(), shape, _nchw(dy).abs(), stride=stride, padding=pad)
+    return ref, 3 * acc_len * U32 * twin
+
+
+def conv_dgrad_ref(dy, w, stride, pad, Hi, Wi):
+    """dx[b, h, w, ci] = sum over taps (r, s) and co of dy[b, (h + pad - r) / stride, (w + pad - s) / stride, co] w[co][ci][r][s]
+    where the division is exact and in range: conv2d_dgrad_f32 (general and small-C_out kernels, fp32 operands) and the
+    tensor-core data gradients of Conv2dFn (fp16 dy and fp16 packed weights: pass those values).  dy [B, Ho, Wo, C_out]
+    NHWC, w (C_out, C_in, kh, kw).  Returns (dx NHWC, bound).
+
+    Every kernel sums at most n = taps x C_out products into one fp32 accumulator: an fma chain on the CUDA cores
+    (2 n U32 twin), the wgmma K loop of the implicit GEMM on the tensor cores (see conv_wgrad_ref: 2.125 n U32 twin):
+        3 n U32 twin + U32 |dx|,   twin = the same sum over |dy| |w|."""
+    B, Ci = dy.shape[0], w.shape[1]
+    Co, kh, kw = w.shape[0], w.shape[2], w.shape[3]
+    g = torch.nn.grad.conv2d_input
+    w64 = _d(w).to(dy.device)
+    ref = g((B, Ci, Hi, Wi), w64, _nchw(dy), stride=stride, padding=pad).permute(0, 2, 3, 1)
+    twin = g((B, Ci, Hi, Wi), w64.abs(), _nchw(dy).abs(), stride=stride, padding=pad).permute(0, 2, 3, 1)
+    return ref, 3 * kh * kw * Co * U32 * twin + U32 * ref.abs()
+
+
+def upsample2x_bwd_ref(dy):
+    """mi_upsample2x_bwd: dx[b, h, w] = (dy[2h, 2w] + dy[2h, 2w + 1]) + (dy[2h + 1, 2w] + dy[2h + 1, 2w + 1]) in fp32, in
+    this order: a fixed-order sum, so the kernel must match it bit for bit.  dy [B, 2H, 2W, C] fp32."""
+    B, H2, W2, C = dy.shape
+    q = dy.float().reshape(B, H2 // 2, 2, W2 // 2, 2, C)
+    return (q[:, :, 0, :, 0] + q[:, :, 0, :, 1]) + (q[:, :, 1, :, 0] + q[:, :, 1, :, 1])

@@ -269,3 +269,181 @@ def test_rel_l2_catches_uniform_errors():
     check_rel_l2(view(o), ref, 2e-3, "attention (emulation)")
     with pytest.raises(AssertionError):
         check_rel_l2(view(o).float() * 1.01, ref, 2e-3, "planted: attention 1% error over the whole output")
+    # fp32 data gradient of a 3x3 conv over 128 output channels computed from fp16-rounded dy
+    B, Ho, Wo, Co, Ci = 2, 16, 16, 128, 32
+    dy, w = torch.randn(B, Ho, Wo, Co, generator=g), torch.randn(Co, Ci, 3, 3, generator=g) * 0.05
+    ref, bound = R.conv_dgrad_ref(dy, w, 1, 1, Ho, Wo)
+    dx = torch.zeros(B, Ho, Wo, Ci)
+    EMU.conv_dgrad(dy, B, Ho, Wo, Co, w, Ci, 3, 3, 1, 1, dx, Ho, Wo)
+    check_rel_l2(dx, ref, 2e-5, "conv_dgrad (emulation)")
+    d = torch.zeros(B, Ho, Wo, Ci)
+    EMU.conv_dgrad(dy.half().float(), B, Ho, Wo, Co, w, Ci, 3, 3, 1, 1, d, Ho, Wo)
+    check(d, ref, bound, "conv_dgrad with fp16-rounded dy (inside the elementwise bound)")
+    with pytest.raises(AssertionError):
+        check_rel_l2(d, ref, 2e-5, "planted: conv_dgrad with fp16-rounded dy")
+
+
+# ---------------------------------------------------------------------------------------------- GroupNorm/FiLM/SiLU backward
+def _gn_case():
+    B, H, W, C, G, eps = 2, 24, 20, 48, 8, 1e-5                  # Cg = 6: groups straddle the kernel's channel quads
+    g = _g(12)
+    x = torch.randn(B, H * W, C, generator=g) * 2 + 0.5
+    x[0, :, 12:18] = 2.5 + 1e-4 * torch.randn(H * W, 6, generator=g)      # image 0, group 2: near-constant (var << eps)
+    x[1, :, 30:36] = 100.0 + torch.randn(H * W, 6, generator=g)          # image 1, group 5: |mean| / std ~ 100
+    dy = torch.randn(B, H * W, C, generator=g)
+    gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
+    ss = torch.randn(B, 2 * C, generator=g) * 0.3
+    dg0, db0 = torch.randn(C, generator=g), torch.randn(C, generator=g)
+    xd = x.double().reshape(B, H * W, G, C // G)
+    sums = torch.stack((xd.sum(dim=(1, 3)), (xd * xd).sum(dim=(1, 3))), dim=-1)          # [B, G, 2], as gn_stats makes them
+    return B, H * W, C, G, eps, x, dy, gamma, beta, ss, dg0, db0, sums
+
+
+def _gn_bwd_fp32(x, dy, sums, gamma, beta, ss, G, eps, dg0, db0, Z, defect=None):
+    """The three passes of gn_silu_bwd (csrc/backward.cu) restated in fp32 torch, Z pixel splits; `defect` plants one
+    subtle mistake.  Returns dx, dgamma, dbeta, dscale, dshift."""
+    B, HW, C = x.shape
+    Cg, n = C // G, (C // G) * HW
+    m = sums[..., 0] / n
+    var = (sums[..., 1] / n - m * m).clamp(min=0)
+    rstd = 1.0 / torch.sqrt(var + eps)
+    if defect == "eps ignored":                                             # on the near-constant group (image 0, group 2)
+        rstd[0, 2] = 1.0 / torch.sqrt(var[0, 2])
+    mean_c = m.float().repeat_interleave(Cg, dim=1)[:, None]
+    rstd_c = rstd.float().repeat_interleave(Cg, dim=1)[:, None]
+    sc, sh = (ss[:, None, :C] + 1.0), ss[:, None, C:]
+    xn = (x - mean_c) * rstd_c
+    v = (xn * gamma + beta) * sc + sh
+    if defect == "silu' before FiLM":                                       # in channel 7
+        v[..., 7] = xn[..., 7] * gamma[7] + beta[7]
+    sg = torch.sigmoid(v)
+    dv = dy * (sg * (1.0 + v * (1.0 - sg)))
+    chunk = -(-HW // Z)
+    A1 = sum(dv[:, z * chunk:(z + 1) * chunk].sum(dim=1) for z in range(Z))
+    A2 = sum((dv * xn)[:, z * chunk:(z + 1) * chunk].sum(dim=1) for z in range(Z))
+    if defect == "split missing":                                           # the second split of (b, c) = (1, 20)
+        A1[1, 20] -= dv[1, chunk:2 * chunk, 20].sum()
+        A2[1, 20] -= (dv * xn)[1, chunk:2 * chunk, 20].sum()
+    sc, sh = sc[:, 0], sh[:, 0]
+    dscale, dshift = gamma * A2 + beta * A1, A1.clone()
+    if defect == "dss swapped":                                             # in image 1
+        dscale[1], dshift[1] = A1[1], gamma * A2[1] + beta * A1[1]
+    dg, db = dg0 + (sc * A2).sum(dim=0), db0 + (sc * A1).sum(dim=0)
+    grp = lambda t: t.reshape(B, G, Cg).sum(dim=2) / n
+    m1, m2 = grp(gamma * sc * A1), grp(gamma * sc * A2)
+    if defect == "neighbour's m1":                                          # image 1, group 3 takes group 4's m1
+        m1[1, 3] = m1[1, 4]
+    m1c, m2c = m1.repeat_interleave(Cg, dim=1)[:, None], m2.repeat_interleave(Cg, dim=1)[:, None]
+    dx = rstd_c * ((gamma * sc)[:, None] * dv - m1c - xn * m2c)
+    return dx, dg, db, dscale, dshift
+
+
+GN_OUTS = ("dx", "dgamma", "dbeta", "dscale", "dshift")
+
+
+def test_gn_silu_bwd_bound():
+    B, HW, C, G, eps, x, dy, gamma, beta, ss, dg0, db0, sums = _gn_case()
+    Z = R.gn_bwd_splits(B, HW, C, 132)
+    assert Z > 1
+    refs = R.gn_silu_bwd_ref(x, dy, gamma, beta, ss, G, eps, dg0, db0, R.gn_bwd_acc_len(B, HW, C, 132))
+    # the emulation (float32 autograd through F.group_norm); the near-constant group is left out of the aggregate: its
+    # elementwise bound is large by nature (rstd ~ eps^-1/2 magnifies the fp32 mean's rounding)
+    dx, dg, db, dss = torch.zeros(B, HW, C), dg0.clone(), db0.clone(), torch.zeros(B, 2 * C)
+    EMU.gn_silu_bwd(x, dy, sums, B, HW, C, G, gamma, beta, ss, 2 * C, eps, dx, dg, db, dss, 2 * C)
+    agg_x, agg_c, agg_bc = torch.ones(B, HW, C, dtype=torch.bool), torch.ones(C, dtype=torch.bool), torch.ones(B, C, dtype=torch.bool)
+    agg_x[0, :, 12:18], agg_c[12:18], agg_bc[0, 12:18] = False, False, False
+    for name, out, (ref, bound), agg in zip(GN_OUTS, (dx, dg, db, dss[:, :C], dss[:, C:]), refs,
+                                            (agg_x, agg_c, agg_c, agg_bc, agg_bc)):
+        check(out, ref, bound, f"gn_silu_bwd {name} (emulation)")
+        check_rel_l2(out[agg], ref[agg], 5e-5, f"gn_silu_bwd {name} (emulation)")
+    # the kernel's own three passes in fp32, then each planted defect
+    outs = _gn_bwd_fp32(x, dy, sums, gamma, beta, ss, G, eps, dg0, db0, Z)
+    for name, out, (ref, bound) in zip(GN_OUTS, outs, refs):
+        check(out, ref, bound, f"gn_silu_bwd {name} (fp32 restatement)")
+    for defect, which in (("split missing", "dbeta"), ("split missing", "dx"), ("neighbour's m1", "dx"),
+                          ("silu' before FiLM", "dx"), ("silu' before FiLM", "dgamma"), ("dss swapped", "dscale"),
+                          ("eps ignored", "dx")):
+        i = GN_OUTS.index(which)
+        out = _gn_bwd_fp32(x, dy, sums, gamma, beta, ss, G, eps, dg0, db0, Z, defect)[i]
+        _fails(out, *refs[i], f"gn_silu_bwd {which}: {defect}")
+
+
+# ---------------------------------------------------------------------------------------------- convolution gradients
+def _wgrad_case(stride, k):
+    B, Ho, Wo, Ci, Co = 2, 16, 24, 64, 128
+    g = _g(13 + k)
+    x16 = torch.randn(B, stride * Ho, stride * Wo, Ci, generator=g).to(F16)
+    dy16 = torch.randn(B, Ho, Wo, Co, generator=g).to(F16)
+    return B, Ho, Wo, Ci, Co, x16, dy16
+
+
+@pytest.mark.parametrize("stride,k", [(1, 3), (2, 4)])
+def test_conv_wgrad_bound(stride, k):
+    """The weight-gradient bound at the tensor-core kernel's summation length, on the emulation of mi_conv2d_wgrad_f16."""
+    B, Ho, Wo, Ci, Co, x16, dy16 = _wgrad_case(stride, k)
+    pad = 1 if stride == 2 else k // 2
+    per, splits = R.wgrad_tc_plan(B, Ho, Wo, Ci, Co, k, 132)
+    assert splits > 1
+    ref, bound = R.conv_wgrad_ref(dy16, x16, stride, pad, k, k, R.wgrad_tc_acc_len(B, Ho, Wo, Ci, Co, k, 132))
+    dw = torch.zeros(Co, Ci, k, k)
+    EMU.conv_wgrad_tc(dy16, x16, B, Ho, Wo, Ci, Co, k, k, dw, stride)
+    check(dw, ref, bound, f"conv_wgrad_tc stride {stride} k {k} (emulation)")
+    check_rel_l2(dw, ref, 1e-5, f"conv_wgrad_tc stride {stride} k {k} (emulation)")
+
+    def without(keep):
+        """dW of the pixels where `keep` [B, Ho, Wo] is True only"""
+        return R.conv_wgrad_ref(dy16 * keep[..., None], x16, stride, pad, k, k, 1)[0].float()
+    boxes = torch.zeros(B, Ho // 8, Wo // 8, dtype=torch.bool)
+    boxes.view(-1)[per:2 * per] = True                                                # the second split's 8x8 boxes
+    split = boxes.repeat_interleave(8, dim=1).repeat_interleave(8, dim=2)
+    d = dw.clone()
+    d[:, :, 0, 1] -= without(split)[:, :, 0, 1]
+    _fails(d, ref, bound, "one split missing from tap (0, 1)")
+    last = torch.zeros(B, Ho, Wo, dtype=torch.bool)
+    last[1, -8:, -8:] = True
+    _fails(dw - without(last), ref, bound, "last 8x8 box of image 1 dropped")
+    # the zero padding above the image replaced by the first row (a tap shift that is wrong at the border only)
+    xp = torch.nn.functional.pad(x16.float().permute(0, 3, 1, 2), (pad, pad, pad, pad))
+    xp[:, :, 0] = xp[:, :, 1]
+    d = torch.nn.grad.conv2d_weight(xp, (Co, Ci, k, k), dy16.float().permute(0, 3, 1, 2), stride=stride)
+    _fails(d, ref, bound, "top border padding replaced by the neighbouring row")
+
+
+@pytest.mark.parametrize("stride,k,Co", [(1, 3, 40), (2, 4, 40), (1, 3, 3)])
+def test_conv_dgrad_bound(stride, k, Co):
+    B, Ho, Wo, Ci = 2, 12, 10, 24
+    pad = 1 if stride == 2 else k // 2
+    Hi, Wi = stride * Ho, stride * Wo
+    g = _g(14 + k + Co)
+    dy = torch.randn(B, Ho, Wo, Co, generator=g)
+    w = torch.randn(Co, Ci, k, k, generator=g) * 0.2
+    dx = torch.zeros(B, Hi, Wi, Ci)
+    EMU.conv_dgrad(dy, B, Ho, Wo, Co, w, Ci, k, k, stride, pad, dx, Hi, Wi)
+    ref, bound = R.conv_dgrad_ref(dy, w, stride, pad, Hi, Wi)
+    what = f"conv_dgrad stride {stride} k {k} C_out {Co}"
+    check(dx, ref, bound, what + " (emulation)")
+    check_rel_l2(dx, ref, 2e-5, what + " (emulation)")
+    last = torch.zeros_like(dy)
+    last[:, :, -1] = dy[:, :, -1]
+    _fails(dx - R.conv_dgrad_ref(last, w, stride, pad, Hi, Wi)[0].float(), ref, bound, what + ": last dy column dropped")
+    wf = w.clone()
+    wf[:, 5] = w[:, 5].flip(1, 2)
+    d = dx.clone()
+    d[..., 5] = R.conv_dgrad_ref(dy, wf, stride, pad, Hi, Wi)[0][..., 5].float()
+    _fails(d, ref, bound, what + ": taps of channel 5 not flipped")
+    if stride == 2:
+        d = dx.clone()
+        d[1, 0::2, 0::2], d[1, 0::2, 1::2] = dx[1, 0::2, 1::2], dx[1, 0::2, 0::2]
+        _fails(d, ref, bound, what + ": output parities (0, 0) and (0, 1) of image 1 swapped")
+
+
+def test_upsample2x_bwd_order():
+    """upsample2x_bwd is a fixed-order sum of four fp32 values: the emulation matches it bit for bit, another order does not."""
+    B, H, W, C = 2, 5, 7, 64
+    dy = torch.randn(B, 2 * H, 2 * W, C, generator=_g(15)) * 1e3
+    dx = torch.zeros(B, H, W, C)
+    EMU.upsample2x_bwd(dy, B, H, W, C, dx)
+    ref = R.upsample2x_bwd_ref(dy)
+    assert torch.equal(dx, ref)
+    q = dy.reshape(B, H, 2, W, 2, C)
+    assert not torch.equal((q[:, :, 0, :, 0] + q[:, :, 1, :, 0]) + (q[:, :, 0, :, 1] + q[:, :, 1, :, 1]), ref)
