@@ -8,7 +8,7 @@ x0 prediction, EXACT per-image dynamic-threshold quantile (radix select), poster
 nothing on the host.  Sampling captures three graph flavours: text-only (one graph serves the DDPM walk and every DDIM
 step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).
 
-Five additions that the reference does not have (all optional, defaults reproduce the reference):
+Six additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -20,9 +20,14 @@ Five additions that the reference does not have (all optional, defaults reproduc
     back to t; then every run pastes in the known region, noised to t (Lugmayr et al. 2022, jump length 1);
   * DPM-Solver++(2M) sampling (`sample(..., sampling_timesteps=S, sampler='dpmpp_2m')`, Lu et al. 2022): a second-order
     multistep solver on the thresholded x0 over S points uniform in log-SNR.  Its step is DDIM's table form plus the
-    previous step's clamped x0 times a third table c3 (mi_step_epilogue_multistep), still one U-Net evaluation per point.
+    previous step's clamped x0 times a third table c3 (mi_step_epilogue_multistep), still one U-Net evaluation per point;
+  * image-to-image and partial cascades (`sample(..., init_images=, skip_steps=k, start_at_unet_number=,
+    start_images=, stop_at_unet_number=)`, SDEdit, Meng et al. 2022): a stage may skip the first k points of its walk and
+    start from its init image noised to the first point it runs, and the cascade may run any contiguous range of stages,
+    fed by the caller's images in place of the stage before it.
 
-`noise_fn` kinds: 'init' (x_T, step -1), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
+`noise_fn` kinds: 'init' (x_T, step -1; with an init image k, the noise z of the start sqrt(a_t0) k + sqrt(1 - a_t0) z,
+t0 the walk's first point), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
 augmentation noise, labelled with the U-Net number).  Inpainting labels the draws of iteration r at grid point t with
 t * R + r (at R = 1 that is t) and takes them in this order: 'renoise' (the re-noising draw, r > 0 only), 'inpaint' (the
 noise of the pasted known region), 'step'.  DPM-Solver++(2M) takes the 'step' draws of DDIM with eta = 0 (one per grid
@@ -53,6 +58,10 @@ def quantile_rank(n: int, q: float):
     lo = torch.floor(rank)
     hi = torch.ceil(rank)
     return int(lo.item()), int(hi.item()), float((rank - lo).item())
+
+
+def _is_int(v):
+    return isinstance(v, int) and not isinstance(v, bool)
 
 
 class _StepGraph:
@@ -441,7 +450,8 @@ class Imagen(nn.Module):
 
     @torch.no_grad()
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
-                       lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None):
+                       lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None,
+                       init_image=None):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
@@ -458,7 +468,10 @@ class Imagen(nn.Module):
         `max_steps` counts iterations.  The draws of each iteration are those of the module docstring.
         A multistep `schedule` (from `noise_scheduler.dpm_solver_schedule`, DPM-Solver++(2M)) carries the previous step's
         clamped x0 from step to step in a history buffer, zeroed at the start of the loop; it cannot be combined with
-        `inpaint` (RePaint's re-noising would break the history)."""
+        `inpaint` (RePaint's re-noising would break the history).
+        `init_image` (not in the reference): the normalised image [B, C, s, s] fp32 that the loop starts from (SDEdit)
+        instead of x_T: noised to the walk's first point t0 with the 'init' draw z, x_t0 = sqrt(a_t0) init + sqrt(1 - a_t0) z
+        (mi_q_sample).  A walk that starts below T-1 (a shortened grid) wants one."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -480,6 +493,12 @@ class Imagen(nn.Module):
                 draws = [[('step', t)] for t, _ in plan]
             B, C, hw = shape[0], shape[1], shape[2] * shape[3]
             img = self._noise('init', shape, -1, device)
+            if exists(init_image):
+                x_t0 = torch.empty(tuple(shape), dtype=F32, device=device)
+                t0 = torch.full((B,), plan[0][0], dtype=torch.long, device=device)
+                ops.q_sample(init_image, img, t0, sch.sqrt_alphas_cumprod, sch.sqrt_one_minus_alphas_cumprod, B, C * hw,
+                             1.0, 0.0, x_t0)
+                img = x_t0
 
             kw = dict(noise_scheduler=noise_scheduler, text_embeds=text_embeds, text_mask=text_mask,
                       lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale)
@@ -528,7 +547,8 @@ class Imagen(nn.Module):
     def sample(self, texts: List[str] = None, text_masks=None, text_embeds=None, cond_scale: float = 1.,
                lowres_sample_noise_level: float = None, return_pil_images: bool = False, device=None,
                distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0., inpaint_images=None,
-               inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim'):
+               inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim', init_images=None,
+               skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -546,17 +566,45 @@ class Imagen(nn.Module):
         'dpmpp_2m', DPM-Solver++(2M) over S points uniform in log-SNR (GaussianDiffusion.dpm_solver_schedule): a
         deterministic second-order multistep solver of the probability-flow ODE, still S U-Net evaluations (2S with
         unbatched guidance), that needs sampling_timesteps, ddim_eta = 0 and no inpainting.  Stages whose entry is None
-        keep the DDPM loop."""
+        keep the DDPM loop.
+        `init_images` (a (b, channels, s, s) float tensor in `input_image_range` for every stage, or one entry per U-Net,
+        each such a tensor or None) and `skip_steps` (None, an int k, or one entry per U-Net) give image-to-image
+        sampling (SDEdit): the stage resizes its init image to its size, walks grid[k:] of its walk (0 <= k < the walk's
+        length; k > 0 needs an init image) and starts from the init image noised to grid[k]; 2M restarts at first order
+        there.  `start_at_unet_number` and `stop_at_unet_number` (default: the last U-Net) run the stages in between
+        only and return the last one's output; `start_images` ((b, channels, s, s) float in `input_image_range`, any
+        square size, required if and only if start_at_unet_number > 1) stand in for the output of the stage before the
+        first one, e.g. to super-resolve the caller's own images."""
         assert sampler in ('ddim', 'dpmpp_2m'), f"sampler must be 'ddim' or 'dpmpp_2m', got {sampler!r}"
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
         if sampler == 'dpmpp_2m':
             assert any(s is not None for s in steps), "sampler='dpmpp_2m' needs sampling_timesteps"
             assert ddim_eta == 0., f"sampler='dpmpp_2m' is deterministic: ddim_eta must be 0, got {ddim_eta}"
             assert not exists(inpaint_images), "sampler='dpmpp_2m' cannot be combined with inpainting"
+        n = len(self.unets)
+        assert _is_int(start_at_unet_number) and 1 <= start_at_unet_number <= n, \
+            f'start_at_unet_number must be between 1 and {n}, got {start_at_unet_number!r}'
+        stop_at_unet_number = default(stop_at_unet_number, n)
+        assert _is_int(stop_at_unet_number) and start_at_unet_number <= stop_at_unet_number <= n, \
+            f'stop_at_unet_number must be between start_at_unet_number ({start_at_unet_number}) and {n}, got ' \
+            f'{stop_at_unet_number!r}'
+        assert not (start_at_unet_number > 1 and not exists(start_images)), \
+            f'start_images are required to start at unet {start_at_unet_number}: they stand in for the output of unet ' \
+            f'{start_at_unet_number - 1}'
+        assert not (start_at_unet_number == 1 and exists(start_images)), \
+            'start_images need start_at_unet_number > 1: the base unet has no low-res input'
+        init_images = self._per_unet(init_images, 'init_images')
+        skips = self._per_unet(skip_steps, 'skip_steps')
+        for i in range(start_at_unet_number, stop_at_unet_number + 1):
+            k, walk_len = default(skips[i - 1], 0), default(steps[i - 1], self.noise_schedulers[i - 1].num_timesteps)
+            assert _is_int(k) and 0 <= k < walk_len, \
+                f'skip_steps of unet {i} must be an int between 0 and {walk_len - 1} (its walk has {walk_len} points), ' \
+                f'got {k!r}'
+            assert k == 0 or exists(init_images[i - 1]), f'skip_steps > 0 needs an init image, and unet {i} has none'
+        skips = tuple(default(k, 0) for k in skips)
         assert exists(inpaint_images) == exists(inpaint_masks), \
             'inpaint_images and inpaint_masks must be given together'
-        assert isinstance(inpaint_resample_times, int) and not isinstance(inpaint_resample_times, bool) \
-            and inpaint_resample_times >= 1, \
+        assert _is_int(inpaint_resample_times) and inpaint_resample_times >= 1, \
             f'inpaint_resample_times must be an int >= 1, got {inpaint_resample_times!r}'
         device = torch.device(default(device, self.device))
         self._reset_unets_all_one_device(device=device)
@@ -565,18 +613,28 @@ class Imagen(nn.Module):
         inpaint = (inpaint_images, inpaint_masks, inpaint_resample_times) if exists(inpaint_images) else None
         with N.device_of(self._temp):
             return self._sample_impl(texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level,
-                                     return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler)
+                                     return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler,
+                                     init_images, skips, start_at_unet_number, stop_at_unet_number, start_images)
+
+    def _per_unet(self, value, name):
+        """`value` once per U-Net: a list or tuple must have one entry per U-Net, anything else applies to every one."""
+        n = len(self.unets)
+        if not isinstance(value, (list, tuple)):
+            return (value,) * n
+        assert len(value) == n, f'{name} must have one entry per unet ({n}), got {len(value)}'
+        return tuple(value)
+
+    def _check_images(self, images, b, name):
+        """`images` must be a (b, channels, s, s) float tensor (b: the full batch of the text conditioning)."""
+        assert torch.is_tensor(images) and images.is_floating_point(), f'{name} must be a float tensor'
+        assert images.dim() == 4 and tuple(images.shape[:2]) == (b, self.channels) and \
+            images.shape[2] == images.shape[3], \
+            f'{name} must be (b, channels, s, s) = ({b}, {self.channels}, s, s), got {tuple(images.shape)}'
 
     def _sampling_steps(self, sampling_timesteps, ddim_eta):
         """Per-U-Net step counts (None = the DDPM loop), validated."""
         assert 0. <= ddim_eta <= 1., f'ddim_eta must be between 0 and 1, got {ddim_eta}'
-        n = len(self.unets)
-        if not isinstance(sampling_timesteps, (list, tuple)):
-            steps = (sampling_timesteps,) * n
-        else:
-            steps = tuple(sampling_timesteps)
-            assert len(steps) == n, \
-                f'sampling_timesteps must have one entry per unet ({n}), got {len(steps)}'
+        steps = self._per_unet(sampling_timesteps, 'sampling_timesteps')
         for s, sch in zip(steps, self.noise_schedulers):
             if s is not None:
                 assert 2 <= s <= sch.num_timesteps, \
@@ -584,7 +642,8 @@ class Imagen(nn.Module):
         return steps
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
-                     device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim'):
+                     device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim', init_images=None,
+                     skips=None, start_at=1, stop_at=None, start_images=None):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -592,21 +651,23 @@ class Imagen(nn.Module):
         assert exists(text_embeds), 'text or text encodings must be passed into Imagen'
         assert not (exists(text_embeds) and text_embeds.shape[-1] != self.text_embed_dim), \
             f'invalid text embedding dimension being passed in (should be {self.text_embed_dim})'
+        b = text_embeds.shape[0]
         inpaint_images = inpaint_masks = None
         if exists(inpaint):
             inpaint_images, inpaint_masks, resample_times = inpaint
-            b = text_embeds.shape[0]
-            assert torch.is_tensor(inpaint_images) and inpaint_images.is_floating_point(), \
-                'inpaint_images must be a float tensor'
-            assert inpaint_images.dim() == 4 and tuple(inpaint_images.shape[:2]) == (b, self.channels) and \
-                inpaint_images.shape[2] == inpaint_images.shape[3], \
-                f'inpaint_images must be (b, channels, s, s) = ({b}, {self.channels}, s, s), got ' \
-                f'{tuple(inpaint_images.shape)}'
+            self._check_images(inpaint_images, b, 'inpaint_images')
             s = inpaint_images.shape[-1]
             assert torch.is_tensor(inpaint_masks) and inpaint_masks.dtype == torch.bool, \
                 'inpaint_masks must be a bool tensor'
             assert tuple(inpaint_masks.shape) == (b, s, s), \
                 f'inpaint_masks must be (b, s, s) = ({b}, {s}, {s}), got {tuple(inpaint_masks.shape)}'
+        n_stages = len(self.unets)
+        init_images = default(init_images, (None,) * n_stages)
+        for i, init in enumerate(init_images, 1):
+            if exists(init):
+                self._check_images(init, b, f'init_images of unet {i}')
+        if exists(start_images):
+            self._check_images(start_images, b, 'start_images')
 
         world, rank = 1, 0
         if distributed:
@@ -616,28 +677,32 @@ class Imagen(nn.Module):
             full_b = text_embeds.shape[0]
             assert full_b % world == 0, f'batch {full_b} must divide evenly over {world} ranks'
             per = full_b // world
-            text_embeds = text_embeds[rank * per:(rank + 1) * per]
-            text_masks = text_masks[rank * per:(rank + 1) * per] if exists(text_masks) else None
-            if exists(inpaint):
-                inpaint_images = inpaint_images[rank * per:(rank + 1) * per]
-                inpaint_masks = inpaint_masks[rank * per:(rank + 1) * per]
+            rows = lambda v: v[rank * per:(rank + 1) * per] if exists(v) else None
+            text_embeds, text_masks, inpaint_images, inpaint_masks, start_images = map(
+                rows, (text_embeds, text_masks, inpaint_images, inpaint_masks, start_images))
+            init_images = tuple(map(rows, init_images))
 
         batch_size = text_embeds.shape[0]
         if exists(inpaint):
             inpaint_images = inpaint_images.to(device=device, dtype=F32).contiguous()
             inpaint_masks = inpaint_masks.to(device=device, dtype=F32)[:, None].contiguous()
+        init_images = tuple(maybe(lambda v: v.to(device=device, dtype=F32).contiguous())(v) for v in init_images)
         text_embeds = text_embeds.to(device=device, dtype=F32).contiguous()
         text_masks = text_masks.to(device).contiguous() if exists(text_masks) else None
         lowres_sample_noise_level = default(lowres_sample_noise_level, self.lowres_sample_noise_level)
         ops = get_ops()
 
         img = None
+        if exists(start_images):
+            # what the finalize of stage start_at - 1 would have left: images in input_image_range
+            img = start_images.to(device=device, dtype=F32).clamp(*self.input_image_range).contiguous()
         gathered = None
-        n_stages = len(self.unets)
+        stop_at = default(stop_at, n_stages)
         steps = default(steps, (None,) * n_stages)
-        for unet_number, unet, channel, image_size, noise_scheduler, n_steps in zip(
-                range(1, n_stages + 1), self.unets, self.sample_channels, self.image_sizes,
-                self.noise_schedulers, steps):
+        skips = default(skips, (0,) * n_stages)
+        stages = list(zip(range(1, n_stages + 1), self.unets, self.sample_channels, self.image_sizes,
+                          self.noise_schedulers, steps, init_images, skips))[start_at - 1:stop_at]
+        for unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip in stages:
             with self._one_unet_in_gpu(unet=unet):
                 lowres_cond_img = lowres_noise_times = None
                 if unet.lowres_cond:
@@ -653,14 +718,23 @@ class Imagen(nn.Module):
                     lowres_cond_img = noised
                 shape = (batch_size, self.channels, image_size, image_size)
                 slot = None
-                if distributed and world > 1 and unet_number == n_stages:
+                if distributed and world > 1 and unet_number == stop_at:
                     # the last stage finalises straight into this rank's slot of the all-gather buffer (no staging copy)
                     gathered = torch.empty((world * batch_size, *shape[1:]), dtype=F32, device=device)
                     slot = gathered[rank * batch_size:(rank + 1) * batch_size]
                 schedule = None
                 if n_steps is not None:
-                    schedule = (noise_scheduler.dpm_solver_schedule(n_steps, device) if sampler == 'dpmpp_2m' else
-                                noise_scheduler.sampling_schedule(n_steps, ddim_eta, device))
+                    schedule = (noise_scheduler.dpm_solver_schedule(n_steps, device, skip=skip) if sampler == 'dpmpp_2m'
+                                else noise_scheduler.sampling_schedule(n_steps, ddim_eta, device))
+                elif skip:
+                    schedule = noise_scheduler.ddpm_schedule(device)
+                if skip and not exists(schedule.c3):
+                    # DDPM / DDIM tables depend only on (t, next t): a shortened walk is the same tables on grid[k:]
+                    schedule = schedule._replace(grid=schedule.grid[skip:])
+                stage_init = None
+                if exists(init):
+                    init = resize_image_to(init, image_size, clamp_range=self.input_image_range)
+                    stage_init = self.normalize_img(init).contiguous()
                 stage_inpaint = None
                 if exists(inpaint):
                     # this stage's known image (normalised) and mask; unchanged when already at the stage's size
@@ -671,7 +745,7 @@ class Imagen(nn.Module):
                 img = self._p_sample_loop(unet, shape, text_embeds=text_embeds, text_mask=text_masks,
                                           cond_scale=cond_scale, lowres_cond_img=lowres_cond_img,
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
-                                          out=slot, schedule=schedule, inpaint=stage_inpaint)
+                                          out=slot, schedule=schedule, inpaint=stage_inpaint, init_image=stage_init)
 
         outputs = img
         if gathered is not None:

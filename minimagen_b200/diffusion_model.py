@@ -109,7 +109,7 @@ class GaussianDiffusion(nn.Module):
         self._schedules[key] = sched
         return sched
 
-    def dpm_solver_schedule(self, steps: int, device) -> SamplingSchedule:
+    def dpm_solver_schedule(self, steps: int, device, skip: int = 0) -> SamplingSchedule:
         """DPM-Solver++(2M) (Lu et al. 2022, Algorithm 2, data prediction) as schedule tables, over a grid uniform in
         log-SNR lambda_t = 0.5 (log a_t - log(1 - a_t)), a = alphas_cumprod.  Grid, ascending: u_0 = 0; for j >= 1, u_j is the
         t whose lambda_t is nearest to linspace(lambda_0, lambda_{T-1}, steps)[j], clamped into [u_{j-1} + 1, T - steps + j]
@@ -122,12 +122,16 @@ class GaussianDiffusion(nn.Module):
             k = S-1 (t = 0):    c1 = 1, c2 = c3 = 0                                    (x = x0, as DDIM)
         with x0 the thresholded data prediction.  sigma = 0.  phi and c2 use sampling_schedule's fp64 expressions, so at
         steps = 2 the tables are those of sampling_schedule(2, 0.).  Computed in fp64, cast to fp32; cached per
-        (steps, device)."""
+        (steps, skip, device).
+        `skip` = k > 0 gives the shortened walk t_k, ..., t_{S-1} (grid[k:], an image-to-image start): the history is zero
+        at its first step, so that step restarts at first order (c1 = phi_k, c3 = 0); every other point keeps its
+        tables."""
         T = self.num_timesteps
-        steps = int(steps)
+        steps, skip = int(steps), int(skip)
         assert 2 <= steps <= T, f'sampling timesteps must be between 2 and {T} (the number of training timesteps)'
+        assert 0 <= skip < steps, f'skip must be between 0 and {steps - 1}, got {skip}'
         device = torch.device(device)
-        key = ('dpmpp_2m', steps, str(device))
+        key = ('dpmpp_2m', steps, skip, str(device))
         sched = self._schedules.get(key)
         if sched is not None:
             return sched
@@ -156,14 +160,15 @@ class GaussianDiffusion(nn.Module):
             r = h[:-1] / h[1:]                                    # r_k, k = 1 .. S-2
             c1[1:-1] = phi[1:-1] * (1. + 1. / (2. * r))
             c3[1:-1] = -phi[1:-1] / (2. * r)
+        c1[skip], c3[skip] = phi[skip], 0.
 
         def table(v, dtype):
             out = torch.zeros(T, dtype=dtype)
             out[grid_up] = v.flip(0).to(dtype)
             return out.to(device)
         next_t = torch.cat((walk[1:], torch.zeros(1, dtype=torch.long)))
-        sched = SamplingSchedule(grid=tuple(walk.tolist()), c1=table(c1, torch.float32), c2=table(c2, torch.float32),
-                                 sigma=torch.zeros(T, dtype=torch.float32, device=device),
+        sched = SamplingSchedule(grid=tuple(walk[skip:].tolist()), c1=table(c1, torch.float32),
+                                 c2=table(c2, torch.float32), sigma=torch.zeros(T, dtype=torch.float32, device=device),
                                  next_t=table(next_t, torch.long), c3=table(c3, torch.float32))
         self._schedules[key] = sched
         return sched
