@@ -257,6 +257,21 @@ int mi_step_epilogue_multistep(const float* x_t, const float* eps_cond, const fl
                                const float* sigma, const float* c3, const float* noise, float* x0_hist, int B, int n,
                                int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
                                float* x0_workspace, void* stream);
+/* mi_step_epilogue and mi_step_epilogue_multistep with a guidance weight per image: image b combines
+ * null + (cond - null) * w[b] (w: fp32 [B], required) instead of cond_scale, which is ignored.  An array of equal values
+ * gives the scalar entry point's bits.  A captured step that reads its weights from a device buffer serves every scale. */
+int mi_step_epilogue_w(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
+                       const long long* t, const float* sqrt_recip_alphas_cumprod,
+                       const float* sqrt_recipm1_alphas_cumprod, const float* posterior_mean_coef1,
+                       const float* posterior_mean_coef2, const float* sigma, const float* noise, int B, int n,
+                       int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
+                       float* x0_workspace, void* stream);
+int mi_step_epilogue_multistep_w(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                                 const float* w, const long long* t, const float* sqrt_recip_alphas_cumprod,
+                                 const float* sqrt_recipm1_alphas_cumprod, const float* c1, const float* c2,
+                                 const float* sigma, const float* c3, const float* noise, float* x0_hist, int B, int n,
+                                 int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
+                                 float* x0_workspace, void* stream);
 /* t[b] <- max(t[b] - 1, 0): the next iteration's timestep of Imagen._p_sample_loop (Imagen.py:398-415 walks the list of
  * diffusion_model.py:81-87), advanced on the device so that a captured step can be replayed back to back */
 int mi_step_advance_t(long long* t, int B, void* stream);

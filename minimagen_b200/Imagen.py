@@ -6,9 +6,10 @@ asserts and messages.  The reverse-diffusion step is executed by the fused step 
 x0 prediction, EXACT per-image dynamic-threshold quantile (radix select), posterior mean and noise add; the whole step
 (both U-Net passes + epilogue) is optionally replayed from a CUDA graph so the ~10^3 kernel launches per step cost
 nothing on the host.  Sampling captures three graph flavours: text-only (one graph serves the DDPM walk and every DDIM
-step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).
+step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).  The guidance weights are per-image
+data in a static buffer, so every flavour's graph serves every `cond_scale` and every negative prompt of its shape.
 
-Six additions that the reference does not have (all optional, defaults reproduce the reference):
+Seven additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -24,7 +25,11 @@ Six additions that the reference does not have (all optional, defaults reproduce
   * image-to-image and partial cascades (`sample(..., init_images=, skip_steps=k, start_at_unet_number=,
     start_images=, stop_at_unet_number=)`, SDEdit, Meng et al. 2022): a stage may skip the first k points of its walk and
     start from its init image noised to the first point it runs, and the cascade may run any contiguous range of stages,
-    fed by the caller's images in place of the stage before it.
+    fed by the caller's images in place of the stage before it;
+  * negative prompts and per-image, per-stage guidance (`sample(..., negative_texts= or negative_text_embeds=,
+    cond_scale=)`): the guidance pass conditions the U-Net on the negative prompt instead of the learned null
+    conditioning, eps = eps_neg + (eps_cond - eps_neg) * w, and w may differ per image and per stage.  The guidance pass
+    runs iff some image's w != 1.
 
 `noise_fn` kinds: 'init' (x_T, step -1; with an init image k, the noise z of the start sqrt(a_t0) k + sqrt(1 - a_t0) z,
 t0 the walk's first point), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
@@ -33,6 +38,8 @@ t * R + r (at R = 1 that is t) and takes them in this order: 'renoise' (the re-n
 noise of the pasted known region), 'step'.  DPM-Solver++(2M) takes the 'step' draws of DDIM with eta = 0 (one per grid
 point, multiplied by a zero sigma).
 """
+import math
+import numbers
 from contextlib import contextmanager
 from typing import Callable, List, Literal, Tuple, Union
 
@@ -64,6 +71,22 @@ def _is_int(v):
     return isinstance(v, int) and not isinstance(v, bool)
 
 
+def _is_guided(cond_scale):
+    """Whether some image's guidance weight differs from 1, i.e. the step runs the guidance pass.  `cond_scale`: a number
+    or a tensor of per-image weights (read back to the host: decide once per loop, never inside a captured step)."""
+    if torch.is_tensor(cond_scale):
+        return bool((cond_scale != 1).any())
+    return cond_scale != 1
+
+
+def _pad_text(embeds, mask, length):
+    """Zero rows and False mask up to `length` rows: exact, since masked rows become null_text_embed either way."""
+    pad = length - embeds.shape[1]
+    if pad == 0:
+        return embeds, mask
+    return F.pad(embeds, (0, 0, 0, pad)), F.pad(mask, (0, pad), value=False)
+
+
 class _StepGraph:
     """One captured denoising step (U-Net pass(es) + step epilogue) over STATIC buffers:
          x      [B, C, s, s]  the image, updated IN PLACE by every replay (x_t -> x_{t-1});
@@ -78,7 +101,9 @@ class _StepGraph:
                 >= 0.5), the RePaint counter r [B] and its limit R [1] (int64), the re-noising tables ra / rb [T] and the
                 draws z_renoise / z_known (`set_inpaint` refreshes them, so one graph serves any mask, image and R).
          hist   multistep graphs only: [B, C, s, s], the previous step's clamped x0 (zeroed at the start of every loop); the
-                sched copy then also has c3 [T].
+                sched copy then also has c3 [T];
+         w      [B] fp32 the per-image guidance weights (`set_cond` refreshes them); guided graphs with a negative prompt
+                also hold static negative_text_embeds / negative_text_mask in `cond`.
     Three flavours: text-only (the step, then mi_step_advance_t_table), inpainting (draws, mi_inpaint_prologue, the step,
     mi_inpaint_advance) and multistep (the draw, mi_step_epilogue_multistep's step, mi_step_advance_t_table).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
     for DDPM; `* ((S-1) R + 1)` when inpainting) -- no per-step host-side tensor ops."""
@@ -89,6 +114,7 @@ class _StepGraph:
         self.cond = {}
         self.sched = None
         self.hist = None
+        self.w = None
         self.inp = None
         self.inject_noise = False
         self.unet = None
@@ -102,22 +128,29 @@ class _StepGraph:
             self.inp[name].copy_(v)
         self.inp['R'].fill_(int(R))
 
-    def set_cond(self, **tensors):
+    def set_cond(self, w=None, **tensors):
+        if w is not None:
+            self.w.copy_(w)
         for k, v in tensors.items():
             if v is not None:
                 self.cond[k].copy_(v)
         self.refresh_static()
 
+    def _static_texts(self):
+        return [te for te in map(self.cond.get, ('text_embeds', 'negative_text_embeds')) if te is not None]
+
     def refresh_static(self):
-        """Step-invariant conditioning of the static buffers (eager, once per sampling loop): the text projection."""
-        te = self.cond.get('text_embeds')
-        if self.unet is not None and te is not None and te.dtype == F32:
-            self.unet.register_static_text(te)
+        """Step-invariant conditioning of the static buffers (eager, once per sampling loop): the text projections of the
+        prompt and of the negative prompt."""
+        if self.unet is not None:
+            for te in self._static_texts():
+                if te.dtype == F32:
+                    self.unet.register_static_text(te)
 
     def release(self):
-        te = self.cond.get('text_embeds')
-        if self.unet is not None and te is not None:
-            self.unet.unregister_static_text(te)
+        if self.unet is not None:
+            for te in self._static_texts():
+                self.unet.unregister_static_text(te)
 
     def replay(self):
         self.graph.replay()
@@ -270,8 +303,13 @@ class Imagen(nn.Module):
                 noise_scheduler.posterior_log_variance_clipped.gather(-1, t).reshape(shp))
 
     def _step(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-              cond_scale, model_output=None, out=None, schedule=None, hist=None):
+              cond_scale, model_output=None, out=None, schedule=None, hist=None, negative_text_embeds=None,
+              negative_text_mask=None, guided=None):
         """x_{t-1} = posterior_mean(x_t, clamp-thresholded x0(x_t, eps)) + [t != 0] * sigma_t * noise.
+        eps = g + (cond - g) * w, with w = `cond_scale` (a number, or an fp32 [B] tensor of per-image weights on x's
+        device) and g the guidance pass: the U-Net conditioned on `negative_text_embeds` / `negative_text_mask` if given,
+        else on the learned null conditioning.  The guidance pass runs iff `guided` (default: some w != 1, which reads a
+        tensor back to the host; a captured step passes it).
         `out` may be `x` itself (the captured step updates the image in place).  `schedule` (a SamplingSchedule) replaces
         the posterior coefficients and sigma by its DDIM tables: the step then goes to the next point of its grid.  A
         multistep schedule (one with c3, DPM-Solver++(2M)) also adds c3[t] * hist, the previous step's clamped x0, and then
@@ -280,11 +318,15 @@ class Imagen(nn.Module):
             return self._step_impl(unet, x, t, noise, noise_scheduler=noise_scheduler, text_embeds=text_embeds,
                                    text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                                    lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
-                                   model_output=model_output, out=out, schedule=schedule, hist=hist)
+                                   model_output=model_output, out=out, schedule=schedule, hist=hist,
+                                   negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
+                                   guided=guided)
 
     def _step_impl(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                   lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None, hist=None):
-        assert not (cond_scale != 1. and not self.can_classifier_guidance), \
+                   lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None, hist=None,
+                   negative_text_embeds=None, negative_text_mask=None, guided=None):
+        guided = _is_guided(cond_scale) if guided is None else guided
+        assert not (guided and not self.can_classifier_guidance), \
             'imagen was not trained with conditional dropout, and thus one cannot use classifier free guidance ' \
             '(cond_scale anything other than 1)'
         ops = get_ops()
@@ -293,21 +335,36 @@ class Imagen(nn.Module):
         sch = noise_scheduler
         kw = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                   lowres_noise_times=lowres_noise_times)
+        neg = exists(negative_text_embeds)
+        # the guidance pass: the negative prompt (keep = 1, no RNG), or the learned null conditioning
+        gkw = dict(kw, text_embeds=negative_text_embeds, text_mask=negative_text_mask) if neg else kw
         eps_null = None
         if exists(model_output):
             eps = model_output.to(F32).contiguous()
         else:
-            if cond_scale != 1 and self.cfg_batched:
-                # conditional and unconditional pass as ONE batch of 2B (per-sample keep mask instead of two forwards)
+            # a negative prompt shares the 2B batch when both prompts have masks (padding to a common length is then
+            # exact) or neither has one and their lengths match
+            batchable = not neg or (exists(text_mask) and exists(negative_text_mask)) or \
+                (not exists(text_mask) and not exists(negative_text_mask) and
+                 text_embeds.shape[1] == negative_text_embeds.shape[1])
+            if guided and self.cfg_batched and batchable:
+                # conditional and guidance pass as ONE batch of 2B (per-sample keep mask instead of two forwards)
                 two = lambda v: torch.cat((v, v), dim=0) if exists(v) else None
                 keep = torch.cat((torch.ones(B, dtype=torch.uint8, device=x.device),
-                                  torch.zeros(B, dtype=torch.uint8, device=x.device)))
-                both = unet._forward_impl(two(x), two(t), cond_keep=keep, **{k: two(v) for k, v in kw.items()})
+                                  torch.full((B,), int(neg), dtype=torch.uint8, device=x.device)))
+                bkw = {k: two(v) for k, v in kw.items()}
+                if neg:
+                    te, tm, nte, ntm = text_embeds, text_mask, negative_text_embeds, negative_text_mask
+                    if exists(tm):
+                        L = max(te.shape[1], nte.shape[1])
+                        (te, tm), (nte, ntm) = _pad_text(te, tm, L), _pad_text(nte, ntm, L)
+                    bkw.update(text_embeds=torch.cat((te, nte)), text_mask=torch.cat((tm, ntm)) if exists(tm) else None)
+                both = unet._forward_impl(two(x), two(t), cond_keep=keep, **bkw)
                 eps, eps_null = both[:B], both[B:]
             else:
                 eps = unet.forward(x, t, **kw)
-                if cond_scale != 1:
-                    eps_null = unet.forward(x, t, cond_drop_prob=1., **kw)
+                if guided:
+                    eps_null = unet.forward(x, t, cond_drop_prob=0. if neg else 1., **gkw)
         x = x.contiguous()
         lo, hi, w = quantile_rank(n, self.dynamic_thresholding_percentile)
         if out is None:
@@ -338,13 +395,18 @@ class Imagen(nn.Module):
 
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
-                   cond_scale, inpaint=False, multistep=False):
+                   cond_scale, inpaint=False, multistep=False, *, negative_text_embeds=None, negative_text_mask=None,
+                   guided=None):
+        """Only whether the step runs the guidance pass is part of the key, not the weights: they are data in the graph's
+        static w buffer.  The negative prompt's signature counts when it is used, i.e. when guided."""
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
+        guided = _is_guided(cond_scale) if guided is None else guided
         p0 = next(unet.parameters())
-        key = (id(unet), tuple(shape), float(cond_scale), bool(self.cfg_batched), exists(self.noise_fn),
+        key = (id(unet), tuple(shape), bool(guided), bool(self.cfg_batched), exists(self.noise_fn),
                noise_scheduler.num_timesteps, sig(text_embeds), sig(text_mask), sig(lowres_cond_img),
                sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
-               self.dynamic_thresholding_percentile)
+               self.dynamic_thresholding_percentile,
+               (sig(negative_text_embeds), sig(negative_text_mask)) if guided else None)
         if inpaint:
             return key + ('inpaint',)
         return key + ('multistep',) if multistep else key
@@ -357,7 +419,8 @@ class Imagen(nn.Module):
         self.max_cached_graphs = 4
 
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                    lowres_noise_times, cond_scale, schedule=None, inpaint=None):
+                    lowres_noise_times, cond_scale, schedule=None, inpaint=None, negative_text_embeds=None,
+                    negative_text_mask=None, guided=None):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
         every later sampling loop of the same signature.  Every lookup refreshes the conditioning tensors in its static
         buffers and installs the walk `schedule` (a SamplingSchedule; None: the DDPM walk) in its static tables: the step
@@ -367,18 +430,28 @@ class Imagen(nn.Module):
         mi_inpaint_prologue, the step, mi_inpaint_advance -- with k, m, R and the walk's re-noising tables installed by
         `_StepGraph.set_inpaint`; neither the mask, the image nor R is part of the signature.
         A multistep `schedule` (with c3) selects the multistep flavour, keyed apart from the other two: static c1 / c2 / c3 /
-        sigma / next_t tables and the x0 history `hist`, stepped by mi_step_epilogue_multistep."""
+        sigma / next_t tables and the x0 history `hist`, stepped by mi_step_epilogue_multistep.
+        `cond_scale` (a number or per-image weights) is installed in the static w buffer: only `guided` (some weight != 1)
+        and, when guided, the negative prompt's shapes are part of the signature."""
         device = self.device
         schedule = default(schedule, lambda: noise_scheduler.ddpm_schedule(device))
         multistep = exists(schedule.c3)
         assert not (multistep and exists(inpaint)), 'a multistep schedule cannot be combined with inpainting'
+        guided = _is_guided(cond_scale) if guided is None else guided
+        if not guided:
+            negative_text_embeds = negative_text_mask = None      # no guidance pass: the graph never reads them
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
-                              lowres_noise_times, cond_scale, exists(inpaint), multistep)
+                              lowres_noise_times, cond_scale, exists(inpaint), multistep,
+                              negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
+                              guided=guided)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
-                    lowres_noise_times=lowres_noise_times)
+                    lowres_noise_times=lowres_noise_times, negative_text_embeds=negative_text_embeds,
+                    negative_text_mask=negative_text_mask)
+        w = (cond_scale.to(device=device, dtype=F32) if torch.is_tensor(cond_scale) else
+             torch.full((shape[0],), float(cond_scale), dtype=F32, device=device))
         g = self._graphs.get(key)
         if g is not None:
-            g.set_cond(**cond)
+            g.set_cond(w=w, **cond)
         else:
             if len(self._graphs) >= self.max_cached_graphs:
                 self._graphs.pop(next(iter(self._graphs))).release()
@@ -389,7 +462,8 @@ class Imagen(nn.Module):
             g.noise = torch.zeros(shape, dtype=F32, device=device)
             g.t = torch.zeros((shape[0],), dtype=torch.long, device=device)
             g.cond = {k: v.clone() for k, v in cond.items() if v is not None}
-            kw = dict(noise_scheduler=noise_scheduler, cond_scale=cond_scale,
+            g.w = w.clone()
+            kw = dict(noise_scheduler=noise_scheduler, cond_scale=g.w, guided=guided,
                       **{k: g.cond.get(k) for k in cond})
             g.refresh_static()
             ops = get_ops()
@@ -451,7 +525,7 @@ class Imagen(nn.Module):
     @torch.no_grad()
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
                        lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None,
-                       init_image=None):
+                       init_image=None, negative_text_embeds=None, negative_text_mask=None):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
@@ -471,7 +545,9 @@ class Imagen(nn.Module):
         `inpaint` (RePaint's re-noising would break the history).
         `init_image` (not in the reference): the normalised image [B, C, s, s] fp32 that the loop starts from (SDEdit)
         instead of x_T: noised to the walk's first point t0 with the 'init' draw z, x_t0 = sqrt(a_t0) init + sqrt(1 - a_t0) z
-        (mi_q_sample).  A walk that starts below T-1 (a shortened grid) wants one."""
+        (mi_q_sample).  A walk that starts below T-1 (a shortened grid) wants one.
+        `cond_scale` (not in the reference: also an fp32 [B] tensor of per-image weights on the sampling device) and
+        `negative_text_embeds` / `negative_text_mask` (not in the reference) guide as in `_step`."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -501,7 +577,9 @@ class Imagen(nn.Module):
                 img = x_t0
 
             kw = dict(noise_scheduler=noise_scheduler, text_embeds=text_embeds, text_mask=text_mask,
-                      lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale)
+                      lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
+                      negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
+                      guided=_is_guided(cond_scale))
             if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
                 g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, **kw)
                 static = dict(step=g.noise)
@@ -548,7 +626,8 @@ class Imagen(nn.Module):
                lowres_sample_noise_level: float = None, return_pil_images: bool = False, device=None,
                distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0., inpaint_images=None,
                inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim', init_images=None,
-               skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None):
+               skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None,
+               negative_texts=None, negative_text_embeds=None, negative_text_masks=None):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -574,7 +653,14 @@ class Imagen(nn.Module):
         there.  `start_at_unet_number` and `stop_at_unet_number` (default: the last U-Net) run the stages in between
         only and return the last one's output; `start_images` ((b, channels, s, s) float in `input_image_range`, any
         square size, required if and only if start_at_unet_number > 1) stand in for the output of the stage before the
-        first one, e.g. to super-resolve the caller's own images."""
+        first one, e.g. to super-resolve the caller's own images.
+        `cond_scale`, the classifier-free guidance weight w, is a number, a 1-D float tensor of b per-image weights (e.g.
+        a guidance sweep in one batch), or one entry per U-Net, each such a number or tensor; every entry must be finite.
+        A stage runs the guidance pass iff some image's w != 1 (at w = 1 everywhere, one U-Net pass per step).
+        `negative_texts` (a str, or a list of 1 or b str, encoded like `texts`) or `negative_text_embeds` ((1 or b, n,
+        text_embed_dim), with optional `negative_text_masks` (1 or b, n) bool; one row is used for every image) replace
+        the learned null conditioning of the guidance pass: eps = eps_neg + (eps_cond - eps_neg) * w.  Captured step graphs
+        are keyed on the shapes only, so changing w or the negative prompt reuses them."""
         assert sampler in ('ddim', 'dpmpp_2m'), f"sampler must be 'ddim' or 'dpmpp_2m', got {sampler!r}"
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
         if sampler == 'dpmpp_2m':
@@ -595,6 +681,15 @@ class Imagen(nn.Module):
             'start_images need start_at_unet_number > 1: the base unet has no low-res input'
         init_images = self._per_unet(init_images, 'init_images')
         skips = self._per_unet(skip_steps, 'skip_steps')
+        scales = self._per_unet(cond_scale, 'cond_scale')
+        for i, w in enumerate(scales, 1):
+            assert torch.is_tensor(w) or (isinstance(w, numbers.Real) and not isinstance(w, bool) and math.isfinite(w)), \
+                f'cond_scale of unet {i} must be a finite number or a 1-D float tensor of per-image weights, got {w!r}'
+        assert not (exists(negative_texts) and exists(negative_text_embeds)), \
+            'negative_texts and negative_text_embeds cannot both be given'
+        assert not (exists(negative_text_masks) and not exists(negative_text_embeds)), \
+            'negative_text_masks need negative_text_embeds'
+        negative = (negative_texts, negative_text_embeds, negative_text_masks)
         for i in range(start_at_unet_number, stop_at_unet_number + 1):
             k, walk_len = default(skips[i - 1], 0), default(steps[i - 1], self.noise_schedulers[i - 1].num_timesteps)
             assert _is_int(k) and 0 <= k < walk_len, \
@@ -612,9 +707,10 @@ class Imagen(nn.Module):
             self.to(device)
         inpaint = (inpaint_images, inpaint_masks, inpaint_resample_times) if exists(inpaint_images) else None
         with N.device_of(self._temp):
-            return self._sample_impl(texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level,
+            return self._sample_impl(texts, text_masks, text_embeds, scales, lowres_sample_noise_level,
                                      return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler,
-                                     init_images, skips, start_at_unet_number, stop_at_unet_number, start_images)
+                                     init_images, skips, start_at_unet_number, stop_at_unet_number, start_images,
+                                     negative)
 
     def _per_unet(self, value, name):
         """`value` once per U-Net: a list or tuple must have one entry per U-Net, anything else applies to every one."""
@@ -631,6 +727,36 @@ class Imagen(nn.Module):
             images.shape[2] == images.shape[3], \
             f'{name} must be (b, channels, s, s) = ({b}, {self.channels}, s, s), got {tuple(images.shape)}'
 
+    def _negative_prompt(self, negative, b, device):
+        """(negative_text_embeds, negative_text_masks) with b rows on `device` (None, None without a negative prompt)."""
+        texts, embeds, masks = negative
+        if exists(texts):
+            texts = [texts] if isinstance(texts, str) else list(texts)
+            assert len(texts) in (1, b) and all(isinstance(v, str) for v in texts), \
+                f'negative_texts must be a str or a list of 1 or b = {b} str, got {len(texts)} entries'
+            embeds, masks = t5_encode_text(texts, name=self.text_encoder_name)
+        if not exists(embeds):
+            return None, None
+        assert torch.is_tensor(embeds) and embeds.dim() == 3 and embeds.shape[0] in (1, b) and \
+            embeds.shape[-1] == self.text_embed_dim, \
+            f'negative_text_embeds must be (1 or b, n, text_embed_dim) = (1 or {b}, n, {self.text_embed_dim}), got ' \
+            f'{tuple(embeds.shape) if torch.is_tensor(embeds) else type(embeds).__name__}'
+        if exists(masks):
+            assert torch.is_tensor(masks) and tuple(masks.shape) == tuple(embeds.shape[:2]), \
+                f'negative_text_masks must be (rows, n) = {tuple(embeds.shape[:2])} like negative_text_embeds, got ' \
+                f'{tuple(masks.shape) if torch.is_tensor(masks) else type(masks).__name__}'
+            masks = masks.to(device).expand(b, -1).contiguous()
+        return embeds.to(device=device, dtype=F32).expand(b, -1, -1).contiguous(), masks
+
+    def _check_scale(self, w, b, unet_number):
+        """A per-image cond_scale tensor: 1-D, float, b finite entries."""
+        if not torch.is_tensor(w):
+            return
+        assert w.is_floating_point() and w.dim() == 1 and w.shape[0] == b, \
+            f'cond_scale of unet {unet_number} must be a 1-D float tensor of b = {b} per-image weights, got ' \
+            f'{tuple(w.shape)} {w.dtype}'
+        assert bool(torch.isfinite(w).all()), f'cond_scale of unet {unet_number} must be finite, got {w.tolist()}'
+
     def _sampling_steps(self, sampling_timesteps, ddim_eta):
         """Per-U-Net step counts (None = the DDPM loop), validated."""
         assert 0. <= ddim_eta <= 1., f'ddim_eta must be between 0 and 1, got {ddim_eta}'
@@ -643,7 +769,7 @@ class Imagen(nn.Module):
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
                      device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim', init_images=None,
-                     skips=None, start_at=1, stop_at=None, start_images=None):
+                     skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None)):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -668,6 +794,10 @@ class Imagen(nn.Module):
                 self._check_images(init, b, f'init_images of unet {i}')
         if exists(start_images):
             self._check_images(start_images, b, 'start_images')
+        scales = self._per_unet(cond_scale, 'cond_scale')
+        for i, w in enumerate(scales, 1):
+            self._check_scale(w, b, i)
+        neg_embeds, neg_masks = self._negative_prompt(negative, b, device)
 
         world, rank = 1, 0
         if distributed:
@@ -678,15 +808,19 @@ class Imagen(nn.Module):
             assert full_b % world == 0, f'batch {full_b} must divide evenly over {world} ranks'
             per = full_b // world
             rows = lambda v: v[rank * per:(rank + 1) * per] if exists(v) else None
-            text_embeds, text_masks, inpaint_images, inpaint_masks, start_images = map(
-                rows, (text_embeds, text_masks, inpaint_images, inpaint_masks, start_images))
+            text_embeds, text_masks, inpaint_images, inpaint_masks, start_images, neg_embeds, neg_masks = map(
+                rows, (text_embeds, text_masks, inpaint_images, inpaint_masks, start_images, neg_embeds, neg_masks))
             init_images = tuple(map(rows, init_images))
+            scales = tuple(rows(w) if torch.is_tensor(w) else w for w in scales)
 
         batch_size = text_embeds.shape[0]
         if exists(inpaint):
             inpaint_images = inpaint_images.to(device=device, dtype=F32).contiguous()
             inpaint_masks = inpaint_masks.to(device=device, dtype=F32)[:, None].contiguous()
         init_images = tuple(maybe(lambda v: v.to(device=device, dtype=F32).contiguous())(v) for v in init_images)
+        scales = tuple(w.to(device=device, dtype=F32).contiguous() if torch.is_tensor(w) else w for w in scales)
+        neg_embeds = maybe(lambda v: v.contiguous())(neg_embeds)
+        neg_masks = maybe(lambda v: v.contiguous())(neg_masks)
         text_embeds = text_embeds.to(device=device, dtype=F32).contiguous()
         text_masks = text_masks.to(device).contiguous() if exists(text_masks) else None
         lowres_sample_noise_level = default(lowres_sample_noise_level, self.lowres_sample_noise_level)
@@ -701,8 +835,8 @@ class Imagen(nn.Module):
         steps = default(steps, (None,) * n_stages)
         skips = default(skips, (0,) * n_stages)
         stages = list(zip(range(1, n_stages + 1), self.unets, self.sample_channels, self.image_sizes,
-                          self.noise_schedulers, steps, init_images, skips))[start_at - 1:stop_at]
-        for unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip in stages:
+                          self.noise_schedulers, steps, init_images, skips, scales))[start_at - 1:stop_at]
+        for unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip, stage_scale in stages:
             with self._one_unet_in_gpu(unet=unet):
                 lowres_cond_img = lowres_noise_times = None
                 if unet.lowres_cond:
@@ -743,9 +877,10 @@ class Imagen(nn.Module):
                     stage_inpaint = (self.normalize_img(k).contiguous(), m.reshape(batch_size, -1).contiguous(),
                                      resample_times)
                 img = self._p_sample_loop(unet, shape, text_embeds=text_embeds, text_mask=text_masks,
-                                          cond_scale=cond_scale, lowres_cond_img=lowres_cond_img,
+                                          cond_scale=stage_scale, lowres_cond_img=lowres_cond_img,
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
-                                          out=slot, schedule=schedule, inpaint=stage_inpaint, init_image=stage_init)
+                                          out=slot, schedule=schedule, inpaint=stage_inpaint, init_image=stage_init,
+                                          negative_text_embeds=neg_embeds, negative_text_mask=neg_masks)
 
         outputs = img
         if gathered is not None:

@@ -26,6 +26,19 @@ def _chk_out(t, dtype, name):
         raise TypeError(f"{name}: expected {dtype}, got {t.dtype}")
 
 
+def _scale_args(cond_scale, B, entry):
+    """(entry point, scale arguments): a Python number takes `entry` itself; an fp32 CUDA tensor of B per-image guidance
+    weights takes `entry`_w, whose w pointer follows the (then ignored) scalar."""
+    if not torch.is_tensor(cond_scale):
+        return entry, (float(cond_scale),)
+    _chk(cond_scale, F32, "cond_scale")
+    if not cond_scale.is_cuda:
+        raise ValueError("cond_scale: a per-image weight tensor must be on a CUDA device")
+    if cond_scale.numel() != B:
+        raise ValueError(f"cond_scale: expected {B} per-image weights, got {cond_scale.numel()}")
+    return entry + "_w", (1.0, N.ptr(cond_scale))
+
+
 class NativeOps:
     name = "native-sm90a"
     attention_tc = True      # wgmma attention core where the shape allows (mi_attention_fwd workspace)
@@ -223,7 +236,8 @@ class NativeOps:
 
     def step_epilogue(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, noise, B, n, rank_lo,
                       rank_hi, weight, min_s, out, s_out=None):
-        """CFG combine + x0 + exact dynamic-threshold quantile + clamp/divide + posterior mean + noise; `out` may be `x_t`."""
+        """CFG combine + x0 + exact dynamic-threshold quantile + clamp/divide + posterior mean + noise; `out` may be `x_t`.
+        `cond_scale`: a number, or an fp32 CUDA tensor of B guidance weights, one per image (mi_step_epilogue_w)."""
         for nm, tt in (("x_t", x_t), ("eps_cond", eps_cond), ("eps_null", eps_null), ("tab_a", tab_a), ("tab_b", tab_b),
                        ("c1", c1), ("c2", c2), ("sigma", sigma), ("noise", noise), ("out", out), ("s_out", s_out)):
             _chk(tt, F32, nm)
@@ -234,14 +248,15 @@ class NativeOps:
             ws = torch.empty(nws, dtype=F32, device=x_t.device)
             if s_out is None:
                 s_out = torch.empty(B, dtype=F32, device=x_t.device)
-        N.call("mi_step_epilogue", N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), float(cond_scale), N.ptr(t), N.ptr(tab_a),
-               N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(noise), B, n, int(rank_lo), int(rank_hi),
+        entry, scale = _scale_args(cond_scale, B, "mi_step_epilogue")
+        N.call(entry, N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), *scale, N.ptr(t), N.ptr(tab_a), N.ptr(tab_b),
+               N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(noise), B, n, int(rank_lo), int(rank_hi),
                float(weight), float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
 
     def step_epilogue_multistep(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist,
                                 B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
         """step_epilogue plus c3[t] * hist in the mean (skipped where c3[t] == 0); then hist <- the clamped x0.
-        `out` may be `x_t`; `hist` [B, n] must not alias the other tensors."""
+        `out` may be `x_t`; `hist` [B, n] must not alias the other tensors.  `cond_scale` as in step_epilogue."""
         for nm, tt in (("x_t", x_t), ("eps_cond", eps_cond), ("eps_null", eps_null), ("tab_a", tab_a), ("tab_b", tab_b),
                        ("c1", c1), ("c2", c2), ("sigma", sigma), ("c3", c3), ("noise", noise), ("hist", hist),
                        ("out", out), ("s_out", s_out)):
@@ -257,8 +272,9 @@ class NativeOps:
             ws = torch.empty(nws, dtype=F32, device=x_t.device)
             if s_out is None:
                 s_out = torch.empty(B, dtype=F32, device=x_t.device)
-        N.call("mi_step_epilogue_multistep", N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), float(cond_scale), N.ptr(t),
-               N.ptr(tab_a), N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(c3), N.ptr(noise), N.ptr(hist), B, n,
+        entry, scale = _scale_args(cond_scale, B, "mi_step_epilogue_multistep")
+        N.call(entry, N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), *scale, N.ptr(t), N.ptr(tab_a), N.ptr(tab_b),
+               N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(c3), N.ptr(noise), N.ptr(hist), B, n,
                int(rank_lo), int(rank_hi), float(weight), float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
 
     def step_advance_t(self, t, B):
