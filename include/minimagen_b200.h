@@ -301,6 +301,15 @@ int mi_inpaint_finalize(const float* x, const float* k, const float* m, int B, i
 int mi_q_sample(const float* x0, const float* noise, const long long* t, const float* sqrt_alphas_cumprod,
                 const float* sqrt_one_minus_alphas_cumprod, int B, int n, float post_scale, float post_shift,
                 float* out, void* stream);
+/* Keyed standard normals (Imagen.sample(seed=)): out [B, n] fp32, row b a pure function of (seeds[b], stage, kind, label,
+ * element index), so an image's draws do not depend on its batch position, the batch size or the launch.  Philox4x32-10
+ * keyed by seeds[b] (int64 on the device, as (lo32, hi32)) over the counter (j / 4, label mod 2^32, kind, stage) for element
+ * j, lane j % 4; Box-Muller on the pairs of each quad (the generator is specified in csrc/step.cu).  kind: 0 'init',
+ * 1 'step', 2 'lowres', 3 'renoise', 4 'inpaint'; stage: the U-Net number (>= 0).  The label is `label` when t is NULL;
+ * otherwise t[b] * (R ? R[0] : 1) + (r ? r[b] : 0), read on the device (t, r [B], R [1] int64), so the draw can sit inside
+ * a captured CUDA graph.  n / 4 must fit in 32 bits. */
+int mi_randn_keyed(float* out, const long long* seeds, int B, long long n, int kind, int stage, const long long* t,
+                   const long long* r, const long long* R, long long label, void* stream);
 
 /* ------------------------------------------------------------------------------------------------- training (backward)
  * The training side of the same path: Imagen.forward / _p_losses (Imagen.py:512-650) back-propagate through Unet.forward

@@ -9,7 +9,7 @@ nothing on the host.  Sampling captures three graph flavours: text-only (one gra
 step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).  The guidance weights are per-image
 data in a static buffer, so every flavour's graph serves every `cond_scale` and every negative prompt of its shape.
 
-Seven additions that the reference does not have (all optional, defaults reproduce the reference):
+Eight additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -29,7 +29,10 @@ Seven additions that the reference does not have (all optional, defaults reprodu
   * negative prompts and per-image, per-stage guidance (`sample(..., negative_texts= or negative_text_embeds=,
     cond_scale=)`): the guidance pass conditions the U-Net on the negative prompt instead of the learned null
     conditioning, eps = eps_neg + (eps_cond - eps_neg) * w, and w may differ per image and per stage.  The guidance pass
-    runs iff some image's w != 1.
+    runs iff some image's w != 1;
+  * per-image seeds (`sample(..., seed=)`): every sampling draw is a pure function of (the image's seed, stage, kind,
+    label, element index), counter-based Philox drawn on the device (mi_randn_keyed, inside the captured step), so an
+    image can be regenerated on its own, at any batch position, batch size or rank count.
 
 `noise_fn` kinds: 'init' (x_T, step -1; with an init image k, the noise z of the start sqrt(a_t0) k + sqrt(1 - a_t0) z,
 t0 the walk's first point), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
@@ -37,6 +40,8 @@ augmentation noise, labelled with the U-Net number).  Inpainting labels the draw
 t * R + r (at R = 1 that is t) and takes them in this order: 'renoise' (the re-noising draw, r > 0 only), 'inpaint' (the
 noise of the pasted known region), 'step'.  DPM-Solver++(2M) takes the 'step' draws of DDIM with eta = 0 (one per grid
 point, multiplied by a zero sigma).
+A seeded run takes exactly these draws, in this order, from mi_randn_keyed with kind 0 'init', 1 'step', 2 'lowres',
+3 'renoise', 4 'inpaint', the same labels (mod 2^32; 'init' is -1) and the U-Net number as the stage.
 """
 import math
 import numbers
@@ -56,6 +61,8 @@ from .ops import get_ops
 from .t5 import get_encoded_dim, t5_encode_text
 
 F32 = torch.float32
+# the `kind` word of a keyed draw's counter (mi_randn_keyed)
+NOISE_KINDS = {'init': 0, 'step': 1, 'lowres': 2, 'renoise': 3, 'inpaint': 4}
 
 
 def quantile_rank(n: int, q: float):
@@ -103,7 +110,9 @@ class _StepGraph:
          hist   multistep graphs only: [B, C, s, s], the previous step's clamped x0 (zeroed at the start of every loop); the
                 sched copy then also has c3 [T];
          w      [B] fp32 the per-image guidance weights (`set_cond` refreshes them); guided graphs with a negative prompt
-                also hold static negative_text_embeds / negative_text_mask in `cond`.
+                also hold static negative_text_embeds / negative_text_mask in `cond`;
+         seeds  seeded graphs only: [B] int64 per-image seeds (`set_cond` refreshes them); the body then draws its noise
+                with mi_randn_keyed at the current t (and r, R) instead of normal_().
     Three flavours: text-only (the step, then mi_step_advance_t_table), inpainting (draws, mi_inpaint_prologue, the step,
     mi_inpaint_advance) and multistep (the draw, mi_step_epilogue_multistep's step, mi_step_advance_t_table).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
     for DDPM; `* ((S-1) R + 1)` when inpainting) -- no per-step host-side tensor ops."""
@@ -115,6 +124,7 @@ class _StepGraph:
         self.sched = None
         self.hist = None
         self.w = None
+        self.seeds = None
         self.inp = None
         self.inject_noise = False
         self.unet = None
@@ -128,9 +138,11 @@ class _StepGraph:
             self.inp[name].copy_(v)
         self.inp['R'].fill_(int(R))
 
-    def set_cond(self, w=None, **tensors):
+    def set_cond(self, w=None, seeds=None, **tensors):
         if w is not None:
             self.w.copy_(w)
+        if seeds is not None:
+            self.seeds.copy_(seeds)
         for k, v in tensors.items():
             if v is not None:
                 self.cond[k].copy_(v)
@@ -285,7 +297,13 @@ class Imagen(nn.Module):
         yield
 
     # -------------------------------------------------------------------------------------------- one reverse step
-    def _noise(self, kind, shape, step, device):
+    def _noise(self, kind, shape, step, device, seeds=None, stage=None):
+        """The draw `kind` labelled `step` (module docstring): keyed by the per-image `seeds` ([B] int64 on `device`) and
+        the U-Net number `stage` when given, else from `noise_fn` or torch's generator."""
+        if exists(seeds):
+            out = torch.empty(tuple(shape), dtype=F32, device=device)
+            get_ops().randn_keyed(out, seeds, shape[0], out[0].numel(), NOISE_KINDS[kind], stage, label=step)
+            return out
         if exists(self.noise_fn):
             return self.noise_fn(kind, shape, step).to(device=device, dtype=F32).contiguous()
         return torch.randn(shape, device=device)
@@ -396,9 +414,11 @@ class Imagen(nn.Module):
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
                    cond_scale, inpaint=False, multistep=False, *, negative_text_embeds=None, negative_text_mask=None,
-                   guided=None):
+                   guided=None, seeded=False, stage=None):
         """Only whether the step runs the guidance pass is part of the key, not the weights: they are data in the graph's
-        static w buffer.  The negative prompt's signature counts when it is used, i.e. when guided."""
+        static w buffer.  The negative prompt's signature counts when it is used, i.e. when guided.  A seeded graph (keyed
+        draws, the seeds in its static buffer) is keyed apart, with the stage its draws carry; an unseeded key is
+        unchanged."""
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         guided = _is_guided(cond_scale) if guided is None else guided
         p0 = next(unet.parameters())
@@ -407,6 +427,8 @@ class Imagen(nn.Module):
                sig(lowres_noise_times), p0.data_ptr(), sum(p._version for p in unet.parameters()),
                self.dynamic_thresholding_percentile,
                (sig(negative_text_embeds), sig(negative_text_mask)) if guided else None)
+        if seeded:
+            key = key + (('seeded', stage),)
         if inpaint:
             return key + ('inpaint',)
         return key + ('multistep',) if multistep else key
@@ -420,7 +442,7 @@ class Imagen(nn.Module):
 
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                     lowres_noise_times, cond_scale, schedule=None, inpaint=None, negative_text_embeds=None,
-                    negative_text_mask=None, guided=None):
+                    negative_text_mask=None, guided=None, seeds=None, stage=None):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
         every later sampling loop of the same signature.  Every lookup refreshes the conditioning tensors in its static
         buffers and installs the walk `schedule` (a SamplingSchedule; None: the DDPM walk) in its static tables: the step
@@ -432,7 +454,10 @@ class Imagen(nn.Module):
         A multistep `schedule` (with c3) selects the multistep flavour, keyed apart from the other two: static c1 / c2 / c3 /
         sigma / next_t tables and the x0 history `hist`, stepped by mi_step_epilogue_multistep.
         `cond_scale` (a number or per-image weights) is installed in the static w buffer: only `guided` (some weight != 1)
-        and, when guided, the negative prompt's shapes are part of the signature."""
+        and, when guided, the negative prompt's shapes are part of the signature.
+        `seeds` ([B] int64 per-image seeds) selects the seeded variant of the flavour, keyed apart with the U-Net number
+        `stage`: its body draws with mi_randn_keyed at the current t (and r, R) and the seeds are installed in its static
+        buffer, so one graph serves every seed."""
         device = self.device
         schedule = default(schedule, lambda: noise_scheduler.ddpm_schedule(device))
         multistep = exists(schedule.c3)
@@ -443,7 +468,7 @@ class Imagen(nn.Module):
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                               lowres_noise_times, cond_scale, exists(inpaint), multistep,
                               negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
-                              guided=guided)
+                              guided=guided, seeded=exists(seeds), stage=stage)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times, negative_text_embeds=negative_text_embeds,
                     negative_text_mask=negative_text_mask)
@@ -451,7 +476,7 @@ class Imagen(nn.Module):
              torch.full((shape[0],), float(cond_scale), dtype=F32, device=device))
         g = self._graphs.get(key)
         if g is not None:
-            g.set_cond(w=w, **cond)
+            g.set_cond(w=w, seeds=seeds, **cond)
         else:
             if len(self._graphs) >= self.max_cached_graphs:
                 self._graphs.pop(next(iter(self._graphs))).release()
@@ -463,6 +488,8 @@ class Imagen(nn.Module):
             g.t = torch.zeros((shape[0],), dtype=torch.long, device=device)
             g.cond = {k: v.clone() for k, v in cond.items() if v is not None}
             g.w = w.clone()
+            if exists(seeds):
+                g.seeds = seeds.to(device=device, dtype=torch.long).clone()
             kw = dict(noise_scheduler=noise_scheduler, cond_scale=g.w, guided=guided,
                       **{k: g.cond.get(k) for k in cond})
             g.refresh_static()
@@ -489,7 +516,15 @@ class Imagen(nn.Module):
                                  z_known=torch.zeros(shape, dtype=F32, device=device))
 
             def body():
-                if not g.inject_noise:
+                if exists(g.seeds):
+                    # keyed draws at the current t (t * R + r when inpainting): those an eager seeded loop takes
+                    n = C * hw
+                    lab = dict(t=g.t, r=p['r'], R=p['R']) if exists(p) else dict(t=g.t)
+                    if exists(p):
+                        ops.randn_keyed(p['z_renoise'], g.seeds, B, n, NOISE_KINDS['renoise'], stage, **lab)
+                        ops.randn_keyed(p['z_known'], g.seeds, B, n, NOISE_KINDS['inpaint'], stage, **lab)
+                    ops.randn_keyed(g.noise, g.seeds, B, n, NOISE_KINDS['step'], stage, **lab)
+                elif not g.inject_noise:
                     if exists(p):
                         p['z_renoise'].normal_()        # drawn every iteration, read only where r > 0
                         p['z_known'].normal_()
@@ -525,7 +560,7 @@ class Imagen(nn.Module):
     @torch.no_grad()
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
                        lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None,
-                       init_image=None, negative_text_embeds=None, negative_text_mask=None):
+                       init_image=None, negative_text_embeds=None, negative_text_mask=None, seeds=None, stage=1):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
@@ -547,7 +582,9 @@ class Imagen(nn.Module):
         instead of x_T: noised to the walk's first point t0 with the 'init' draw z, x_t0 = sqrt(a_t0) init + sqrt(1 - a_t0) z
         (mi_q_sample).  A walk that starts below T-1 (a shortened grid) wants one.
         `cond_scale` (not in the reference: also an fp32 [B] tensor of per-image weights on the sampling device) and
-        `negative_text_embeds` / `negative_text_mask` (not in the reference) guide as in `_step`."""
+        `negative_text_embeds` / `negative_text_mask` (not in the reference) guide as in `_step`.
+        `seeds` (not in the reference): [B] int64 per-image seeds on the sampling device; every draw of the loop is then
+        keyed by them and by `stage` (the U-Net number), eager or captured (module docstring)."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -568,7 +605,8 @@ class Imagen(nn.Module):
             else:
                 draws = [[('step', t)] for t, _ in plan]
             B, C, hw = shape[0], shape[1], shape[2] * shape[3]
-            img = self._noise('init', shape, -1, device)
+            keyed = dict(seeds=seeds, stage=stage) if exists(seeds) else {}
+            img = self._noise('init', shape, -1, device, **keyed)
             if exists(init_image):
                 x_t0 = torch.empty(tuple(shape), dtype=F32, device=device)
                 t0 = torch.full((B,), plan[0][0], dtype=torch.long, device=device)
@@ -581,7 +619,7 @@ class Imagen(nn.Module):
                       negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
                       guided=_is_guided(cond_scale))
             if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
-                g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, **kw)
+                g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, **keyed, **kw)
                 static = dict(step=g.noise)
                 if exists(inpaint):
                     static.update(renoise=g.inp['z_renoise'], inpaint=g.inp['z_known'])
@@ -602,7 +640,7 @@ class Imagen(nn.Module):
                     img = img.clone()           # the prologue works in place; x_T may be the caller's draw
                 hist = torch.zeros(tuple(shape), dtype=F32, device=device) if multistep else None
                 for (t, r), iteration in zip(plan, draws):
-                    z = {kind: self._noise(kind, shape, label, device) for kind, label in iteration}
+                    z = {kind: self._noise(kind, shape, label, device, **keyed) for kind, label in iteration}
                     times = torch.full((B,), t, device=device, dtype=torch.long)
                     if exists(inpaint):
                         reps = torch.full((B,), r, device=device, dtype=torch.long)
@@ -627,7 +665,7 @@ class Imagen(nn.Module):
                distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0., inpaint_images=None,
                inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim', init_images=None,
                skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None,
-               negative_texts=None, negative_text_embeds=None, negative_text_masks=None):
+               negative_texts=None, negative_text_embeds=None, negative_text_masks=None, seed=None):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -660,7 +698,21 @@ class Imagen(nn.Module):
         `negative_texts` (a str, or a list of 1 or b str, encoded like `texts`) or `negative_text_embeds` ((1 or b, n,
         text_embed_dim), with optional `negative_text_masks` (1 or b, n) bool; one row is used for every image) replace
         the learned null conditioning of the guidance pass: eps = eps_neg + (eps_cond - eps_neg) * w.  Captured step graphs
-        are keyed on the shapes only, so changing w or the negative prompt reuses them."""
+        are keyed on the shapes only, so changing w or the negative prompt reuses them.
+        `seed` (None, an int s >= 0 with s + b - 1 < 2^63, or a list or 1-D integer tensor of b seeds in [0, 2^63)) makes
+        every draw of image i a pure function of its seed: an int s gives image i the seed s + i, so image 7 of a seed-s
+        batch is image 0 of a seed-(s + 7) run, and an image's result does not depend on the batch it is sampled in,
+        its position there, the rank count, graph or eager execution, or whether the stage before ran in the same call
+        (up to the rounding of batched kernels).  The generator: Philox4x32-10 (Random123 / cuRAND round constants M = 0xD2511F53, 0xCD9E8D57,
+        W = 0x9E3779B9, 0xBB67AE85) keyed by the seed as (lo32, hi32), over the counter (j / 4, label mod 2^32, kind,
+        stage) for element j of the image's flattened C*H*W data (lane j % 4); kind 0 'init', 1 'step', 2 'lowres',
+        3 'renoise', 4 'inpaint' with the `noise_fn` labels of the module docstring, stage the U-Net number.  Each pair
+        (x_a, x_b) of a quad gives u = ((x_a >> 9) + 0.5) 2^-23 and v = (x_b >> 8) 2^-24, both exact in fp32, and the
+        normals sqrt(-2 ln u) cos(2 pi v), sqrt(-2 ln u) sin(2 pi v) (precise logf / sqrtf / cospif / sinpif), so
+        |z| <= 5.77.  The draws run on the device, inside the captured step.  Cannot be combined with `noise_fn`; labels
+        must fit in 32 bits (timesteps * inpaint_resample_times < 2^31).  None (the default) draws from torch's
+        generator as before; with `distributed=True` that is each rank's own generator, which the caller must seed
+        per rank for the ranks to draw different noise."""
         assert sampler in ('ddim', 'dpmpp_2m'), f"sampler must be 'ddim' or 'dpmpp_2m', got {sampler!r}"
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
         if sampler == 'dpmpp_2m':
@@ -701,6 +753,14 @@ class Imagen(nn.Module):
             'inpaint_images and inpaint_masks must be given together'
         assert _is_int(inpaint_resample_times) and inpaint_resample_times >= 1, \
             f'inpaint_resample_times must be an int >= 1, got {inpaint_resample_times!r}'
+        if exists(seed):
+            self._check_seed(seed)
+            R = inpaint_resample_times if exists(inpaint_images) else 1
+            for i in range(start_at_unet_number, stop_at_unet_number + 1):
+                T = self.noise_schedulers[i - 1].num_timesteps
+                assert T * R < 2 ** 31, \
+                    f'with a seed, timesteps * inpaint_resample_times must be below 2^31 (the 32-bit draw labels), got ' \
+                    f'{T} * {R} for unet {i}'
         device = torch.device(default(device, self.device))
         self._reset_unets_all_one_device(device=device)
         if self._temp.device != device:
@@ -710,7 +770,32 @@ class Imagen(nn.Module):
             return self._sample_impl(texts, text_masks, text_embeds, scales, lowres_sample_noise_level,
                                      return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler,
                                      init_images, skips, start_at_unet_number, stop_at_unet_number, start_images,
-                                     negative)
+                                     negative, seed)
+
+    def _check_seed(self, seed):
+        """`seed`: an int >= 0, or a non-empty list or 1-D integer tensor of seeds in [0, 2^63); never with noise_fn."""
+        assert not exists(self.noise_fn), 'seed and noise_fn cannot both be given: noise_fn supplies every draw'
+        if _is_int(seed):
+            assert seed >= 0, f'seed must be >= 0, got {seed}'
+            return
+        ok = (isinstance(seed, (list, tuple)) and len(seed) > 0 and all(_is_int(s) for s in seed)) or \
+            (torch.is_tensor(seed) and seed.dim() == 1 and seed.numel() > 0 and not seed.is_floating_point() and
+             not seed.is_complex() and seed.dtype != torch.bool)
+        assert ok, f'seed must be an int, or a list or 1-D integer tensor of per-image seeds, got {seed!r}'
+        values = seed.tolist() if torch.is_tensor(seed) else list(seed)
+        assert all(0 <= s < 2 ** 63 for s in values), f'per-image seeds must be between 0 and 2^63 - 1, got {values}'
+
+    def _seeds(self, seed, b, device):
+        """The per-image seeds of the full batch of b images as a [b] int64 tensor on `device` (None without a seed):
+        an int s gives image i the seed s + i."""
+        if seed is None:
+            return None
+        if _is_int(seed):
+            assert seed + b - 1 < 2 ** 63, f'seed + b - 1 must be below 2^63, got seed {seed} with b = {b}'
+            return torch.arange(seed, seed + b, dtype=torch.long, device=device)
+        seeds = seed if torch.is_tensor(seed) else torch.tensor(seed, dtype=torch.long)
+        assert seeds.numel() == b, f'seed must have one entry per image (b = {b}), got {seeds.numel()}'
+        return seeds.to(device=device, dtype=torch.long).contiguous()
 
     def _per_unet(self, value, name):
         """`value` once per U-Net: a list or tuple must have one entry per U-Net, anything else applies to every one."""
@@ -769,7 +854,7 @@ class Imagen(nn.Module):
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
                      device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim', init_images=None,
-                     skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None)):
+                     skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None), seed=None):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -798,6 +883,7 @@ class Imagen(nn.Module):
         for i, w in enumerate(scales, 1):
             self._check_scale(w, b, i)
         neg_embeds, neg_masks = self._negative_prompt(negative, b, device)
+        seeds = self._seeds(seed, b, device)
 
         world, rank = 1, 0
         if distributed:
@@ -808,8 +894,9 @@ class Imagen(nn.Module):
             assert full_b % world == 0, f'batch {full_b} must divide evenly over {world} ranks'
             per = full_b // world
             rows = lambda v: v[rank * per:(rank + 1) * per] if exists(v) else None
-            text_embeds, text_masks, inpaint_images, inpaint_masks, start_images, neg_embeds, neg_masks = map(
-                rows, (text_embeds, text_masks, inpaint_images, inpaint_masks, start_images, neg_embeds, neg_masks))
+            text_embeds, text_masks, inpaint_images, inpaint_masks, start_images, neg_embeds, neg_masks, seeds = map(
+                rows, (text_embeds, text_masks, inpaint_images, inpaint_masks, start_images, neg_embeds, neg_masks,
+                       seeds))
             init_images = tuple(map(rows, init_images))
             scales = tuple(rows(w) if torch.is_tensor(w) else w for w in scales)
 
@@ -843,7 +930,8 @@ class Imagen(nn.Module):
                     sch = self.lowres_noise_schedule
                     lowres_noise_times = sch._get_times(batch_size, lowres_sample_noise_level, device=device)
                     lowres_cond_img = resize_image_to(img, image_size, pad_mode='reflect').to(F32).contiguous()
-                    aug_noise = self._noise('lowres', lowres_cond_img.shape, unet_number, device)
+                    aug_noise = self._noise('lowres', lowres_cond_img.shape, unet_number, device,
+                                            **(dict(seeds=seeds, stage=unet_number) if exists(seeds) else {}))
                     noised = torch.empty_like(lowres_cond_img)
                     # NB: like the reference (Imagen.py:483 vs :393) the [0,1] image is noised BEFORE normalisation
                     ops.q_sample(lowres_cond_img, aug_noise, lowres_noise_times, sch.sqrt_alphas_cumprod,
@@ -880,7 +968,8 @@ class Imagen(nn.Module):
                                           cond_scale=stage_scale, lowres_cond_img=lowres_cond_img,
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
                                           out=slot, schedule=schedule, inpaint=stage_inpaint, init_image=stage_init,
-                                          negative_text_embeds=neg_embeds, negative_text_mask=neg_masks)
+                                          negative_text_embeds=neg_embeds, negative_text_mask=neg_masks, seeds=seeds,
+                                          stage=unet_number)
 
         outputs = img
         if gathered is not None:

@@ -64,6 +64,7 @@ SIGNATURES = {
     "mi_inpaint_advance": [_P, _P, _P, _P, _I, _I, _P],
     "mi_inpaint_finalize": [_P, _P, _P, _I, _I, _I, _I, _P, _P],
     "mi_q_sample": [_P, _P, _P, _P, _P, _I, _I, _F, _F, _P, _P],
+    "mi_randn_keyed": [_P, _P, _I, _L, _I, _I, _P, _P, _P, _L, _P],
     # training side (backward)
     "mi_gemm_f32": [_P, _P, _P, _I, _I, _I, _L, _L, _L, _L, _L, _L, _I, _I, _L, _L, _L, _L, _L, _L, _F, _I, _P],
     "mi_colsum_f32": [_P, _L, _I, _P, _I, _P],

@@ -350,6 +350,10 @@ int mi_q_sample(const float* x0, const float* noise, const long long* t, const f
                 int n, float post_scale, float post_shift, float* out, void* stream) {
     return check(mi::q_sample(x0, noise, t, tab_a, tab_b, B, n, post_scale, post_shift, out, S(stream)), "mi_q_sample");
 }
+int mi_randn_keyed(float* out, const long long* seeds, int B, long long n, int kind, int stage, const long long* t,
+                   const long long* r, const long long* R, long long label, void* stream) {
+    return check(mi::randn_keyed(out, seeds, B, n, kind, stage, t, r, R, label, S(stream)), "mi_randn_keyed");
+}
 
 int mi_gemm_f32(const float* A, const float* B, float* C, int M, int N, int K, long long a_sm, long long a_sk,
                 long long b_sk, long long b_sn, long long c_sm, long long c_sn, int Z1, int Z2, long long a_b1,

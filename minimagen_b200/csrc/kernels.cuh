@@ -94,6 +94,8 @@ int inpaint_finalize(const float* x, const float* k, const float* m, int B, int 
                      cudaStream_t st);
 int q_sample(const float* x0, const float* noise, const long long* t, const float* tab_a, const float* tab_b, int B,
              int n_per_img, float post_scale, float post_shift, float* out, cudaStream_t st);
+int randn_keyed(float* out, const long long* seeds, int B, long long n, int kind, int stage, const long long* t,
+                const long long* r, const long long* R, long long label, cudaStream_t st);
 
 // backward.cu: fp32 backward kernels of the training side (SURVEY 8f-2)
 int gemm_f32(const float* A, const float* B, float* C, int M, int N, int K, long long a_sm, long long a_sk, long long b_sk,

@@ -14,7 +14,23 @@
 // The select of step 2 exists twice, and each is the other's test reference: quantile_kernel (one CTA per image, keys
 // streamed from global memory, any n) and the one inside step_epilogue_kernel (an 8-CTA cluster per image, keys held in
 // registers, n <= 196 608).  Both end in step_threshold.
+//
+// Keyed sampling noise (mi_randn_keyed, Imagen.sample(seed=)): a stateless counter-based generator, so that every draw is
+// a pure function of (image seed, stage, draw kind, label, element index) -- independent of the batch layout, the rank
+// count, graph or eager execution and skipped steps, and computable inside a captured graph that reads everything from
+// device buffers.
+//   key      the image's 64-bit seed s as (lo32, hi32)
+//   counter  (q, label mod 2^32, kind, stage): element j of the image's flattened C*H*W NCHW data is lane j % 4 of quad
+//            q = j / 4; kind is 0 'init', 1 'step', 2 'lowres', 3 'renoise', 4 'inpaint'; stage is the U-Net number
+//   bits     Philox4x32-10 with the Random123 / cuRAND constants M = 0xD2511F53, 0xCD9E8D57, W = 0x9E3779B9, 0xBB67AE85
+//   normals  Box-Muller on each pair (x_a, x_b) = (x0, x1), (x2, x3) of the quad:
+//              u = ((x_a >> 9) + 0.5) 2^-23 in (0, 1) and v = (x_b >> 8) 2^-24 in [0, 1), both exact in fp32
+//              (u keeps 23 bits: (m + 0.5) with a 24-bit m would need 25 significant bits);
+//              rho = sqrtf(-2 logf(u)); the pair's normals are rho cospif(2v) and rho sinpif(2v).
+//            Precise functions, products rounded on their own (__fmul_rn).  |z| <= sqrt(-2 ln 2^-24) = 5.77 by
+//            construction, since u >= 2^-24.
 #include <cuda_runtime.h>
+#include <curand_philox4x32_x.h>
 #include <float.h>
 #include <stdint.h>
 
@@ -437,7 +453,60 @@ __global__ void inpaint_finalize_kernel(const float* __restrict__ x, const float
     out[idx] = v;
 }
 
+// Box-Muller on one pair of Philox words (header comment): u, v and 2v are exact; logf and sincospif (cospif and sinpif
+// with one argument reduction) are the precise library functions (1 ulp), sqrtf is correctly rounded.
+__device__ __forceinline__ float2 box_muller(uint32_t xa, uint32_t xb) {
+    const float u = __fmul_rn(__fadd_rn((float)(xa >> 9), 0.5f), 0x1p-23f);
+    const float v2 = __fmul_rn((float)(xb >> 8), 0x1p-23f);                 // 2v
+    const float rho = sqrtf(__fmul_rn(-2.f, logf(u)));
+    float s, c;
+    sincospif(v2, &s, &c);
+    return make_float2(__fmul_rn(rho, c), __fmul_rn(rho, s));
+}
+
+// out [B, n]: image b's keyed normals, one Philox call (four values) per thread.  The label is the host's `label`, or
+// t[b] * (R ? R[0] : 1) + (r ? r[b] : 0) read on the device when t is given (a captured step draws at the current t).
+// vec4: n % 4 == 0 and out 16-byte aligned, one float4 store per thread; otherwise scalar stores up to the row's end.
+__global__ void __launch_bounds__(256)
+randn_keyed_kernel(float* __restrict__ out, const long long* __restrict__ seeds, long long n, int kind, int stage,
+                   const long long* __restrict__ t, const long long* __restrict__ r, const long long* __restrict__ R,
+                   long long label, int vec4) {
+    pdl_wait();
+    pdl_trigger();
+    const int b = blockIdx.y;
+    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= (n + 3) / 4) return;
+    const long long lab = t ? t[b] * (R ? R[0] : 1LL) + (r ? r[b] : 0LL) : label;
+    const unsigned long long s = (unsigned long long)seeds[b];
+    const uint4 x = curand_Philox4x32_10(make_uint4((uint32_t)q, (uint32_t)lab, (uint32_t)kind, (uint32_t)stage),
+                                         make_uint2((uint32_t)s, (uint32_t)(s >> 32)));
+    const float2 z01 = box_muller(x.x, x.y), z23 = box_muller(x.z, x.w);
+    float* row = out + (long long)b * n;
+    const long long j = 4 * q;
+    if (vec4) {
+        *reinterpret_cast<float4*>(row + j) = make_float4(z01.x, z01.y, z23.x, z23.y);
+        return;
+    }
+    const float z[4] = {z01.x, z01.y, z23.x, z23.y};
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        if (j + k < n) row[j + k] = z[k];
+}
+
 }  // namespace
+
+int randn_keyed(float* out, const long long* seeds, int B, long long n, int kind, int stage, const long long* t,
+                const long long* r, const long long* R, long long label, cudaStream_t st) {
+    if (B < 0 || n < 0 || kind < 0 || kind > 4 || stage < 0) return -1;
+    if (B == 0 || n == 0) return 0;
+    if (!out || !seeds) return -1;
+    const long long nq = (n + 3) / 4;
+    if (nq > (1LL << 32) || B > 65535) return -1;           // the quad index is a 32-bit counter word
+    const int vec4 = n % 4 == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+    dim3 grid((unsigned)((nq + 255) / 256), B);
+    launch_k(randn_keyed_kernel, grid, 256, 0, st, out, seeds, n, kind, stage, t, r, R, label, vec4);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
 
 int inpaint_prologue(float* x, const long long* t, const long long* r, const float* ra, const float* rb,
                      const float* sqrt_acp, const float* sqrt_1m_acp, const float* k, const float* m,

@@ -330,6 +330,17 @@ class NativeOps:
         N.call("mi_q_sample", N.ptr(x0), N.ptr(noise), N.ptr(t), N.ptr(tab_a), N.ptr(tab_b), B, n, float(post_scale),
                float(post_shift), N.ptr(out), N.stream())
 
+    def randn_keyed(self, out, seeds, B, n, kind, stage, t=None, r=None, R=None, label=0):
+        """out [B, n] fp32 <- image b's keyed normals for (seeds[b], stage, kind, label) (mi_randn_keyed).  The label is
+        `label`, or t[b] * R[0] + r[b] read on the device when t ([B] int64) is given (r, R optional)."""
+        _chk(out, F32, "out"); _chk(seeds, I64, "seeds"); _chk(t, I64, "t"); _chk(r, I64, "r"); _chk(R, I64, "R")
+        if seeds.numel() < B:
+            raise ValueError(f"seeds: expected at least {B} per-image seeds, got {seeds.numel()}")
+        if out.numel() != B * n:
+            raise ValueError(f"out: expected {B * n} values, got {out.numel()}")
+        N.call("mi_randn_keyed", N.ptr(out), N.ptr(seeds), int(B), int(n), int(kind), int(stage), N.ptr(t), N.ptr(r),
+               N.ptr(R), int(label), N.stream())
+
 
     # ---------------------------------------------------------------- training side (backward kernels, fp32)
     def gemm_f32(self, A, B, C, M, N, K, a_str, b_str, c_str, Z1=1, Z2=1, a_b=(0, 0), b_b=(0, 0), c_b=(0, 0), alpha=1.0,
