@@ -17,6 +17,11 @@ def _strided(out, shape, strides):
     return out.as_strided(shape, strides, out.storage_offset())
 
 
+def _sat16(y):
+    """fp32 -> fp16 with saturation (csrc/sat_half.cuh): beyond +-65504 -> +-65504, not inf."""
+    return y.clamp(-65504.0, 65504.0).to(F16)
+
+
 def _cat_src(src0, c0, src1, c1, scale1, lead_shape):
     a = src0.reshape(*lead_shape, c0)
     if src1 is None or c1 == 0:
@@ -111,7 +116,7 @@ class EmuOps:
         if out_f32 is not None:
             _strided(out_f32, (B, H, W, nv), (sb, sh, sw, out_sc)).copy_(y)
         if out_f16 is not None:
-            _strided(out_f16, (B, H, W, nv), (sb, sh, sw, out_sc)).copy_(y.to(F16))
+            _strided(out_f16, (B, H, W, nv), (sb, sh, sw, out_sc)).copy_(_sat16(y))
 
     def conv_res1x1_supported(self, H, W, c_in, c_out, x_cin):
         t16 = W == 16 and H % 16 == 0
@@ -199,7 +204,7 @@ class EmuOps:
             ss = scale_shift.as_strided((B, 2 * C), (ss_ld, 1), scale_shift.storage_offset())
             y = y * (ss[:, None, :C] + 1.0) + ss[:, None, C:]
         y = y * torch.sigmoid(y)
-        out.reshape(B, hw, C).copy_(y.to(out.dtype))
+        out.reshape(B, hw, C).copy_(_sat16(y) if out.dtype == F16 else y)
 
     def cast_act(self, src0, c0, src1, c1, scale1, B, H, W, mode, out):
         self._log("cast_act")

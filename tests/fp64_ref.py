@@ -1,5 +1,7 @@
-"""TEST INFRASTRUCTURE ONLY: float64 references of the token-side kernels and of the image-side training kernels
-(GroupNorm/SiLU backward, convolution weight and data gradients, upsample backward) with elementwise error bounds.
+"""TEST INFRASTRUCTURE ONLY: float64 references of the token-side kernels, of the image-side forward kernels (implicit-GEMM,
+direct and stem convolutions, the conv epilogue's GroupNorm statistics, GroupNorm statistics and GroupNorm/FiLM/SiLU, the
+fused GroupNorm conv) and of the image-side training kernels (GroupNorm/SiLU backward, convolution weight and data
+gradients, upsample backward) with elementwise error bounds.
 
 Every reference takes the operands exactly as the kernel reads them (fp16-rounded where the kernel reads fp16, the null
 key/value included), computes in float64 on the operands' device, and returns (reference, bound): |kernel - reference| <=
@@ -537,3 +539,234 @@ def upsample2x_bwd_ref(dy):
     B, H2, W2, C = dy.shape
     q = dy.float().reshape(B, H2 // 2, 2, W2 // 2, 2, C)
     return (q[:, :, 0, :, 0] + q[:, :, 0, :, 1]) + (q[:, :, 1, :, 0] + q[:, :, 1, :, 1])
+
+
+# ---------------------------------------------------------------------------------------------- convolution forward
+U64 = 2.0 ** -53            # unit roundoff of fp64: the double sums and atomics of the statistics
+ETA_SILU = 2.0 ** -118      # |SiLU(v)| where the fp32 SiLU flushes to 0 (v < -87: 1 + e^-v > 2^126)
+
+
+def unpack_conv_weight(wp, kh, kw, c_in):
+    """The first kh * kw * c_in columns of a packed [C_out][taps * C_in (+ C_x)] weight (tap-major, channel-minor, the
+    layout of mi_pack_conv_weight_f16) as float64 OIHW."""
+    return _d(wp[:, :kh * kw * c_in]).reshape(wp.shape[0], kh, kw, c_in).permute(0, 3, 1, 2)
+
+
+def conv_nhwc(a, w, mode):
+    """Float64 convolution of the NHWC operand `a` with OIHW `w` as mi_conv2d_igemm_f16 reads it in `mode`; NHWC result.
+      mode 0: 'same' k x k conv of a [B, H, W, C];
+      mode 1: the 4x4 stride-2 pad-1 conv of the phase-split a [B, 4, H, W, C] (phase p = (h & 1) * 2 + (w & 1));
+      modes 2..5: sub-pixel phase (pa, pb) = ((mode - 2) >> 1, (mode - 2) & 1) of a [B, H, W, C]: the 2x2 taps of output
+                  pixel (y, x) read the pixels (y + pa - 1 + r, x + pb - 1 + s);
+      mode 6: the 4x4 stride-2 pad-1 conv of a [B, 2H, 2W, C] read in place."""
+    F = torch.nn.functional
+    if mode == 1:
+        B, _, H, W, C = a.shape
+        full = a.new_zeros(B, 2 * H, 2 * W, C)
+        for p in range(4):
+            full[:, (p >> 1)::2, (p & 1)::2] = a[:, p]
+        a, mode = full, 6
+    x = a.permute(0, 3, 1, 2)
+    if mode == 6:
+        y = F.conv2d(x, w, stride=2, padding=1)
+    elif mode == 0:
+        y = F.conv2d(x, w, padding=(w.shape[2] // 2, w.shape[3] // 2))
+    else:
+        pa, pb = (mode - 2) >> 1, (mode - 2) & 1
+        H, W = x.shape[2], x.shape[3]
+        y = F.conv2d(F.pad(x, (1, 1, 1, 1))[:, :, pa:pa + H + 1, pb:pb + W + 1], w)
+    return y.permute(0, 2, 3, 1)
+
+
+def conv_fwd_ref(a, wp, kh, kw, mode=0, bias=None, residual=None, x=None):
+    """conv + bias + residual of mi_conv2d_igemm_f16 / mi_conv3x3_res1x1_f16 (and, with fp32 operands, mi_conv2d_direct_f32):
+    a the fp16 operand as the kernel reads it (see conv_nhwc; a two-source virtual concat is the channel concat of both
+    sources, the skip scale folded into the packed weight), wp the packed fp16 weight [C_out][kh kw C_in (+ C_x)], x the
+    operand of the folded 1x1 conv [B, H, W, C_x] (columns kh kw C_in ... of wp, read at the centre tap), residual
+    [B, H, W, C_out].  Returns (reference NHWC, bound of the fp32 output); half_out gives the fp16 output's.
+
+    Every output element is one fp32 accumulation of n = taps C_in (+ C_x) exact fp16 products, then the bias and the
+    residual adds.  The wgmma k-groups truncate instead of rounding (2.125 U32 twin per product, see conv_wgrad_ref), so
+        3 (n + 2) U32 twin,   twin = sum |a| |w| + |bias| + |residual|.
+    conv_direct_f32 is an fma chain over taps x ceil4(C_in) products (2 n U32 twin): the same form with that n; the stem's
+    15-tap GEMM over 128 unrolled channels has n = 15 x 128."""
+    c_in = a.shape[-1]
+    w = unpack_conv_weight(wp, kh, kw, c_in).to(a.device)
+    a64 = _d(a)
+    ref, twin = conv_nhwc(a64, w, mode), conv_nhwc(a64.abs(), w.abs(), mode)
+    n = kh * kw * c_in
+    if x is not None:
+        wx, x64 = _d(wp[:, n:]).to(a.device), _d(x)
+        ref, twin = ref + x64 @ wx.t(), twin + x64.abs() @ wx.abs().t()
+        n += x.shape[-1]
+    for t in (bias, residual):
+        if t is not None:
+            ref, twin = ref + _d(t), twin + _d(t).abs()
+    return ref, 3 * (n + 2) * U32 * twin
+
+
+def conv_stats_acc_len():
+    """Rounding steps behind one (image, 16-channel block) statistic of the conv epilogue (csrc/conv_tc.cu): a thread adds
+    its 8 values of the block (2 rows x 2 column pairs, each pair summed first; for the squares one product and one fma per
+    pair) in fp32 -- at most 8 roundings on any value's path -- then 5 xor-shuffle levels add the warp's 32 partials in
+    fp32; the rest (per warp or per warpgroup) is fp64."""
+    return 8 + 5 + 1
+
+
+def conv_stats_ref(out32, sb=16):
+    """The epilogue's GroupNorm statistics, per (image, sb-channel block), of the kernel's OWN fp32 output out32
+    [B, ..., C] (valid pixels only; the phases of modes 2..5 all in one tensor): float64 (sum, sum of squares) [B, C/sb, 2]
+    and their bound
+        2 acc_len U32 sum|f|  (resp. sum f^2)  +  P U64 (same),
+    acc_len = conv_stats_acc_len(), P the pixel count (more than the fp64 adds of any reduction order).  Because it compares
+    with the output the kernel wrote, not with reference statistics, the bound is tight enough to see one warp's 16 rows, a
+    tile credited to the wrong image, or masked rows that were counted."""
+    f = _d(out32)
+    B, C = f.shape[0], f.shape[-1]
+    fb = f.reshape(B, -1, C // sb, sb)
+    P = fb.shape[1]
+    s, q, t = fb.sum(dim=(1, 3)), (fb * fb).sum(dim=(1, 3)), fb.abs().sum(dim=(1, 3))
+    c = 2 * conv_stats_acc_len() * U32 + P * U64
+    return torch.stack((s, q), dim=-1), torch.stack((c * t, c * q), dim=-1)
+
+
+# ---------------------------------------------------------------------------------------------- GroupNorm forward
+def _f32(v):
+    """A Python scale as the fp32 number the kernels multiply by."""
+    return float(torch.tensor(float(v), dtype=torch.float32))
+
+
+def gn_concat(src0, src1=None, scale1=1.0):
+    """The virtual concat cat(src0, src1 * scale1) [B, HW, C] in float64, src1 scaled by the fp32 scale1 (exact here; the
+    kernels' fp32 product rounds by U32 of it)."""
+    x = _d(src0)
+    if src1 is not None:
+        x = torch.cat((x, _d(src1) * _f32(scale1)), dim=-1)
+    return x
+
+
+def gn_stats_plan(C, HW):
+    """(chunk, planes, L) of gn_stats_kernel (csrc/elementwise.cu, gn_stats): the grid covers `chunk` = clamp(32768 / C, 4,
+    HW) pixels per CTA; its 256 threads split into `planes` = 256 / (C / 8) pixel planes of C / 8 channel vectors (1 plane
+    when C > 2048); a thread's fp32 chain adds every planes-th pixel of the chunk, L = ceil(chunk / planes) values."""
+    chunk = min(max(32768 // C, 4), HW)
+    V = C // 8
+    planes = 256 // V if V <= 256 else 1
+    return chunk, planes, -(-chunk // planes)
+
+
+def gn_stats_ref(src0, groups, src1=None, scale1=1.0, L=None):
+    """mi_gn_stats: per (image, group) float64 (sum, sum of squares) [B, G, 2] of the virtual concat, and the bound
+        (L + 3) U32 sum|x|  (resp. sum x^2)  +  (HW + 2048) U64 (same).
+    A thread's fp32 chain of L values (gn_stats_plan) rounds at most L times on any value's path, the squares once more
+    and the fp32 product x * scale1 once (U32 |x|, 2 U32 x^2); the 8 partials of a thread, the CTA's shared-memory sum and
+    the atomics per chunk are fp64."""
+    x = gn_concat(src0, src1, scale1)
+    B, HW, C = x.shape
+    if L is None:
+        L = gn_stats_plan(C, HW)[2]
+    xg = x.reshape(B, HW, groups, C // groups)
+    s, q, t = xg.sum(dim=(1, 3)), (xg * xg).sum(dim=(1, 3)), xg.abs().sum(dim=(1, 3))
+    c = (L + 3) * U32 + (HW + 2048) * U64
+    return torch.stack((s, q), dim=-1), torch.stack((c * t, c * q), dim=-1)
+
+
+def group_sums(stats0, C0, groups, stats1=None, C1=0, scale1=1.0, sb=16):
+    """Per-source block statistics [B, C_s / sb, 2] (of a conv epilogue, or gn_stats with C_s / sb groups) gathered into
+    the groups of the virtual concat, as gn_apply_silu_kernel and the fused GroupNorm conv gather them (the second source's
+    sums times scale1, its squares times scale1^2).  Works for bounds too (they are non-negative)."""
+    s1 = _f32(scale1)
+    parts = [_d(stats0)]
+    if stats1 is not None and C1:
+        t = _d(stats1).clone()
+        t[..., 0] *= s1
+        t[..., 1] *= s1 * s1
+        parts.append(t)
+    blocks = torch.cat(parts, dim=1)                                   # [B, (C0 + C1) / sb, 2]
+    B = blocks.shape[0]
+    return blocks.reshape(B, groups, -1, 2).sum(dim=2)
+
+
+def _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, fast):
+    """y = SiLU(((x - mean) rstd gamma + beta) (scale + 1) + shift) in float64 from the statistics `sums` [B, G, 2], and
+    the bound of the kernel's fp32 y before any fp16 rounding.  See gn_apply_silu_ref."""
+    B, HW, C = x.shape
+    Cg = C // groups
+    n = Cg * HW
+    dev = x.device
+    sums = _d(sums).to(dev)
+    mean = sums[..., 0] / n
+    var = (sums[..., 1] / n - mean * mean).clamp(min=0)
+    V = var + eps
+    rstd = 1.0 / torch.sqrt(V)
+    spread = lambda t: t.repeat_interleave(Cg, dim=1)[:, None, :]              # [B, G] -> [B, 1, C]
+    g, be = _d(gamma).to(dev), _d(beta).to(dev)
+    if ss is not None:
+        s64 = _d(ss).to(dev)
+        sc, sh = (s64[:, :C] + 1.0)[:, None], s64[:, C:2 * C][:, None]
+    else:
+        sc, sh = torch.ones((), dtype=F64, device=dev), torch.zeros((), dtype=F64, device=dev)
+    m_c, r_c = spread(mean), spread(rstd)
+    A = r_c * g * sc
+    Bc = (be - m_c * r_c * g) * sc + sh
+    v = x * A + Bc
+    y = _silu(v)
+    ev = U32 * (6 * (x * A).abs() + sc.abs() * (7 * (m_c * r_c * g).abs() + 3 * be.abs()) + Bc.abs() + v.abs())
+    if sums_err is not None:
+        e = _d(sums_err).to(dev)
+        dm = e[..., 0] / n
+        dvar = e[..., 1] / n + (2 * mean.abs() + dm) * dm + 4 * U64 * sums[..., 1].abs() / n
+        lo = (V - dvar).clamp(min=eps)
+        drs = dvar / (lo.sqrt() * V.sqrt() * (lo.sqrt() + V.sqrt()))
+        ev = ev + (g * sc).abs() * ((x - m_c).abs() * spread(drs) + spread(rstd + drs) * spread(dm))
+    if fast:
+        rel = 2 * U32 * (2 + 1.16 * v.abs()) * torch.sigmoid(-v) + 8 * U32
+    else:
+        rel = 8 * U32
+    return y, 2 * (1.1 * ev + rel * y.abs()) + ETA_SILU
+
+
+def gn_apply_silu_ref(src0, groups, gamma, beta, ss, eps, sums, sums_err=None, src1=None, scale1=1.0, out16=False,
+                      fast=None):
+    """mi_gn_apply_silu: y = SiLU(GroupNorm(x) (scale + 1) + shift) over the virtual concat x = cat(src0, src1 * scale1)
+    [B, HW, C], ss [B, 2C] = [scale | shift] (a view without the row gaps) or None.  `sums` [B, G, 2] are the statistics the
+    reference normalises with; `sums_err` (optional) bounds how far the kernel's statistics are from them.  Returns the
+    reference and the bound of the output (fp16 when out16).  fast: the __expf / __fdividef SiLU the kernel uses for fp16
+    outputs (default: out16).
+
+    (a) Exact statistics (sums_err None): the kernel casts mean and rstd to fp32 and folds
+            a = rstd gamma,  bb = beta - mean a,  a *= sc,  bb = bb sc + shift,  v = fmaf(x, a, bb),
+        with sc = scale + 1 rounded once.  Each step rounds once: a is off by 4 U32 |a|, bb by 4 U32 |mean a| (the
+        cancellation term) plus 3 U32 |beta - mean a| before the FiLM, so with A = rstd gamma sc, Bc the exact coefficients
+            |dv| <= U32 (6 |x A| + |sc| (7 |mean rstd gamma| + 3 |beta|) + |Bc| + |v|)
+        (6 |x A| includes the fp32 product x * scale1 of the second source).  SiLU has slope <= 1.1; silu_f (expf, a
+        division) is good to 8 U32 |y|; on fp16 outputs __expf is off by (2 + 1.16 |v|) ulp of e^-v, weighted by
+        e^-v / (1 + e^-v) in y, and __fdividef adds 2 ulp -- and returns 0 once 1 + e^-v > 2^126 (ETA_SILU absolute):
+            2 (1.1 |dv| + rel |y|) + ETA_SILU,   then half_out for fp16.
+    (b) Statistics a kernel produced (sums_err = their bound): mean is off by dm = e_sum / n, var = sq / n - mean^2 by
+        dvar = e_sq / n + (2 |mean| + dm) dm -- relative to var that grows with (|mean| / std)^2 -- and rstd by
+        |1/sqrt(V - dvar) - 1/sqrt(V)| (V = var + eps); v moves by |gamma sc| (|x - mean| drstd + (rstd + drstd) dm)."""
+    x = gn_concat(src0, src1, scale1)
+    y, bound = _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, out16 if fast is None else fast)
+    return half_out(y, bound) if out16 else (y, bound)
+
+
+def conv_gn_ref(src0, groups, gamma, beta, ss, eps, sums, wp, bias=None, residual=None, src1=None, scale1=1.0):
+    """mi_conv3x3_gn_silu_f16: GroupNorm -> FiLM -> SiLU (gn_apply_silu_ref (a), fast SiLU, statistics `sums` [B, G, 2]
+    gathered with group_sums) in float64, then the 3x3 conv with the fp16 packed weight wp, + bias + residual.  src0 / src1
+    [B, H, W, C_s].  Returns (reference NHWC, bound of the fp32 output).
+
+    The kernel rounds the activated operand a to fp16 (sat_half: U16 |a|, 2^-25 among subnormals) after an fp32 error e_a
+    (the bound of (a) before rounding), so
+        3 (n + 2) U32 (conv(|a|, |w|) + |bias| + |residual|)  +  conv(U16 |a| + e_a + 2^-25, |w|),   n = 9 C."""
+    B, H, W, _ = src0.shape
+    x = gn_concat(src0.reshape(B, H * W, -1), None if src1 is None else src1.reshape(B, H * W, -1), scale1)
+    C = x.shape[-1]
+    a, ea = _gn_silu(x, groups, gamma, beta, ss, eps, sums, None, True)
+    a, ea = a.reshape(B, H, W, C), ea.reshape(B, H, W, C)
+    w = unpack_conv_weight(wp, 3, 3, C).to(x.device)
+    ref, twin = conv_nhwc(a, w, 0), conv_nhwc(a.abs(), w.abs(), 0)
+    for t in (bias, residual):
+        if t is not None:
+            ref, twin = ref + _d(t), twin + _d(t).abs()
+    return ref, 3 * (9 * C + 2) * U32 * twin + conv_nhwc(U16 * a.abs() + ea + 2.0 ** -25, w.abs(), 0)

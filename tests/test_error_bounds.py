@@ -1,6 +1,7 @@
 """The float64 error bounds of tests/fp64_ref.py, proven on the CPU: the torch emulation of each kernel's contract
-(tests/emu_ops.py) passes every bound, and each planted defect -- a kernel that is only subtly wrong -- fails it.  (The
-fp16 saturation range is left to the GPU tests: the emulation converts with .to(float16), which gives inf there.)"""
+(tests/emu_ops.py) passes every bound, and each planted defect -- a kernel that is only subtly wrong -- fails it.  Where the
+emulation's arithmetic differs from the kernel's in structure (the conv epilogue's statistics, gn_stats's chains, the
+GroupNorm coefficient fold), an fp32 restatement of the kernel's own order passes the bound too."""
 import pytest
 import torch
 
@@ -447,3 +448,361 @@ def test_upsample2x_bwd_order():
     assert torch.equal(dx, ref)
     q = dy.reshape(B, H, 2, W, 2, C)
     assert not torch.equal((q[:, :, 0, :, 0] + q[:, :, 1, :, 0]) + (q[:, :, 0, :, 1] + q[:, :, 1, :, 1]), ref)
+
+
+# ---------------------------------------------------------------------------------------------- convolution forward
+F64 = torch.float64
+
+
+def _conv_operands(B, H, W, Cin, Cout, k, mode, seed, C1=0):
+    """fp16 operand(s) in the layout of `mode`, the OIHW fp32 weight, bias, residual"""
+    g = _g(seed)
+    lead = (B, 2 * H, 2 * W) if mode == 6 else (B, 4, H, W) if mode == 1 else (B, H, W)
+    a0 = torch.randn(*lead, Cin, generator=g).to(F16)
+    a1 = torch.randn(*lead, C1, generator=g).to(F16) if C1 else None
+    w = torch.randn(Cout, Cin + C1, k, k, generator=g) * (k * k * (Cin + C1)) ** -0.5
+    return a0, a1, w, torch.randn(Cout, generator=g), torch.randn(B, H, W, Cout, generator=g)
+
+
+def _emu_conv(a0, a1, wp, B, H, W, Cout, k, mode, bias, res, stats=True):
+    o, o16 = torch.zeros(B, H, W, Cout), torch.zeros(B, H, W, Cout, dtype=F16)
+    st = torch.zeros(B, Cout // 16, 2, dtype=F64) if stats else None
+    kw = dict(act2=a1, lda2=a1.shape[-1], c_in1=a0.shape[-1]) if a1 is not None else {}
+    Cin = a0.shape[-1] + (a1.shape[-1] if a1 is not None else 0)
+    EMU.conv_igemm(a0, B, H, W, a0.shape[-1], 0, Cin, wp, Cout, k, k, mode, bias, res, o, o16,
+                   (H * W * Cout, W * Cout, Cout), out_stats=st, **kw)
+    return o, o16, st
+
+
+def _epilogue_stats_fp32(out32):
+    """The conv epilogue's statistics in the kernel's own order (csrc/conv_tc.cu): lane 4 rr + cc of a warp holds rows
+    rr, rr + 8 of its 16 and columns 8 jj + 2 cc + e of each 16-channel block; it adds its two column pairs (j = 2q, 2q + 1)
+    of both rows in fp32, pair sums first; five xor-shuffle levels add the 32 lanes in fp32; warps are added in fp64."""
+    B, C = out32.shape[0], out32.shape[-1]
+    f = out32.float().reshape(B, -1, 2, 8, C // 16, 2, 4, 2)          # [B, warp, r, rr, q, jj, cc, e]
+    ps = f[..., 0] + f[..., 1]
+    pq = f[..., 0] * f[..., 0] + f[..., 1] * f[..., 1]
+    lanes = torch.arange(32)
+    out = []
+    for p in (ps, pq):
+        t = ((p[:, :, 0, :, :, 0] + p[:, :, 1, :, :, 0]) + p[:, :, 0, :, :, 1]) + p[:, :, 1, :, :, 1]   # [B, warp, rr, q, cc]
+        t = t.permute(0, 1, 3, 2, 4).reshape(B, -1, C // 16, 32)
+        for o in (1, 2, 4, 8, 16):
+            t = t + t[..., lanes ^ o]
+        out.append(t[..., 0].double().sum(dim=1))
+    return torch.stack(out, dim=-1)
+
+
+CONV_FWD_CASES = [
+    # B, H, W, C_in, C_out, k, mode
+    (2, 16, 16, 128, 64, 3, 0), (3, 8, 8, 64, 32, 1, 0), (2, 8, 16, 64, 32, 4, 1), (2, 8, 8, 64, 32, 4, 6),
+    (2, 8, 8, 64, 32, 2, 2), (1, 4, 136, 64, 32, 3, 0),
+]
+
+
+@pytest.mark.parametrize("B,H,W,Cin,Cout,k,mode", CONV_FWD_CASES)
+def test_conv_fwd_bound(B, H, W, Cin, Cout, k, mode):
+    """The emulation of mi_conv2d_igemm_f16 (fp32 and fp16 outputs, block statistics) passes conv_fwd_ref / conv_stats_ref,
+    and the kernel-ordered fp32 statistics of the same output pass conv_stats_ref.  Modes 2..5 write one interleaved
+    2H x 2W output."""
+    a0, _, w, bias, res = _conv_operands(B, H, W, Cin, Cout, k, mode, seed=20 + mode + k)
+    what = f"conv mode {mode} k {k} {H}x{W}"
+    if mode == 2:
+        o, o16 = torch.zeros(B, 2 * H, 2 * W, Cout), torch.zeros(B, 2 * H, 2 * W, Cout, dtype=F16)
+        ref, bound = torch.zeros(B, 2 * H, 2 * W, Cout, dtype=F64), torch.zeros(B, 2 * H, 2 * W, Cout, dtype=F64)
+        st = torch.zeros(B, Cout // 16, 2, dtype=F64)
+        strides = (4 * H * W * Cout, 4 * W * Cout, 2 * Cout)
+        for p in range(4):
+            wp = EMU.pack_conv_weight(w + 0.1 * p)
+            off = ((p >> 1) * 2 * W + (p & 1)) * Cout
+            EMU.conv_igemm(a0, B, H, W, Cin, 0, Cin, wp, Cout, 2, 2, 2 + p, bias, None, o.view(-1)[off:], o16.view(-1)[off:],
+                           strides, out_stats=st)
+            r, bd = R.conv_fwd_ref(a0, wp, 2, 2, 2 + p, bias)
+            ref[:, p >> 1::2, p & 1::2], bound[:, p >> 1::2, p & 1::2] = r, bd
+    else:
+        wp = EMU.pack_conv_weight(w)
+        o, o16, st = _emu_conv(a0, None, wp, B, H, W, Cout, k, mode, bias, res)
+        ref, bound = R.conv_fwd_ref(a0, wp, k, k, mode, bias, res)
+    check(o, ref, bound, what + " (emulation)")
+    check_rel_l2(o, ref, 2e-5, what + " (emulation)")
+    check(o16, *half_out(ref, bound), what + " fp16 (emulation)")
+    check_rel_l2(o16, ref, 1e-3, what + " fp16 (emulation)")
+    sref, sbound = R.conv_stats_ref(o)
+    check(st, sref, sbound, what + " statistics (emulation)")
+    check(_epilogue_stats_fp32(o), sref, sbound, what + " statistics (fp32 restatement)")
+    if mode == 2:
+        d = o.clone()
+        d[1, 0::2, 1::2], d[1, 1::2, 0::2] = o[1, 1::2, 0::2], o[1, 0::2, 1::2]
+        _fails(d, ref, bound, what + ": sub-pixel phases (0, 1) and (1, 0) of image 1 swapped")
+    if W == 136:
+        # the masked columns 136..255 of each row's second 128-pixel tile counted with their bias value (acc = 0)
+        d = st.clone()
+        nb = (256 - W) * H
+        bb = bias.double().reshape(-1, 16)
+        d[..., 0] += nb * bb.sum(dim=1)
+        d[..., 1] += nb * (bb * bb).sum(dim=1)
+        _fails(d, sref, sbound, what + ": masked ragged-W rows counted")
+
+
+def test_conv_fwd_defects():
+    """Planted defects of the implicit-GEMM conv and its statistics fail the bounds (3x3, C_in = 128: two 64-channel
+    k-blocks per tap; 16 x 16 images: a 128-pixel tile is 8 rows of one image)."""
+    B, H, W, Cin, Cout, k = 2, 16, 16, 128, 64, 3
+    a0, _, w, bias, res = _conv_operands(B, H, W, Cin, Cout, k, 0, seed=30)
+    wp = EMU.pack_conv_weight(w)
+    o, _, st = _emu_conv(a0, None, wp, B, H, W, Cout, k, 0, bias, res)
+    ref, bound = R.conv_fwd_ref(a0, wp, k, k, 0, bias, res)
+    check(o, ref, bound, "conv 3x3 (emulation)")
+    w64 = R.unpack_conv_weight(wp, k, k, Cin)
+    a64 = a0.double()
+    # 1. the second k-block (channels 64..127) of tap (1, 2) missing in the first tile of image 1
+    wpart = torch.zeros_like(w64)
+    wpart[:, 64:, 1, 2] = w64[:, 64:, 1, 2]
+    d = o.clone()
+    d[1, :8] -= R.conv_nhwc(a64, wpart, 0)[1, :8].float()
+    _fails(d, ref, bound, "one k-block of one tap missing in one tile")
+    # 2. the right-border taps read the first pixel of the next row instead of the zero padding
+    xp = torch.nn.functional.pad(a64.permute(0, 3, 1, 2), (1, 1, 1, 1))
+    xp[:, :, 1:H, W + 1] = xp[:, :, 2:H + 1, 1]
+    d = (torch.nn.functional.conv2d(xp, w64).permute(0, 2, 3, 1) + bias.double() + res.double()).float()
+    _fails(d, ref, bound, "right-border tap reads the next row")
+    # 3. the bias shifted by one 16-channel block
+    _fails(o - bias + bias.roll(16), ref, bound, "bias shifted by one 16-channel block")
+    # statistics: 4. one warp's 16 rows missing from block 1 of image 0; 5. the first tile of image 0 credited to image 1
+    sref, sbound = R.conv_stats_ref(o)
+    f = o.double().reshape(B, H * W, Cout)
+    d = st.clone()
+    d[0, 1, 0] -= f[0, 16:32, 16:32].sum()
+    d[0, 1, 1] -= (f[0, 16:32, 16:32] ** 2).sum()
+    _fails(d, sref, sbound, "one warp's 16 rows missing from one statistics block")
+    t = f[0, :128].reshape(128, Cout // 16, 16)
+    ts = torch.stack((t.sum(dim=(0, 2)), (t * t).sum(dim=(0, 2))), dim=-1)
+    d = st.clone()
+    d[0] -= ts
+    d[1] += ts
+    _fails(d, sref, sbound, "a tile's statistics added to image b + 1")
+
+
+def test_conv_fwd_concat_and_res1x1():
+    """The two-source virtual concat (skip scale folded into the packed weight) and the folded res_conv 1x1: the emulation
+    passes; the second source without its scale fails."""
+    B, H, W, C0, C1, Cout = 2, 8, 16, 64, 64, 128
+    a0, a1, w, bias, res = _conv_operands(B, H, W, C0, Cout, 3, 0, seed=31, C1=C1)
+    wsc = w.clone()
+    wsc[:, C0:] *= 0.7071
+    wp = EMU.pack_conv_weight(wsc)
+    o, _, _ = _emu_conv(a0, a1, wp, B, H, W, Cout, 3, 0, bias, res)
+    a = torch.cat((a0, a1), dim=-1)
+    ref, bound = R.conv_fwd_ref(a, wp, 3, 3, 0, bias, res)
+    check(o, ref, bound, "conv concat (emulation)")
+    d, _, _ = _emu_conv(a0, a1, EMU.pack_conv_weight(w), B, H, W, Cout, 3, 0, bias, res)
+    _fails(d, ref, bound, "second source without its scale")
+    # folded 1x1 over x = cat(x0, x1)
+    g = _g(32)
+    x0, x1 = torch.randn(B, H, W, 64, generator=g).to(F16), torch.randn(B, H, W, 64, generator=g).to(F16)
+    w3 = torch.randn(Cout, C0, 3, 3, generator=g) * (9 * C0) ** -0.5
+    w1 = torch.randn(Cout, 128, 1, 1, generator=g) * 128 ** -0.5
+    wp = torch.cat((EMU.pack_conv_weight(w3), EMU.pack_conv_weight(w1)), dim=1).contiguous()
+    o, st = torch.zeros(B, H, W, Cout), torch.zeros(B, Cout // 16, 2, dtype=F64)
+    EMU.conv_res1x1(a0, B, H, W, C0, C0, None, 0, 0, x0, 64, 128, x1, 64, 64, wp, Cout, bias, res, o, None, st)
+    ref, bound = R.conv_fwd_ref(a0, wp, 3, 3, 0, bias, res, x=torch.cat((x0, x1), dim=-1))
+    check(o, ref, bound, "conv res1x1 (emulation)")
+    check_rel_l2(o, ref, 2e-5, "conv res1x1 (emulation)")
+    check(st, *R.conv_stats_ref(o), "conv res1x1 statistics (emulation)")
+    d = o.clone()
+    d[0] -= (x1[0].double() @ R._d(wp[:, 9 * C0 + 64:]).t()).float()
+    _fails(d, ref, bound, "folded 1x1: second x source dropped in image 0")
+
+
+def test_conv_direct_and_stem_bound():
+    """conv_direct_f32 (fp32 operands, n = taps x ceil4(C_in)) and the stem's 15-tap GEMM over 128 unrolled channels
+    (n = 15 x 128) have the conv_fwd_ref form."""
+    g = _g(33)
+    B, H, W, Cin, ldi, Cout, k = 2, 12, 12, 6, 8, 16, 7
+    x = torch.zeros(B, H, W, ldi)
+    x[..., :Cin] = torch.randn(B, H, W, Cin, generator=g)
+    w, b = torch.randn(Cout, Cin, k, k, generator=g) * 0.1, torch.randn(Cout, generator=g)
+    o = torch.zeros(B, H, W, Cout)
+    EMU.conv_direct(x, B, H, W, Cin, ldi, w, Cout, k, k, 1, k // 2, b, None, o, H, W, (H * W * Cout, W * Cout, Cout, 1))
+    wpad = torch.zeros(Cout, ldi, k, k)
+    wpad[:, :Cin] = w
+    wp = wpad.permute(0, 2, 3, 1).reshape(Cout, -1)
+    ref, bound = R.conv_fwd_ref(x, wp, k, k, 0, b)
+    check(o, ref, bound, "conv_direct (emulation)")
+    d = o.clone()
+    d[..., 3] -= R.conv_nhwc(x.double()[..., Cin - 1:Cin], w[3:4, Cin - 1:Cin].double(), 0)[..., 0].float()
+    _fails(d, ref, bound, "conv_direct: last input channel dropped in output channel 3")
+    # stem: unroll the (fp16) image, 15-tap vertical GEMM == the float64 k = 3 / 7 / 15 convs of the fp16 operands
+    from minimagen_b200.layers import CrossEmbedLayer
+    torch.manual_seed(0)
+    layer = CrossEmbedLayer(6, (3, 7, 15), dim_out=64, stride=1)
+    img = torch.randn(B, 6, 16, 16, generator=g)
+    a = torch.zeros(B, 16, 16, 128, dtype=F16)
+    EMU.stem_unroll(img[:, :3], 3, img[:, 3:], 3, B, 16, 16, a)
+    wp16, sbias = layer._stem_weights()
+    ref, bound = R.conv_fwd_ref(a, wp16, 15, 1, 0, sbias)
+    x16 = img.half().double()
+    direct = torch.cat([torch.nn.functional.conv2d(x16, c.weight.detach().half().double(), c.bias.detach().double(),
+                                                   padding=c.padding) for c in layer.convs], dim=1).permute(0, 2, 3, 1)
+    assert (direct - ref).abs().max() < 1e-12                  # the unrolled GEMM is the three convs
+    o = torch.zeros(B, 16, 16, 64)
+    EMU.conv_igemm(a, B, 16, 16, 128, 0, 128, wp16, 64, 15, 1, 0, sbias, None, o, None, (16 * 16 * 64, 16 * 64, 64))
+    check(o, ref, bound, "stem 15-tap GEMM (emulation)")
+
+
+# ---------------------------------------------------------------------------------------------- GroupNorm forward
+def _gn_stats_fp32(x32, groups, chunk, planes, lost_chunk=None):
+    """gn_stats_kernel in its own order: per chunk of pixels, per plane, an fp32 chain over every planes-th pixel, two
+    values per step (s += v0 + v1, q += v0 v0 + v1 v1), a single value at the end; the per-(chunk, plane, channel) chains
+    are added in fp64.  x32 [B, HW, C] is the fp32 concat the kernel loads (src1 * scale1 rounded)."""
+    B, HW, C = x32.shape
+    S = torch.zeros(B, C, dtype=F64)
+    Q = torch.zeros(B, C, dtype=F64)
+    for k, p0 in enumerate(range(0, HW, chunk)):
+        if k == lost_chunk:
+            continue
+        xs = x32[:, p0:p0 + chunk]
+        L = -(-xs.shape[1] // planes)
+        xs = torch.cat((xs, xs.new_zeros(B, L * planes - xs.shape[1], C)), dim=1).reshape(B, L, planes, C)
+        xs = torch.cat((xs, xs.new_zeros(B, L % 2, planes, C)), dim=1)        # zeros add exactly
+        s, q = torch.zeros(B, planes, C), torch.zeros(B, planes, C)
+        for i in range(0, xs.shape[1], 2):
+            v0, v1 = xs[:, i], xs[:, i + 1]
+            s = s + (v0 + v1)
+            q = q + (v0 * v0 + v1 * v1)
+        S += s.double().sum(dim=1)
+        Q += q.double().sum(dim=1)
+    return torch.stack((S.reshape(B, groups, -1).sum(dim=2), Q.reshape(B, groups, -1).sum(dim=2)), dim=-1)
+
+
+@pytest.mark.parametrize("HW,C0,C1,groups", [(1000, 48, 0, 16), (1000, 48, 0, 8), (300, 256, 128, 8), (50, 4096, 0, 32)])
+def test_gn_stats_bound(HW, C0, C1, groups):
+    """gn_stats_ref on the emulation and on the kernel-ordered fp32 chains (gn_stats_plan); a lost chunk and the straddling
+    8-channel vector credited to its first group (Cg = 3, 6) fail."""
+    B, C = 2, C0 + C1
+    g = _g(HW + C)
+    s0 = torch.randn(B, HW, C0, generator=g) * 2 + 0.5
+    s1 = torch.randn(B, HW, C1, generator=g) if C1 else None
+    scale1 = 0.7071 if C1 else 1.0
+    sums = torch.zeros(B, groups, 2, dtype=F64)
+    EMU.gn_stats(s0, C0, s1, C1, scale1, B, HW, groups, sums)
+    chunk, planes, L = R.gn_stats_plan(C, HW)
+    ref, bound = R.gn_stats_ref(s0, groups, s1, scale1, L)
+    what = f"gn_stats HW={HW} C={C} G={groups}"
+    check(sums, ref, bound, what + " (emulation)")
+    x32 = torch.cat((s0, s1 * scale1), dim=-1) if C1 else s0
+    check(_gn_stats_fp32(x32, groups, chunk, planes), ref, bound, what + " (fp32 restatement)")
+    if HW > chunk:
+        _fails(_gn_stats_fp32(x32, groups, chunk, planes, lost_chunk=1), ref, bound, what + ": one chunk lost")
+    Cg = C // groups
+    if Cg in (3, 6):
+        d = sums.clone()
+        v = x32.double()[..., 8:16]                    # the vector straddling groups 8 // Cg and 15 // Cg
+        for c in range(8):
+            if (8 + c) // Cg != 8 // Cg:
+                d[:, 8 // Cg, 0] += v[..., c].sum(dim=1)
+                d[:, (8 + c) // Cg, 0] -= v[..., c].sum(dim=1)
+        _fails(d, ref, bound, what + ": straddling vector's last channels credited to its first group")
+
+
+def _gn_apply_fp32(x32, sums, groups, gamma, beta, ss, eps, out16, defect=None):
+    """gn_apply_silu_kernel in its own order: fp64 mean / var / rstd cast to fp32; a = rstd gamma, bb = beta - mean a,
+    FiLM a *= sc, bb = fma(bb, sc, shift); v = fma(x, a, bb) (an fma: exact product in fp64, one rounding); SiLU in fp32."""
+    B, HW, C = x32.shape
+    Cg, n = C // groups, (C // groups) * HW
+    mean = sums[..., 0] / n
+    var = (sums[..., 1] / n - mean * mean).clamp(min=0)
+    rstd = 1.0 / torch.sqrt(var + eps)
+    if defect == "eps ignored":                                  # on the near-constant group (image 0, group 2)
+        rstd[0, 2] = 1.0 / torch.sqrt(var[0, 2])
+    if defect == "neighbour's mean":                             # image 1, group 3 takes group 4's mean
+        mean[1, 3] = mean[1, 4]
+    m, r = mean.float().repeat_interleave(Cg, dim=1), rstd.float().repeat_interleave(Cg, dim=1)
+    a = r * gamma
+    bb = beta - m * a
+    if ss is not None:
+        sc = ss[:, :C] + 1.0
+        if defect == "scale without +1":                         # image 0
+            sc[0] = ss[0, :C]
+        a = a * sc
+        bb = (bb.double() * sc.double() + ss[:, C:2 * C].double()).float()
+    v = (x32.double() * a.double()[:, None] + bb.double()[:, None]).float()
+    y = v / (1.0 + torch.exp(-v))
+    return y.clamp(-65504, 65504).half() if out16 else y
+
+
+def _gn_apply_case():
+    B, HW, C0, C1, G = 2, 96, 32, 16, 8                        # Cg = 6: groups straddle the two sources and 8-vectors
+    C = C0 + C1
+    g = _g(34)
+    s0 = torch.randn(B, HW, C0, generator=g) * 2 + 0.5
+    s1 = torch.randn(B, HW, C1, generator=g)
+    s0[0, :, 12:18] = 2.5 + 1e-4 * torch.randn(HW, 6, generator=g)          # image 0, group 2: near-constant
+    s1[1, :, 0:6] = 100.0 / 0.7071 + torch.randn(HW, 6, generator=g)         # image 1, group 5 (after the scale): |mean|/std ~ 100
+    gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
+    gamma[45] = 3e4                                              # v beyond 65504 and below -88 in channel 45
+    ss = torch.randn(B, 2 * C, generator=g) * 0.3
+    return B, HW, C0, C1, G, C, s0, s1, gamma, beta, ss
+
+
+@pytest.mark.parametrize("out16", [False, True])
+def test_gn_apply_silu_bound(out16):
+    """gn_apply_silu_ref (a) on the emulation and on the kernel's coefficient fold; (b) with the kernel-ordered gn_stats of
+    the same input; planted defects fail."""
+    B, HW, C0, C1, G, C, s0, s1, gamma, beta, ss = _gn_apply_case()
+    sums, sums_err = R.gn_stats_ref(s0, G, s1, 0.7071)
+    x32 = torch.cat((s0, s1 * 0.7071), dim=-1)
+    out = torch.zeros(B, HW, C, dtype=F16 if out16 else torch.float32)
+    EMU.gn_apply_silu(s0, C0, s1, C1, 0.7071, B, HW, G, sums, 0, None, 0, gamma, beta, ss, 2 * C, 1e-5, out)
+    ref, bound = R.gn_apply_silu_ref(s0, G, gamma, beta, ss, 1e-5, sums, src1=s1, scale1=0.7071, out16=out16)
+    what = f"gn_apply_silu out16={out16}"
+    check(out, ref, bound, what + " (emulation)")
+    assert (out.double().abs().max() == 65504.0) if out16 else (out.abs().max() > 65504.0)
+    fold = _gn_apply_fp32(x32, sums, G, gamma, beta, ss, 1e-5, out16)
+    check(fold, ref, bound, what + " (fp32 coefficient fold)")
+    # the aggregate leaves out the saturating channel 45 and the near-constant and |mean|/std ~ 100 groups, whose elementwise
+    # bounds are large by nature
+    agg = torch.ones(B, HW, C, dtype=torch.bool)
+    agg[..., 45], agg[0, :, 12:18], agg[1, :, 30:36] = False, False, False
+    check_rel_l2(fold[agg], ref[agg], 1e-3 if out16 else 5e-6, what + " (fp32 coefficient fold)")
+    for defect in ("eps ignored", "neighbour's mean", "scale without +1"):
+        _fails(_gn_apply_fp32(x32, sums, G, gamma, beta, ss, 1e-5, out16, defect), ref, bound, f"{what}: {defect}")
+    # (b): the statistics of the kernel-ordered gn_stats chains, the reference on the exact ones
+    chunk, planes, L = R.gn_stats_plan(C, HW)
+    ks = _gn_stats_fp32(x32, G, chunk, planes)
+    fold = _gn_apply_fp32(x32, ks, G, gamma, beta, ss, 1e-5, out16)
+    ref, bound = R.gn_apply_silu_ref(s0, G, gamma, beta, ss, 1e-5, sums, sums_err, src1=s1, scale1=0.7071, out16=out16)
+    check(fold, ref, bound, what + " (b) with kernel-ordered statistics")
+    check(fold[1, :, 30:36], ref[1, :, 30:36], bound[1, :, 30:36], what + " (b) the |mean|/std ~ 100 group")
+
+
+def test_conv_gn_bound():
+    """mi_conv3x3_gn_silu_f16's emulation (gn_apply_silu to fp16, then the conv) passes conv_gn_ref; the FiLM scale
+    without +1 in image 0 fails."""
+    B, H, W, C0, C1, Cout, G = 2, 32, 8, 64, 64, 128, 8
+    C = C0 + C1
+    g = _g(35)
+    x0, x1 = torch.randn(B, H, W, C0, generator=g) * 1.5 + 0.3, torch.randn(B, H, W, C1, generator=g)
+    gamma, beta = torch.randn(C, generator=g), torch.randn(C, generator=g)
+    ss = torch.randn(B, 2 * C, generator=g) * 0.3
+    w = torch.randn(Cout, C, 3, 3, generator=g) * (9 * C) ** -0.5
+    bias, res = torch.randn(Cout, generator=g), torch.randn(B, H, W, Cout, generator=g)
+    wp = EMU.pack_conv_weight(w)
+    st = []
+    for t, Cc in ((x0, C0), (x1, C1)):
+        s = torch.zeros(B, Cc // 16, 2, dtype=F64)
+        EMU.gn_stats(t, Cc, None, 0, 1.0, B, H * W, Cc // 16, s)
+        st.append(s)
+    o = torch.zeros(B, H, W, Cout)
+    EMU.conv_gn(x0, C0, x1, C1, 0.7071, B, H, W, G, st[0], st[1], gamma, beta, ss, 2 * C, 1e-5, wp, Cout, bias, res, o,
+                None, None)
+    sums = R.group_sums(st[0], C0, G, st[1], C1, 0.7071)
+    ref, bound = R.conv_gn_ref(x0, G, gamma, beta, ss, 1e-5, sums, wp, bias, res, src1=x1, scale1=0.7071)
+    check(o, ref, bound, "conv_gn (emulation)")
+    check_rel_l2(o, ref, 1.5e-3, "conv_gn (emulation)")
+    ss2 = ss.clone()
+    ss2[0, :C] -= 1.0
+    d = o.clone()
+    EMU.conv_gn(x0, C0, x1, C1, 0.7071, B, H, W, G, st[0], st[1], gamma, beta, ss2, 2 * C, 1e-5, wp, Cout, bias, res, d,
+                None, None)
+    _fails(d, ref, bound, "conv_gn: FiLM scale without +1 in image 0")
