@@ -6,6 +6,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "clamp_nan.cuh"
 #include "kernels.cuh"
 #include "launch.cuh"
 #include "sat_half.cuh"
@@ -743,7 +744,7 @@ resize_sep_kernel(const float* __restrict__ in, int Hin, int Win, float* __restr
         for (int i = 0; i < ty; ++i) col = __fadd_rn(col, __fmul_rn(wy[y * ty + i], src[(long long)iy[y * ty + i] * Win + xi]));
         acc = __fadd_rn(acc, __fmul_rn(wx[x * tx + j], col));
     }
-    if (has_clamp) acc = fminf(fmaxf(acc, lo), hi);
+    if (has_clamp) acc = clamp_nan(acc, lo, hi);      // a NaN stays NaN, as torch.clamp
     out[idx] = acc;
 }
 

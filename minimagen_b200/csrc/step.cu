@@ -36,6 +36,7 @@
 
 #include <cooperative_groups.h>
 
+#include "clamp_nan.cuh"
 #include "kernels.cuh"
 #include "launch.cuh"
 
@@ -59,11 +60,15 @@ __device__ __forceinline__ float guided_x0(const float* x_t, const float* eps_co
 
 // The threshold from the two selected order statistics (bit patterns of |x0|): at::lerp in its vectorised CPU form,
 // base + coeff * (end - start) with weight < 0.5 ? (start, w) : (end, w - 1), then s.clamp_(min=min_s).
-__device__ __forceinline__ float step_threshold(uint32_t v_lo, uint32_t v_hi, float weight, float min_s) {
+// NaN follows torch: has_nan (some |x0| key above +inf's 0x7F800000) gives s = NaN, as torch.quantile of a row containing
+// NaN; lerp(inf, inf) is NaN (at least n - rank_lo values are +-inf); and the min_s clamp keeps a NaN.  The posterior
+// then makes the whole image NaN (clamp(x0, -s, s) / s), as the reference does.
+__device__ __forceinline__ float step_threshold(uint32_t v_lo, uint32_t v_hi, float weight, float min_s, bool has_nan) {
+    if (has_nan) return __uint_as_float(0x7FFFFFFFu);
     const float lo = __uint_as_float(v_lo), hi = __uint_as_float(v_hi);
     const float diff = __fsub_rn(hi, lo);
     const float s = (weight < 0.5f) ? fmaf(weight, diff, lo) : fmaf(__fsub_rn(weight, 1.0f), diff, hi);
-    return fmaxf(s, min_s);
+    return fmax_nan(s, min_s);
 }
 
 // Step 3 at element idx: xs = clamp(x0, -s, s) / s, mean = c1 * xs + c2 * x_t, and out = mean + sig * noise.
@@ -101,6 +106,8 @@ x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, con
 constexpr int kSelThreads = 1024;
 
 __device__ __forceinline__ uint32_t absbits(float v) { return __float_as_uint(v) & 0x7FFFFFFFu; }
+// |v| bit patterns above +inf's are NaN
+constexpr uint32_t kInfBits = 0x7F800000u;
 
 __global__ void __launch_bounds__(kSelThreads)
 quantile_kernel(const float* __restrict__ x0, int n, int rank_lo, int rank_hi, float weight, float min_s,
@@ -114,6 +121,8 @@ quantile_kernel(const float* __restrict__ x0, int n, int rank_lo, int rank_hi, f
     const int tid = threadIdx.x, lane = tid & 31;
     uint32_t prefix = 0, maskbits = 0, k = (uint32_t)rank_lo;
     const int n_round = (n + 31) & ~31;
+    bool nan_key = false;                       // this thread has seen a NaN (pass 0 reads every key)
+    int has_nan = 0;
 
     for (int pass = 0; pass < 4; ++pass) {
         const int shift = 24 - 8 * pass;
@@ -123,12 +132,14 @@ quantile_kernel(const float* __restrict__ x0, int n, int rank_lo, int rank_hi, f
             unsigned bin = 256;
             if (i < n) {
                 const uint32_t key = absbits(x[i]);
+                nan_key |= key > kInfBits;
                 if ((key & maskbits) == prefix) bin = (key >> shift) & 0xFF;
             }
             const unsigned peers = __match_any_sync(0xffffffffu, bin);
             if (lane == (__ffs(peers) - 1)) atomicAdd(&hist[bin], __popc(peers));
         }
-        __syncthreads();
+        if (pass == 0) has_nan = __syncthreads_or(nan_key);
+        else __syncthreads();
         if (tid == 0) {
             uint32_t cum = 0;
             int d = 0;
@@ -170,7 +181,7 @@ quantile_kernel(const float* __restrict__ x0, int n, int rank_lo, int rank_hi, f
         v_hi = sh_min[0];
         if (v_hi == 0xFFFFFFFFu) v_hi = v_lo;   // cannot happen for rank_hi < n
     }
-    if (tid == 0) s_out[blockIdx.x] = step_threshold(v_lo, v_hi, weight, min_s);
+    if (tid == 0) s_out[blockIdx.x] = step_threshold(v_lo, v_hi, weight, min_s, has_nan);
 }
 
 // kHist: the multistep form (mi_step_epilogue_multistep) of posterior_elem.  The extra arguments come last so that the
@@ -223,8 +234,10 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
     pdl_trigger();
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
-    __shared__ unsigned hist[256];       // this CTA's histogram of the current pass (read remotely by the peers)
-    __shared__ unsigned ghist[256];      // cluster-wide histogram
+    // this CTA's histogram of the current pass (read remotely by the peers) and the cluster-wide one; entry 256 is not a
+    // bin: it holds whether this CTA's x0 has a NaN, so that ghist[256] != 0 when the image has one
+    __shared__ unsigned hist[257];
+    __shared__ unsigned ghist[257];
     __shared__ uint32_t sh_prefix, sh_k, sh_eq, sh_cta_min, sh_maskbits;
     __shared__ uint32_t sh_min[32];
     const int img = blockIdx.x / kSelCluster;
@@ -239,16 +252,22 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
     const float scale = image_scale(w, cond_scale, img);
 
     float x0v[kSelPerThread];
+    bool nan_key = false;
 #pragma unroll
     for (int j = 0; j < kSelPerThread; ++j) {
         const int i = tid + j * kSelThreads;
         x0v[j] = i < cnt ? guided_x0(x_t, eps_cond, eps_null, scale, ca, cb, base + i) : 0.f;
+        nan_key |= isnan(x0v[j]);       // (not absbits(.) > kInfBits: ptxas would keep those keys for pass 0, and spill)
     }
     // Each pass reads its mask from shared memory.  With the mask a compile-time constant of the unrolled passes, ptxas
     // precomputes the next pass's masked keys next to x0v, and at 64 registers that spills.  Thread 0 updates it after
     // the barrier that ends the pass's reads.
     uint32_t prefix = 0, k = (uint32_t)rank_lo;
-    if (tid == 0) sh_maskbits = 0;
+    const int cta_nan = __syncthreads_or(nan_key);
+    if (tid == 0) {
+        sh_maskbits = 0;
+        hist[256] = cta_nan;                                       // never re-zeroed: summed again by every pass
+    }
     for (int pass = 0; pass < 4; ++pass) {
         const int shift = 24 - 8 * pass;
         if (tid < 256) hist[tid] = 0;
@@ -263,7 +282,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
             if (live && lane == (__ffs(peers) - 1)) atomicAdd(&hist[bin], __popc(peers));
         }
         cluster.sync();                                            // every CTA's histogram is complete
-        if (tid < 256) {
+        if (tid < 257) {
             unsigned tt = 0;
 #pragma unroll
             for (int r = 0; r < kSelCluster; ++r) tt += *cluster.map_shared_rank(&hist[tid], r);
@@ -329,7 +348,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
         v_hi = sh_min[0];
         if (v_hi == 0xFFFFFFFFu) v_hi = v_lo;
     }
-    const float sb = step_threshold(v_lo, v_hi, weight, min_s);
+    const float sb = step_threshold(v_lo, v_hi, weight, min_s, ghist[256] != 0);
     if (s_out && rank == 0 && tid == 0) s_out[img] = sb;
 
     const float c1 = tab_c1[tb], c2 = tab_c2[tb];
@@ -369,7 +388,7 @@ __global__ void finalize_kernel(const float* __restrict__ x, long long n, int un
     pdl_trigger();
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    float v = fminf(fmaxf(x[i], -1.f), 1.f);
+    float v = clamp_nan(x[i], -1.f, 1.f);
     if (unnormalize) v = __fmul_rn(__fadd_rn(v, 1.f), 0.5f);
     out[i] = v;
 }
@@ -448,7 +467,7 @@ __global__ void inpaint_finalize_kernel(const float* __restrict__ x, const float
     if (i >= n_per_img) return;
     const long long idx = (long long)b * n_per_img + i;
     float v = m[(long long)b * hw + i % hw] >= 0.5f ? k[idx] : x[idx];
-    v = fminf(fmaxf(v, -1.f), 1.f);
+    v = clamp_nan(v, -1.f, 1.f);
     if (unnormalize) v = __fmul_rn(__fadd_rn(v, 1.f), 0.5f);
     out[idx] = v;
 }

@@ -344,7 +344,10 @@ class EmuOps:
     def step_quantile(self, x0, B, n, rank_lo, rank_hi, weight, min_s, s):
         self._log("step_quantile")
         srt = x0.reshape(B, n).abs().sort(dim=-1).values
-        lo, hi = srt[:, rank_lo], srt[:, rank_hi]
+        # torch.quantile: a row containing NaN (sorted last) takes both order statistics from its last element -> NaN
+        nan = srt[:, -1].isnan()
+        lo = torch.where(nan, srt[:, -1], srt[:, rank_lo])
+        hi = torch.where(nan, srt[:, -1], srt[:, rank_hi])
         w = torch.tensor(weight, dtype=F32)
         s.copy_(torch.lerp(lo, hi, w).clamp(min=min_s))
 

@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE ONLY: float64 references of the token-side kernels, of the image-side forward kernels (implicit-GEMM,
 direct and stem convolutions, the conv epilogue's GroupNorm statistics, GroupNorm statistics and GroupNorm/FiLM/SiLU, the
-fused GroupNorm conv) and of the image-side training kernels (GroupNorm/SiLU backward, convolution weight and data
-gradients, upsample backward) with elementwise error bounds.
+fused GroupNorm conv), of the image-side training kernels (GroupNorm/SiLU backward, convolution weight and data
+gradients, upsample backward) and of the sampling loop's kernels outside the U-Net (the step epilogue's x0, threshold and
+posterior, q_sample, the cascade resize, the timestep embedding and the text-token pooling) with elementwise error bounds.
 
 Every reference takes the operands exactly as the kernel reads them (fp16-rounded where the kernel reads fp16, the null
 key/value included), computes in float64 on the operands' device, and returns (reference, bound): |kernel - reference| <=
@@ -770,3 +771,139 @@ def conv_gn_ref(src0, groups, gamma, beta, ss, eps, sums, wp, bias=None, residua
         if t is not None:
             ref, twin = ref + _d(t), twin + _d(t).abs()
     return ref, 3 * (9 * C + 2) * U32 * twin + conv_nhwc(U16 * a.abs() + ea + 2.0 ** -25, w.abs(), 0)
+
+
+# ---------------------------------------------------------------------------------------------- sampling step
+# Operands of the step kernels as they read them: per-image scalars gathered from the fp32 schedule tables at t [B], the
+# guidance weight w (a number or [B]) as fp32, [B, n] images.  The elementwise bounds hold for finite data; NaN and inf
+# are checked for parity with the torch restatement instead.
+def _per_image(tab, t):
+    return _d(tab.detach().cpu()[t.detach().cpu()])[:, None]
+
+
+def _scale_col(w, B):
+    if torch.is_tensor(w):
+        return _d(w.detach().cpu()).reshape(B, 1)
+    return torch.full((B, 1), _f32(w), dtype=F64)
+
+
+def step_x0_ref(x_t, eps_cond, eps_null, w, t, tab_a, tab_b):
+    """guided_x0 (csrc/step.cu): e = nl + (c - nl) w, x0 = a[t] x - b[t] e, every product and sum rounded on its own.
+    First-order error: fl(c - nl) and the product w (c - nl) put 2 U32 |w| |c - nl| on p, the sum adds U32 |nl + p|, so
+    e is off by U32 |nl| + 3 U32 |w| |c - nl|; b e adds U32 |b e|, a x one U32 |a x|, the subtraction U32 |x0|:
+        |dx0| <= U32 (2 |a x| + |b| (3 |nl| + 5 |w| (|c| + |nl|)))  <=  5 U32 (|a x| + |b| (|nl| + |w| (|c| + |nl|)))
+    (without eps_null: 2 U32 (|a x| + |b c|)), + ETA32 for products that underflow.  Returns (x0, bound) [B, n]."""
+    x, c = _d(x_t).cpu(), _d(eps_cond).cpu()
+    B = x.shape[0]
+    a, b = _per_image(tab_a, t), _per_image(tab_b, t)
+    if eps_null is None:
+        e, te = c, c.abs()
+    else:
+        nl, wc = _d(eps_null).cpu(), _scale_col(w, B)
+        e = nl + (c - nl) * wc
+        te = nl.abs() + wc.abs() * (c.abs() + nl.abs())
+    x0 = a * x - b * e
+    return x0, 5 * U32 * ((a * x).abs() + b.abs() * te) + ETA32
+
+
+def step_threshold_ref(x0, x0_bound, rank_lo, rank_hi, weight, min_s):
+    """The dynamic threshold s [B] from the float64 x0 [B, n] and its bound: the order statistics lo, hi of |x0| at
+    rank_lo / rank_hi, s = max(lo + w (hi - lo), min_s) with the fp32 weight w of quantile_rank.  Order statistics are
+    1-Lipschitz in the sup norm, so the kernel's selected values (of its fp32 x0) are within D = max_i x0_bound_i of lo and
+    hi -- per image, not per element; the lerp is a convex combination (1-Lipschitz too) rounded twice (hi - lo, then one
+    fma), and the clamp is 1-Lipschitz:
+        |s - s64| <= D (1 + 3 U32) + U32 (|hi - lo| + |s64|) + ETA32.
+    Returns (s, bound) [B]."""
+    srt = x0.abs().sort(dim=-1).values
+    lo, hi = srt[:, rank_lo], srt[:, rank_hi]
+    wt = _f32(weight)
+    s = (lo + wt * (hi - lo)).clamp(min=_f32(min_s))
+    D = x0_bound.amax(dim=-1)
+    return s, D * (1 + 3 * U32) + U32 * ((hi - lo).abs() + s.abs()) + ETA32
+
+
+def step_posterior_ref(x0, x0_bound, s, s_bound, x_t, noise, t, tab_c1, tab_c2, tab_sigma, tab_c3=None, hist=None):
+    """posterior_elem: xs = clamp(x0, -s, s) / s, out = c1[t] xs + c2[t] x + c3[t] h + sigma[t] z with sigma = 0 at t = 0;
+    the multistep form (tab_c3, hist given) also returns xs, the new history.  clamp(x, -s, s) is 1-Lipschitz in x and in
+    s, and |clamp / s| <= 1, so with dx = x0_bound, ds = s_bound
+        |xs - xs64| <= (dx + 2 ds) / (s64 - ds) + U32 (|xs64| + ...)  =: dxs,
+    and the four products and three sums of the output put at most four roundings on each term:
+        |out - out64| <= |c1| dxs (1 + 4 U32) + 4 U32 (|c1 xs| + |c2 x| + |c3 h| + |sigma z|) + ETA32.
+    Returns (out, out_bound, xs, xs_bound) [B, n] (xs for the history)."""
+    x, z = _d(x_t).cpu(), _d(noise).cpu()
+    sc, ds = s[:, None], s_bound[:, None]
+    xs = torch.minimum(torch.maximum(x0, -sc), sc) / sc
+    dxs0 = (x0_bound + 2 * ds) / (sc - ds)
+    dxs = dxs0 + U32 * (xs.abs() + dxs0) + ETA32
+    c1, c2 = _per_image(tab_c1, t), _per_image(tab_c2, t)
+    sig = torch.where(t.detach().cpu()[:, None] == 0, torch.zeros((), dtype=F64), _per_image(tab_sigma, t))
+    out = c1 * xs + c2 * x + sig * z
+    twin = (c1 * xs).abs() + (c2 * x).abs() + (sig * z).abs()
+    if tab_c3 is not None:
+        c3, h = _per_image(tab_c3, t), _d(hist).cpu()
+        out = out + c3 * h
+        twin = twin + (c3 * h).abs()
+    return out, c1.abs() * dxs * (1 + 4 * U32) + 4 * U32 * twin + ETA32, xs, dxs
+
+
+def q_sample_ref(x0, noise, t, tab_a, tab_b, post_scale, post_shift):
+    """q_sample_kernel: v = a[t] x0 + b[t] z (three roundings), then v * post_scale + post_shift (two more):
+        |out - out64| <= 4 U32 (|post_scale| (|a x0| + |b z|) + |post_shift|) + ETA32."""
+    x, z = _d(x0).cpu(), _d(noise).cpu()
+    a, b = _per_image(tab_a, t), _per_image(tab_b, t)
+    ps, sh = _f32(post_scale), _f32(post_shift)
+    ref = (a * x + b * z) * ps + sh
+    return ref, 4 * U32 * (abs(ps) * ((a * x).abs() + (b * z).abs()) + abs(sh)) + ETA32
+
+
+def resize_ref(x, iy, wy, ix, wx, clamp=None):
+    """resize_sep_kernel: out[p, y, x] = clamp(sum_j wx[x, j] sum_i wy[y, i] in[p, iy[y, i], ix[x, j]]) over the fp32 tap
+    tables, x [P, Hin, Win].  The kernel's inner chain (ty products and sums from 0) and outer chain (one product, tx sums)
+    round at most ty + tx + 1 times on any term's path; the clamp is 1-Lipschitz:
+        |out - out64| <= (ty + tx + 2) U32 * twin + ETA32,   twin = the same sums over |w| and |in|.
+    Returns (out, bound) [P, Hout, Wout]."""
+    xd = _d(x).cpu()
+    iy, ix = iy.detach().cpu().long(), ix.detach().cpu().long()
+    wy, wx = _d(wy).cpu(), _d(wx).cpu()
+
+    def sep(v, wyv, wxv):
+        rows = (v[:, iy, :] * wyv[None, :, :, None]).sum(2)                 # [P, Hout, Win]
+        return (rows[:, :, ix] * wxv[None, None, :, :]).sum(3)              # [P, Hout, Wout]
+    ref, twin = sep(xd, wy, wx), sep(xd.abs(), wy.abs(), wx.abs())
+    if clamp is not None:
+        ref = ref.clamp(_f32(clamp[0]), _f32(clamp[1]))
+    return ref, (iy.shape[1] + ix.shape[1] + 2) * U32 * twin + ETA32
+
+
+def posemb_ref(t, dim):
+    """posemb_kernel: out = cat(sin(arg), cos(arg)), arg_j = t exp(-j ln(1e4) / (half - 1)), half = dim / 2.  The kernel
+    rounds the step ln(1e4) / (half - 1) to fp32 (U32), j * step once more (U32), then expf (2 ulp, 4 U32) and the product
+    with t (U32): with e_j = j ln(1e4) / (half - 1) <= ln(1e4) the argument is off by
+        |d arg| <= |arg| (2 U32 e_j + 6 U32),
+    and sin / cos (1-Lipschitz) add their own 2 ulp (4 U32 |out|):
+        |out - out64| <= |arg| (2 e_j + 6) U32 + 4 U32 |out64| + ETA32.     Returns (out, bound) [B, dim]."""
+    half = dim // 2
+    j = torch.arange(half, dtype=F64)
+    e = j * (math.log(10000.0) / (half - 1))
+    arg = _d(t).cpu()[:, None] * torch.exp(-e)[None, :]
+    ref = torch.cat((arg.sin(), arg.cos()), dim=-1)
+    darg = arg.abs() * (2 * e + 6) * U32
+    return ref, torch.cat((darg, darg), dim=-1) + 4 * U32 * ref.abs() + ETA32
+
+
+def text_pool_ref(rows):
+    """text_tokens_kernel's pooled mean of the max_len conditioning rows it wrote, rows [B, max_len, D]: the kernel adds
+    them one by one in fp32 from 0 (max_len - 1 roundings on the first row's path) and divides by max_len (one more):
+        |pooled - mean64| <= max_len U32 mean(|rows|) + ETA32.
+    Returns (mean, bound) [B, D]; `text_pool_fp32` is the same sum in the kernel's own order."""
+    r = _d(rows).cpu()
+    L = r.shape[1]
+    return r.mean(dim=1), L * U32 * r.abs().mean(dim=1) + ETA32
+
+
+def text_pool_fp32(rows):
+    """The serial fp32 sum of the rows [B, max_len, D], then the division by max_len, in the kernel's order."""
+    s = torch.zeros(rows.shape[0], rows.shape[2], dtype=torch.float32)
+    for l in range(rows.shape[1]):
+        s = s + rows[:, l].float().cpu()
+    return s / float(rows.shape[1])

@@ -806,3 +806,216 @@ def test_conv_gn_bound():
     EMU.conv_gn(x0, C0, x1, C1, 0.7071, B, H, W, G, st[0], st[1], gamma, beta, ss2, 2 * C, 1e-5, wp, Cout, bias, res, d,
                 None, None)
     _fails(d, ref, bound, "conv_gn: FiLM scale without +1 in image 0")
+
+
+# ---------------------------------------------------------------------------------------------- sampling step
+# The step kernels compute op by op in fp32 in the order torch evaluates the restatement (un-fused products and sums, an
+# exact select, at::lerp), so the emulation below is also the fp32 restatement in the kernels' order.
+def _schedule(kind, T=1000):
+    """(a, b, c1, c2, sigma, c3) fp32 tables of GaussianDiffusion's DDPM, DDIM (eta 0.5) or DPM-Solver++(2M) walk.  The
+    library's sigma[0] is 0 or 1e-10, where a kernel that forgot to zero the noise at t = 0 would stay below any bound; the
+    tests give sigma[0] = 0.25 so that the zeroing shows."""
+    from minimagen_b200.diffusion_model import GaussianDiffusion
+    gd = GaussianDiffusion(timesteps=T)
+    sch = {"ddpm": gd.ddpm_schedule, "ddim": lambda d: gd.sampling_schedule(50, 0.5, d),
+           "dpmpp": lambda d: gd.dpm_solver_schedule(20, d)}[kind]("cpu")
+    sigma = sch.sigma.clone()
+    sigma[0] = 0.25
+    return gd.sqrt_recip_alphas_cumprod, gd.sqrt_recipm1_alphas_cumprod, sch.c1, sch.c2, sigma, sch.c3, sch.grid
+
+
+def _step_data(B, n, seed, grid):
+    g = _g(seed)
+    x = torch.randn(B, n, generator=g) * 1.3
+    x[-1] *= 0.2                                       # the last image's |x0| quantile is below min_s = 1 at t = 0
+    eps, eps0, noise = (torch.randn(B, n, generator=g) for _ in range(3))
+    hist = torch.randn(B, n, generator=g)
+    t = torch.tensor([grid[0], grid[len(grid) // 2], 0][:B])
+    w = torch.tensor([7.0, 3.0, 1.5][:B])
+    return x, eps, eps0, noise, hist, t, w
+
+
+def step_fp32(x, eps, eps0, w, t, tabs, lo, hi, wt, min_s, noise, hist=None, defect=None):
+    """The step epilogue in fp32, op by op in the kernels' order: (x0, s, out, new hist).  `defect` plants one error."""
+    a, b, c1, c2, sigma, c3 = tabs
+    B = x.shape[0]
+    wc = w.reshape(B, 1) if torch.is_tensor(w) else w
+    if defect == "w0":
+        wc = w[0]
+    e = eps if eps0 is None else eps0 + (eps - eps0) * wc
+    x0 = a[t][:, None] * x - b[t][:, None] * e
+    s = torch.empty(B)
+    EMU.step_quantile(x0, B, x0.shape[1], lo + (defect == "rank"), hi, wt, min_s, s)
+    if defect == "lerp":
+        srt = x0.abs().sort(dim=-1).values
+        s = torch.lerp(srt[:, lo], srt[:, hi], torch.tensor(1 - wt)).clamp(min=min_s)
+    if defect == "min_s":
+        EMU.step_quantile(x0, B, x0.shape[1], lo, hi, wt, 0.0, s)
+    if defect == "neighbour":
+        s = s.roll(1)
+    sb = s[:, None]
+    xs = x0.clamp(-sb, sb) / sb
+    mean = c1[t][:, None] * xs + c2[t][:, None] * x
+    if hist is not None:
+        c3t = c3[t][:, None]
+        mean = torch.where(c3t != 0, mean + c3t * hist, mean)
+    sig = sigma[t] if defect == "sigma0" else torch.where(t == 0, torch.zeros(()), sigma[t])
+    return x0, s, mean + sig[:, None] * noise, xs
+
+
+def _step_refs(x, eps, eps0, w, t, tabs, lo, hi, wt, min_s, noise, hist):
+    a, b, c1, c2, sigma, c3 = tabs
+    x0r, bx0 = R.step_x0_ref(x, eps, eps0, w, t, a, b)
+    sr, bs = R.step_threshold_ref(x0r, bx0, lo, hi, wt, min_s)
+    o = R.step_posterior_ref(x0r, bx0, sr, bs, x, noise, t, c1, c2, sigma, c3 if hist is not None else None, hist)
+    return (x0r, bx0), (sr, bs), o
+
+
+@pytest.mark.parametrize("kind", ["ddpm", "ddim", "dpmpp"])
+@pytest.mark.parametrize("cfg", [True, False])
+def test_step_bounds(kind, cfg):
+    from minimagen_b200.Imagen import quantile_rank
+    *tabs, grid = _schedule(kind)
+    B, n = 3, 3 * 64 * 64
+    x, eps, eps0, noise, hist, t, w = _step_data(B, n, 5, grid)
+    eps0 = eps0 if cfg else None
+    hist = hist if kind == "dpmpp" else None
+    lo, hi, wt = quantile_rank(n, 0.9)
+    (x0r, bx0), (sr, bs), (outr, bo, xsr, bxs) = _step_refs(x, eps, eps0, w, t, tabs, lo, hi, wt, 1.0, noise, hist)
+    x0, s, out, xs = step_fp32(x, eps, eps0, w, t, tabs, lo, hi, wt, 1.0, noise, hist)
+    check(x0, x0r, bx0, f"{kind} x0")
+    check(s, sr, bs, f"{kind} s")
+    check(out, outr, bo, f"{kind} out")
+    check_rel_l2(out, outr, 1e-6, f"{kind} out")
+    if hist is not None:
+        check(xs, xsr, bxs, f"{kind} hist")
+    # the emulation of the ops interface, scalar weight (the library's own entry point)
+    if kind != "dpmpp":
+        o2, s2 = torch.empty_like(x), torch.empty(B)
+        c1, c2, sigma = tabs[2], tabs[3], tabs[4]
+        EMU.step_epilogue(x, eps, eps0, 3.0, t, tabs[0], tabs[1], c1, c2, sigma, noise, B, n, lo, hi, wt, 1.0, o2, s2)
+        (_, bx2), (sr2, bs2), (or2, bo2, _, _) = _step_refs(x, eps, eps0, 3.0, t, tabs, lo, hi, wt, 1.0, noise, None)
+        check(s2, sr2, bs2, f"{kind} emu s")
+        check(o2, or2, bo2, f"{kind} emu out")
+
+
+@pytest.mark.parametrize("defect", ["rank", "lerp", "min_s", "neighbour", "w0", "sigma0"])
+def test_step_defects(defect):
+    """Each planted defect of the select or the step fails the bound of s or of out (the last image's s is below min_s = 1,
+    the three images have different t and guidance weights, t = 0 is one of them)."""
+    from minimagen_b200.Imagen import quantile_rank
+    *tabs, grid = _schedule("ddpm")
+    B, n = 3, 3 * 64 * 64
+    x, eps, eps0, noise, _, t, w = _step_data(B, n, 5, grid)
+    lo, hi, wt = quantile_rank(n, 0.9)
+    _, (sr, bs), (outr, bo, _, _) = _step_refs(x, eps, eps0, w, t, tabs, lo, hi, wt, 1.0, noise, None)
+    _, s, out, _ = step_fp32(x, eps, eps0, w, t, tabs, lo, hi, wt, 1.0, noise, defect=defect)
+    _fails(out, outr, bo, f"step defect {defect}")
+    if defect in ("rank", "lerp", "min_s", "neighbour"):
+        _fails(s, sr, bs, f"step defect {defect} (s)")
+
+
+def test_step_quantile_nan_follows_torch():
+    """The emulated select gives NaN for a row containing NaN, and NaN (lerp(inf, inf)) when both order statistics are inf,
+    as torch.quantile; the restatement's clamp / divide then makes the whole image NaN."""
+    from minimagen_b200.Imagen import quantile_rank
+    from oracle import restatement as RS
+    B, n = 3, 1000
+    x0 = torch.randn(B, n, generator=_g(3))
+    x0[0, 17] = float("nan")
+    x0[1, :150] = float("inf")
+    lo, hi, wt = quantile_rank(n, 0.9)
+    s = torch.empty(B)
+    EMU.step_quantile(x0, B, n, lo, hi, wt, 1.0, s)
+    ref = torch.quantile(x0.abs(), 0.9, dim=-1).clamp(min=1.0)
+    assert torch.equal(s.isnan(), torch.tensor([True, True, False])) and torch.equal(s[2], ref[2])
+    tabs = RS.ddpm_tables(1000)
+    t = torch.tensor([5, 5, 5])
+    out = torch.empty(B, n)
+    EMU.step_epilogue(x0, torch.zeros(B, n), None, 1.0, t, torch.ones(1000), torch.zeros(1000),
+                      tabs["posterior_mean_coef1"], tabs["posterior_mean_coef2"], torch.zeros(1000), torch.zeros(B, n),
+                      B, n, lo, hi, wt, 1.0, out)
+    assert out[:2].isnan().all() and not out[2].isnan().any()
+
+
+def test_q_sample_bound():
+    from oracle import restatement as RS
+    tabs = RS.ddpm_tables(1000)
+    g = _g(8)
+    x0, z = torch.rand(3, 5000, generator=g), torch.randn(3, 5000, generator=g)
+    t = torch.tensor([0, 500, 999])
+    a, b = tabs["sqrt_alphas_cumprod"], tabs["sqrt_one_minus_alphas_cumprod"]
+    for ps, sh in ((1.0, 0.0), (2.0, -1.0)):
+        o = torch.empty(3, 5000)
+        EMU.q_sample(x0, z, t, a, b, 3, 5000, ps, sh, o)
+        ref, bound = R.q_sample_ref(x0, z, t, a, b, ps, sh)
+        check(o, ref, bound, f"q_sample ({ps}, {sh})")
+        if sh:
+            EMU.q_sample(x0, z, t, a, b, 3, 5000, ps, 0.0, o)        # post_shift dropped
+            _fails(o, ref, bound, "q_sample without post_shift")
+
+
+def resize_fp32(x, iy, wy, ix, wx, clamp=None, swap_strides=False):
+    """resize_sep_kernel in fp32 in its own order (sequential taps, rows inside columns).  swap_strides: the plane read
+    with Hin and Win exchanged (in[xi][yi] of a [Win, Hin] view), an x/y mix-up that stays in bounds."""
+    P, Hin, Win = x.shape
+    v = x.reshape(P, Win, Hin).transpose(1, 2) if swap_strides else x
+    acc = torch.zeros(P, iy.shape[0], ix.shape[0])
+    for j in range(ix.shape[1]):
+        col = torch.zeros(P, iy.shape[0], ix.shape[0])
+        cols = v[:, :, ix[:, j].long()]                                       # [P, Hin, Wout]
+        for i in range(iy.shape[1]):
+            col = col + wy[:, i][None, :, None] * cols[:, iy[:, i].long(), :]
+        acc = acc + wx[:, j][None, None, :] * col
+    return acc.clamp(*clamp) if clamp is not None else acc
+
+
+@pytest.mark.parametrize("H,W,scale,pad,clamp", [(40, 72, 2.0, "reflect", None), (40, 72, 0.25, "reflect", (-1.0, 1.0)),
+                                                 (64, 64, 4.0, "constant", (0.0, 1.0))])
+def test_resize_bound(H, W, scale, pad, clamp):
+    from minimagen_b200.helpers import resize_tables
+    x = torch.randn(2, H, W, generator=_g(9)) * 0.8
+    ho, iy, wy = resize_tables(H, scale, pad, "cpu")
+    wo, ix, wx = resize_tables(W, scale, pad, "cpu")
+    ref, bound = R.resize_ref(x, iy, wy, ix, wx, clamp)
+    o = torch.empty(2, ho, wo)
+    EMU.resize_separable(x, 2, H, W, o, ho, wo, iy, wy, ix, wx, clamp=clamp)
+    check(o, ref, bound, f"resize {H}x{W} x{scale} emulation")
+    check(resize_fp32(x, iy, wy, ix, wx, clamp), ref, bound, f"resize {H}x{W} x{scale} fp32 order")
+    if H != W:
+        _fails(resize_fp32(x, iy, wy, ix, wx, clamp, swap_strides=True), ref, bound, "resize: Hin/Win strides swapped")
+    if pad == "reflect":
+        # a border tap reflected off by one: -tap - 1 instead of -tap (the 'symmetric' boundary)
+        _, iy1, wy1 = resize_tables(H, scale, "symmetric", "cpu")
+        _fails(resize_fp32(x, iy1, wy1, ix, wx, clamp), ref, bound, "resize: border tap off by one")
+
+
+@pytest.mark.parametrize("dim", [8, 128, 1024])
+def test_posemb_bound(dim):
+    t = torch.tensor([0, 1, 17, 500, 999])
+    o = torch.empty(5, dim)
+    EMU.posemb(t, 5, dim, o)
+    ref, bound = R.posemb_ref(t, dim)
+    check(o, ref, bound, f"posemb {dim}")
+    half = dim // 2
+    e = torch.exp(torch.arange(half) * -(torch.log(torch.tensor(10000.0)) / half))          # half instead of half - 1
+    arg = t[:, None].float() * e[None, :]
+    _fails(torch.cat((arg.sin(), arg.cos()), dim=-1), ref, bound, "posemb: half instead of half - 1")
+    _fails(torch.cat((o[:, half:], o[:, :half]), dim=-1), ref, bound, "posemb: sin and cos swapped")
+
+
+@pytest.mark.parametrize("L,D", [(11, 16), (300, 40)])
+def test_text_pool_bound(L, D):
+    B, max_len, m, off = 3, 256, 260, 4
+    g = _g(10)
+    proj, null = torch.randn(B, L, D, generator=g), torch.randn(max_len, D, generator=g)
+    mask = (torch.rand(B, L, generator=g) > 0.3).to(torch.uint8)
+    keep = torch.tensor([1, 0, 1], dtype=torch.uint8)
+    c, p = torch.full((B, m, D), float("nan")), torch.empty(B, D)
+    EMU.text_tokens(proj, B, L, D, mask, keep, null, max_len, c, m, off, p)
+    rows = c[:, off:off + max_len]
+    ref, bound = R.text_pool_ref(rows)
+    check(p, ref, bound, "text pooled (emulation)")
+    check(R.text_pool_fp32(rows), ref, bound, "text pooled (fp32 serial)")
+    if L < max_len:
+        _fails(rows.sum(dim=1) / L, ref, bound, "text pooled / Lc")
