@@ -426,7 +426,8 @@ class Conv2d(nn.Conv2d):
         kh, kw = self.kernel_size
         strides = (H * W * Cout, W * Cout, Cout)
         dev = a.device
-        if a.dtype == F16:
+        if a.dim() == 5:      # the operand's layout, not its dtype, names the path
+            assert a.dtype == F16
             # Downsample: 4-phase split operand (mode 1) or the fp16 activation read in place with TMA element strides (6)
             mode = (6 if in_place_s2 else 1) if self._geom == 'down' else 0
             # epilogue statistics credit a warp's 32 pixel rows to ONE image: needs whole images per 32-row slab
@@ -440,6 +441,7 @@ class Conv2d(nn.Conv2d):
                            self.bias, residual, o32, o16, strides, act2=a2, lda2=a2.shape[-1] if exists(a2) else 0,
                            c_in1=c_in1, out_stats=st)
             return Act(o32, o16, st)
+        assert a.dtype == F32
         out = torch.empty((B, H, W, Cout), dtype=F32, device=dev)
         Hin, Win = a.shape[1], a.shape[2]
         ops.conv_direct(a, B, Hin, Win, Cin, a.shape[3], self.weight.detach(), Cout, kh, kw, self.stride[0],
@@ -498,7 +500,8 @@ class Conv2d(nn.Conv2d):
         kh, kw = self.kernel_size
         if out is None:
             out = torch.empty((B, Cout, H, W), dtype=F32, device=a.device)
-        if a.dtype == F16:
+        if a.dim() == 5:
+            assert a.dtype == F16
             Np = (Cout + 15) // 16 * 16
             key = (self.weight.data_ptr(), self.weight._version, self.bias._version if exists(self.bias) else -1)
             if getattr(self, "_nchw_key", None) != key:
@@ -862,7 +865,7 @@ class CrossAttention(nn.Module):
         if tc_o:
             y = _linear_rows(None, o, B * n, inner, self.to_out[0].weight, self._po, C)
         else:
-            y = _linear_rows(o.float(), None, B * n, inner, self.to_out[0].weight, self._po, C)
+            y = _linear_rows(o.to(F32), None, B * n, inner, self.to_out[0].weight, self._po, C)
         o32, o16 = self.to_out[1].run_rows(y, B * n, C, residual=rows if residual else None, both=True)
         return Act(o32.reshape(B, H, W, C), o16.reshape(B, 1, H, W, C))
 
@@ -916,7 +919,7 @@ class Attention(nn.Module):
         if _tc_linear_ok(B * n, inner, C):
             y = _linear_rows(None, o, B * n, inner, self.to_out[0].weight, self._po, C)
         else:
-            y = _linear_rows(o.float(), None, B * n, inner, self.to_out[0].weight, self._po, C)
+            y = _linear_rows(o.to(F32), None, B * n, inner, self.to_out[0].weight, self._po, C)
         o32, o16 = self.to_out[1].run_rows(y, B * n, C, residual=rows if residual else None, both=True)
         return Act(o32.reshape(B, H, W, C), o16.reshape(B, 1, H, W, C))
 

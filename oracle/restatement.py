@@ -90,11 +90,12 @@ def _chan_ln(sd, p, x, eps=1e-5):
     return (x - mean) / (var + eps).sqrt() * sd[p + '.g']
 
 
-def _posemb(t, dim):
-    """layers.SinusoidalPosEmb (layers.py:455-465)"""
+def _posemb(t, dim, dtype=torch.float32):
+    """layers.SinusoidalPosEmb (layers.py:455-465); `dtype` float64 for a float64 run of the network"""
     half = dim // 2
     step = math.log(10000) / (half - 1)
-    freqs = torch.exp(torch.arange(half, device=t.device) * -step)
+    ar = torch.arange(half, device=t.device)
+    freqs = torch.exp((ar.double() if dtype == torch.float64 else ar) * -step)
     arg = t[:, None] * freqs[None, :]
     return torch.cat((arg.sin(), arg.cos()), dim=-1)
 
@@ -106,6 +107,11 @@ def _block(sd, p, x, scale_shift=None, groups=8):
         scale, shift = scale_shift
         x = x * (scale + 1) + shift
     return _conv(sd, p + '.project', F.silu(x), padding=1)
+
+
+def _softmax_dtype(sim):
+    """The reference softmaxes in fp32 whatever it is fed; a float64 run of this restatement stays float64."""
+    return torch.float64 if sim.dtype == torch.float64 else torch.float32
 
 
 def _split_heads(x, h):
@@ -128,7 +134,7 @@ def _cross_attention(sd, p, x, context, heads=8, mask=None):
     if mask is not None:
         mk = F.pad(mask, (1, 0), value=True)[:, None, None, :]
         sim = sim.masked_fill(~mk, -torch.finfo(sim.dtype).max)
-    out = sim.softmax(dim=-1, dtype=torch.float32) @ v
+    out = sim.softmax(dim=-1, dtype=_softmax_dtype(sim)) @ v
     out = out.permute(0, 2, 1, 3).reshape(b, x.shape[1], -1)
     return _ln(sd, p + '.to_out.1', F.linear(out, sd[p + '.to_out.0.weight']))
 
@@ -147,7 +153,7 @@ def _attention(sd, p, x, heads=8, mask=None):
     if mask is not None:
         mk = F.pad(mask, (1, 0), value=True)[:, None, None, :]
         sim = sim.masked_fill(~mk, -torch.finfo(sim.dtype).max)
-    out = torch.einsum('bhij,bjd->bhid', sim.softmax(dim=-1, dtype=torch.float32), v)
+    out = torch.einsum('bhij,bjd->bhid', sim.softmax(dim=-1, dtype=_softmax_dtype(sim)), v)
     out = out.permute(0, 2, 1, 3).reshape(b, x.shape[1], -1)
     return _ln(sd, p + '.to_out.1', F.linear(out, sd[p + '.to_out.0.weight']))
 
@@ -203,7 +209,7 @@ def unet_forward(sd, cfg, x, time, lowres_cond_img=None, lowres_noise_times=None
 
     # --- time conditioning
     def time_branch(prefix, times):
-        hid = F.silu(_linear(sd, prefix + 'hiddens.1', _posemb(times, dim)))
+        hid = F.silu(_linear(sd, prefix + 'hiddens.1', _posemb(times, dim, x.dtype)))
         return _linear(sd, prefix + 'cond.0', hid), _linear(sd, prefix + 'tokens.0', hid).reshape(bsz, 2, -1)
     t, time_tokens = time_branch('to_time_', time)
     if lowres:

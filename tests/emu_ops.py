@@ -4,6 +4,16 @@ It mirrors the CONTRACT of every C-ABI entry point (layouts, packing order, stri
 output semantics) with plain torch ops, so that the host-side orchestration in minimagen_b200/{layers,Unet,Imagen}.py
 can be executed -- and compared against the real reference -- on a box without a GPU.  The product never imports this
 file; on a GPU box the native library is the only backend.
+
+Two modes, chosen by the storage-dtype pair of the U-Net ops (the sampler's step ops are fp32 in both):
+
+  EmuOps()                                       lo = fp16, hi = fp32: the kernels' storage types.  Tensor-core operands and
+                                                 fp16 outputs are rounded (saturating) to fp16 like the kernels do, so a
+                                                 network agrees with the fp32 reference at the operand-rounding level (~1e-3).
+  EmuOps(lo=torch.float64, hi=torch.float64)     exact mode: no rounding and no saturation anywhere.  Together with the host
+                                                 modules' dtype constants set to float64 (tests/test_lowering_exact.py) the
+                                                 orchestration becomes a pure DATAFLOW: it must agree with a float64 run of the
+                                                 reference restatement to ~1e-10 per element, whatever the network amplifies.
 """
 import math
 
@@ -17,11 +27,6 @@ def _strided(out, shape, strides):
     return out.as_strided(shape, strides, out.storage_offset())
 
 
-def _sat16(y):
-    """fp32 -> fp16 with saturation (csrc/sat_half.cuh): beyond +-65504 -> +-65504, not inf."""
-    return y.clamp(-65504.0, 65504.0).to(F16)
-
-
 def _cat_src(src0, c0, src1, c1, scale1, lead_shape):
     a = src0.reshape(*lead_shape, c0)
     if src1 is None or c1 == 0:
@@ -32,8 +37,14 @@ def _cat_src(src0, c0, src1, c1, scale1, lead_shape):
 class EmuOps:
     name = "torch-emulation (tests only)"
 
-    def __init__(self):
+    def __init__(self, lo=F16, hi=F32):
+        self.lo, self.hi = lo, hi
         self.calls = []
+        self.conv_log = []      # per host call: conv_igemm (mode, kh, kw, c_in, c_out); conv_res1x1 ('res1x1', two x sources, x_cin, c_in, c_out)
+
+    def _sat16(self, y):
+        """hi -> lo; fp32 -> fp16 saturates (csrc/sat_half.cuh): beyond +-65504 -> +-65504, not inf."""
+        return y.clamp(-65504.0, 65504.0).to(F16) if self.lo == F16 else y.to(self.lo)
 
     def _log(self, name):
         self.calls.append(name)
@@ -59,7 +70,7 @@ class EmuOps:
         if w.dim() == 2:
             w = w[:, :, None, None]
         O, I, KH, KW = w.shape
-        return (w.detach().float() * scale).permute(0, 2, 3, 1).reshape(O, KH * KW * I).to(F16).contiguous()
+        return (w.detach().to(self.hi) * scale).permute(0, 2, 3, 1).reshape(O, KH * KW * I).to(self.lo).contiguous()
 
     def pack_conv_weight_dgrad(self, w):
         if w.dim() == 2:
@@ -70,20 +81,21 @@ class EmuOps:
     def conv_igemm(self, act, B, H, W, lda, c_off, c_in, wp, c_out, kh, kw, mode, bias, residual, out_f32, out_f16,
                    out_strides, block_n=0, out_sc=1, n_valid=0, act2=None, lda2=0, c_off2=0, c_in1=0, out_stats=None):
         self._log("conv_igemm")
-        assert act.dtype == F16 and wp.dtype == F16
+        self.conv_log.append((mode, kh, kw, c_in, c_out))
+        assert act.dtype == self.lo and wp.dtype == self.lo
         P = 4 if mode == 1 else 1
         if mode == 6:
-            a = act.reshape(B, 2 * H, 2 * W, lda)[..., c_off:c_off + c_in].float()
-            w = wp.float().reshape(c_out, kh, kw, c_in).permute(0, 3, 1, 2)
+            a = act.reshape(B, 2 * H, 2 * W, lda)[..., c_off:c_off + c_in].to(self.hi)
+            w = wp.to(self.hi).reshape(c_out, kh, kw, c_in).permute(0, 3, 1, 2)
             y = F.conv2d(a.permute(0, 3, 1, 2), w, None, stride=2, padding=1).permute(0, 2, 3, 1)
             return self._conv_finish(y, B, H, W, c_out, bias, residual, out_f32, out_f16, out_strides, out_sc, n_valid,
                                      out_stats)
         if act2 is None:
-            a = act.reshape(B, P, H, W, lda)[..., c_off:c_off + c_in].float()
+            a = act.reshape(B, P, H, W, lda)[..., c_off:c_off + c_in].to(self.hi)
         else:
-            a = torch.cat((act.reshape(B, P, H, W, lda)[..., c_off:c_off + c_in1].float(),
-                           act2.reshape(B, P, H, W, lda2)[..., c_off2:c_off2 + (c_in - c_in1)].float()), dim=-1)
-        w = wp.float().reshape(c_out, kh, kw, c_in).permute(0, 3, 1, 2)           # OIHW
+            a = torch.cat((act.reshape(B, P, H, W, lda)[..., c_off:c_off + c_in1].to(self.hi),
+                           act2.reshape(B, P, H, W, lda2)[..., c_off2:c_off2 + (c_in - c_in1)].to(self.hi)), dim=-1)
+        w = wp.to(self.hi).reshape(c_out, kh, kw, c_in).permute(0, 3, 1, 2)           # OIHW
         if mode == 0:
             y = F.conv2d(a[:, 0].permute(0, 3, 1, 2), w, None, stride=1, padding=(kh // 2, kw // 2))
         elif mode >= 2:
@@ -93,7 +105,7 @@ class EmuOps:
             y = F.conv2d(x[:, :, pa:pa + H + 1, pb:pb + W + 1], w, None)
         else:
             # un-split the 4 phases back to the (2H, 2W) input: phase p = (h&1)*2 + (w&1)
-            full = torch.zeros((B, 2 * H, 2 * W, c_in))
+            full = torch.zeros((B, 2 * H, 2 * W, c_in), dtype=self.hi)
             for p in range(4):
                 full[:, (p >> 1)::2, (p & 1)::2] = a[:, p]
             y = F.conv2d(full.permute(0, 3, 1, 2), w, None, stride=2, padding=1)
@@ -116,7 +128,7 @@ class EmuOps:
         if out_f32 is not None:
             _strided(out_f32, (B, H, W, nv), (sb, sh, sw, out_sc)).copy_(y)
         if out_f16 is not None:
-            _strided(out_f16, (B, H, W, nv), (sb, sh, sw, out_sc)).copy_(_sat16(y))
+            _strided(out_f16, (B, H, W, nv), (sb, sh, sw, out_sc)).copy_(self._sat16(y))
 
     def conv_res1x1_supported(self, H, W, c_in, c_out, x_cin):
         t16 = W == 16 and H % 16 == 0
@@ -126,16 +138,17 @@ class EmuOps:
     def conv_res1x1(self, act, B, H, W, lda, c_in, act2, lda2, c_in1, x, ldx, x_cin, x2, ldx2, x_cin1, wp, c_out, bias,
                     residual, out_f32, out_f16, out_stats):
         self._log("conv_res1x1")
+        self.conv_log.append(("res1x1", x2 is not None, x_cin, c_in, c_out))
         K3 = 9 * c_in
-        y = torch.zeros((B, H, W, c_out))
+        y = torch.zeros((B, H, W, c_out), dtype=self.hi)
         st = (H * W * c_out, W * c_out, c_out)
         self.conv_igemm(act, B, H, W, lda, 0, c_in, wp[:, :K3].contiguous(), c_out, 3, 3, 0, None, None, y, None, st,
                         act2=act2, lda2=lda2, c_in1=c_in1)
-        self.calls.pop()
-        y1 = torch.zeros((B, H, W, c_out))
+        self.calls.pop(), self.conv_log.pop()
+        y1 = torch.zeros((B, H, W, c_out), dtype=self.hi)
         self.conv_igemm(x, B, H, W, ldx, 0, x_cin, wp[:, K3:].contiguous(), c_out, 1, 1, 0, None, None, y1, None, st,
                         act2=x2, lda2=ldx2, c_in1=x_cin1)
-        self.calls.pop()
+        self.calls.pop(), self.conv_log.pop()
         self._conv_finish(y + y1, B, H, W, c_out, bias, residual, out_f32, out_f16, st, 1, 0, out_stats)
 
     def conv_gn_supported(self, H, W, c0, c1, c_out, groups):
@@ -147,13 +160,13 @@ class EmuOps:
                 wp, c_out, bias, residual, out_f32, out_f16, out_stats):
         self._log("conv_gn")
         C = c0 + c1
-        a = torch.zeros((B, 1, H, W, C), dtype=F16)
+        a = torch.zeros((B, 1, H, W, C), dtype=self.lo)
         self.gn_apply_silu(src0, c0, src1, c1, scale1, B, H * W, groups, stats0, 16, stats1, 16, gamma, beta, scale_shift,
                            ss_ld, eps, a)
         self.calls.pop()
         self.conv_igemm(a, B, H, W, C, 0, C, wp, c_out, 3, 3, 0, bias, residual, out_f32, out_f16,
                         (H * W * c_out, W * c_out, c_out), out_stats=out_stats)
-        self.calls.pop()
+        self.calls.pop(), self.conv_log.pop()
 
     def conv_direct(self, inp, B, Hin, Win, c_in, ldi, w, c_out, kh, kw, stride, pad, bias, residual, out, Hout, Wout,
                     out_strides):
@@ -170,7 +183,7 @@ class EmuOps:
     # ---------------------------------------------------------------- normalisation / casts
     def gn_stats(self, src0, c0, src1, c1, scale1, B, hw, groups, sums):
         self._log("gn_stats")
-        x = _cat_src(src0.float(), c0, src1.float() if src1 is not None else None, c1, scale1, (B, hw)).double()
+        x = _cat_src(src0.to(self.hi), c0, src1.to(self.hi) if src1 is not None else None, c1, scale1, (B, hw)).double()
         C = c0 + c1
         xg = x.reshape(B, hw, groups, C // groups)
         sums[:, :, 0] += xg.sum(dim=(1, 3))
@@ -179,7 +192,7 @@ class EmuOps:
     def gn_apply_silu(self, src0, c0, src1, c1, scale1, B, hw, groups, stats0, sb0, stats1, sb1, gamma, beta,
                       scale_shift, ss_ld, eps, out):
         self._log("gn_apply_silu")
-        x = _cat_src(src0.float(), c0, src1.float() if src1 is not None else None, c1, scale1, (B, hw))
+        x = _cat_src(src0.to(self.hi), c0, src1.to(self.hi) if src1 is not None else None, c1, scale1, (B, hw))
         C = c0 + c1
         n = (C // groups) * hw
         if sb0 == 0:
@@ -197,18 +210,18 @@ class EmuOps:
         mean = sums[:, :, 0] / n
         var = (sums[:, :, 1] / n - mean * mean).clamp(min=0)
         rstd = 1.0 / torch.sqrt(var + eps)
-        mean_c = mean.float().repeat_interleave(C // groups, dim=1)[:, None, :]
-        rstd_c = rstd.float().repeat_interleave(C // groups, dim=1)[:, None, :]
+        mean_c = mean.to(self.hi).repeat_interleave(C // groups, dim=1)[:, None, :]
+        rstd_c = rstd.to(self.hi).repeat_interleave(C // groups, dim=1)[:, None, :]
         y = (x - mean_c) * rstd_c * gamma.detach() + beta.detach()
         if scale_shift is not None:
             ss = scale_shift.as_strided((B, 2 * C), (ss_ld, 1), scale_shift.storage_offset())
             y = y * (ss[:, None, :C] + 1.0) + ss[:, None, C:]
         y = y * torch.sigmoid(y)
-        out.reshape(B, hw, C).copy_(_sat16(y) if out.dtype == F16 else y)
+        out.reshape(B, hw, C).copy_(self._sat16(y) if out.dtype == self.lo else y)
 
     def cast_act(self, src0, c0, src1, c1, scale1, B, H, W, mode, out):
         self._log("cast_act")
-        x = _cat_src(src0.float(), c0, src1.float() if src1 is not None else None, c1, scale1, (B, H, W))
+        x = _cat_src(src0.to(self.hi), c0, src1.to(self.hi) if src1 is not None else None, c1, scale1, (B, H, W))
         C = c0 + c1
         if mode == 0:
             out.reshape(-1)[:B * H * W * C].reshape(B, H, W, C).copy_(x.to(out.dtype))     # the kernel writes the first B*H*W rows
@@ -231,7 +244,7 @@ class EmuOps:
         if out_f32 is not None:
             out_f32.reshape(rows, C).copy_(y)
         if out_f16 is not None:
-            out_f16.reshape(rows, C).copy_(y.to(F16))
+            out_f16.reshape(rows, C).copy_(y.to(self.lo))
 
     # ---------------------------------------------------------------- conditioning
     def linear_f32(self, inp, M, K, W, bias, Nout, in_act, out_act, addend, out_f32, out_f16, out_scale=1.0):
@@ -248,20 +261,20 @@ class EmuOps:
         if out_f32 is not None:
             out_f32.reshape(M, Nout).copy_(y)
         if out_f16 is not None:
-            out_f16.reshape(M, Nout).copy_(y.to(F16))
+            out_f16.reshape(M, Nout).copy_(y.to(self.lo))
 
     def posemb(self, t, B, dim, out):
         self._log("posemb")
         half = dim // 2
         step = math.log(10000) / (half - 1)
-        emb = torch.exp(torch.arange(half) * -step)
+        emb = torch.exp(torch.arange(half).to(self.hi) * -step)
         arg = t[:, None] * emb[None, :]
         out.copy_(torch.cat((arg.sin(), arg.cos()), dim=-1))
 
     def text_tokens(self, proj, B, L, D, mask, keep, null_embed, max_len, c_out, m, row_off, pooled):
         self._log("text_tokens")
         Lc = min(L, max_len)
-        tok = torch.zeros((B, max_len, D))
+        tok = torch.zeros((B, max_len, D), dtype=self.hi)
         tok[:, :Lc] = proj.reshape(B, L, D)[:, :Lc]
         cond = keep.bool()[:, None].expand(B, max_len).clone()
         if mask is not None:
@@ -296,10 +309,10 @@ class EmuOps:
         x = a if b is None or cb == 0 else torch.cat((a, b), dim=1)            # B,C,H,W
         C = x.shape[1]
         xp = F.pad(x, (7, 8))                                                   # w + j - 7, j in [0,16)
-        o = torch.zeros((B, H, W, 16, 8))
+        o = torch.zeros((B, H, W, 16, 8), dtype=self.hi)
         for j in range(15):
             o[:, :, :, j, :C] = xp[:, :, :, j:j + W].permute(0, 2, 3, 1)
-        out.reshape(B, H, W, 128).copy_(o.reshape(B, H, W, 128).to(F16))
+        out.reshape(B, H, W, 128).copy_(o.reshape(B, H, W, 128).to(self.lo))
 
     def resize_separable(self, inp, planes, hin, win, out, hout, wout, iy, wy, ix, wx, clamp=None):
         self._log("resize_separable")
@@ -317,11 +330,11 @@ class EmuOps:
     # ---------------------------------------------------------------- attention
     def attention(self, q, q_bs, ldq, k, v, kv_bs, ldkv, kv_hs, null_kv, mask, B, heads, n, m, out, o_bs, ldo):
         self._log("attention")
-        qq = q.as_strided((B, heads, n, 64), (q_bs, 64, ldq, 1), q.storage_offset()).float()
-        kk = k.as_strided((B, heads, m, 64), (kv_bs, kv_hs, ldkv, 1), k.storage_offset()).float()
-        vv = v.as_strided((B, heads, m, 64), (kv_bs, kv_hs, ldkv, 1), v.storage_offset()).float()
-        nk = null_kv.detach()[0].to(F16).float().reshape(1, 1, 1, 64).expand(B, heads, 1, 64)
-        nv = null_kv.detach()[1].to(F16).float().reshape(1, 1, 1, 64).expand(B, heads, 1, 64)
+        qq = q.as_strided((B, heads, n, 64), (q_bs, 64, ldq, 1), q.storage_offset()).to(self.hi)
+        kk = k.as_strided((B, heads, m, 64), (kv_bs, kv_hs, ldkv, 1), k.storage_offset()).to(self.hi)
+        vv = v.as_strided((B, heads, m, 64), (kv_bs, kv_hs, ldkv, 1), v.storage_offset()).to(self.hi)
+        nk = null_kv.detach()[0].to(self.lo).to(self.hi).reshape(1, 1, 1, 64).expand(B, heads, 1, 64)
+        nv = null_kv.detach()[1].to(self.lo).to(self.hi).reshape(1, 1, 1, 64).expand(B, heads, 1, 64)
         kk = torch.cat((nk, kk), dim=2)
         vv = torch.cat((nv, vv), dim=2)
         sim = qq @ kk.transpose(-1, -2)
@@ -330,7 +343,7 @@ class EmuOps:
             sim = sim.masked_fill(~mk, -torch.finfo(sim.dtype).max)
         attn = sim.softmax(dim=-1)
         o = attn @ vv                                                       # B,h,n,64
-        out.as_strided((B, heads, n, 64), (o_bs, 64, ldo, 1), out.storage_offset()).copy_(o.to(F16))
+        out.as_strided((B, heads, n, 64), (o_bs, 64, ldo, 1), out.storage_offset()).copy_(o.to(self.lo))
 
     # ---------------------------------------------------------------- DDPM step
     def step_x0(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0):
@@ -422,8 +435,8 @@ class EmuOps:
     def conv_wgrad_tc(self, dy16, x16, B, Ho, Wo, c_in, c_out, kh, kw, dw, stride=1):
         self._log("conv_wgrad_tc")
         pad = 1 if stride == 2 else kh // 2
-        g = torch.nn.grad.conv2d_weight(x16.float().reshape(B, stride * Ho, stride * Wo, c_in).permute(0, 3, 1, 2),
-                                        (c_out, c_in, kh, kw), dy16.float().reshape(B, Ho, Wo, c_out).permute(0, 3, 1, 2),
+        g = torch.nn.grad.conv2d_weight(x16.to(self.hi).reshape(B, stride * Ho, stride * Wo, c_in).permute(0, 3, 1, 2),
+                                        (c_out, c_in, kh, kw), dy16.to(self.hi).reshape(B, Ho, Wo, c_out).permute(0, 3, 1, 2),
                                         stride=stride, padding=pad)
         dw.reshape(c_out, c_in, kh, kw).copy_(g)
 
