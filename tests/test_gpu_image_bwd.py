@@ -128,6 +128,7 @@ WGRAD_TC_CASES = [
     (1, 8, 8, 128, 128, 3, 1),          # one box: one split
     # stride 2, the 4x4 pad-1 Downsample: TMA element-stride boxes, padding row at coordinate -1
     (2, 16, 16, 128, 128, 4, 2), (3, 8, 16, 64, 256, 4, 2), (1, 32, 32, 192, 128, 4, 2), (2, 32, 32, 256, 256, 4, 2),
+    (2, 8, 8, 1024, 512, 3, 1),         # the 8x8 level of the cfg-3 U-Net's training step
 ]
 
 
@@ -147,6 +148,29 @@ def test_conv_wgrad_tc(native, B, Ho, Wo, cin, cout, k, stride):
     per, splits = R.wgrad_tc_plan(B, Ho, Wo, cin, cout, k, _sms())
     ref, bound = R.conv_wgrad_ref(dy16, x16, stride, pad, k, k, R.wgrad_tc_acc_len(B, Ho, Wo, cin, cout, k, _sms()))
     what = f"conv_wgrad_tc B={B} {Ho}x{Wo} {cin}->{cout} k={k} stride={stride} splits={splits} boxes/split={per}"
+    check(dw, ref, bound, what)
+    check_rel_l2(dw, ref, REL_WGRAD_TC, what)
+    last = torch.zeros_like(dy16)
+    last[-1, -8:, -8:] = dy16[-1, -8:, -8:]
+    _rejects(dw - R.conv_wgrad_ref(last, x16, stride, pad, k, k, 1)[0], ref, bound, what + ": last 8x8 box dropped")
+
+
+@pytest.mark.parametrize("B,Ho,Wo,cin,cout,k,stride", [(2, 8, 8, 1024, 512, 3, 1), (2, 16, 16, 128, 128, 4, 2)])
+def test_conv_wgrad_tc_subnormal_dy(native, B, Ho, Wo, cin, cout, k, stride):
+    """dy of the deep levels of a training step is small enough to round to fp16 subnormals (the cfg-3 U-Net's 8x8
+    1024 -> 512 conv: |dy| ~ 1e-8).  The wgmma k-group aligns such a product as if its subnormal factor were 2^-14
+    (fp64_ref.align_mag), so the error is measured against that; the bound must hold and still see a dropped box."""
+    gen = torch.Generator().manual_seed(B * 1000 + Ho + cin + 7)
+    x16 = torch.randn(B, stride * Ho, stride * Wo, cin, generator=gen).cuda().half()
+    dy16 = (torch.randn(B, Ho, Wo, cout, generator=gen) * 2.0 ** -22).cuda().half()
+    sub = (dy16 != 0) & (dy16.abs() < R.FP16_MIN_NORMAL)
+    assert sub.float().mean() > 0.85
+    pad = 1 if stride == 2 else k // 2
+    dw = torch.full((cout, cin, k, k), float("nan"), device="cuda")
+    native.conv_wgrad_tc(dy16, x16, B, Ho, Wo, cin, cout, k, k, dw, stride)
+    torch.cuda.synchronize()
+    ref, bound = R.conv_wgrad_ref(dy16, x16, stride, pad, k, k, R.wgrad_tc_acc_len(B, Ho, Wo, cin, cout, k, _sms()))
+    what = f"conv_wgrad_tc subnormal dy B={B} {Ho}x{Wo} {cin}->{cout} k={k} stride={stride}"
     check(dw, ref, bound, what)
     check_rel_l2(dw, ref, REL_WGRAD_TC, what)
     last = torch.zeros_like(dy16)
