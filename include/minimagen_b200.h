@@ -81,7 +81,9 @@ int mi_pack_conv_weight_dgrad_f16(const float* w_oihw, int c_out, int c_in, int 
  *             Block (layers.py:136) for free; needs out_sc = 1
  *   block_n   0 = auto, or one of 16/32/64/128/256 (tile width; must divide c_out).  The width also sets the schedule:
  *             256-wide tiles are split between the two consumer warpgroups, narrower ones alternate between them whole so
- *             that one tile's epilogue overlaps the next tile's MMAs
+ *             that one tile's epilogue overlaps the next tile's MMAs.  At c_out = 128, 256 selects the transposed
+ *             schedule (128 channels x 256 pixels of one image per tile; needs out_sc = 1, n_valid = c_out and a grid
+ *             that tiles by 256 pixels inside an image, else auto), which auto also picks when it gives every SM a tile
  *   workspace reserved, pass NULL / 0
  * Requirements: c_in % 64 == 0, c_out % 16 == 0, W a power of two >= 8 (or W >= 128), see mi_conv2d_igemm_supported.
  * A plain GEMM  out[M][N] = act[M][K] * w[N][K]^T  is the case B=1, H=1, W=M, kh=kw=1. */

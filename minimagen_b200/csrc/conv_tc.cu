@@ -28,6 +28,14 @@
 // In the TMA kernel the producer warpgroup gives its registers to the consumers (setmaxnreg 40 / 232): that is what lets
 // a consumer hold 128 accumulators, of a 256-wide cooperative tile or of a 128-wide ping-pong one.
 //
+// Transposed schedule (C_out = 128, TR): D^T[128 channels, pixels] = Wp . A^T runs on the cooperative 256-wide kernel
+// unchanged but for the producer and the epilogue.  The weight box (64 K x 128 channels) fills the 16 KiB stage slot and
+// is the wgmma A operand; a 256-pixel activation box (BW = 256, or BW = W and BH = 256 / W, one image) fills the 32 KiB
+// slot and is B.  Consumer cw owns output channels [64 cw, 64 cw + 64) of 256 pixels, so a C_out = 128 conv moves the
+// operand bytes per FLOP of a 128x256 tile instead of a 128x128 one.  Its epilogue stores channel-strided from the
+// fragments (8 channels x 4 pixels per warp store) and, every value of a warp being in one 16-channel block of one image,
+// sums its statistics with one shuffle reduction and one atomic pair per warp and tile.
+//
 // Fused GroupNorm variant (Block.forward, minimagen/layers.py:131-145: GroupNorm -> (scale + 1, shift) -> SiLU -> 3x3 conv):
 // the whole producer warpgroup builds the A tile instead of TMA -- it reads the fp32 NHWC source(s) (optionally the virtual
 // concat cat(x, skip * s), Unet.py:445), applies y = SiLU(x * A[b,c] + Bc[b,c]) with per-(image, channel) coefficients folded
@@ -76,7 +84,7 @@ struct Cfg {
 
 __device__ __forceinline__ float silu(float v) { return __fdividef(v, 1.0f + __expf(-v)); }
 
-template <int BLOCK_N, bool GN>
+template <int BLOCK_N, bool GN, bool TR = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmX,
@@ -85,8 +93,10 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     using C = Cfg<BLOCK_N>;
     constexpr int STAGES = C::kStages;
     static_assert(2 * STAGES * 8 <= 256, "barrier block overlaps the GroupNorm scratch");
-    constexpr bool PP = !GN && BLOCK_N <= 128;    // ping-pong schedule (else cooperative)
+    static_assert(!TR || (BLOCK_N == 256 && !GN), "the transposed tile is the cooperative 256-wide one");
+    constexpr bool PP = !GN && !TR && BLOCK_N <= 128;    // ping-pong schedule (else cooperative)
     constexpr int HALVES = PP ? 2 : 1;            // 64-row halves of a tile one consumer computes
+    constexpr int TILE_PIX = TR ? BLOCK_N : kConvBlockM;   // pixels per tile
 
     extern __shared__ uint8_t smem_raw[];
     // SWIZZLE_128B operands need 1024-byte aligned stage bases
@@ -121,7 +131,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int tiles_m = args.tiles_w * args.tiles_h * args.tiles_b;
     const int total_tiles = tiles_m * args.tiles_n;
     const int BW = 1 << args.bw_log2, BH = 1 << args.bh_log2;
-    const int BB = kConvBlockM >> (args.bw_log2 + args.bh_log2);
+    const int BB = TILE_PIX >> (args.bw_log2 + args.bh_log2);
 
     if (wg == 0) {
         if constexpr (!GN) {
@@ -140,8 +150,10 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     for (int kb = 0; kb < num_kb; ++kb) {
                         ptx::mbar_wait(&empty_bar[stage], phase ^ 1, err, 100 + stage);
                         if (ptx::elect_one()) {
-                            uint8_t* sa = smem + stage * C::kStageBytes;
-                            uint8_t* sb = sa + kABytes;
+                            // transposed: the 128-channel weight tile is the wgmma A operand (16 KiB slot), the
+                            // 256-pixel activation tile the B operand
+                            uint8_t* sa = smem + stage * C::kStageBytes + (TR ? kABytes : 0);
+                            uint8_t* sb = smem + stage * C::kStageBytes + (TR ? 0 : kABytes);
                             ptx::mbar_arrive_expect_tx(&full_bar[stage], C::kStageBytes);
                             if (kb < num_tap_kb) {
                                 const int t = kb / args.chunks_per_tap, j = kb - t * args.chunks_per_tap;
@@ -372,6 +384,81 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int tw0 = (mt % args.tiles_w) * BW;
             const int th0 = ((mt / args.tiles_w) % args.tiles_h) * BH;
             const int tb0 = (mt / (args.tiles_w * args.tiles_h)) * BB;
+            if constexpr (TR) {
+                // ---- transposed epilogue: fragment element 4j + 2r + e = output channel c0 + 8r, tile pixel 8j + cq + e.
+                // The tile is whole and in image tb0, and the warp's values are all in 16-channel block c0 / 16: one
+                // statistics pair per warp.  Like the row-major epilogue, a thread sums 8 values in fp32 (then fp64).
+                const int c0 = 64 * cw + 16 * wq + (lane >> 2);
+                const float bv[2] = {args.bias ? __ldg(args.bias + c0) : 0.f, args.bias ? __ldg(args.bias + c0 + 8) : 0.f};
+                const long long base = (long long)tb0 * args.out_sb + (long long)th0 * args.out_sh +
+                                       (long long)(tw0 + cq) * args.out_sw + c0;
+                float* const o32 = args.out_f32 ? args.out_f32 + base : nullptr;
+                __half* const o16 = args.out_f16 ? args.out_f16 + base : nullptr;
+                const float* const res = args.residual ? args.residual + base : nullptr;
+                // offsets inside a tile fit in 31 bits (host); pixels 8j .. 8j + 7 lie in one tile row (BW >= 8), so
+                // the offset of pixel 8j steps by 8 columns, or to the next row where 8j wraps BW
+                const int sw = (int)args.out_sw, step = 8 * sw, wrap = (int)args.out_sh - (BW - 8) * sw;
+                float* a = acc[0];
+                // pass 1: bias and residual into the accumulators.  The residual may be the output buffer itself, so a
+                // load cannot move above an earlier store: with no store between them the loads are in flight together
+                // instead of each waiting behind the previous element's store
+                int oj = 0;
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                    if (j > 0) oj += ((8 * j) & (BW - 1)) ? step : wrap;
+#pragma unroll
+                    for (int r = 0; r < 2; ++r)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float& f = a[4 * j + 2 * r + e];
+                            f += bv[r];
+                            if (res) f += res[oj + e * sw + 8 * r];
+                        }
+                }
+                // pass 2: stores and statistics
+                const bool stats = args.stats != nullptr;
+                double su = 0.0, sq = 0.0;
+                oj = 0;
+#pragma unroll
+                for (int jj = 0; jj < BLOCK_N / 16; ++jj) {
+                    float s8 = 0.f, q8 = 0.f;
+#pragma unroll
+                    for (int j = 2 * jj; j < 2 * jj + 2; ++j) {
+                        if (j > 0) oj += ((8 * j) & (BW - 1)) ? step : wrap;
+#pragma unroll
+                        for (int r = 0; r < 2; ++r) {
+                            const float* f = a + 4 * j + 2 * r;
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int o = oj + e * sw + 8 * r;
+                                if (o32) o32[o] = f[e];
+                                if (o16) o16[o] = sat_half(f[e]);
+                            }
+                            if (stats) {
+                                s8 += f[0] + f[1];
+                                q8 += f[0] * f[0] + f[1] * f[1];
+                            }
+                        }
+                    }
+                    if (stats) {
+                        su += (double)s8;
+                        sq += (double)q8;
+                    }
+                }
+                if (stats) {
+#pragma unroll
+                    for (int o = 1; o <= 16; o <<= 1) {
+                        su += __shfl_xor_sync(0xffffffffu, su, o);
+                        sq += __shfl_xor_sync(0xffffffffu, sq, o);
+                    }
+                    if (lane == 0) {
+                        double* dst = args.stats + ((long long)tb0 * args.stats_blocks + (c0 >> 4)) * 2;
+                        atomicAdd(dst, su);
+                        atomicAdd(dst + 1, sq);
+                    }
+                }
+                continue;
+            }
             const bool fast = vec && n0 + BLOCK_N <= args.n_valid;
 #pragma unroll
             for (int hf = 0; hf < HALVES; ++hf) {
@@ -503,12 +590,12 @@ int num_sms_of_current_device() {
     return n;
 }
 
-// 128-pixel tile box: BW x BH pixels x BB images
-void tile_geometry(int H, int W, int B, ConvTcArgs& a) {
-    int BW = W >= 128 ? 128 : W;
-    int BH = 128 / BW;
+// tile box of tile_pix (128, or 256 for the transposed schedule) pixels: BW x BH pixels x BB images
+void tile_geometry(int H, int W, int B, int tile_pix, ConvTcArgs& a) {
+    int BW = W >= tile_pix ? tile_pix : W;
+    int BH = tile_pix / BW;
     if (BH > H) BH = H;
-    const int BB = 128 / (BW * BH);
+    const int BB = tile_pix / (BW * BH);
     a.bw_log2 = ilog2_exact(BW);
     a.bh_log2 = ilog2_exact(BH);
     a.tiles_w = (W + BW - 1) / BW;
@@ -539,12 +626,12 @@ int pick_block_n(int Cout, int tiles_m, int hint, int num_sms) {
 }
 
 CUresult encode_act(PFN_encodeTiled enc, CUtensorMap* m, const void* ptr, cuuint64_t channels, cuuint64_t ld, int W, int H,
-                    int phases, int B, int in_stride, const ConvTcArgs& a) {
+                    int phases, int B, int in_stride, int tile_pix, const ConvTcArgs& a) {
     // (C, W, H, P, B), fp16, box (64, BW, BH, 1, BB), 128B swizzle, OOB -> zeros.  in_stride == 2 (Downsample read in place):
     // the tensor is the (2H x 2W) input, the box spans 2*BW x 2*BH pixels and the element strides make TMA keep every second
-    // pixel -> the same 128-pixel tile lands in shared memory
+    // pixel -> the same tile_pix-pixel tile lands in shared memory
     const cuuint64_t IS = in_stride;
-    const int BW = 1 << a.bw_log2, BH = 1 << a.bh_log2, BB = kConvBlockM >> (a.bw_log2 + a.bh_log2);
+    const int BW = 1 << a.bw_log2, BH = 1 << a.bh_log2, BB = tile_pix >> (a.bw_log2 + a.bh_log2);
     cuuint64_t gdim[5] = {channels, (cuuint64_t)W * IS, (cuuint64_t)H * IS, (cuuint64_t)phases, (cuuint64_t)B};
     cuuint64_t gstr[4] = {ld * 2, (cuuint64_t)W * IS * ld * 2, (cuuint64_t)H * IS * W * IS * ld * 2,
                           (cuuint64_t)phases * H * IS * W * IS * ld * 2};
@@ -565,14 +652,29 @@ CUresult encode_weights(PFN_encodeTiled enc, CUtensorMap* m, const void* ptr, cu
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-template <int BLOCK_N, bool GN>
+// The transposed schedule computes D^T[C_out = 128, pixels] = W . A^T on the cooperative 256-wide kernel: the weight tile
+// is the wgmma A operand (M = the 128 output channels, 64 per consumer) and a 256-pixel activation tile the B operand
+// (N = 256), so a C_out = 128 conv gets the 128x256 tile's operand bytes per FLOP.  It needs whole 256-pixel tiles inside
+// one image (the statistics of a warp then fall in one image), TMA boxes of <= 256 pixels per dimension (the in-place
+// stride-2 read doubles them), and every channel stored channel-contiguous (its stores go 8 channels x 4 pixels a warp).
+bool transposed_ok(const ConvTcProblem& p, const ConvTcArgs& a) {
+    if (p.Cout != 128 || a.n_valid != p.Cout || a.out_sc != 1) return false;
+    const int BW = p.W >= 256 ? 256 : p.W;
+    if (p.W % BW || ilog2_exact(BW) < 3 || BW * a.in_stride > 256) return false;
+    const int BH = 256 / BW;
+    // the epilogue addresses a tile's outputs with 32-bit offsets from its first pixel
+    if (BH * a.out_sh + BW * a.out_sw + p.Cout > INT32_MAX) return false;
+    return p.H % BH == 0 && BH * a.in_stride <= 256;
+}
+
+template <int BLOCK_N, bool GN, bool TR = false>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& tmB, const CUtensorMap& tmX,
            const CUtensorMap& tmX2, const ConvTcArgs& args, const GnPrologueArgs& gn, uint32_t extra_smem,
            cudaStream_t stream) {
     using C = Cfg<BLOCK_N>;
     static bool attr_set = false;   // per-template-instance; benign race (idempotent call)
     if (!attr_set) {
-        if (cudaFuncSetAttribute(conv_wg_kernel<BLOCK_N, GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) !=
+        if (cudaFuncSetAttribute(conv_wg_kernel<BLOCK_N, GN, TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) !=
             cudaSuccess)
             return -10;
         attr_set = true;
@@ -580,8 +682,8 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmA2, const CUtensorMap& t
     const int total_tiles = args.tiles_w * args.tiles_h * args.tiles_b * args.tiles_n;
     const int num_sms = num_sms_of_current_device();
     const int grid = total_tiles < num_sms ? total_tiles : num_sms;
-    const uint32_t smem = C::kSmemBytes + (!GN && BLOCK_N <= 128 ? stat_scratch_bytes(BLOCK_N) : 0u) + extra_smem;
-    launch_k(conv_wg_kernel<BLOCK_N, GN>, grid, kNumThreads, smem, stream, tmA, tmA2, tmB, tmX, tmX2, args, gn);
+    const uint32_t smem = C::kSmemBytes + (!GN && !TR && BLOCK_N <= 128 ? stat_scratch_bytes(BLOCK_N) : 0u) + extra_smem;
+    launch_k(conv_wg_kernel<BLOCK_N, GN, TR>, grid, kNumThreads, smem, stream, tmA, tmA2, tmB, tmX, tmX2, args, gn);
     return cudaGetLastError() == cudaSuccess ? 0 : -11;
 }
 
@@ -630,7 +732,6 @@ int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream) {
     ConvTcArgs a{};
     a.num_taps = p.num_taps;
     a.chunks_per_tap = p.Cin / kConvBlockK;
-    tile_geometry(p.H, p.W, p.B, a);
     a.a_chan_off = p.a_chan_off;
     a.in_stride = p.in_stride == 2 ? 2 : 1;
     a.out_sb = p.out_sb; a.out_sh = p.out_sh; a.out_sw = p.out_sw;
@@ -641,20 +742,32 @@ int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream) {
     a.stats = p.stats; a.stats_blocks = p.Cout / 16;
     for (int t = 0; t < p.num_taps; ++t) { a.dh[t] = p.dh[t]; a.dw[t] = p.dw[t]; a.ph[t] = p.ph[t]; }
 
+    // schedule: the block_n hint 256 asks for the transposed one at C_out = 128, any other width the row-major tiles.
+    // Without a hint the transposed schedule runs where it applies and gives every SM a tile: on an H100 SXM at 700 W
+    // every cfg-3 C_out = 128 class measured faster on it, the sub-pixel phases and the residual (block2) epilogue
+    // included (tools/bench_ops.py conv 256 128)
+    const int num_sms = num_sms_of_current_device();
+    const int hint = p.block_n_hint < 0 ? -p.block_n_hint : p.block_n_hint;
+    const bool tr_ok = transposed_ok(p, a);
+    const bool tr = hint == 256 ? tr_ok
+                                : (hint == 0 || p.Cout % hint != 0) && tr_ok && (long long)p.B * p.H * p.W / 256 >= num_sms;
+    const int tile_pix = tr ? 256 : kConvBlockM;
+    tile_geometry(p.H, p.W, p.B, tile_pix, a);
     const int tiles_m = a.tiles_w * a.tiles_h * a.tiles_b;
-    const int block_n = pick_block_n(p.Cout, tiles_m, p.block_n_hint, num_sms_of_current_device());
+    const int block_n = tr ? 128 : pick_block_n(p.Cout, tiles_m, p.block_n_hint, num_sms);
     a.tiles_n = p.Cout / block_n;
 
     CUtensorMap tmA, tmA2, tmB, tmX, tmX2;
     a.a_split = (p.act2 ? p.Cin1 : p.Cin) / kConvBlockK;
     a.a_chan_off2 = p.a_chan_off2;
-    if (encode_act(enc, &tmA, p.act, p.a_channels, p.lda, p.W, p.H, p.phases, p.B, a.in_stride, a) != CUDA_SUCCESS) return -6;
+    if (encode_act(enc, &tmA, p.act, p.a_channels, p.lda, p.W, p.H, p.phases, p.B, a.in_stride, tile_pix, a) != CUDA_SUCCESS)
+        return -6;
     tmA2 = tmA;
     if (p.act2) {
         if (p.Cin1 <= 0 || p.Cin1 % kConvBlockK || p.Cin1 >= p.Cin || (p.lda2 % 8) || (reinterpret_cast<uintptr_t>(p.act2) & 15) ||
             a.in_stride != 1)
             return -8;
-        if (encode_act(enc, &tmA2, p.act2, p.lda2, p.lda2, p.W, p.H, p.phases, p.B, 1, a) != CUDA_SUCCESS) return -6;
+        if (encode_act(enc, &tmA2, p.act2, p.lda2, p.lda2, p.W, p.H, p.phases, p.B, 1, tile_pix, a) != CUDA_SUCCESS) return -6;
     }
     // folded 1x1 conv over a second operand x (res_conv): its own tensor map(s), read at the centre tap
     tmX = tmA; tmX2 = tmA;
@@ -667,14 +780,17 @@ int conv_tc_launch(const ConvTcProblem& p, cudaStream_t stream) {
         a.x_chunks = p.Cx / kConvBlockK;
         a.x_split = (p.x_act2 ? p.Cx1 : p.Cx) / kConvBlockK;
         a.x_chan_off = p.x_chan_off; a.x_chan_off2 = p.x_chan_off2;
-        if (encode_act(enc, &tmX, p.x_act, p.x_lda, p.x_lda, p.W, p.H, 1, p.B, 1, a) != CUDA_SUCCESS) return -6;
+        if (encode_act(enc, &tmX, p.x_act, p.x_lda, p.x_lda, p.W, p.H, 1, p.B, 1, tile_pix, a) != CUDA_SUCCESS) return -6;
         tmX2 = tmX;
-        if (p.x_act2 && encode_act(enc, &tmX2, p.x_act2, p.x_lda2, p.x_lda2, p.W, p.H, 1, p.B, 1, a) != CUDA_SUCCESS) return -6;
+        if (p.x_act2 &&
+            encode_act(enc, &tmX2, p.x_act2, p.x_lda2, p.x_lda2, p.W, p.H, 1, p.B, 1, tile_pix, a) != CUDA_SUCCESS)
+            return -6;
     }
     const cuuint64_t K = (cuuint64_t)p.num_taps * p.Cin + (p.x_act ? (cuuint64_t)p.Cx : 0);
     if (encode_weights(enc, &tmB, p.wpacked, K, p.Cout, block_n) != CUDA_SUCCESS) return -7;
 
     const GnPrologueArgs gn{};
+    if (tr) return launch<256, false, true>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
     switch (block_n) {
         case 256: return launch<256, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
         case 128: return launch<128, false>(tmA, tmA2, tmB, tmX, tmX2, a, gn, 0, stream);
@@ -712,7 +828,7 @@ int conv_gn_launch(const ConvGnProblem& p, cudaStream_t stream) {
     a.chunks_per_tap = C / kConvBlockK;
     a.a_split = p.C0 / kConvBlockK;
     a.in_stride = 1;
-    tile_geometry(p.H, p.W, p.B, a);
+    tile_geometry(p.H, p.W, p.B, kConvBlockM, a);
     a.out_sb = (long long)p.H * p.W * p.Cout; a.out_sh = (long long)p.W * p.Cout; a.out_sw = p.Cout; a.out_sc = 1;
     a.n_valid = p.Cout;
     a.out_f32 = p.out_f32; a.out_f16 = p.out_f16; a.bias = p.bias; a.residual = p.residual; a.err_flag = p.err_flag;

@@ -59,7 +59,8 @@ struct ConvTcProblem {
     long long out_sc;       // 0 or 1 = contiguous channels
     int n_valid;            // 0 = all C_out channels are stored
     int block_n_hint;       // 0 = auto; otherwise the preferred tile width (sign ignored): 256 runs the cooperative
-                            // schedule, <= 128 the ping-pong one (see conv_tc.cu)
+                            // schedule (at C_out = 128 the transposed one, where its geometry allows), <= 128 the
+                            // ping-pong one (see conv_tc.cu)
     double* stats;          // optional GroupNorm block statistics of the output (pre-zeroed), see ConvTcArgs
     int* err_flag;
 };

@@ -193,12 +193,20 @@ CONV_SHAPES = [("3x3 1024->1024 @16", 16, 1024, 0, 1024, 3), ("3x3 2048->1024 @1
                ("3x3 256->128 @128", 128, 256, 0, 128, 3), ("1x1 1024->512 @32", 32, 1024, 0, 512, 1)]
 
 
-def conv_auto_block_n(c_out, tiles_m, num_sms):
-    """The tile width conv_tc.cu's pick_block_n selects without a hint (C_out % 64 == 0 here)."""
+def conv_tile(c_out, pixels, hint, num_sms):
+    """(label, pixels per tile, output channels per tile) of the schedule conv_tc.cu's conv_tc_launch selects, for the
+    shapes here (C_out % 64 == 0, grids that tile by 256 pixels inside one image): the transposed tile "t256" (256 pixels
+    x 128 channels) at C_out = 128 for the hint 256, or without a hint when it gives every SM a tile; else the 128-pixel
+    tile of the width the hint or pick_block_n selects."""
+    hint = abs(hint)
+    if c_out == 128 and (hint == 256 or ((hint == 0 or c_out % hint) and pixels // 256 >= num_sms)):
+        return "t256", 256, 128
+    if hint and c_out % hint == 0:
+        return f"n{hint}", 128, hint
     for bn in (256, 128):
-        if c_out % bn == 0 and tiles_m * (c_out // bn) >= num_sms:
-            return bn
-    return 64
+        if c_out % bn == 0 and pixels // 128 * (c_out // bn) >= num_sms:
+            return f"n{bn}", 128, bn
+    return "n64", 128, 64
 
 
 # k-block sweep: 3x3 convs at b=32 whose k-blocks per tile (9 C_in / 64) run from 9 to 72, at the two cfg-3 geometries
@@ -206,13 +214,15 @@ def conv_auto_block_n(c_out, tiles_m, num_sms):
 SWEEP_SHAPES = [(128, 128, (64, 128, 256, 512)), (64, 256, (64, 128, 256, 512))]   # (H = W, C_out, C_in sweep)
 
 
-def conv_operand_bytes(tiles_m, c_out, k_blocks, block_n):
-    """L2 -> SM operand bytes of one launch: per tile and k-block one TMA stage, a 128x64 A box and a block_n x 64 B box."""
-    return tiles_m * (c_out // block_n) * k_blocks * (128 * 64 * 2 + block_n * 64 * 2)
+def conv_operand_bytes(pixels, c_out, k_blocks, tile_px, tile_ch):
+    """L2 -> SM operand bytes of one launch: per tile and k-block one TMA stage, a tile_px x 64 activation box and a
+    tile_ch x 64 weight box."""
+    return pixels // tile_px * (c_out // tile_ch) * k_blocks * (tile_px + tile_ch) * 64 * 2
 
 
 def bench_conv(ops, hints=(0,)):
-    """Usage: bench_ops.py conv [block_n ...] -- 0 = the library's own choice (default)."""
+    """Usage: bench_ops.py conv [block_n ...] -- 0 = the library's own choice (default); 256 runs the C_out = 128 shapes on
+    the transposed tile, 128 on the 128-wide ping-pong one."""
     B = 32
     num_sms = torch.cuda.get_device_properties(dev).multi_processor_count
     rows = [(lbl, H, c0, c1, co, k, False) for (lbl, H, c0, c1, co, k) in CONV_SHAPES]
@@ -224,7 +234,6 @@ def bench_conv(ops, hints=(0,)):
         out = torch.empty(B, H, H, c_out, device=dev, dtype=F16)
         stats = torch.zeros(B, c_out // 16, 2, device=dev, dtype=F64)
         bias = torch.randn(c_out, device=dev)
-        tiles_m = B * H * H // 128
         k_blocks = k * k * c_in // 64
         flop = 2.0 * B * H * H * c_out * k * k * c_in
         if res:
@@ -245,11 +254,35 @@ def bench_conv(ops, hints=(0,)):
                                                      (H * H * c_out, H * c_out, c_out), block_n=hint, act2=act2, lda2=c1,
                                                      c_in1=c0 if c1 else 0, out_stats=stats)
             ms = timeit([f], reps=20)
-            bn = hint if hint and c_out % hint == 0 else conv_auto_block_n(c_out, tiles_m, num_sms)
-            nbytes = conv_operand_bytes(tiles_m, c_out, k_blocks, bn)
-            res_line.append(f"n{bn:<3d} {ms * 1e3:8.1f} us {flop / ms / 1e9:6.1f} TFLOP/s L2->SM {nbytes / ms / 1e9:5.2f} TB/s")
+            lbl_t, tpx, tch = conv_tile(c_out, B * H * H, hint, num_sms)
+            nbytes = conv_operand_bytes(B * H * H, c_out, k_blocks, tpx, tch)
+            res_line.append(f"{lbl_t:4s} {ms * 1e3:8.1f} us {flop / ms / 1e9:6.1f} TFLOP/s L2->SM {nbytes / ms / 1e9:5.2f} TB/s")
         print(f"conv {lbl:40s} " + "  |  ".join(res_line), flush=True)
+    bench_conv_phases(ops, hints, num_sms)
     bench_conv_sweep(ops, hints, num_sms)
+
+
+def bench_conv_phases(ops, hints, num_sms):
+    """One sub-pixel phase of the Upsample conv (2x2 taps on the low-res grid, every second pixel of every second row of
+    the 2H x 2W output), with the fp16 + statistics epilogue: the cfg-3 classes 128->128 onto 256x256 and 256->128 onto
+    128x128."""
+    B, c_out = 32, 128
+    for (H, c_in) in ((128, 128), (64, 256)):
+        act = torch.randn(B, H, H, c_in, device=dev).to(F16)
+        wp = (torch.randn(c_out, 4 * c_in, device=dev) * 0.01).to(F16)
+        bias = torch.randn(c_out, device=dev)
+        out = torch.empty(B, 2 * H, 2 * H, c_out, device=dev, dtype=F16)
+        stats = torch.zeros(B, c_out // 16, 2, device=dev, dtype=F64)
+        flop = 2.0 * B * H * H * c_out * 4 * c_in
+        line = []
+        for hint in hints:
+            f = lambda hint=hint: ops.conv_igemm(act, B, H, H, c_in, 0, c_in, wp, c_out, 2, 2, 2, bias, None, None, out,
+                                                 (4 * H * H * c_out, 4 * H * c_out, 2 * c_out), block_n=hint,
+                                                 out_stats=stats)
+            ms = timeit([f], reps=20)
+            lbl_t = conv_tile(c_out, B * H * H, hint, num_sms)[0]
+            line.append(f"{lbl_t:4s} {ms * 1e3:8.1f} us {flop / ms / 1e9:6.1f} TFLOP/s")
+        print(f"conv sub-pixel phase {c_in}->{c_out} onto {2 * H}x{2 * H}{'':14s} " + "  |  ".join(line), flush=True)
 
 
 def bench_conv_sweep(ops, hints, num_sms):
@@ -259,7 +292,6 @@ def bench_conv_sweep(ops, hints, num_sms):
     import numpy as np
     B = 32
     for (H, c_out, c_ins) in SWEEP_SHAPES:
-        tiles_m = B * H * H // 128
         for epi in ("f16", "block2"):
             pts = {}
             for c_in in c_ins:
@@ -273,20 +305,20 @@ def bench_conv_sweep(ops, hints, num_sms):
                 k_blocks = 9 * c_in // 64
                 line = []
                 for hint in hints:
-                    bn = hint if hint and c_out % hint == 0 else conv_auto_block_n(c_out, tiles_m, num_sms)
+                    lbl_t, tpx, tch = conv_tile(c_out, B * H * H, hint, num_sms)
                     f = lambda hint=hint: ops.conv_igemm(act, B, H, H, c_in, 0, c_in, wp, c_out, 3, 3, 0, bias, res, out32,
                                                          out16, (H * H * c_out, H * c_out, c_out), block_n=hint,
                                                          out_stats=stats)
                     ms = timeit([f], reps=20)
-                    per_tile = ms * 1e3 / (tiles_m * (c_out // bn) / num_sms)
-                    pts.setdefault((hint, bn), []).append((k_blocks, per_tile))
-                    line.append(f"n{bn:<3d} {ms * 1e3:8.1f} us {per_tile:6.2f} us/tile "
+                    per_tile = ms * 1e3 / (B * H * H // tpx * (c_out // tch) / num_sms)
+                    pts.setdefault((hint, lbl_t), []).append((k_blocks, per_tile))
+                    line.append(f"{lbl_t:4s} {ms * 1e3:8.1f} us {per_tile:6.2f} us/tile "
                                 f"{2.0 * B * H * H * c_out * 9 * c_in / ms / 1e9:6.1f} TFLOP/s")
                 print(f"conv sweep 3x3 {c_in:4d}->{c_out} @{H} {epi:6s} kb={k_blocks:3d} " + "  |  ".join(line), flush=True)
-            for (hint, bn), p in sorted(pts.items()):
+            for (hint, lbl_t), p in sorted(pts.items()):
                 kb, us = np.array(p).T
                 c, F = np.polyfit(kb, us, 1)
-                print(f"conv sweep fit C_out={c_out} @{H} {epi:6s} n{bn:<3d}{'' if hint else ' (auto)'}: F = {F:5.2f} us/tile, "
+                print(f"conv sweep fit C_out={c_out} @{H} {epi:6s} {lbl_t:4s}{'' if hint else ' (auto)'}: F = {F:5.2f} us/tile, "
                       f"{c:5.3f} us per k-block",
                       flush=True)
 
