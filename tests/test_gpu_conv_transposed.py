@@ -21,22 +21,28 @@ pytestmark = pytest.mark.gpu
 F16, F64 = torch.float16, torch.float64
 EMU = EmuOps()
 STAGES = 4        # ring stages of the 256-wide kernel (48 KiB each)
+CONV_WG_KERNEL = re.compile(r"conv_wg_kernel<(\d+), *(?:\(bool\))?(\w+), *(?:\(bool\))?(\w+)>")
+
+
+def conv_instance(name):
+    """(BLOCK_N, GN, transposed) of a conv_wg_kernel record's name, or None for any other kernel."""
+    m = CONV_WG_KERNEL.search(name)
+    return None if m is None else (int(m.group(1)), m.group(2) in ("true", "1"), m.group(3) in ("true", "1"))
 
 
 def _schedules(fn):
     """Run fn under the profiler; the set of conv_wg_kernel instances (BLOCK_N, GN, transposed) it launched.  fn must
     give the same result when run again: a profiling session that returns no kernel record at all is repeated (up to
     three sessions) rather than read as "no conv ran"."""
-    pat = re.compile(r"conv_wg_kernel<(\d+), *(?:\(bool\))?(\w+), *(?:\(bool\))?(\w+)>")
     found = set()
     for _ in range(3):
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
             fn()
             torch.cuda.synchronize()
         for ev in prof.events():
-            m = pat.search(ev.name)
-            if m:
-                found.add((int(m.group(1)), m.group(2) in ("true", "1"), m.group(3) in ("true", "1")))
+            inst = conv_instance(ev.name)
+            if inst:
+                found.add(inst)
         if found:
             break
     return found
