@@ -274,6 +274,24 @@ int mi_step_epilogue_multistep_w(const float* x_t, const float* eps_cond, const 
                                  const float* sigma, const float* c3, const float* noise, float* x0_hist, int B, int n,
                                  int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
                                  float* x0_workspace, void* stream);
+/* mi_step_epilogue_w and mi_step_epilogue_multistep_w with a guidance table w_sched [T] fp32 (required; Imagen.sample(
+ * guidance_interval=, guidance_schedule=)): image b combines with w_b(t[b]), where w_b(t) = w[b] if w_sched[t] == 1 and
+ * otherwise 1 + (w[b] - 1) * w_sched[t], rounded op by op in fp32.  Bit for bit the _w entry point called with the array
+ * w_eff[b] = w_b(t[b]), in the fused and the three-kernel form.  A captured step that reads the table from a device
+ * buffer serves every interval and schedule. */
+int mi_step_epilogue_ws(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
+                        const float* w_sched, const long long* t, const float* sqrt_recip_alphas_cumprod,
+                        const float* sqrt_recipm1_alphas_cumprod, const float* posterior_mean_coef1,
+                        const float* posterior_mean_coef2, const float* sigma, const float* noise, int B, int n,
+                        int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
+                        float* x0_workspace, void* stream);
+int mi_step_epilogue_multistep_ws(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                                  const float* w, const float* w_sched, const long long* t,
+                                  const float* sqrt_recip_alphas_cumprod, const float* sqrt_recipm1_alphas_cumprod,
+                                  const float* c1, const float* c2, const float* sigma, const float* c3,
+                                  const float* noise, float* x0_hist, int B, int n, int rank_lo, int rank_hi,
+                                  float weight, float min_s, float* out, float* s_out, float* x0_workspace,
+                                  void* stream);
 /* t[b] <- max(t[b] - 1, 0): the next iteration's timestep of Imagen._p_sample_loop (Imagen.py:398-415 walks the list of
  * diffusion_model.py:81-87), advanced on the device so that a captured step can be replayed back to back */
 int mi_step_advance_t(long long* t, int B, void* stream);

@@ -9,7 +9,7 @@ nothing on the host.  Sampling captures three graph flavours: text-only (one gra
 step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).  The guidance weights are per-image
 data in a static buffer, so every flavour's graph serves every `cond_scale` and every negative prompt of its shape.
 
-Eight additions that the reference does not have (all optional, defaults reproduce the reference):
+Nine additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -32,7 +32,12 @@ Eight additions that the reference does not have (all optional, defaults reprodu
     runs iff some image's w != 1;
   * per-image seeds (`sample(..., seed=)`): every sampling draw is a pure function of (the image's seed, stage, kind,
     label, element index), counter-based Philox drawn on the device (mi_randn_keyed, inside the captured step), so an
-    image can be regenerated on its own, at any batch position, batch size or rank count.
+    image can be regenerated on its own, at any batch position, batch size or rank count;
+  * guidance intervals and guidance-weight schedules (`sample(..., guidance_interval=(sigma_lo, sigma_hi),
+    guidance_schedule='linear' or 'cosine')`, Kynkaanniemi et al. 2024; Wang et al. 2024): a per-stage fp32 table s[t]
+    (GaussianDiffusion.guidance_table) scales each image's w - 1 at timestep t (mi_step_epilogue_ws), and a grid point
+    with s[t] = 0 runs without the guidance pass, one U-Net evaluation.  A captured stage keeps a guided and an unguided
+    graph over the same static buffers and replays the one each grid point needs.
 
 `noise_fn` kinds: 'init' (x_T, step -1; with an init image k, the noise z of the start sqrt(a_t0) k + sqrt(1 - a_t0) z,
 t0 the walk's first point), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
@@ -112,26 +117,37 @@ class _StepGraph:
          w      [B] fp32 the per-image guidance weights (`set_cond` refreshes them); guided graphs with a negative prompt
                 also hold static negative_text_embeds / negative_text_mask in `cond`;
          seeds  seeded graphs only: [B] int64 per-image seeds (`set_cond` refreshes them); the body then draws its noise
-                with mi_randn_keyed at the current t (and r, R) instead of normal_().
+                with mi_randn_keyed at the current t (and r, R) instead of normal_();
+         gtab   guidance-table graphs only: [T] fp32, the stage's guidance table (`set_guidance` installs a loop's, so one
+                graph serves every interval and schedule); the guided body then steps with mi_step_epilogue_ws(_multistep).
+    A guidance-table graph is a pair: `graph`, the guided step, and `graph_unguided`, the same step without the guidance
+    pass (one U-Net evaluation, the unguided epilogue), captured when a loop first needs it over the same static buffers,
+    in the same memory pool.  The two never run at once: `replay(guided)` picks one per grid point, and the state they
+    carry (x, t, the history of 2M, the RePaint counter) passes from one to the other as it is.
     Three flavours: text-only (the step, then mi_step_advance_t_table), inpainting (draws, mi_inpaint_prologue, the step,
     mi_inpaint_advance) and multistep (the draw, mi_step_epilogue_multistep's step, mi_step_advance_t_table).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
     for DDPM; `* ((S-1) R + 1)` when inpainting) -- no per-step host-side tensor ops."""
 
     def __init__(self):
-        self.graph = None
+        self.graph = self.graph_unguided = None
         self.x = self.t = self.noise = None
         self.cond = {}
         self.sched = None
         self.hist = None
         self.w = None
         self.seeds = None
+        self.gtab = None
         self.inp = None
         self.inject_noise = False
         self.unet = None
+        self.body = None
 
     def set_schedule(self, sched):
         for name in ('c1', 'c2', 'sigma', 'next_t') + (('c3',) if self.sched.c3 is not None else ()):
             getattr(self.sched, name).copy_(getattr(sched, name))
+
+    def set_guidance(self, table):
+        self.gtab.copy_(table)
 
     def set_inpaint(self, k, m, R, ra, rb):
         for name, v in (('k', k), ('m', m), ('ra', ra), ('rb', rb)):
@@ -164,8 +180,9 @@ class _StepGraph:
             for te in self._static_texts():
                 self.unet.unregister_static_text(te)
 
-    def replay(self):
-        self.graph.replay()
+    def replay(self, guided=True):
+        """guided=False: the unguided graph of a guidance-table pair."""
+        (self.graph if guided else self.graph_unguided).replay()
 
 
 class Imagen(nn.Module):
@@ -322,7 +339,7 @@ class Imagen(nn.Module):
 
     def _step(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
               cond_scale, model_output=None, out=None, schedule=None, hist=None, negative_text_embeds=None,
-              negative_text_mask=None, guided=None):
+              negative_text_mask=None, guided=None, guidance_table=None):
         """x_{t-1} = posterior_mean(x_t, clamp-thresholded x0(x_t, eps)) + [t != 0] * sigma_t * noise.
         eps = g + (cond - g) * w, with w = `cond_scale` (a number, or an fp32 [B] tensor of per-image weights on x's
         device) and g the guidance pass: the U-Net conditioned on `negative_text_embeds` / `negative_text_mask` if given,
@@ -331,18 +348,21 @@ class Imagen(nn.Module):
         `out` may be `x` itself (the captured step updates the image in place).  `schedule` (a SamplingSchedule) replaces
         the posterior coefficients and sigma by its DDIM tables: the step then goes to the next point of its grid.  A
         multistep schedule (one with c3, DPM-Solver++(2M)) also adds c3[t] * hist, the previous step's clamped x0, and then
-        stores this step's clamped x0 in `hist` ([B, C, s, s] fp32, zeros before the first step)."""
+        stores this step's clamped x0 in `hist` ([B, C, s, s] fp32, zeros before the first step).
+        `guidance_table` ([T] fp32 on x's device, GaussianDiffusion.guidance_table): a guided step then combines image b
+        with w_b(t) = w_b where the table is 1 at t, else 1 + (w_b - 1) * table[t] (mi_step_epilogue_ws); whether the
+        step is guided at all stays the caller's choice (`guided`)."""
         with N.device_of(x):
             return self._step_impl(unet, x, t, noise, noise_scheduler=noise_scheduler, text_embeds=text_embeds,
                                    text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                                    lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
                                    model_output=model_output, out=out, schedule=schedule, hist=hist,
                                    negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
-                                   guided=guided)
+                                   guided=guided, guidance_table=guidance_table)
 
     def _step_impl(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                    lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None, hist=None,
-                   negative_text_embeds=None, negative_text_mask=None, guided=None):
+                   negative_text_embeds=None, negative_text_mask=None, guided=None, guidance_table=None):
         guided = _is_guided(cond_scale) if guided is None else guided
         assert not (guided and not self.can_classifier_guidance), \
             'imagen was not trained with conditional dropout, and thus one cannot use classifier free guidance ' \
@@ -391,7 +411,18 @@ class Imagen(nn.Module):
         # (mi_step_epilogue; images too large for its register-resident select take the three-kernel form inside the ABI)
         c1, c2, sigma = ((sch.posterior_mean_coef1, sch.posterior_mean_coef2, sch.sigma) if schedule is None else
                          (schedule.c1, schedule.c2, schedule.sigma))
-        if exists(schedule) and exists(schedule.c3):
+        if exists(guidance_table) and exists(eps_null):
+            # the scheduled weights w_b(t) (mi_step_epilogue_ws / mi_step_epilogue_multistep_ws)
+            if exists(schedule) and exists(schedule.c3):
+                assert exists(hist), 'a multistep schedule needs the x0 history (hist=)'
+                ops.step_epilogue_multistep_scheduled(x, eps, eps_null, cond_scale, guidance_table, t,
+                                                      sch.sqrt_recip_alphas_cumprod, sch.sqrt_recipm1_alphas_cumprod, c1,
+                                                      c2, sigma, schedule.c3, noise, hist, B, n, lo, hi, w, 1.0, out)
+            else:
+                ops.step_epilogue_scheduled(x, eps, eps_null, cond_scale, guidance_table, t, sch.sqrt_recip_alphas_cumprod,
+                                            sch.sqrt_recipm1_alphas_cumprod, c1, c2, sigma, noise, B, n, lo, hi, w, 1.0,
+                                            out)
+        elif exists(schedule) and exists(schedule.c3):
             assert exists(hist), 'a multistep schedule needs the x0 history (hist=)'
             ops.step_epilogue_multistep(x, eps, eps_null, cond_scale, t, sch.sqrt_recip_alphas_cumprod,
                                         sch.sqrt_recipm1_alphas_cumprod, c1, c2, sigma, schedule.c3, noise, hist, B, n,
@@ -414,11 +445,12 @@ class Imagen(nn.Module):
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
                    cond_scale, inpaint=False, multistep=False, *, negative_text_embeds=None, negative_text_mask=None,
-                   guided=None, seeded=False, stage=None):
+                   guided=None, seeded=False, stage=None, scheduled=False):
         """Only whether the step runs the guidance pass is part of the key, not the weights: they are data in the graph's
         static w buffer.  The negative prompt's signature counts when it is used, i.e. when guided.  A seeded graph (keyed
         draws, the seeds in its static buffer) is keyed apart, with the stage its draws carry; an unseeded key is
-        unchanged."""
+        unchanged.  So is a guidance-table graph pair (`scheduled`: the table in its static buffer), with a
+        'guidance_table' suffix; neither the interval nor the schedule is part of the key."""
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         guided = _is_guided(cond_scale) if guided is None else guided
         p0 = next(unet.parameters())
@@ -429,6 +461,8 @@ class Imagen(nn.Module):
                (sig(negative_text_embeds), sig(negative_text_mask)) if guided else None)
         if seeded:
             key = key + (('seeded', stage),)
+        if scheduled:
+            key = key + ('guidance_table',)
         if inpaint:
             return key + ('inpaint',)
         return key + ('multistep',) if multistep else key
@@ -442,7 +476,7 @@ class Imagen(nn.Module):
 
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                     lowres_noise_times, cond_scale, schedule=None, inpaint=None, negative_text_embeds=None,
-                    negative_text_mask=None, guided=None, seeds=None, stage=None):
+                    negative_text_mask=None, guided=None, seeds=None, stage=None, guidance_table=None, unguided=False):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
         every later sampling loop of the same signature.  Every lookup refreshes the conditioning tensors in its static
         buffers and installs the walk `schedule` (a SamplingSchedule; None: the DDPM walk) in its static tables: the step
@@ -457,7 +491,13 @@ class Imagen(nn.Module):
         and, when guided, the negative prompt's shapes are part of the signature.
         `seeds` ([B] int64 per-image seeds) selects the seeded variant of the flavour, keyed apart with the U-Net number
         `stage`: its body draws with mi_randn_keyed at the current t (and r, R) and the seeds are installed in its static
-        buffer, so one graph serves every seed."""
+        buffer, so one graph serves every seed.
+        `guidance_table` ([T] fp32, for a guided loop whose table is neither all ones nor all zeros on its walk) selects
+        the guidance-table pair of the flavour, keyed apart: the guided graph steps with mi_step_epilogue_ws(_multistep)
+        and reads the table from its static buffer (`_StepGraph.set_guidance` installs it), so one pair serves every
+        interval and schedule.  `unguided` (the loop has grid points without the guidance pass) captures the pair's
+        unguided graph if it does not exist yet: the same body with one U-Net pass, over the same static buffers and in
+        the guided graph's memory pool.  The pair is one entry of `max_cached_graphs`."""
         device = self.device
         schedule = default(schedule, lambda: noise_scheduler.ddpm_schedule(device))
         multistep = exists(schedule.c3)
@@ -465,10 +505,11 @@ class Imagen(nn.Module):
         guided = _is_guided(cond_scale) if guided is None else guided
         if not guided:
             negative_text_embeds = negative_text_mask = None      # no guidance pass: the graph never reads them
+        scheduled = guided and exists(guidance_table)
         key = self._graph_key(unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                               lowres_noise_times, cond_scale, exists(inpaint), multistep,
                               negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
-                              guided=guided, seeded=exists(seeds), stage=stage)
+                              guided=guided, seeded=exists(seeds), stage=stage, scheduled=scheduled)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times, negative_text_embeds=negative_text_embeds,
                     negative_text_mask=negative_text_mask)
@@ -490,7 +531,9 @@ class Imagen(nn.Module):
             g.w = w.clone()
             if exists(seeds):
                 g.seeds = seeds.to(device=device, dtype=torch.long).clone()
-            kw = dict(noise_scheduler=noise_scheduler, cond_scale=g.w, guided=guided,
+            if scheduled:
+                g.gtab = guidance_table.to(device=device, dtype=F32).clone()
+            kw = dict(noise_scheduler=noise_scheduler, cond_scale=g.w, guidance_table=g.gtab,
                       **{k: g.cond.get(k) for k in cond})
             g.refresh_static()
             ops = get_ops()
@@ -515,7 +558,7 @@ class Imagen(nn.Module):
                                  z_renoise=torch.zeros(shape, dtype=F32, device=device),
                                  z_known=torch.zeros(shape, dtype=F32, device=device))
 
-            def body():
+            def body(step_guided=guided):
                 if exists(g.seeds):
                     # keyed draws at the current t (t * R + r when inpainting): those an eager seeded loop takes
                     n = C * hw
@@ -533,34 +576,46 @@ class Imagen(nn.Module):
                     ops.inpaint_prologue(g.x, g.t, p['r'], p['ra'], p['rb'], noise_scheduler.sqrt_alphas_cumprod,
                                          noise_scheduler.sqrt_one_minus_alphas_cumprod, p['k'], p['m'], p['z_renoise'],
                                          p['z_known'], T, B, C, hw)
-                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, hist=g.hist, **kw)
+                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, hist=g.hist, guided=step_guided, **kw)
                 if exists(p):
                     ops.inpaint_advance(g.t, p['r'], g.sched.next_t, p['R'], T, B)   # next repeat, or next grid point
                 else:
                     ops.step_advance_t_table(g.t, g.sched.next_t, T, B)              # t <- next grid point
 
-            # warm-up on a side stream (packs weights, sizes the caching allocator), then capture
-            side = torch.cuda.Stream(device=device)
-            side.wait_stream(torch.cuda.current_stream(device))
-            with torch.cuda.stream(side):
-                body()
-            torch.cuda.current_stream(device).wait_stream(side)
-            torch.cuda.synchronize(device)
-            g.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g.graph):
-                body()
+            g.body = body
+            g.graph = self._capture(body, device)
             self._graphs[key] = g
+        if scheduled and unguided and g.graph_unguided is None:
+            g.graph_unguided = self._capture(lambda: g.body(False), device, pool=g.graph.pool())
         g.set_schedule(schedule)
+        if scheduled:
+            g.set_guidance(guidance_table)
         if exists(inpaint):
             k, m, R = inpaint
             _, ra, rb = noise_scheduler.inpaint_tables(schedule, device)
             g.set_inpaint(k, m, R, ra, rb)
         return g
 
+    @staticmethod
+    def _capture(body, device, pool=None):
+        """`body` captured in a new CUDA graph (in `pool` when given), after one warm-up run on a side stream (packs
+        weights, sizes the caching allocator)."""
+        side = torch.cuda.Stream(device=device)
+        side.wait_stream(torch.cuda.current_stream(device))
+        with torch.cuda.stream(side):
+            body()
+        torch.cuda.current_stream(device).wait_stream(side)
+        torch.cuda.synchronize(device)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=pool):
+            body()
+        return graph
+
     @torch.no_grad()
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
                        lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None,
-                       init_image=None, negative_text_embeds=None, negative_text_mask=None, seeds=None, stage=1):
+                       init_image=None, negative_text_embeds=None, negative_text_mask=None, seeds=None, stage=1,
+                       guidance_table=None):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
@@ -584,7 +639,11 @@ class Imagen(nn.Module):
         `cond_scale` (not in the reference: also an fp32 [B] tensor of per-image weights on the sampling device) and
         `negative_text_embeds` / `negative_text_mask` (not in the reference) guide as in `_step`.
         `seeds` (not in the reference): [B] int64 per-image seeds on the sampling device; every draw of the loop is then
-        keyed by them and by `stage` (the U-Net number), eager or captured (module docstring)."""
+        keyed by them and by `stage` (the U-Net number), eager or captured (module docstring).
+        `guidance_table` (not in the reference; [T] fp32 on the sampling device, GaussianDiffusion.guidance_table) schedules
+        a guided loop's weights: iteration (t, r) runs the guidance pass iff table[t] != 0 (decided on the host from the
+        same fp32 values), with w_b(t) as in `_step`.  A table that is 1 at every point of the walk runs exactly the loop
+        without it, and one that is 0 at every point the unguided loop (as cond_scale = 1).  The draws do not depend on it."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -614,12 +673,24 @@ class Imagen(nn.Module):
                              1.0, 0.0, x_t0)
                 img = x_t0
 
+            guided = _is_guided(cond_scale)
+            on = [guided] * len(plan)           # whether iteration i runs the guidance pass
+            if guided and exists(guidance_table):
+                s = guidance_table.cpu()
+                on = [bool(s[t] != 0) for t, _ in plan]
+                if all(bool(s[t] == 1) for t, _ in plan):
+                    guidance_table = None       # the table changes nothing: the loop without it
+                elif not any(on):
+                    guided, guidance_table = False, None        # the unguided loop
+            else:
+                guidance_table = None
             kw = dict(noise_scheduler=noise_scheduler, text_embeds=text_embeds, text_mask=text_mask,
                       lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
-                      negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
-                      guided=_is_guided(cond_scale))
+                      negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask, guided=guided,
+                      guidance_table=guidance_table)
             if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
-                g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, **keyed, **kw)
+                g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, unguided=not all(on), **keyed,
+                                     **kw)
                 static = dict(step=g.noise)
                 if exists(inpaint):
                     static.update(renoise=g.inp['z_renoise'], inpaint=g.inp['z_known'])
@@ -628,18 +699,20 @@ class Imagen(nn.Module):
                     g.hist.zero_()
                 g.x.copy_(img)
                 g.t.fill_(plan[0][0])
-                for iteration in draws:
+                for iteration, step_guided in zip(draws, on):
                     if g.inject_noise:
                         for kind, label in iteration:
                             static[kind].copy_(self._noise(kind, shape, label, device))
-                    g.replay()                  # [prologue +] step in place; then t (and r) <- the next iteration's
+                    # [prologue +] step in place; then t (and r) <- the next iteration's.  Without a table the graph is
+                    # the only one of its key (guided or not as the whole loop); a pair replays the one this point needs
+                    g.replay(step_guided or not exists(guidance_table))
                 img = g.x
             else:
                 if exists(inpaint):
                     _, ra, rb = sch.inpaint_tables(walk, device)
                     img = img.clone()           # the prologue works in place; x_T may be the caller's draw
                 hist = torch.zeros(tuple(shape), dtype=F32, device=device) if multistep else None
-                for (t, r), iteration in zip(plan, draws):
+                for (t, r), iteration, step_guided in zip(plan, draws, on):
                     z = {kind: self._noise(kind, shape, label, device, **keyed) for kind, label in iteration}
                     times = torch.full((B,), t, device=device, dtype=torch.long)
                     if exists(inpaint):
@@ -648,7 +721,7 @@ class Imagen(nn.Module):
                         ops.inpaint_prologue(img, times, reps, ra, rb, sch.sqrt_alphas_cumprod,
                                              sch.sqrt_one_minus_alphas_cumprod, k, m, z.get('renoise', z['inpaint']),
                                              z['inpaint'], sch.num_timesteps, B, C, hw)
-                    img = self._step(unet, img, times, z['step'], schedule=walk, hist=hist, **kw)
+                    img = self._step(unet, img, times, z['step'], schedule=walk, hist=hist, **dict(kw, guided=step_guided))
 
             if out is None:
                 out = torch.empty(tuple(shape), dtype=F32, device=device)
@@ -665,7 +738,8 @@ class Imagen(nn.Module):
                distributed: bool = False, sampling_timesteps=None, ddim_eta: float = 0., inpaint_images=None,
                inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim', init_images=None,
                skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None,
-               negative_texts=None, negative_text_embeds=None, negative_text_masks=None, seed=None):
+               negative_texts=None, negative_text_embeds=None, negative_text_masks=None, seed=None,
+               guidance_interval=None, guidance_schedule=None):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -712,7 +786,21 @@ class Imagen(nn.Module):
         |z| <= 5.77.  The draws run on the device, inside the captured step.  Cannot be combined with `noise_fn`; labels
         must fit in 32 bits (timesteps * inpaint_resample_times < 2^31).  None (the default) draws from torch's
         generator as before; with `distributed=True` that is each rank's own generator, which the caller must seed
-        per rank for the ranks to draw different noise."""
+        per rank for the ranks to draw different noise.
+        `guidance_interval` (None, a pair (sigma_lo, sigma_hi) with 0 <= sigma_lo < sigma_hi, sigma_lo finite and sigma_hi
+        possibly inf, or one entry per U-Net, each None or such a pair) and `guidance_schedule` (None, 'linear' or
+        'cosine', or one entry per U-Net) schedule the guidance of each guided stage over its walk (Kynkaanniemi et al.
+        2024, "Applying Guidance in a Limited Interval"; after Wang et al. 2024, "Analysis of Classifier-Free Guidance
+        Weight Schedulers").  The stage's fp32 table s[t] over its T timesteps is computed in fp64 from its own
+        alphas_cumprod a and cast: with sigma_t = sqrt((1 - a_t) / a_t) (the VE noise level the intervals are quoted in,
+        inf where a_t = 0) and tau = t / (T - 1), shape(t) is 1 (None), 2 (1 - tau) ('linear') or 1 + cos(pi tau)
+        ('cosine') -- both ramps average 1 and are 0 at t = T - 1 -- and s[t] = shape(t) if sigma_lo < sigma_t <= sigma_hi
+        (every t without an interval), else 0.  Image b at timestep t is guided with w_b where s[t] == 1, and with
+        fp32(1 + fp32(fp32(w_b - 1) * s[t])) elsewhere.  A grid point with s[t] == 0 runs without the guidance pass (one
+        U-Net evaluation, the conditional prediction alone), for the whole batch; an inpainting iteration follows its t.
+        A stage whose table is 1 at every point it walks runs exactly as without the arguments, one whose table is 0
+        there as at cond_scale = 1 (the negative prompt is then not read), and a stage where every w_b == 1 ignores them.
+        The draws do not depend on them."""
         assert sampler in ('ddim', 'dpmpp_2m'), f"sampler must be 'ddim' or 'dpmpp_2m', got {sampler!r}"
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
         if sampler == 'dpmpp_2m':
@@ -742,6 +830,11 @@ class Imagen(nn.Module):
         assert not (exists(negative_text_masks) and not exists(negative_text_embeds)), \
             'negative_text_masks need negative_text_embeds'
         negative = (negative_texts, negative_text_embeds, negative_text_masks)
+        guidance = (self._guidance_intervals(guidance_interval),
+                    self._per_unet(guidance_schedule, 'guidance_schedule'))
+        for i, sched in enumerate(guidance[1], 1):
+            assert sched in (None, 'linear', 'cosine'), \
+                f"guidance_schedule of unet {i} must be None, 'linear' or 'cosine', got {sched!r}"
         for i in range(start_at_unet_number, stop_at_unet_number + 1):
             k, walk_len = default(skips[i - 1], 0), default(steps[i - 1], self.noise_schedulers[i - 1].num_timesteps)
             assert _is_int(k) and 0 <= k < walk_len, \
@@ -770,7 +863,7 @@ class Imagen(nn.Module):
             return self._sample_impl(texts, text_masks, text_embeds, scales, lowres_sample_noise_level,
                                      return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler,
                                      init_images, skips, start_at_unet_number, stop_at_unet_number, start_images,
-                                     negative, seed)
+                                     negative, seed, guidance)
 
     def _check_seed(self, seed):
         """`seed`: an int >= 0, or a non-empty list or 1-D integer tensor of seeds in [0, 2^63); never with noise_fn."""
@@ -796,6 +889,19 @@ class Imagen(nn.Module):
         seeds = seed if torch.is_tensor(seed) else torch.tensor(seed, dtype=torch.long)
         assert seeds.numel() == b, f'seed must have one entry per image (b = {b}), got {seeds.numel()}'
         return seeds.to(device=device, dtype=torch.long).contiguous()
+
+    def _guidance_intervals(self, value):
+        """`guidance_interval` once per U-Net, validated: one pair (sigma_lo, sigma_hi) applies to every U-Net, a list or
+        tuple of anything else has one entry per U-Net, each None or a pair."""
+        real = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool)
+        pair = lambda v: isinstance(v, (list, tuple)) and len(v) == 2 and all(map(real, v))
+        intervals = (value,) * len(self.unets) if pair(value) else self._per_unet(value, 'guidance_interval')
+        for i, v in enumerate(intervals, 1):
+            assert v is None or pair(v), f'guidance_interval of unet {i} must be None or a pair (sigma_lo, sigma_hi), ' \
+                                         f'got {v!r}'
+            assert v is None or (math.isfinite(v[0]) and 0 <= v[0] < v[1]), \
+                f'guidance_interval of unet {i} must have 0 <= sigma_lo < sigma_hi with a finite sigma_lo, got {v!r}'
+        return tuple(None if v is None else (float(v[0]), float(v[1])) for v in intervals)
 
     def _per_unet(self, value, name):
         """`value` once per U-Net: a list or tuple must have one entry per U-Net, anything else applies to every one."""
@@ -854,7 +960,8 @@ class Imagen(nn.Module):
 
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
                      device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim', init_images=None,
-                     skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None), seed=None):
+                     skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None), seed=None,
+                     guidance=None):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -921,9 +1028,12 @@ class Imagen(nn.Module):
         stop_at = default(stop_at, n_stages)
         steps = default(steps, (None,) * n_stages)
         skips = default(skips, (0,) * n_stages)
+        intervals, gscheds = default(guidance, ((None,) * n_stages, (None,) * n_stages))
         stages = list(zip(range(1, n_stages + 1), self.unets, self.sample_channels, self.image_sizes,
-                          self.noise_schedulers, steps, init_images, skips, scales))[start_at - 1:stop_at]
-        for unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip, stage_scale in stages:
+                          self.noise_schedulers, steps, init_images, skips, scales, intervals,
+                          gscheds))[start_at - 1:stop_at]
+        for (unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip, stage_scale, interval,
+             gsched) in stages:
             with self._one_unet_in_gpu(unet=unet):
                 lowres_cond_img = lowres_noise_times = None
                 if unet.lowres_cond:
@@ -957,6 +1067,9 @@ class Imagen(nn.Module):
                 if exists(init):
                     init = resize_image_to(init, image_size, clamp_range=self.input_image_range)
                     stage_init = self.normalize_img(init).contiguous()
+                gtab = None
+                if exists(interval) or exists(gsched):
+                    gtab = noise_scheduler.guidance_table(interval, gsched, device)
                 stage_inpaint = None
                 if exists(inpaint):
                     # this stage's known image (normalised) and mask; unchanged when already at the stage's size
@@ -969,7 +1082,7 @@ class Imagen(nn.Module):
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
                                           out=slot, schedule=schedule, inpaint=stage_inpaint, init_image=stage_init,
                                           negative_text_embeds=neg_embeds, negative_text_mask=neg_masks, seeds=seeds,
-                                          stage=unet_number)
+                                          stage=unet_number, guidance_table=gtab)
 
         outputs = img
         if gathered is not None:

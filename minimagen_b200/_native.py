@@ -57,6 +57,9 @@ SIGNATURES = {
     "mi_step_epilogue_w": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P, _P, _P, _P],
     "mi_step_epilogue_multistep_w": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P,
                                      _P, _P, _P],
+    "mi_step_epilogue_ws": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P, _P, _P, _P],
+    "mi_step_epilogue_multistep_ws": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F,
+                                      _P, _P, _P, _P],
     "mi_step_advance_t": [_P, _I, _P],
     "mi_step_advance_t_table": [_P, _P, _I, _I, _P],
     "mi_step_finalize": [_P, _L, _I, _P, _P],

@@ -269,7 +269,7 @@ int mi_attention_fwd(const void* q, long long q_bs, int ldq, const void* k, cons
 }
 int mi_step_x0(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const long long* t,
                const float* tab_a, const float* tab_b, int B, int n, float* x0, void* stream) {
-    return check(mi::step_x0(x_t, eps_cond, eps_null, cond_scale, nullptr, t, tab_a, tab_b, B, n, x0, S(stream)),
+    return check(mi::step_x0(x_t, eps_cond, eps_null, cond_scale, nullptr, nullptr, t, tab_a, tab_b, B, n, x0, S(stream)),
                  "mi_step_x0");
 }
 int mi_step_quantile(const float* x0, int B, int n, int rank_lo, int rank_hi, float weight, float min_s, float* s,
@@ -287,7 +287,7 @@ int mi_step_epilogue(const float* x_t, const float* eps_cond, const float* eps_n
                      const float* tab_a, const float* tab_b, const float* c1, const float* c2, const float* sigma,
                      const float* noise, int B, int n, int rank_lo, int rank_hi, float weight, float min_s, float* out,
                      float* s_out, float* x0_workspace, void* stream) {
-    return check(mi::step_epilogue(x_t, eps_cond, eps_null, cond_scale, nullptr, t, tab_a, tab_b, c1, c2, sigma, noise, B,
+    return check(mi::step_epilogue(x_t, eps_cond, eps_null, cond_scale, nullptr, nullptr, t, tab_a, tab_b, c1, c2, sigma, noise, B,
                                    n, rank_lo, rank_hi, weight, min_s, out, s_out, x0_workspace, S(stream)),
                  "mi_step_epilogue");
 }
@@ -296,7 +296,7 @@ int mi_step_epilogue_w(const float* x_t, const float* eps_cond, const float* eps
                        const float* sigma, const float* noise, int B, int n, int rank_lo, int rank_hi, float weight,
                        float min_s, float* out, float* s_out, float* x0_workspace, void* stream) {
     if (!w) return fail(-1, "mi_step_epilogue_w: w is required");
-    return check(mi::step_epilogue(x_t, eps_cond, eps_null, cond_scale, w, t, tab_a, tab_b, c1, c2, sigma, noise, B, n,
+    return check(mi::step_epilogue(x_t, eps_cond, eps_null, cond_scale, w, nullptr, t, tab_a, tab_b, c1, c2, sigma, noise, B, n,
                                    rank_lo, rank_hi, weight, min_s, out, s_out, x0_workspace, S(stream)),
                  "mi_step_epilogue_w");
 }
@@ -305,7 +305,7 @@ int mi_step_epilogue_multistep(const float* x_t, const float* eps_cond, const fl
                                const float* c2, const float* sigma, const float* c3, const float* noise, float* x0_hist,
                                int B, int n, int rank_lo, int rank_hi, float weight, float min_s, float* out,
                                float* s_out, float* x0_workspace, void* stream) {
-    return check(mi::step_epilogue_multistep(x_t, eps_cond, eps_null, cond_scale, nullptr, t, tab_a, tab_b, c1, c2,
+    return check(mi::step_epilogue_multistep(x_t, eps_cond, eps_null, cond_scale, nullptr, nullptr, t, tab_a, tab_b, c1, c2,
                                              sigma, c3, noise, x0_hist, B, n, rank_lo, rank_hi, weight, min_s, out,
                                              s_out, x0_workspace, S(stream)),
                  "mi_step_epilogue_multistep");
@@ -317,10 +317,31 @@ int mi_step_epilogue_multistep_w(const float* x_t, const float* eps_cond, const 
                                  float weight, float min_s, float* out, float* s_out, float* x0_workspace,
                                  void* stream) {
     if (!w) return fail(-1, "mi_step_epilogue_multistep_w: w is required");
-    return check(mi::step_epilogue_multistep(x_t, eps_cond, eps_null, cond_scale, w, t, tab_a, tab_b, c1, c2, sigma, c3,
+    return check(mi::step_epilogue_multistep(x_t, eps_cond, eps_null, cond_scale, w, nullptr, t, tab_a, tab_b, c1, c2, sigma, c3,
                                              noise, x0_hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out,
                                              x0_workspace, S(stream)),
                  "mi_step_epilogue_multistep_w");
+}
+int mi_step_epilogue_ws(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
+                        const float* w_sched, const long long* t, const float* tab_a, const float* tab_b, const float* c1,
+                        const float* c2, const float* sigma, const float* noise, int B, int n, int rank_lo, int rank_hi,
+                        float weight, float min_s, float* out, float* s_out, float* x0_workspace, void* stream) {
+    if (!w || !w_sched) return fail(-1, "mi_step_epilogue_ws: w and w_sched are required");
+    return check(mi::step_epilogue(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_a, tab_b, c1, c2, sigma, noise,
+                                   B, n, rank_lo, rank_hi, weight, min_s, out, s_out, x0_workspace, S(stream)),
+                 "mi_step_epilogue_ws");
+}
+int mi_step_epilogue_multistep_ws(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
+                                  const float* w, const float* w_sched, const long long* t, const float* tab_a,
+                                  const float* tab_b, const float* c1, const float* c2, const float* sigma,
+                                  const float* c3, const float* noise, float* x0_hist, int B, int n, int rank_lo,
+                                  int rank_hi, float weight, float min_s, float* out, float* s_out, float* x0_workspace,
+                                  void* stream) {
+    if (!w || !w_sched) return fail(-1, "mi_step_epilogue_multistep_ws: w and w_sched are required");
+    return check(mi::step_epilogue_multistep(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_a, tab_b, c1, c2,
+                                             sigma, c3, noise, x0_hist, B, n, rank_lo, rank_hi, weight, min_s, out,
+                                             s_out, x0_workspace, S(stream)),
+                 "mi_step_epilogue_multistep_ws");
 }
 int mi_step_advance_t(long long* t, int B, void* stream) {
     return check(mi::step_advance_t(t, B, S(stream)), "mi_step_advance_t");

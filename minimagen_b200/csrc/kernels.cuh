@@ -62,9 +62,10 @@ typedef CUresult (*PFN_tmaEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint
 PFN_tmaEncodeTiled get_tma_encode();
 
 // step.cu
-// w (optional, [B]): per-image guidance weights in place of cond_scale
+// w (optional, [B]): per-image guidance weights in place of cond_scale; w_sched (optional, [T]): the guidance table that
+// schedules them per timestep (step.cu header)
 int step_x0(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
-            const long long* t, const float* tab_recip, const float* tab_recipm1, int B, int n_per_img, float* x0,
+            const float* w_sched, const long long* t, const float* tab_recip, const float* tab_recipm1, int B, int n_per_img, float* x0,
             cudaStream_t st);
 int step_quantile(const float* x0, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
                   float* s_out, cudaStream_t st);
@@ -73,12 +74,13 @@ int step_posterior(const float* x0, const float* x_t, const float* noise, const 
                    cudaStream_t st);
 bool step_epilogue_fused_ok(int n_per_img);
 int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
-                  const long long* t,
+                  const float* w_sched, const long long* t,
                   const float* tab_recip, const float* tab_recipm1, const float* tab_c1, const float* tab_c2,
                   const float* tab_sigma, const float* noise, int B, int n_per_img, int rank_lo, int rank_hi,
                   float weight, float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st);
 int step_epilogue_multistep(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
-                            const float* w, const long long* t, const float* tab_recip, const float* tab_recipm1, const float* tab_c1,
+                            const float* w, const float* w_sched, const long long* t, const float* tab_recip,
+                            const float* tab_recipm1, const float* tab_c1,
                             const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
                             float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
                             float* out, float* s_out, float* x0_ws, cudaStream_t st);

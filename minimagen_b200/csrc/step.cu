@@ -9,7 +9,9 @@
 // The per-image schedule gathers (helpers.extract) happen inside the kernels from the fp32 tables.
 // Products and sums are kept un-fused (__fmul_rn/__fadd_rn) so that the arithmetic matches torch's op-by-op rounding.
 // The guidance weight w is cond_scale for every image, or w[b] per image when the optional array w [B] is given (the _w
-// entry points): one captured step then serves every scale and every per-image scale vector.
+// entry points): one captured step then serves every scale and every per-image scale vector.  The _ws entry points also
+// take a guidance table w_sched [T] (Imagen.sample(guidance_interval=, guidance_schedule=)): image b then combines with
+// w_b(t[b]) = w[b] where w_sched[t[b]] == 1, else 1 + (w[b] - 1) * w_sched[t[b]], rounded op by op.
 // Steps 1 and 3 are written once (guided_x0, posterior_elem) and shared by the three-kernel form and the fused kernel.
 // The select of step 2 exists twice, and each is the other's test reference: quantile_kernel (one CTA per image, keys
 // streamed from global memory, any n) and the one inside step_epilogue_kernel (an 8-CTA cluster per image, keys held in
@@ -44,8 +46,13 @@ namespace mi {
 
 namespace {
 
-// The guidance weight of image b.
-__device__ __forceinline__ float image_scale(const float* w, float cond_scale, int b) { return w ? w[b] : cond_scale; }
+// The guidance weight of image b at its timestep tb, scheduled by w_sched[tb] when the table is given.
+__device__ __forceinline__ float image_scale(const float* w, const float* w_sched, float cond_scale, int b, long long tb) {
+    const float wb = w ? w[b] : cond_scale;
+    if (!w_sched) return wb;
+    const float s = w_sched[tb];
+    return s == 1.f ? wb : __fadd_rn(1.f, __fmul_rn(__fsub_rn(wb, 1.f), s));
+}
 
 // Step 1 at element idx: eps = null + (cond - null) * w when eps_null is given, then x0 = a[t] * x_t - b[t] * eps.
 __device__ __forceinline__ float guided_x0(const float* x_t, const float* eps_cond, const float* eps_null,
@@ -91,7 +98,8 @@ __device__ __forceinline__ void posterior_elem(float x0, float s, float c1, floa
 __global__ void __launch_bounds__(256)
 x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
           float cond_scale, const long long* __restrict__ t, const float* __restrict__ tab_recip,
-          const float* __restrict__ tab_recipm1, int n_per_img, float* __restrict__ x0, const float* __restrict__ w) {
+          const float* __restrict__ tab_recipm1, int n_per_img, float* __restrict__ x0, const float* __restrict__ w,
+          const float* __restrict__ w_sched) {
     pdl_wait();
     pdl_trigger();
     const int b = blockIdx.y;
@@ -99,7 +107,8 @@ x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, con
     if (i >= n_per_img) return;
     const long long idx = (long long)b * n_per_img + i;
     const long long tb = t[b];
-    x0[idx] = guided_x0(x_t, eps_cond, eps_null, image_scale(w, cond_scale, b), tab_recip[tb], tab_recipm1[tb], idx);
+    x0[idx] = guided_x0(x_t, eps_cond, eps_null, image_scale(w, w_sched, cond_scale, b, tb), tab_recip[tb],
+                        tab_recipm1[tb], idx);
 }
 
 // One CTA per image.  Exact k-th order statistics of |x| by 4 x 8-bit radix passes over the float bit patterns.
@@ -229,7 +238,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
                      const float* __restrict__ tab_c2, const float* __restrict__ tab_sigma,
                      const float* __restrict__ noise, int n, int rank_lo, int rank_hi, float weight, float min_s,
                      float* out, float* __restrict__ s_out, const float* __restrict__ tab_c3,
-                     float* __restrict__ x0_hist, const float* __restrict__ w) {
+                     float* __restrict__ x0_hist, const float* __restrict__ w, const float* __restrict__ w_sched) {
     pdl_wait();
     pdl_trigger();
     namespace cg = cooperative_groups;
@@ -249,7 +258,7 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
     const long long base = (long long)img * n + beg;
     const long long tb = t[img];
     const float ca = tab_recip[tb], cb = tab_recipm1[tb];
-    const float scale = image_scale(w, cond_scale, img);
+    const float scale = image_scale(w, w_sched, cond_scale, img, tb);
 
     float x0v[kSelPerThread];
     bool nan_key = false;
@@ -560,10 +569,11 @@ int inpaint_finalize(const float* x, const float* k, const float* m, int B, int 
 }
 
 int step_x0(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
-            const long long* t, const float* tab_recip, const float* tab_recipm1, int B, int n_per_img, float* x0,
-            cudaStream_t st) {
+            const float* w_sched, const long long* t, const float* tab_recip, const float* tab_recipm1, int B,
+            int n_per_img, float* x0, cudaStream_t st) {
     dim3 grid((n_per_img + 255) / 256, B);
-    launch_k(x0_kernel, grid, 256, 0, st, x_t, eps_cond, eps_null, cond_scale, t, tab_recip, tab_recipm1, n_per_img, x0, w);
+    launch_k(x0_kernel, grid, 256, 0, st, x_t, eps_cond, eps_null, cond_scale, t, tab_recip, tab_recipm1, n_per_img, x0, w,
+             w_sched);
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
@@ -597,20 +607,20 @@ bool step_epilogue_fused_ok(int n_per_img) {
 
 template <bool kHist>
 static int step_epilogue_impl(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
-                              const float* w, const long long* t, const float* tab_recip, const float* tab_recipm1, const float* tab_c1,
-                              const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
+                              const float* w, const float* w_sched, const long long* t, const float* tab_recip,
+                              const float* tab_recipm1, const float* tab_c1, const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
                               float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight,
                               float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st) {
     if (rank_lo < 0 || rank_hi < rank_lo || rank_hi >= n_per_img) return -1;
     if (step_epilogue_fused_ok(n_per_img)) {
         launch_k(step_epilogue_kernel<kHist>, B * kSelCluster, kSelThreads, 0, st, x_t, eps_cond, eps_null, cond_scale,
                  t, tab_recip, tab_recipm1, tab_c1, tab_c2, tab_sigma, noise, n_per_img, rank_lo, rank_hi, weight, min_s,
-                 out, s_out, tab_c3, x0_hist, w);
+                 out, s_out, tab_c3, x0_hist, w, w_sched);
         return cudaGetLastError() == cudaSuccess ? 0 : -2;
     }
     // images beyond the register-resident select (> 196 608 values, e.g. 3 x 1024 x 1024): x0 through the caller's scratch
     if (!x0_ws || !s_out) return -1;
-    int rc = step_x0(x_t, eps_cond, eps_null, cond_scale, w, t, tab_recip, tab_recipm1, B, n_per_img, x0_ws, st);
+    int rc = step_x0(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, B, n_per_img, x0_ws, st);
     if (rc) return rc;
     rc = step_quantile(x0_ws, B, n_per_img, rank_lo, rank_hi, weight, min_s, s_out, st);
     if (rc) return rc;
@@ -619,22 +629,23 @@ static int step_epilogue_impl(const float* x_t, const float* eps_cond, const flo
 }
 
 int step_epilogue(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
-                  const long long* t,
+                  const float* w_sched, const long long* t,
                   const float* tab_recip, const float* tab_recipm1, const float* tab_c1, const float* tab_c2,
                   const float* tab_sigma, const float* noise, int B, int n_per_img, int rank_lo, int rank_hi,
                   float weight, float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st) {
-    return step_epilogue_impl<false>(x_t, eps_cond, eps_null, cond_scale, w, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
+    return step_epilogue_impl<false>(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
                                      tab_sigma, nullptr, noise, nullptr, B, n_per_img, rank_lo, rank_hi, weight, min_s,
                                      out, s_out, x0_ws, st);
 }
 
 int step_epilogue_multistep(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
-                            const float* w, const long long* t, const float* tab_recip, const float* tab_recipm1, const float* tab_c1,
+                            const float* w, const float* w_sched, const long long* t, const float* tab_recip,
+                            const float* tab_recipm1, const float* tab_c1,
                             const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
                             float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
                             float* out, float* s_out, float* x0_ws, cudaStream_t st) {
     if (!tab_c3 || !x0_hist) return -1;
-    return step_epilogue_impl<true>(x_t, eps_cond, eps_null, cond_scale, w, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
+    return step_epilogue_impl<true>(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
                                     tab_sigma, tab_c3, noise, x0_hist, B, n_per_img, rank_lo, rank_hi, weight, min_s,
                                     out, s_out, x0_ws, st);
 }

@@ -8,6 +8,7 @@ per-timestep noise scale the fused step kernel gathers (reference computes it ev
 The tensor methods are kept for API parity (they are one-line broadcasts of table lookups); the sampling loop does
 NOT go through them -- it uses the fused step kernels (minimagen_b200/csrc/step.cu).
 """
+import math
 from typing import NamedTuple, Optional, Tuple
 
 import torch
@@ -213,6 +214,38 @@ class GaussianDiffusion(nn.Module):
         tabs = (walk.next_t, ra.to(torch.float32).to(device), rb.to(torch.float32).to(device))
         self._schedules[key] = tabs
         return tabs
+
+    def guidance_table(self, interval, schedule, device):
+        """Guidance table of a guidance interval and a guidance-weight schedule (no reference counterpart), [T] fp32 on
+        `device`.  With a = alphas_cumprod (fp64), sigma_t = sqrt((1 - a_t) / a_t) (the VE noise level; inf where a_t = 0)
+        and tau = t / (T - 1):
+            shape(t) = 1 (schedule None), 2 (1 - tau) ('linear') or 1 + cos(pi tau) ('cosine'),
+            s[t]     = shape(t) if sigma_lo < sigma_t <= sigma_hi (every t when `interval` is None), else 0,
+        computed in fp64 and cast to fp32.  A step at t guides image b with w_b where s[t] == 1, with
+        1 + (w_b - 1) s[t] elsewhere, and skips the guidance pass where s[t] == 0.  Cached per (interval, schedule, device)."""
+        device = torch.device(device)
+        key = ('guidance', None if interval is None else tuple(map(float, interval)), schedule, str(device))
+        tab = self._schedules.get(key)
+        if tab is not None:
+            return tab
+        T = self.num_timesteps
+        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        tau = torch.arange(T, dtype=torch.float64) / (T - 1)
+        if schedule is None:
+            s = torch.ones(T, dtype=torch.float64)
+        elif schedule == 'linear':
+            s = 2. * (1. - tau)
+        elif schedule == 'cosine':
+            s = 1. + torch.cos(math.pi * tau)
+        else:
+            raise ValueError(f"guidance schedule must be None, 'linear' or 'cosine', got {schedule!r}")
+        if interval is not None:
+            lo, hi = map(float, interval)
+            sigma = ((1. - acp) / acp).sqrt()                     # 1 / 0 = inf at T = 20's last timestep
+            s = torch.where((sigma > lo) & (sigma <= hi), s, torch.zeros_like(s))
+        tab = s.to(torch.float32).to(device)
+        self._schedules[key] = tab
+        return tab
 
     # ---- integer timestep generators (diffusion_model.py:68-87)
     def _get_times(self, batch_size, noise_level, *, device):

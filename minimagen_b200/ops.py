@@ -277,6 +277,48 @@ class NativeOps:
                N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(c3), N.ptr(noise), N.ptr(hist), B, n,
                int(rank_lo), int(rank_hi), float(weight), float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
 
+    def step_epilogue_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2, sigma, noise, B,
+                                n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """step_epilogue with the guidance weights scheduled by the table `w_sched` ([T] fp32 on x's device, a
+        GaussianDiffusion.guidance_table): image b combines with w_b(t[b]) = w_b where w_sched[t[b]] == 1, else
+        1 + (w_b - 1) * w_sched[t[b]] (mi_step_epilogue_ws).  `cond_scale` as in step_epilogue."""
+        self._scheduled("mi_step_epilogue_ws", x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2, sigma,
+                        None, noise, None, B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def step_epilogue_multistep_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2,
+                                          sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """step_epilogue_multistep with the guidance weights scheduled by `w_sched` as in step_epilogue_scheduled
+        (mi_step_epilogue_multistep_ws)."""
+        if c3 is None or hist is None:
+            raise ValueError("step_epilogue_multistep_scheduled: c3 and hist are required")
+        self._scheduled("mi_step_epilogue_multistep_ws", x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1,
+                        c2, sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def _scheduled(self, entry, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2, sigma, c3, noise,
+                   hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out):
+        for nm, tt in (("x_t", x_t), ("eps_cond", eps_cond), ("eps_null", eps_null), ("w_sched", w_sched),
+                       ("tab_a", tab_a), ("tab_b", tab_b), ("c1", c1), ("c2", c2), ("sigma", sigma), ("c3", c3),
+                       ("noise", noise), ("hist", hist), ("out", out), ("s_out", s_out)):
+            _chk(tt, F32, nm)
+        _chk(t, I64, "t")
+        if w_sched is None or not w_sched.is_cuda:
+            raise ValueError("w_sched: the guidance table must be an fp32 tensor on a CUDA device")
+        if hist is not None and hist.numel() != B * n:
+            raise ValueError(f"hist: expected {B * n} values, got {hist.numel()}")
+        if not torch.is_tensor(cond_scale):
+            cond_scale = torch.full((B,), float(cond_scale), dtype=F32, device=x_t.device)
+        _, scale = _scale_args(cond_scale, B, entry)
+        ws = None
+        nws = int(N.load().mi_step_epilogue_workspace_floats(B, n))
+        if nws:
+            ws = torch.empty(nws, dtype=F32, device=x_t.device)
+            if s_out is None:
+                s_out = torch.empty(B, dtype=F32, device=x_t.device)
+        tail = (N.ptr(noise),) if hist is None else (N.ptr(c3), N.ptr(noise), N.ptr(hist))
+        N.call(entry, N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), *scale, N.ptr(w_sched), N.ptr(t), N.ptr(tab_a),
+               N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), *tail, B, n, int(rank_lo), int(rank_hi), float(weight),
+               float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
+
     def step_advance_t(self, t, B):
         _chk(t, I64, "t")
         N.call("mi_step_advance_t", N.ptr(t), B, N.stream())
