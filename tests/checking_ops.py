@@ -17,9 +17,15 @@ checkers are not vacuous).
 `sms` is the SM count the per-kernel summation plans (and so the bounds' accumulation lengths) depend on: the device's
 multi_processor_count, or 132 (an H100 SXM) for the CPU emulation.
 
-The image-sized checkers (convolutions, GroupNorm, casts, the stem) build their float64 references and compare a few images
-at a time (`_image_slices`): every bound is per element, so slicing changes no verdict, and a forward at the benchmark's
-size (b = 32 at 256 x 256, activations of 2 GiB per tensor in float64) keeps its reference memory to a few GiB.
+The image-sized checkers (convolutions, GroupNorm, casts, the stem, the NCHW -> NHWC copy) build their float64 references
+and compare a few images at a time, and when one image's reference exceeds SLICE_ELEMENTS (a 1024 x 1024 conv: 8 - 16x
+over), one band of rows at a time (`_bands`).  A conv band reads the rows its taps reach beyond it (the halo of its mode:
+k // 2 rows for a k x k or the 15 x 1 stem conv, one phase row for the phase-split stride-2 conv and the sub-pixel Upsample
+phases, two input rows for the stride-2 conv read in place) and keeps only its own output rows.  Every elementwise bound is
+per element, so banding changes no verdict; the statistics (the conv epilogue's increment, gn_stats) are reduced per band
+in float64 and the bands' sums, and bounds, added before the one comparison per image.  So a forward at 256 x 256 (b = 32,
+2 GiB per activation in float64) or at 1024 x 1024 keeps its reference memory to a few GiB.  `images` restricts the
+comparisons to some images (a test of a large batch that checks the images next to an index boundary).
 """
 import contextlib
 import io
@@ -53,31 +59,50 @@ def default_sms():
     return torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
 
 
-SLICE_ELEMENTS = 1 << 26        # float64 elements per reference tensor of one slice of images (512 MiB)
+SLICE_ELEMENTS = 1 << 26        # float64 elements per reference tensor of one piece of a check (512 MiB)
 
 
-def _image_slices(B, per_image):
-    """Slices of the B images such that one slice's largest tensor (per_image elements per image) stays within
-    SLICE_ELEMENTS; one slice when everything fits."""
-    step = max(1, SLICE_ELEMENTS // max(1, per_image))
-    return [slice(b, min(B, b + step)) for b in range(0, B, step)]
+def _bands(B, H, per_row, halo=0, step=1, images=None):
+    """The pieces a check computes its reference in: [(image slice, [(h0, h1), ...] its bands of rows)].  Whole images, a
+    few at a time, while one image's largest reference tensor (H rows of per_row elements) fits SLICE_ELEMENTS; else one
+    image at a time in bands of rows whose reference, with the `halo` rows read beyond the band on either side, fits.
+    Band edges are multiples of `step`.  images: only these images, one slice each."""
+    if H * per_row > SLICE_ELEMENTS:
+        rows = max(step, (SLICE_ELEMENTS // per_row - 2 * halo) // step * step)
+        bands = [(h, min(H, h + rows)) for h in range(0, H, rows)]
+        return [(slice(b, b + 1), bands) for b in (range(B) if images is None else images)]
+    if images is not None:
+        return [(slice(b, b + 1), [(0, H)]) for b in images]
+    n = max(1, SLICE_ELEMENTS // max(1, H * per_row))
+    return [(slice(b, min(B, b + n)), [(0, H)]) for b in range(0, B, n)]
 
 
 def _at(t, i):
     return None if t is None else t[i]
 
 
+def _rows(t, i, h0, h1):
+    return None if t is None else t[i, h0:h1]
+
+
+def _add(acc, part):
+    """Elementwise sum of (reference, bound) pairs; acc None to start."""
+    return part if acc is None else (acc[0] + part[0], acc[1] + part[1])
+
+
 class CheckingOps:
-    def __init__(self, inner, sms=None, fresh_accumulators=False, only=None, strict=True):
+    def __init__(self, inner, sms=None, fresh_accumulators=False, only=None, strict=True, images=None):
         """only: check just these methods (the others run unchecked): lets a run with one planted defect skip the float64
         references of every other call.  strict=False: a failed check is recorded in `failures` and the run goes on (the
         outputs are the backend's own either way), so that one run gives both the verdict and the gradients;
-        `raise_failures` raises the first one afterwards."""
+        `raise_failures` raises the first one afterwards.  images: the image-sized checkers compare only these images."""
         self.inner = inner
         self.sms = default_sms() if sms is None else sms
         self.fresh = fresh_accumulators
         self.only = only
         self.strict = strict
+        self.images = images
+        self.image, self.per_image = None, {}   # the one image being compared; (method, image) -> worst |err| / bound
         self.failures = []
         self.called, self.checked = set(), set()
         self.family = {}                       # method -> [calls, worst |err| / bound]
@@ -131,6 +156,9 @@ class CheckingOps:
         f = self.family.setdefault(name, [0, 0.0])
         f[1] = max(f[1], ratio)
         self.last = max(self.last, ratio)
+        if self.image is not None:
+            key = (name, self.image)
+            self.per_image[key] = max(self.per_image.get(key, 0.0), ratio)
 
     def _count(self, name):
         self.family.setdefault(name, [0, 0.0])[0] += 1
@@ -155,15 +183,28 @@ class CheckingOps:
         for fam, (calls, worst) in sorted(self.family.items()):
             print(f"  {fam:28s} {calls:5d} calls   worst |err|/bound {worst:.3g}")
 
-    def _stats_increment(self, name, acc, before, f, e, sb=16):
-        """acc - before against the (sum, sum of squares) per (image, sb channels) of this call's output: `f` the fp32 values
-        the kernel summed (its own fp32 output), or their reference with elementwise bound `e` when only fp16 was stored.
-        Per image: acc, before and f may be the same slice of images of a call (the caller counts the call)."""
-        ref, bound = R.conv_stats_ref(f, sb)
+    def _bands(self, B, H, per_row, halo=0, step=1):
+        """_bands with this proxy's `images`; while a piece of one image is compared, its ratios also go to per_image."""
+        for i, rows in _bands(B, H, per_row, halo, step, self.images):
+            self.image = i.start if i.stop - i.start == 1 else None
+            yield i, rows
+        self.image = None
+
+    @staticmethod
+    def _stats_band(f, e, P, sb=16):
+        """The float64 (sum, sum of squares) per (image, sb channels) of one band of this call's output, and its bound (the
+        image has P pixels): `f` the fp32 values the kernel summed (its own fp32 output), or their reference with
+        elementwise bound `e` when only fp16 was stored.  Both add up over the bands of an image."""
+        ref, bound = R.conv_stats_ref(f, sb, P)
         if e is not None:
             B, C = f.shape[0], f.shape[-1]
             blk = lambda t: t.reshape(B, -1, C // sb, sb).sum(dim=(1, 3))
             bound = bound + torch.stack((blk(e), blk(2 * f.abs() * e + e * e)), dim=-1)
+        return ref, bound
+
+    def _stats_increment(self, name, acc, before, ref, bound):
+        """acc - before against the statistics `ref` (bound `bound`) of this call's output, summed over its bands.  Per
+        image: acc, before and ref may be the same slice of images of a call (the caller counts the call)."""
         bound = bound + 4 * R.U64 * (before.abs() + acc.abs())             # the subtraction below
         self._note(name + " statistics", R.check(acc - before, ref, bound, name + " statistics increment"))
 
@@ -177,7 +218,10 @@ class CheckingOps:
     def _check_conv_igemm(self, act, B, H, W, lda, c_off, c_in, wp, c_out, kh, kw, mode, bias, residual, out_f32, out_f16,
                           out_strides, block_n=0, out_sc=1, n_valid=0, act2=None, lda2=0, c_off2=0, c_in1=0, out_stats=None):
         self._count("conv_igemm")
-        self.features.add(f"conv_igemm mode {mode}")
+        self.features |= {f"conv_igemm mode {mode}", f"conv_igemm c_out={c_out}", f"conv_igemm K={kh * kw * c_in}",
+                          f"conv_igemm W={W}"}
+        if H * W < 128:
+            self.features.add("conv_igemm multi-image tiles")               # a 128-pixel tile spans 128 / (H W) images
         nv = n_valid if n_valid else c_out
         sb_, sh, sw = out_strides
         view = lambda t: None if t is None else _strided(t, (B, H, W, nv), (sb_, sh, sw, out_sc))
@@ -198,12 +242,24 @@ class CheckingOps:
         res = None if residual is None else _strided(residual, (B, H, W, c_out), (sb_, sh, sw, 1))
         if out_stats is not None:
             self._count("conv_igemm statistics")
-            acc, before, own = out_stats.reshape(B, -1, 2), before.reshape(B, -1, 2), o32 is not None
-        for i in _image_slices(B, H * W * max(4 * c_in, c_out)):
-            ref, bound = R.conv_fwd_ref(a[i], wp, kh, kw, mode, bias, _at(res, i))
-            self._out("conv_igemm", _at(o32, i), _at(o16, i), ref[..., :nv], bound[..., :nv])
+            acc, before = out_stats.reshape(B, -1, 2), before.reshape(B, -1, 2)
+        # a band of output rows [h0, h1) reads input rows [s h0 - halo, s h1 + halo) (s = 2: the stride-2 conv read in
+        # place, whose input has 2H rows; mode 1's input rows are phase rows)
+        s, halo = (2, 2) if mode == 6 else (1, kh // 2 if mode == 0 else 1)
+        for i, rows in self._bands(B, H, W * max(4 * c_in, c_out), halo):
+            st = None
+            for h0, h1 in rows:
+                lo, hi = max(0, s * h0 - halo), min(s * H, s * h1 + halo)
+                ref, bound = R.conv_fwd_ref(a[i][..., lo:hi, :, :], wp, kh, kw, mode, bias,
+                                            None if res is None else res[i, lo // s:hi // s])
+                band = slice(h0 - lo // s, h1 - lo // s)                     # the band's rows of the slab's output
+                ref, bound = ref[:, band], bound[:, band]
+                self._out("conv_igemm", _rows(o32, i, h0, h1), _rows(o16, i, h0, h1), ref[..., :nv], bound[..., :nv])
+                if out_stats is not None:
+                    st = _add(st, self._stats_band(o32[i, h0:h1], None, H * W) if o32 is not None else
+                             self._stats_band(ref, bound, H * W))
             if out_stats is not None:
-                self._stats_increment("conv_igemm", acc[i], before[i], o32[i] if own else ref, None if own else bound)
+                self._stats_increment("conv_igemm", acc[i], before[i], *st)
 
     def _check_conv_res1x1(self, act, B, H, W, lda, c_in, act2, lda2, c_in1, x, ldx, x_cin, x2, ldx2, x_cin1, wp, c_out,
                            bias, residual, out_f32, out_f16, out_stats):
@@ -221,12 +277,20 @@ class CheckingOps:
         res, o32, o16 = rs(residual), rs(out_f32), rs(out_f16)
         if out_stats is not None:
             self._count("conv_res1x1 statistics")
-            acc, before, own = out_stats.reshape(B, -1, 2), before.reshape(B, -1, 2), o32 is not None
-        for i in _image_slices(B, H * W * max(c_in + x_cin, c_out)):
-            ref, bound = R.conv_fwd_ref(a[i], wp, 3, 3, 0, bias, _at(res, i), x=xs[i])
-            self._out("conv_res1x1", _at(o32, i), _at(o16, i), ref, bound)
+            acc, before = out_stats.reshape(B, -1, 2), before.reshape(B, -1, 2)
+        for i, rows in self._bands(B, H, W * max(c_in + x_cin, c_out), 1):
+            st = None
+            for h0, h1 in rows:
+                lo, hi = max(0, h0 - 1), min(H, h1 + 1)
+                ref, bound = R.conv_fwd_ref(a[i, lo:hi], wp, 3, 3, 0, bias, None if res is None else res[i, lo:hi],
+                                            x=xs[i, lo:hi])
+                ref, bound = ref[:, h0 - lo:h1 - lo], bound[:, h0 - lo:h1 - lo]
+                self._out("conv_res1x1", _rows(o32, i, h0, h1), _rows(o16, i, h0, h1), ref, bound)
+                if out_stats is not None:
+                    st = _add(st, self._stats_band(o32[i, h0:h1], None, H * W) if o32 is not None else
+                             self._stats_band(ref, bound, H * W))
             if out_stats is not None:
-                self._stats_increment("conv_res1x1", acc[i], before[i], o32[i] if own else ref, None if own else bound)
+                self._stats_increment("conv_res1x1", acc[i], before[i], *st)
 
     def _check_conv_gn(self, src0, c0, src1, c1, scale1, B, H, W, groups, stats0, stats1, gamma, beta, scale_shift, ss_ld,
                        eps, wp, c_out, bias, residual, out_f32, out_f16, out_stats):
@@ -245,8 +309,9 @@ class CheckingOps:
         self._out("conv_gn", rs(out_f32, c_out), rs(out_f16, c_out), ref, bound)
         if out_stats is not None:
             self._count("conv_gn statistics")
-            own = out_f32 is not None
-            self._stats_increment("conv_gn", out_stats, before, rs(out_f32, c_out) if own else ref, None if own else bound)
+            st = (self._stats_band(rs(out_f32, c_out), None, H * W) if out_f32 is not None else
+                  self._stats_band(ref, bound, H * W))
+            self._stats_increment("conv_gn", out_stats, before, *st)
 
     def _check_conv_direct(self, inp, B, Hin, Win, c_in, ldi, w, c_out, kh, kw, stride, pad, bias, residual, out, Hout, Wout,
                            out_strides):
@@ -284,8 +349,11 @@ class CheckingOps:
         before = self._accumulator(sums).reshape(B, -1, 2)
         yield
         acc, s0, s1 = sums.reshape(B, -1, 2), src0.reshape(B, hw, c0), src1.reshape(B, hw, c1) if c1 else None
-        for i in _image_slices(B, hw * (c0 + c1)):
-            ref, bound = R.gn_stats_ref(s0[i], groups, _at(s1, i), scale1)
+        for i, bands in self._bands(B, hw, c0 + c1):
+            st = None
+            for p0, p1 in bands:
+                st = _add(st, R.gn_stats_ref(s0[i, p0:p1], groups, None if s1 is None else s1[i, p0:p1], scale1, HW=hw))
+            ref, bound = st
             bound = bound + 4 * R.U64 * (before[i].abs() + acc[i].abs())
             self._note("gn_stats", R.check(acc[i] - before[i], ref, bound, "gn_stats increment"))
 
@@ -300,10 +368,12 @@ class CheckingOps:
         sums = sums.reshape(B, groups, 2)
         ss = None if scale_shift is None else _strided(scale_shift, (B, 2 * C), (ss_ld, 1))
         s0, s1, o = src0.reshape(B, hw, c0), src1.reshape(B, hw, c1) if c1 else None, out.reshape(B, hw, C)
-        for i in _image_slices(B, hw * C):
-            ref, bound = R.gn_apply_silu_ref(s0[i], groups, gamma, beta, _at(ss, i), eps, sums[i], src1=_at(s1, i),
-                                             scale1=scale1, out16=out.dtype == F16)
-            self._note("gn_apply_silu", R.check(o[i], ref, bound, "gn_apply_silu"))
+        for i, bands in self._bands(B, hw, C):
+            for p0, p1 in bands:
+                ref, bound = R.gn_apply_silu_ref(s0[i, p0:p1], groups, gamma, beta, _at(ss, i), eps, sums[i],
+                                                 src1=None if s1 is None else s1[i, p0:p1], scale1=scale1,
+                                                 out16=out.dtype == F16, HW=hw)
+                self._note("gn_apply_silu", R.check(o[i, p0:p1], ref, bound, "gn_apply_silu"))
 
     def _check_cast_act(self, src0, c0, src1, c1, scale1, B, H, W, mode, out):
         self._count("cast_act")
@@ -312,19 +382,27 @@ class CheckingOps:
         o = out.reshape(-1)[:n_out]                                        # mode 0 writes the first B*H*W rows of `out`
         o.fill_(NAN)
         yield
-        s0, s1, ob = src0.reshape(B, H, W, c0), src1.reshape(B, H, W, c1) if c1 else None, o.reshape(B, -1)
-        for i in _image_slices(B, 4 * H * W * C):
-            x = R.gn_concat(s0[i], _at(s1, i), scale1)
-            if mode == 1:
-                x = x.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2)
-            elif mode == 2:
-                x = torch.stack([x[:, (p >> 1)::2, (p & 1)::2] for p in range(4)], dim=1)
-            bound = R.U32 * x.abs() if c1 else torch.zeros_like(x)         # the fp32 product with the skip scale
-            ref, bound = R.half_out(x, bound) if out.dtype == F16 else (x, bound)
-            self._note("cast_act", R.check(ob[i].reshape(x.shape), ref, bound, f"cast_act mode {mode}"))
+        s0, s1 = src0.reshape(B, H, W, c0), src1.reshape(B, H, W, c1) if c1 else None
+        # the output rows of input rows [h0, h1): the same rows, rows [2 h0, 2 h1) of the nearest x2 upsample, or phase
+        # rows [h0 / 2, h1 / 2) of each of the four phases (bands of even rows)
+        ob = o.reshape((B, H, W, C) if mode == 0 else (B, 2 * H, 2 * W, C) if mode == 1 else (B, 4, H // 2, W // 2, C))
+        for i, rows in self._bands(B, H, 4 * W * C, step=2 if mode == 2 else 1):
+            for h0, h1 in rows:
+                x = R.gn_concat(s0[i, h0:h1], None if s1 is None else s1[i, h0:h1], scale1)
+                if mode == 0:
+                    got = ob[i, h0:h1]
+                elif mode == 1:
+                    x, got = x.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2), ob[i, 2 * h0:2 * h1]
+                else:
+                    x = torch.stack([x[:, (p >> 1)::2, (p & 1)::2] for p in range(4)], dim=1)
+                    got = ob[i, :, h0 // 2:h1 // 2]
+                bound = R.U32 * x.abs() if c1 else torch.zeros_like(x)     # the fp32 product with the skip scale
+                ref, bound = R.half_out(x, bound) if out.dtype == F16 else (x, bound)
+                self._note("cast_act", R.check(got, ref, bound, f"cast_act mode {mode}"))
 
     def _check_ln_rows(self, inp, rows, C, gamma, beta, eps, pre_gelu, residual, out_f32, out_f16):
         self._count("ln_rows")
+        self.features.add(f"ln_rows C={C}")
         for o in (out_f32, out_f16):
             if o is not None:
                 o.fill_(NAN)
@@ -361,6 +439,8 @@ class CheckingOps:
 
     def _check_text_tokens(self, proj, B, L, D, mask, keep, null_embed, max_len, c_out, m, row_off, pooled):
         self._count("text_tokens")
+        if not keep.bool().all():
+            self.features.add(f"text_tokens null rows B={B}")
         rows = c_out.reshape(B, m, D)[:, row_off:row_off + max_len]
         rows.fill_(NAN)
         pooled.fill_(NAN)
@@ -398,11 +478,14 @@ class CheckingOps:
         self._count("nchw_to_nhwc")
         out.fill_(NAN)
         yield
-        want = torch.zeros((B, hw, c_pad), dtype=F32, device=a.device)
-        want[:, :, :ca] = a.reshape(B, ca, hw).permute(0, 2, 1)
-        if b is not None and cb:
-            want[:, :, ca:ca + cb] = b.reshape(B, cb, hw).permute(0, 2, 1)
-        assert torch.equal(out.reshape(B, hw, c_pad), want), "nchw_to_nhwc is a transposing copy with zero padding"
+        for i, bands in self._bands(B, hw, 2 * c_pad):
+            for p0, p1 in bands:
+                want = torch.zeros((i.stop - i.start, p1 - p0, c_pad), dtype=F32, device=a.device)
+                want[:, :, :ca] = a.reshape(B, ca, hw)[i, :, p0:p1].permute(0, 2, 1)
+                if b is not None and cb:
+                    want[:, :, ca:ca + cb] = b.reshape(B, cb, hw)[i, :, p0:p1].permute(0, 2, 1)
+                assert torch.equal(out.reshape(B, hw, c_pad)[i, p0:p1], want), \
+                    "nchw_to_nhwc is a transposing copy with zero padding"
         self._note("nchw_to_nhwc", 0.0)
 
     def _check_stem_unroll(self, a, ca, b, cb, B, H, W, out):
@@ -411,17 +494,19 @@ class CheckingOps:
         yield
         x = a if b is None or cb == 0 else torch.cat((a, b), dim=1)
         o = out.reshape(B, H, W, 128)
-        for i in _image_slices(B, H * W * 128):
-            xp = torch.nn.functional.pad(x[i], (7, 8))
-            want = torch.zeros((xp.shape[0], H, W, 16, 8), dtype=F64, device=a.device)
-            for j in range(15):
-                want[:, :, :, j, :x.shape[1]] = xp[:, :, :, j:j + W].permute(0, 2, 3, 1)
-            ref, bound = R.half_out(want.reshape(-1, H, W, 128), torch.zeros((), dtype=F64, device=a.device))
-            self._note("stem_unroll", R.check(o[i], ref, bound, "stem_unroll"))
+        for i, rows in self._bands(B, H, W * 128):
+            for h0, h1 in rows:
+                xp = torch.nn.functional.pad(x[i, :, h0:h1], (7, 8))       # the window is horizontal: no halo rows
+                want = torch.zeros((xp.shape[0], h1 - h0, W, 16, 8), dtype=F64, device=a.device)
+                for j in range(15):
+                    want[:, :, :, j, :x.shape[1]] = xp[:, :, :, j:j + W].permute(0, 2, 3, 1)
+                ref, bound = R.half_out(want.reshape(-1, h1 - h0, W, 128), torch.zeros((), dtype=F64, device=a.device))
+                self._note("stem_unroll", R.check(o[i, h0:h1], ref, bound, "stem_unroll"))
 
     # ---------------------------------------------------------------- attention
     def _check_attention(self, q, q_bs, ldq, k, v, kv_bs, ldkv, kv_hs, null_kv, mask, B, heads, n, m, out, o_bs, ldo):
         self._count("attention")
+        self.features.add(f"attention B={B} n={n}")
         o = _strided(out, (B, heads, n, 64), (o_bs, 64, ldo, 1))
         o.fill_(NAN)
         yield

@@ -638,18 +638,19 @@ def conv_stats_acc_len():
     return 8 + 5 + 1
 
 
-def conv_stats_ref(out32, sb=16):
+def conv_stats_ref(out32, sb=16, P=None):
     """The epilogue's GroupNorm statistics, per (image, sb-channel block), of the kernel's OWN fp32 output out32
     [B, ..., C] (valid pixels only; the phases of modes 2..5 all in one tensor): float64 (sum, sum of squares) [B, C/sb, 2]
     and their bound
         2 acc_len U32 sum|f|  (resp. sum f^2)  +  P U64 (same),
     acc_len = conv_stats_acc_len(), P the pixel count (more than the fp64 adds of any reduction order).  Because it compares
     with the output the kernel wrote, not with reference statistics, the bound is tight enough to see one warp's 16 rows, a
-    tile credited to the wrong image, or masked rows that were counted."""
+    tile credited to the wrong image, or masked rows that were counted.  P (default: out32's pixels) is the image's pixel
+    count when out32 is one band of rows: both results are then linear in the band's values and add up over the bands."""
     f = _d(out32)
     B, C = f.shape[0], f.shape[-1]
     fb = f.reshape(B, -1, C // sb, sb)
-    P = fb.shape[1]
+    P = fb.shape[1] if P is None else P
     s, q, t = fb.sum(dim=(1, 3)), (fb * fb).sum(dim=(1, 3)), fb.abs().sum(dim=(1, 3))
     c = 2 * conv_stats_acc_len() * U32 + P * U64
     return torch.stack((s, q), dim=-1), torch.stack((c * t, c * q), dim=-1)
@@ -680,17 +681,19 @@ def gn_stats_plan(C, HW):
     return chunk, planes, -(-chunk // planes)
 
 
-def gn_stats_ref(src0, groups, src1=None, scale1=1.0, L=None):
+def gn_stats_ref(src0, groups, src1=None, scale1=1.0, L=None, HW=None):
     """mi_gn_stats: per (image, group) float64 (sum, sum of squares) [B, G, 2] of the virtual concat, and the bound
         (L + 3) U32 sum|x|  (resp. sum x^2)  +  (HW + 2048) U64 (same).
     A thread's fp32 chain of L values (gn_stats_plan) rounds at most L times on any value's path, the squares once more
     and the fp32 product x * scale1 once (U32 |x|, 2 U32 x^2); the 8 partials of a thread, the CTA's shared-memory sum and
-    the atomics per chunk are fp64."""
+    the atomics per chunk are fp64.  HW (default: the sources' pixels) is the image's pixel count when the sources are
+    one band of its pixels: the results then add up over the bands."""
     x = gn_concat(src0, src1, scale1)
-    B, HW, C = x.shape
+    B, _, C = x.shape
+    HW = x.shape[1] if HW is None else HW
     if L is None:
         L = gn_stats_plan(C, HW)[2]
-    xg = x.reshape(B, HW, groups, C // groups)
+    xg = x.reshape(B, -1, groups, C // groups)
     s, q, t = xg.sum(dim=(1, 3)), (xg * xg).sum(dim=(1, 3)), xg.abs().sum(dim=(1, 3))
     c = (L + 3) * U32 + (HW + 2048) * U64
     return torch.stack((s, q), dim=-1), torch.stack((c * t, c * q), dim=-1)
@@ -712,10 +715,12 @@ def group_sums(stats0, C0, groups, stats1=None, C1=0, scale1=1.0, sb=16):
     return blocks.reshape(B, groups, -1, 2).sum(dim=2)
 
 
-def _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, fast):
-    """y = SiLU(((x - mean) rstd gamma + beta) (scale + 1) + shift) in float64 from the statistics `sums` [B, G, 2], and
-    the bound of the kernel's fp32 y before any fp16 rounding.  See gn_apply_silu_ref."""
-    B, HW, C = x.shape
+def _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, fast, HW=None):
+    """y = SiLU(((x - mean) rstd gamma + beta) (scale + 1) + shift) in float64 from the statistics `sums` [B, G, 2] over
+    HW pixels per image (default: x's), and the bound of the kernel's fp32 y before any fp16 rounding.  See
+    gn_apply_silu_ref."""
+    B, _, C = x.shape
+    HW = x.shape[1] if HW is None else HW
     Cg = C // groups
     n = Cg * HW
     dev = x.device
@@ -752,12 +757,12 @@ def _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, fast):
 
 
 def gn_apply_silu_ref(src0, groups, gamma, beta, ss, eps, sums, sums_err=None, src1=None, scale1=1.0, out16=False,
-                      fast=None):
+                      fast=None, HW=None):
     """mi_gn_apply_silu: y = SiLU(GroupNorm(x) (scale + 1) + shift) over the virtual concat x = cat(src0, src1 * scale1)
     [B, HW, C], ss [B, 2C] = [scale | shift] (a view without the row gaps) or None.  `sums` [B, G, 2] are the statistics the
     reference normalises with; `sums_err` (optional) bounds how far the kernel's statistics are from them.  Returns the
     reference and the bound of the output (fp16 when out16).  fast: the __expf / __fdividef SiLU the kernel uses for fp16
-    outputs (default: out16).
+    outputs (default: out16).  HW: the image's pixel count when the sources are one band of its pixels (default: theirs).
 
     (a) Exact statistics (sums_err None): the kernel casts mean and rstd to fp32 and folds
             a = rstd gamma,  bb = beta - mean a,  a *= sc,  bb = bb sc + shift,  v = fmaf(x, a, bb),
@@ -772,7 +777,7 @@ def gn_apply_silu_ref(src0, groups, gamma, beta, ss, eps, sums, sums_err=None, s
         dvar = e_sq / n + (2 |mean| + dm) dm -- relative to var that grows with (|mean| / std)^2 -- and rstd by
         |1/sqrt(V - dvar) - 1/sqrt(V)| (V = var + eps); v moves by |gamma sc| (|x - mean| drstd + (rstd + drstd) dm)."""
     x = gn_concat(src0, src1, scale1)
-    y, bound = _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, out16 if fast is None else fast)
+    y, bound = _gn_silu(x, groups, gamma, beta, ss, eps, sums, sums_err, out16 if fast is None else fast, HW)
     return half_out(y, bound) if out16 else (y, bound)
 
 

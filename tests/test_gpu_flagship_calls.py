@@ -1,23 +1,28 @@
-"""Every kernel call of the flagship workload at the benchmark's size against float64: the cfg-3 super-resolution U-Net
-(`Unet(**Super.defaults, lowres_cond=True, text_embed_dim=768)`) at 256 x 256 with b = 32, as `bench.py` runs it.
+"""Every kernel call of the workloads bench.py reports, at the benchmark's sizes, against float64: the flagship cfg-3
+super-resolution U-Net (`Unet(**Super.defaults, lowres_cond=True, text_embed_dim=768)`) at 256 x 256 with b = 32, and the
+secondary rows cfg 2b, cfg 4's base stage and cfg 5, each as `bench.workload` defines it.
 
 test_gpu_lowering_calls.py checks every call of a forward at 32 - 64 px with b <= 16.  `conv_tc_launch` (csrc/conv_tc.cu)
 picks the conv schedule from the problem size and the SM count, so those sizes never reach the schedules that carry the
 benchmark's conv time: the 256-wide cooperative tiles, the transposed C_out = 128 schedule and the 128-wide ping-pong tiles
 (at b = 2 nearly every conv steps down to 64-wide tiles, and at 64 px the deepest level runs on the fp32 direct conv).  Here:
 
-  * test_every_call_of_the_cfg3_forward_at_benchmark_size: the conditional and the null pass of one guided step through
-    `CheckingOps` (tests/checking_ops.py), with the assertions of test_every_call_of_a_forward.  A Python restatement of
-    the schedule choice (`conv_schedule`) names the kernel instance of every conv call, and one profiler session over the
-    whole checked run counts the conv_wg_kernel launches per instance: the two counts must agree, so the per-schedule
-    table (calls, worst |err| / bound) is about the schedules that actually ran;
+  * test_every_call_of_the_cfg3_forward_at_benchmark_size, test_every_call_of_a_secondary_forward_at_benchmark_size[row]:
+    one forward of each bench.py row (FORWARDS: cfg 3's conditional and null pass; cfg 2b at b = 64; cfg 4's base stage
+    as one cfg_batched 2 x 64 batch, half of it on the null-text rows; cfg 5 at b = 2, 1024 x 1024) through
+    `CheckingOps` (tests/checking_ops.py), with the assertions of
+    test_every_call_of_a_forward, and the routes the row exists for.  A Python restatement of the schedule choice
+    (`conv_schedule`) names the kernel instance of every conv call, and one profiler session over the whole checked run
+    counts the conv_wg_kernel launches per instance: the two counts must agree, so the per-schedule table (calls, worst
+    |err| / bound) is about the schedules that actually ran;
   * test_step_epilogue_many_cluster_waves: the step epilogue at B = 32 and 64 -- the fused cluster kernel (8 CTAs per
-    image) then launches several waves of clusters -- and the three-kernel form, against float64, with non-finite images
-    past the first wave;
-  * test_one_cfg3_sampling_step_at_benchmark_size: Imagen.sample's eager loop at b = 32, the loop's own kernels checked.
+    image) then launches several waves of clusters -- and the three-kernel form, at cfg 5's n = 3 x 1024^2 too, against
+    float64, with non-finite images past the first wave;
+  * test_one_cfg3_sampling_step_at_benchmark_size, test_two_cfg5_sampling_steps_at_benchmark_size: Imagen.sample's eager
+    loop (64 -> 256 px at b = 32; 256 -> 1024 px at b = 2), the loop's own kernels checked.
 
-The float64 references of the image-sized calls are computed a few images at a time (checking_ops._image_slices).  Each
-test prints its wall time and peak device memory.
+The float64 references of the image-sized calls are computed a few images, or at 1024 px a band of rows, at a time
+(checking_ops._bands).  Each test prints its wall time and peak device memory.
 """
 import collections
 import inspect
@@ -40,11 +45,6 @@ pytestmark = pytest.mark.gpu
 
 INT32_MAX = 2 ** 31 - 1
 TRANSPOSED, COOP256, PINGPONG128 = (256, False, True), (256, False, False), (128, False, False)
-
-
-def _cfg3():
-    from minimagen_b200.Unet import Super
-    return dict(Super.defaults, lowres_cond=True, text_embed_dim=768)
 
 
 # ------------------------------------------------------------------------------------------------ schedule restatement
@@ -168,10 +168,33 @@ def _profiled_launches(fn):
 
 
 # ------------------------------------------------------------------------------------------------ the forward
-def test_every_call_of_the_cfg3_forward_at_benchmark_size(native):
+# bench.py row -> (workload, batch, how the batch runs, the routes the case exists for: CheckingOps features)
+FORWARDS = {
+    # the headline: the conditional and the null pass of one guided step
+    "cfg3": ("cfg3", 32, "guided", set()),
+    # Base.defaults at dim 128: C_out = 384 convs, LayerNorm rows of 384 (the generic ln_rows kernel), the 8x8 level's
+    # 128-pixel tiles spanning two images
+    "cfg2b": ("cfg2b", 64, "one pass", {"conv_igemm c_out=384", "ln_rows C=384", "conv_igemm multi-image tiles"}),
+    # cfg 4's base stage: the cfg-2a U-Net with both halves of a guided step in one 2B = 128 batch (Imagen.cfg_batched), the
+    # second half on the null-text rows; its 4096-token self-attention at B = 128
+    "cfg4_base": ("cfg2a", 64, "cfg_batched", {"attention B=128 n=4096", "text_tokens null rows B=128"}),
+    # cfg 5 as measure_config(per_gpu=16, micro=2, cond_scale=1) runs it: 1024-wide rows, the 2048 + 2048-channel concat
+    # convs at 64x64 (K = 36 864), the 4096-token self-attention and its LayerNorm rows at 2048 channels
+    "cfg5": ("cfg5", 2, "one pass", {"conv_igemm W=1024", "conv_igemm K=36864", "attention B=2 n=4096", "ln_rows C=2048"}),
+}
+
+
+def _check_forward(native, row):
+    """Every call of one forward of a bench.py row at the row's size (bench.workload: config, image size, text width)
+    through CheckingOps, with the schedule restatement checked against the profiler's launch counts; the case must reach
+    the routes it is listed for."""
+    import bench
     import minimagen_b200.ops as ops_mod
     from minimagen_b200.Unet import Unet
-    cfg, s, b = _cfg3(), 256, 32
+    name, b, how, routes = FORWARDS[row]
+    wl = bench.workload(name)
+    cfg, s = wl["cfg"], wl["size"]
+    assert cfg["text_embed_dim"] == wl["E"]
     props = torch.cuda.get_device_properties(0)
     sms = props.multi_processor_count
     torch.manual_seed(0)
@@ -179,14 +202,21 @@ def test_every_call_of_the_cfg3_forward_at_benchmark_size(native):
     x, t, kw = _inputs(cfg, s, b)
     tm = kw["text_mask"]
     tm[b // 2, 11:] = False                                 # ragged rows besides _inputs' last one, one with a single token
-    tm[3, 1:] = False
+    tm[min(3, b - 1), 1:] = False
 
     def run():
         proxy = CheckingOps(native)
         log = ScheduleLog(proxy, sms)
         ops_mod.set_ops(log)                                # the `native` fixture restores the previous backend afterwards
         with torch.no_grad():
-            out = u.forward_with_cond_scale(x, t, cond_scale=3., **kw)     # the conditional and the null pass
+            if how == "guided":
+                out = u.forward_with_cond_scale(x, t, cond_scale=3., **kw)   # the conditional and the null pass
+            elif how == "cfg_batched":
+                two = lambda v: torch.cat((v, v))
+                keep = torch.cat((torch.ones(b, dtype=torch.uint8), torch.zeros(b, dtype=torch.uint8))).cuda()
+                out = u._forward_impl(two(x), two(t), cond_keep=keep, **{k: two(v) for k, v in kw.items()})
+            else:
+                out = u(x, t, **kw)
         return out, proxy, log
 
     torch.cuda.synchronize()
@@ -197,14 +227,15 @@ def test_every_call_of_the_cfg3_forward_at_benchmark_size(native):
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
     assert torch.isfinite(out).all()
     n_acc = proxy.assert_accumulators_disjoint()
-    print(f"\ncfg 3 U-Net, b = {b} at {s}x{s}, conditional + null pass on {props.name} ({sms} SMs): {dt:.1f} s under the "
+    passes = 2 if how == "guided" else 1
+    print(f"\n{row} U-Net ({name}), b = {b} at {s}x{s}, {how} on {props.name} ({sms} SMs): {dt:.1f} s under the "
           f"profiler, peak {peak:.1f} GiB allocated, {n_acc} statistics accumulators (zero when handed out, disjoint)")
     proxy.report()
     predicted = log.counts()
     print("  conv schedule                      calls   worst |err|/bound   profiler launches   per forward")
     for inst in sorted(set(predicted) | set(launches), key=lambda i: (-i[2], -i[0], i[1])):
         calls, worst = log.per.get(inst, (0, 0.0))
-        print(f"  {instance_name(inst):32s} {calls:7d}   {worst:17.3g}   {launches[inst]:17d}   {calls / 2:11g}")
+        print(f"  {instance_name(inst):32s} {calls:7d}   {worst:17.3g}   {launches[inst]:17d}   {calls / passes:11g}")
     if "conv_direct" in proxy.family:
         calls, worst = proxy.family["conv_direct"]
         print(f"  {'fp32 direct':32s} {calls:7d}   {worst:17.3g}")
@@ -212,8 +243,20 @@ def test_every_call_of_the_cfg3_forward_at_benchmark_size(native):
     assert not unchecked, f"kernels that ran without a float64 check: {sorted(unchecked)}"
     assert {"conv_igemm", "gn_apply_silu", "attention", "ln_rows", "linear_f32"} <= proxy.checked
     assert launches == predicted, f"profiler {dict(launches)} vs restatement {dict(predicted)}"
+    missing = routes - proxy.features
+    assert not missing, f"routes not reached: {sorted(missing)}; reached: {sorted(proxy.features)}"
+    return sms, launches
+
+
+def test_every_call_of_the_cfg3_forward_at_benchmark_size(native):
+    sms, launches = _check_forward(native, "cfg3")
     if sms == 132:
         assert {TRANSPOSED, COOP256, PINGPONG128} <= set(launches), "a schedule of the benchmark was not reached"
+
+
+@pytest.mark.parametrize("row", [r for r in FORWARDS if r != "cfg3"])
+def test_every_call_of_a_secondary_forward_at_benchmark_size(native, row):
+    _check_forward(native, row)
 
 
 # ------------------------------------------------------------------------------------------------ the step epilogue
@@ -227,16 +270,20 @@ def _step_call(native, multi, x, eps, eps0, w, t, tabs, noise, hist, lo, hi, wt,
         native.step_epilogue(x, eps, eps0, w, t, a, b_, c1, c2, sigma, noise, B, n, lo, hi, wt, 1.0, out, s_out=s)
 
 
+CFG5_N = 3 * 1024 * 1024                                    # one cfg-5 image: 3 x 1024 x 1024, 16 x FUSED_MAX
+
+
 @pytest.mark.parametrize("kind", ["ddpm", "dpmpp"])
-@pytest.mark.parametrize("n", [FUSED_MAX, FUSED_MAX + 1])
-@pytest.mark.parametrize("B", [32, 64])
+@pytest.mark.parametrize("B,n", [(32, FUSED_MAX), (32, FUSED_MAX + 1), (64, FUSED_MAX), (64, FUSED_MAX + 1), (2, CFG5_N),
+                                 (16, CFG5_N)])
 def test_step_epilogue_many_cluster_waves(native, B, n, kind):
     """At n = FUSED_MAX the fused cluster kernel runs B clusters of 8 CTAs, several waves at B = 32 and 64; n + 1 takes
-    the three-kernel form.  out, s and the history against float64 (test_step_epilogue_bounds' references and bounds) for
-    scalar and per-image guidance weights, out separate from x_t and aliasing it; s bit for bit torch.quantile of step_x0's
-    output.  Then images B - 4 (one NaN), B - 3 (15 % +inf) and B - 2 (two +-inf), past the first wave, must give the NaN
-    pattern the torch restatement gives (as test_step_nan_and_inf_parity at B = 4), and the clean images the bits of a run
-    without them."""
+    the three-kernel form, and so does cfg 5's n = 3 x 1024^2 (at its benchmark batch, 2, and at 16).  out, s and the
+    history against float64 (test_step_epilogue_bounds' references and bounds) for scalar and per-image guidance weights,
+    out separate from x_t and aliasing it; s bit for bit torch.quantile of step_x0's output.  Then (B >= 4) images B - 4
+    (one NaN), B - 3 (15 % +inf) and B - 2 (two +-inf), past the first wave, must give the NaN pattern the torch
+    restatement gives (as test_step_nan_and_inf_parity at B = 4), and the clean images the bits of a run without them."""
+    assert n <= 2 ** 24, "torch.quantile, the reference of s, takes rows of up to 2^24 elements"
     from minimagen_b200.Imagen import quantile_rank
     tabs, grid = _tabs_cuda(kind)
     multi = kind == "dpmpp"
@@ -275,6 +322,9 @@ def test_step_epilogue_many_cluster_waves(native, B, n, kind):
             native.step_x0(xc, ec, e0c, w, tc, tabs[0], tabs[1], B, n, x0n)
             assert torch.equal(s.cpu(), torch.quantile(x0n.abs().cpu(), 0.9, dim=-1).clamp(min=1.0)), f"{what}: s not exact"
 
+    if B < 4:
+        print(f"{kind} B={B} n={n}: {time.time() - t0:.1f} s")
+        return
     # non-finite images past the first wave of clusters
     xb, eb = x.clone(), eps.clone()
     eb[B - 4, n // 2] = float("nan")
@@ -311,26 +361,28 @@ LOOP = {"step_epilogue", "step_epilogue_multistep", "step_advance_t", "step_adva
         "resize_separable", "q_sample"}
 
 
-def test_one_cfg3_sampling_step_at_benchmark_size(native):
-    """Imagen.sample(start_at_unet_number=2) from random 64 x 64 images, two DDIM steps with guidance w = 3, eager (a loop
-    of two steps is not captured): the loop's own kernels -- the cascade resize of the start images, q_sample of the low-res
-    conditioning, the step epilogue, the finalize -- checked against float64; the U-Net calls run unchecked (see the
-    forward test above)."""
+def _two_sampling_steps(native, name, b):
+    """Imagen.sample(start_at_unet_number=2) with the bench.py row's U-Net as the second stage, from random images of the
+    first stage's size, two DDIM steps with guidance w = 3, eager (a loop of two steps is not captured): the loop's own
+    kernels -- the cascade resize of the start images, q_sample of the low-res conditioning, the step epilogue, the
+    finalize -- checked against float64; the U-Net calls run unchecked (see the forward test above)."""
+    import bench
     import minimagen_b200.ops as ops_mod
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import BaseTest, Unet
-    b = 32
+    wl = bench.workload(name)
+    size, low = wl["size"], wl["size"] // 4
     torch.manual_seed(0)
-    u = Unet(**_cfg3()).eval()
-    first = Unet(**dict(BaseTest.defaults, text_embed_dim=768)).eval()
-    im = Imagen(unets=(first, u), text_encoder_name="t5_base", image_sizes=(64, 256), timesteps=1000,
+    u = Unet(**wl["cfg"]).eval()
+    first = Unet(**dict(BaseTest.defaults, text_embed_dim=wl["E"])).eval()
+    im = Imagen(unets=(first, u), text_encoder_name="t5_base", image_sizes=(low, size), timesteps=1000,
                 cond_drop_prob=0.1).eval().cuda()
     im.use_cuda_graph = False
     g = torch.Generator().manual_seed(11)
-    te = torch.randn(b, 20, 768, generator=g).cuda()
+    te = torch.randn(b, 20, wl["E"], generator=g).cuda()
     tm = torch.ones(b, 20, dtype=torch.bool)
     tm[-1, 5:] = False
-    start = torch.rand(b, 3, 64, 64, generator=g).cuda()
+    start = torch.rand(b, 3, low, low, generator=g).cuda()
     proxy = CheckingOps(native, only=LOOP)
     ops_mod.set_ops(proxy)                                  # the `native` fixture restores the previous backend afterwards
     torch.cuda.synchronize()
@@ -339,9 +391,19 @@ def test_one_cfg3_sampling_step_at_benchmark_size(native):
     out = im.sample(text_embeds=te, text_masks=tm.cuda(), cond_scale=3., sampling_timesteps=2, start_at_unet_number=2,
                     start_images=start)
     torch.cuda.synchronize()
-    print(f"\ntwo cfg-3 sampling steps, b = {b}: {time.time() - t0:.1f} s, peak "
+    print(f"\ntwo {name} sampling steps, b = {b}, {low} -> {size} px: {time.time() - t0:.1f} s, peak "
           f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB allocated")
     proxy.report()
-    assert tuple(out.shape) == (b, 3, 256, 256) and torch.isfinite(out).all()
+    assert tuple(out.shape) == (b, 3, size, size) and torch.isfinite(out).all()
     assert proxy.family["step_epilogue"][0] == 2
     assert {"step_epilogue", "step_finalize", "resize_separable", "q_sample"} <= proxy.checked
+
+
+def test_one_cfg3_sampling_step_at_benchmark_size(native):
+    _two_sampling_steps(native, "cfg3", 32)
+
+
+def test_two_cfg5_sampling_steps_at_benchmark_size(native):
+    """cfg 5's loop at its benchmark batch: the resize 256 -> 1024 and images of n = 3 x 1024^2 in the step epilogue's
+    three-kernel form."""
+    _two_sampling_steps(native, "cfg5", 2)
