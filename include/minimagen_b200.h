@@ -85,7 +85,10 @@ int mi_pack_conv_weight_dgrad_f16(const float* w_oihw, int c_out, int c_in, int 
  *             schedule (128 channels x 256 pixels of one image per tile; needs out_sc = 1, n_valid = c_out and a grid
  *             that tiles by 256 pixels inside an image, else auto), which auto also picks when it gives every SM a tile
  *   workspace reserved, pass NULL / 0
- * Requirements: c_in % 64 == 0, c_out % 16 == 0, W a power of two >= 8 (or W >= 128), see mi_conv2d_igemm_supported.
+ * Requirements: c_in % 64 == 0, c_out % 16 == 0, and W >= 128, or a power of two >= 8, or a multiple of 8 whose largest
+ * power-of-two divisor BW gives 128 / BW rows dividing H (W = 96, 48, 24 at H % 4, 8, 16 == 0); see
+ * mi_conv2d_igemm_supported.  Tiles are BW x BH pixel boxes of one image where such a box tiles it exactly (any other
+ * W >= 128 masks the last tile of each row).
  * A plain GEMM  out[M][N] = act[M][K] * w[N][K]^T  is the case B=1, H=1, W=M, kh=kw=1. */
 int mi_conv2d_igemm_supported(int H, int W, int c_in, int c_out);
 int mi_conv2d_igemm_f16(const void* act_f16, int B, int H, int W, int lda, int c_off, int c_in, const void* act2_f16,

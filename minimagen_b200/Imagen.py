@@ -9,7 +9,7 @@ nothing on the host.  Sampling captures three graph flavours: text-only (one gra
 step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).  The guidance weights are per-image
 data in a static buffer, so every flavour's graph serves every `cond_scale` and every negative prompt of its shape.
 
-Nine additions that the reference does not have (all optional, defaults reproduce the reference):
+Ten additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -37,7 +37,11 @@ Nine additions that the reference does not have (all optional, defaults reproduc
     guidance_schedule='linear' or 'cosine')`, Kynkaanniemi et al. 2024; Wang et al. 2024): a per-stage fp32 table s[t]
     (GaussianDiffusion.guidance_table) scales each image's w - 1 at timestep t (mi_step_epilogue_ws), and a grid point
     with s[t] = 0 runs without the guidance pass, one U-Net evaluation.  A captured stage keeps a guided and an unguided
-    graph over the same static buffers and replays the one each grid point needs.
+    graph over the same static buffers and replays the one each grid point needs;
+  * non-square images (`sample(..., image_sizes=((h1, w1), (h2, w2)))`): each stage samples (b, c, h, w) at its own size,
+    all with one aspect ratio, and every image argument follows the stage shape.  The implicit-GEMM convolutions tile a
+    width that is a multiple of 8 but not a power of two with exact BW x BH one-image boxes (csrc/conv_tc.cu tile_box), so
+    a 64 x 96 or 256 x 384 stage stays on the tensor cores.  Training keeps the reference's square resize.
 
 `noise_fn` kinds: 'init' (x_T, step -1; with an init image k, the noise z of the start sqrt(a_t0) k + sqrt(1 - a_t0) z,
 t0 the walk's first point), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
@@ -739,7 +743,7 @@ class Imagen(nn.Module):
                inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim', init_images=None,
                skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None,
                negative_texts=None, negative_text_embeds=None, negative_text_masks=None, seed=None,
-               guidance_interval=None, guidance_schedule=None):
+               guidance_interval=None, guidance_schedule=None, image_sizes=None):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -748,6 +752,14 @@ class Imagen(nn.Module):
         timesteps) samples a stage with S DDIM steps over round(linspace(0, T-1, S)) instead of all T DDPM steps;
         `ddim_eta` in [0, 1] scales their noise (0: deterministic given x_T; 1 at S = T: the DDPM sampler).  None (the
         default) runs the DDPM loop.
+        `image_sizes` (None, or one entry per U-Net, each an int s or a pair (h, w)) sets the size each stage samples at;
+        None keeps the constructor's square `image_sizes`.  Only the stages that run are read: their h and w must be
+        positive multiples of the U-Net's downsampling factor (2 to the number of its Downsample convs), and they must
+        share one aspect ratio (h_i * w_j == h_j * w_i), so every inter-stage resize scales both axes alike.  A level whose
+        width is a multiple of 8 runs the tensor-core convolutions on exact BW x BH tiles (csrc/conv_tc.cu tile_box); one
+        whose width is not (e.g. the 12- and 6-pixel levels of a 64 x 96 memory-efficient U-Net) runs the fp32 direct
+        convolution there.  The image arguments below then have the run's aspect ratio instead of being square: "s, s"
+        reads "h, w".
         `inpaint_images` (b, channels, s, s) float in `input_image_range` and `inpaint_masks` (b, s, s) bool, given
         together (b: the full batch of the text conditioning), inpaint: True marks a pixel kept from `inpaint_images`,
         False one the model generates.  Every stage resizes both to its size (known where the resized mask >= 0.5) and
@@ -764,7 +776,8 @@ class Imagen(nn.Module):
         length; k > 0 needs an init image) and starts from the init image noised to grid[k]; 2M restarts at first order
         there.  `start_at_unet_number` and `stop_at_unet_number` (default: the last U-Net) run the stages in between
         only and return the last one's output; `start_images` ((b, channels, s, s) float in `input_image_range`, any
-        square size, required if and only if start_at_unet_number > 1) stand in for the output of the stage before the
+        size of the run's aspect ratio, required if and only if start_at_unet_number > 1) stand in for the output of the
+        stage before the
         first one, e.g. to super-resolve the caller's own images.
         `cond_scale`, the classifier-free guidance weight w, is a number, a 1-D float tensor of b per-image weights (e.g.
         a guidance sweep in one batch), or one entry per U-Net, each such a number or tensor; every entry must be finite.
@@ -835,6 +848,7 @@ class Imagen(nn.Module):
         for i, sched in enumerate(guidance[1], 1):
             assert sched in (None, 'linear', 'cosine'), \
                 f"guidance_schedule of unet {i} must be None, 'linear' or 'cosine', got {sched!r}"
+        sizes = self._stage_sizes(image_sizes, start_at_unet_number, stop_at_unet_number)
         for i in range(start_at_unet_number, stop_at_unet_number + 1):
             k, walk_len = default(skips[i - 1], 0), default(steps[i - 1], self.noise_schedulers[i - 1].num_timesteps)
             assert _is_int(k) and 0 <= k < walk_len, \
@@ -863,7 +877,36 @@ class Imagen(nn.Module):
             return self._sample_impl(texts, text_masks, text_embeds, scales, lowres_sample_noise_level,
                                      return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler,
                                      init_images, skips, start_at_unet_number, stop_at_unet_number, start_images,
-                                     negative, seed, guidance)
+                                     negative, seed, guidance, sizes)
+
+    @staticmethod
+    def downsample_factor(unet):
+        """2 to the number of stride-2 (Downsample) convs in `unet.downs`: the factor by which its deepest level is
+        smaller than the image, which both sides of a sampled size must be multiples of."""
+        return 2 ** sum(1 for m in unet.downs.modules() if isinstance(m, nn.Conv2d) and tuple(m.stride) == (2, 2))
+
+    def _stage_sizes(self, image_sizes, start, stop):
+        """(h, w) per U-Net: the constructor's squares, or `image_sizes` (an int s or a pair (h, w) per U-Net) validated
+        for the stages start..stop that run; the entries of the others are not read (None)."""
+        n = len(self.unets)
+        if image_sizes is None:
+            return tuple((s, s) for s in self.image_sizes)
+        assert isinstance(image_sizes, (list, tuple)) and len(image_sizes) == n, \
+            f'image_sizes must have one entry per unet ({n}), got {image_sizes!r}'
+        sizes = [None] * n
+        for i in range(start, stop + 1):
+            v = image_sizes[i - 1]
+            pair = isinstance(v, (list, tuple)) and len(v) == 2 and all(map(_is_int, v))
+            assert _is_int(v) or pair, f'image size of unet {i} must be an int or a pair (h, w), got {v!r}'
+            h, w = (v, v) if _is_int(v) else (int(v[0]), int(v[1]))
+            f = self.downsample_factor(self.unets[i - 1])
+            assert h > 0 and w > 0 and h % f == 0 and w % f == 0, \
+                f'image size of unet {i} must be positive multiples of its downsampling factor {f}, got {h} x {w}'
+            h0, w0 = sizes[start - 1] if i > start else (h, w)
+            assert h * w0 == w * h0, \
+                f'the unets that run must share one aspect ratio: unet {i} samples {h} x {w}, unet {start} {h0} x {w0}'
+            sizes[i - 1] = (h, w)
+        return tuple(sizes)
 
     def _check_seed(self, seed):
         """`seed`: an int >= 0, or a non-empty list or 1-D integer tensor of seeds in [0, 2^63); never with noise_fn."""
@@ -911,12 +954,16 @@ class Imagen(nn.Module):
         assert len(value) == n, f'{name} must have one entry per unet ({n}), got {len(value)}'
         return tuple(value)
 
-    def _check_images(self, images, b, name):
-        """`images` must be a (b, channels, s, s) float tensor (b: the full batch of the text conditioning)."""
+    def _check_images(self, images, b, name, aspect=(1, 1)):
+        """`images` must be a (b, channels, h, w) float tensor with h:w = `aspect` ((1, 1): square; b: the full batch of
+        the text conditioning)."""
         assert torch.is_tensor(images) and images.is_floating_point(), f'{name} must be a float tensor'
-        assert images.dim() == 4 and tuple(images.shape[:2]) == (b, self.channels) and \
-            images.shape[2] == images.shape[3], \
-            f'{name} must be (b, channels, s, s) = ({b}, {self.channels}, s, s), got {tuple(images.shape)}'
+        ok = images.dim() == 4 and tuple(images.shape[:2]) == (b, self.channels) and \
+            images.shape[2] * aspect[1] == images.shape[3] * aspect[0]
+        if aspect[0] == aspect[1]:
+            assert ok, f'{name} must be (b, channels, s, s) = ({b}, {self.channels}, s, s), got {tuple(images.shape)}'
+        assert ok, f'{name} must be (b, channels, h, w) = ({b}, {self.channels}, h, w) with h:w = {aspect[0]}:' \
+                   f'{aspect[1]} (the aspect ratio of the stages that run), got {tuple(images.shape)}'
 
     def _negative_prompt(self, negative, b, device):
         """(negative_text_embeds, negative_text_masks) with b rows on `device` (None, None without a negative prompt)."""
@@ -961,7 +1008,7 @@ class Imagen(nn.Module):
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
                      device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim', init_images=None,
                      skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None), seed=None,
-                     guidance=None):
+                     guidance=None, sizes=None):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -970,22 +1017,27 @@ class Imagen(nn.Module):
         assert not (exists(text_embeds) and text_embeds.shape[-1] != self.text_embed_dim), \
             f'invalid text embedding dimension being passed in (should be {self.text_embed_dim})'
         b = text_embeds.shape[0]
+        n_stages = len(self.unets)
+        stop_at = default(stop_at, n_stages)
+        sizes = default(sizes, tuple((s, s) for s in self.image_sizes))
+        g = math.gcd(*sizes[start_at - 1])
+        aspect = (sizes[start_at - 1][0] // g, sizes[start_at - 1][1] // g)
         inpaint_images = inpaint_masks = None
         if exists(inpaint):
             inpaint_images, inpaint_masks, resample_times = inpaint
-            self._check_images(inpaint_images, b, 'inpaint_images')
-            s = inpaint_images.shape[-1]
+            self._check_images(inpaint_images, b, 'inpaint_images', aspect)
+            h, w = inpaint_images.shape[-2:]
             assert torch.is_tensor(inpaint_masks) and inpaint_masks.dtype == torch.bool, \
                 'inpaint_masks must be a bool tensor'
-            assert tuple(inpaint_masks.shape) == (b, s, s), \
-                f'inpaint_masks must be (b, s, s) = ({b}, {s}, {s}), got {tuple(inpaint_masks.shape)}'
-        n_stages = len(self.unets)
+            assert tuple(inpaint_masks.shape) == (b, h, w), \
+                (f'inpaint_masks must be (b, s, s) = ({b}, {h}, {w}), got {tuple(inpaint_masks.shape)}' if h == w else
+                 f'inpaint_masks must be (b, h, w) = ({b}, {h}, {w}) like inpaint_images, got {tuple(inpaint_masks.shape)}')
         init_images = default(init_images, (None,) * n_stages)
         for i, init in enumerate(init_images, 1):
             if exists(init):
-                self._check_images(init, b, f'init_images of unet {i}')
+                self._check_images(init, b, f'init_images of unet {i}', aspect)
         if exists(start_images):
-            self._check_images(start_images, b, 'start_images')
+            self._check_images(start_images, b, 'start_images', aspect)
         scales = self._per_unet(cond_scale, 'cond_scale')
         for i, w in enumerate(scales, 1):
             self._check_scale(w, b, i)
@@ -1025,11 +1077,10 @@ class Imagen(nn.Module):
             # what the finalize of stage start_at - 1 would have left: images in input_image_range
             img = start_images.to(device=device, dtype=F32).clamp(*self.input_image_range).contiguous()
         gathered = None
-        stop_at = default(stop_at, n_stages)
         steps = default(steps, (None,) * n_stages)
         skips = default(skips, (0,) * n_stages)
         intervals, gscheds = default(guidance, ((None,) * n_stages, (None,) * n_stages))
-        stages = list(zip(range(1, n_stages + 1), self.unets, self.sample_channels, self.image_sizes,
+        stages = list(zip(range(1, n_stages + 1), self.unets, self.sample_channels, sizes,
                           self.noise_schedulers, steps, init_images, skips, scales, intervals,
                           gscheds))[start_at - 1:stop_at]
         for (unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip, stage_scale, interval,
@@ -1048,7 +1099,7 @@ class Imagen(nn.Module):
                                  sch.sqrt_one_minus_alphas_cumprod, batch_size, lowres_cond_img[0].numel(), 1.0, 0.0,
                                  noised)
                     lowres_cond_img = noised
-                shape = (batch_size, self.channels, image_size, image_size)
+                shape = (batch_size, self.channels, *image_size)
                 slot = None
                 if distributed and world > 1 and unet_number == stop_at:
                     # the last stage finalises straight into this rank's slot of the all-gather buffer (no staging copy)

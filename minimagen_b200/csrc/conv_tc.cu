@@ -30,7 +30,7 @@
 //
 // Transposed schedule (C_out = 128, TR): D^T[128 channels, pixels] = Wp . A^T runs on the cooperative 256-wide kernel
 // unchanged but for the producer and the epilogue.  The weight box (64 K x 128 channels) fills the 16 KiB stage slot and
-// is the wgmma A operand; a 256-pixel activation box (BW = 256, or BW = W and BH = 256 / W, one image) fills the 32 KiB
+// is the wgmma A operand; a 256-pixel activation box (BW x BH = 256 of one image, tile_box) fills the 32 KiB
 // slot and is B.  Consumer cw owns output channels [64 cw, 64 cw + 64) of 256 pixels, so a C_out = 128 conv moves the
 // operand bytes per FLOP of a 128x256 tile instead of a 128x128 one.  Its epilogue stores channel-strided from the
 // fragments (8 channels x 4 pixels per warp store) and, every value of a warp being in one 16-channel block of one image,
@@ -590,11 +590,26 @@ int num_sms_of_current_device() {
     return n;
 }
 
-// tile box of tile_pix (128, or 256 for the transposed schedule) pixels: BW x BH pixels x BB images
-void tile_geometry(int H, int W, int B, int tile_pix, ConvTcArgs& a) {
-    int BW = W >= tile_pix ? tile_pix : W;
-    int BH = tile_pix / BW;
+// Tile box of tile_pix (128, or 256 for the transposed schedule) pixels: BW x BH pixels x BB images, BW and BH powers of
+// two.  W a power of two or a multiple of tile_pix: BW = min(W, tile_pix), BH = tile_pix / BW (at most H; a short image
+// spans BB images).  Any other W that is a multiple of 8 and whose largest power-of-two divisor BW (< tile_pix) gives
+// BH = tile_pix / BW rows dividing H: exact one-image tiles of that box (W = 96: 32 x 4; 48: 16 x 8; 24: 8 x 16 at 128
+// pixels).  Otherwise BW = tile_pix, BH = 1 and the last tile of every row is masked (W > tile_pix only).
+void tile_box(int H, int W, int tile_pix, int& BW, int& BH) {
+    const int low = W & -W;                                  // largest power of two dividing W
+    if (low != W && W % tile_pix != 0 && low >= 8 && H % (tile_pix / low) == 0) {
+        BW = low;
+        BH = tile_pix / low;
+        return;
+    }
+    BW = W >= tile_pix ? tile_pix : W;
+    BH = tile_pix / BW;
     if (BH > H) BH = H;
+}
+
+void tile_geometry(int H, int W, int B, int tile_pix, ConvTcArgs& a) {
+    int BW, BH;
+    tile_box(H, W, tile_pix, BW, BH);
     const int BB = tile_pix / (BW * BH);
     a.bw_log2 = ilog2_exact(BW);
     a.bh_log2 = ilog2_exact(BH);
@@ -659,9 +674,9 @@ CUresult encode_weights(PFN_encodeTiled enc, CUtensorMap* m, const void* ptr, cu
 // stride-2 read doubles them), and every channel stored channel-contiguous (its stores go 8 channels x 4 pixels a warp).
 bool transposed_ok(const ConvTcProblem& p, const ConvTcArgs& a) {
     if (p.Cout != 128 || a.n_valid != p.Cout || a.out_sc != 1) return false;
-    const int BW = p.W >= 256 ? 256 : p.W;
-    if (p.W % BW || ilog2_exact(BW) < 3 || BW * a.in_stride > 256) return false;
-    const int BH = 256 / BW;
+    int BW, BH;
+    tile_box(p.H, p.W, 256, BW, BH);
+    if (p.W % BW || ilog2_exact(BW) < 3 || BW * a.in_stride > 256 || BW * BH != 256) return false;
     // the epilogue addresses a tile's outputs with 32-bit offsets from its first pixel
     if (BH * a.out_sh + BW * a.out_sw + p.Cout > INT32_MAX) return false;
     return p.H % BH == 0 && BH * a.in_stride <= 256;
@@ -696,7 +711,8 @@ const char* conv_tc_strerror(int code) {
         case 0: return "ok";
         case -1: return "conv_tc: C_in (per tap) must be a positive multiple of 64";
         case -2: return "conv_tc: C_out must be a multiple of 16";
-        case -3: return "conv_tc: W must be a power of two >= 8 or a multiple of 128; H*W tiling unsupported";
+        case -3: return "conv_tc: W must be >= 128, a power of two >= 8, or a multiple of 8 whose largest power-of-two divisor BW gives " \
+                       "128 / BW rows dividing H";
         case -4: return "conv_tc: too many taps (max 16)";
         case -5: return "conv_tc: cuTensorMapEncodeTiled unavailable";
         case -6: return "conv_tc: tensor map encode failed (activations)";
@@ -711,8 +727,12 @@ const char* conv_tc_strerror(int code) {
 
 bool conv_tc_supported(int H, int W, int Cin, int Cout) {
     if (Cin <= 0 || Cin % kConvBlockK != 0 || Cout <= 0 || Cout % 16 != 0) return false;
-    if (W >= 128) return true;                            // BW = 128, BH = 1, BB = 1; ragged tail rows are masked
-    if (ilog2_exact(W) < 3) return false;                 // W in {8,16,32,64}
+    if (W >= 128) return true;                            // BW = 128, BH = 1, or an exact box (tile_box); else ragged
+    if (ilog2_exact(W) < 0) {                             // W % 8 == 0: BW = W & -W, BH = 128 / BW rows of one image
+        const int low = W & -W;
+        return W > 0 && low >= 8 && H % (128 / low) == 0;
+    }
+    if (W < 8) return false;                              // W in {8,16,32,64}
     const int bh = 128 / W;
     if (H >= bh) return H % bh == 0;                      // BH = 128 / W rows of one image
     return ilog2_exact(H) >= 0;                           // BH = H, the tile spans 128 / (W*H) images

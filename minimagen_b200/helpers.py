@@ -136,16 +136,26 @@ def resize_tables(n_in, scale, pad_mode, device):
 
 def resize_image_to(image, target_image_size, clamp_range=None, pad_mode='reflect'):
     """Inter-stage resize of the cascade (helpers.py:138-164 -> resize_right.resize; called at Imagen.py:482): one
-    separable-resampling kernel (mi_resize_separable) driven by the tap tables above."""
-    orig = image.shape[-1]
-    if orig == target_image_size:
-        return image
+    separable-resampling kernel (mi_resize_separable) driven by the tap tables above.  `target_image_size` is an int, as
+    in the reference (both axes scaled by target / width), or a pair (h, w): each axis gets its own scale, h / H and
+    w / W."""
+    if isinstance(target_image_size, (tuple, list)):
+        th, tw = map(int, target_image_size)
+        if tuple(image.shape[-2:]) == (th, tw):
+            return image
+        scale_h, scale_w = th / image.shape[-2], tw / image.shape[-1]
+    else:
+        orig = image.shape[-1]
+        if orig == target_image_size:
+            return image
+        scale_h = scale_w = target_image_size / orig
     from .ops import get_ops
-    scale = target_image_size / orig
     x = image.to(torch.float32).contiguous()
     B, C, H, W = x.shape
-    ho, iy, wy = resize_tables(H, scale, pad_mode, x.device)
-    wo, ix, wx = resize_tables(W, scale, pad_mode, x.device)
+    ho, iy, wy = resize_tables(H, scale_h, pad_mode, x.device)
+    wo, ix, wx = resize_tables(W, scale_w, pad_mode, x.device)
+    if isinstance(target_image_size, (tuple, list)):
+        assert (ho, wo) == (th, tw), f'resizing {H} x {W} to {th} x {tw} gives {ho} x {wo}'
     out = torch.empty((B, C, ho, wo), dtype=torch.float32, device=x.device)
     get_ops().resize_separable(x, B * C, H, W, out, ho, wo, iy, wy, ix, wx, clamp=clamp_range)
     return out
