@@ -295,6 +295,29 @@ int mi_step_epilogue_multistep_ws(const float* x_t, const float* eps_cond, const
                                   const float* noise, float* x0_hist, int B, int n, int rank_lo, int rank_hi,
                                   float weight, float min_s, float* out, float* s_out, float* x0_workspace,
                                   void* stream);
+/* Guidance rescale (Lin et al. 2024, sec. 3.4; Imagen.sample(guidance_rescale=)).  For image b with c = eps_cond[b],
+ * g = eps_null + (c - eps_null) * w_b(t[b]) (the guided prediction exactly as the _w / _ws entry points form it; w [B]
+ * required, w_sched [T] optional as in mi_step_epilogue_ws) and phi [B] fp32 in [0, 1]:
+ *   SS_c = sum (c - mean c)^2, SS_g = sum (g - mean g)^2   over the image's n values, in fp64,
+ *   f[b] = fp32(phi_b * sqrt(SS_c / SS_g) + (1 - phi_b))  evaluated in fp64 and rounded once; 1 where SS_g == 0, NaN
+ *   where the image has a NaN.
+ * Deterministic (fixed reduction order, no atomics): the same inputs give the same bits, eager or captured.  workspace:
+ * mi_guidance_rescale_workspace_doubles(B, n) doubles (8-byte aligned), caller-allocated. */
+long long mi_guidance_rescale_workspace_doubles(int B, int n);
+int mi_guidance_rescale_factor(const float* eps_cond, const float* eps_null, const float* w, const float* w_sched,
+                               const long long* t, const float* phi, int B, int n, float* f, double* workspace,
+                               void* stream);
+/* The guided step with the guided prediction rescaled per image: eps = fp32(g * f[b]) in place of g, everything after it
+ * (x0, threshold, posterior) as mi_step_epilogue_ws / mi_step_epilogue_multistep_ws.  Bit for bit mi_step_epilogue
+ * called with eps_cond = fp32(g * f) and eps_null = NULL.  eps_null, w [B] and f [B] are required; w_sched [T] is
+ * optional; c3 and x0_hist are given together (the multistep form) or both NULL.  Same workspace rule as
+ * mi_step_epilogue. */
+int mi_step_epilogue_rescaled(const float* x_t, const float* eps_cond, const float* eps_null, const float* w,
+                              const float* w_sched, const float* f, const long long* t,
+                              const float* x0_tab_a, const float* x0_tab_b, const float* c1, const float* c2,
+                              const float* sigma, const float* c3, const float* noise, float* x0_hist, int B, int n,
+                              int rank_lo, int rank_hi, float weight, float min_s, float* out, float* s_out,
+                              float* x0_workspace, void* stream);
 /* t[b] <- max(t[b] - 1, 0): the next iteration's timestep of Imagen._p_sample_loop (Imagen.py:398-415 walks the list of
  * diffusion_model.py:81-87), advanced on the device so that a captured step can be replayed back to back */
 int mi_step_advance_t(long long* t, int B, void* stream);

@@ -60,6 +60,9 @@ SIGNATURES = {
     "mi_step_epilogue_ws": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P, _P, _P, _P],
     "mi_step_epilogue_multistep_ws": [_P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F,
                                       _P, _P, _P, _P],
+    "mi_guidance_rescale_workspace_doubles": [_I, _I],
+    "mi_guidance_rescale_factor": [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P],
+    "mi_step_epilogue_rescaled": [_P] * 15 + [_I, _I, _I, _I, _F, _F, _P, _P, _P, _P],
     "mi_step_advance_t": [_P, _I, _P],
     "mi_step_advance_t_table": [_P, _P, _I, _I, _P],
     "mi_step_finalize": [_P, _L, _I, _P, _P],
@@ -83,7 +86,8 @@ SIGNATURES = {
     "mi_upsample2x_bwd": [_P, _I, _I, _I, _I, _P, _P],
 }
 _RESTYPES = {"mi_last_error": c_char_p, "mi_conv2d_igemm_workspace_bytes": c_longlong,
-             "mi_attention_workspace_bytes": c_longlong, "mi_conv2d_wgrad_f16_workspace_bytes": c_longlong, "mi_step_epilogue_workspace_floats": c_longlong}
+             "mi_attention_workspace_bytes": c_longlong, "mi_conv2d_wgrad_f16_workspace_bytes": c_longlong, "mi_step_epilogue_workspace_floats": c_longlong,
+             "mi_guidance_rescale_workspace_doubles": c_longlong}
 
 _lib = None
 launch_count = 0   # number of kernel launches issued through this binding (bench.py reports it)

@@ -343,6 +343,26 @@ int mi_step_epilogue_multistep_ws(const float* x_t, const float* eps_cond, const
                                              s_out, x0_workspace, S(stream)),
                  "mi_step_epilogue_multistep_ws");
 }
+long long mi_guidance_rescale_workspace_doubles(int B, int n) { return mi::guidance_rescale_workspace_doubles(B, n); }
+int mi_guidance_rescale_factor(const float* eps_cond, const float* eps_null, const float* w, const float* w_sched,
+                               const long long* t, const float* phi, int B, int n, float* f, double* workspace,
+                               void* stream) {
+    return check(mi::guidance_rescale_factor(eps_cond, eps_null, w, w_sched, t, phi, B, n, f, workspace, S(stream)),
+                 "mi_guidance_rescale_factor");
+}
+int mi_step_epilogue_rescaled(const float* x_t, const float* eps_cond, const float* eps_null, const float* w,
+                              const float* w_sched, const float* f, const long long* t, const float* tab_a,
+                              const float* tab_b, const float* c1, const float* c2, const float* sigma, const float* c3,
+                              const float* noise, float* x0_hist, int B, int n, int rank_lo, int rank_hi, float weight,
+                              float min_s, float* out, float* s_out, float* x0_workspace, void* stream) {
+    if (!eps_null || !w || !f) return fail(-1, "mi_step_epilogue_rescaled: eps_null, w and f are required");
+    if ((c3 == nullptr) != (x0_hist == nullptr))
+        return fail(-1, "mi_step_epilogue_rescaled: c3 and x0_hist are given together or not at all");
+    return check(mi::step_epilogue_rescaled(x_t, eps_cond, eps_null, w, w_sched, f, t, tab_a, tab_b, c1, c2, sigma, c3,
+                                            noise, x0_hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out,
+                                            x0_workspace, S(stream)),
+                 "mi_step_epilogue_rescaled");
+}
 int mi_step_advance_t(long long* t, int B, void* stream) {
     return check(mi::step_advance_t(t, B, S(stream)), "mi_step_advance_t");
 }

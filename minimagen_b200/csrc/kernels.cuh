@@ -84,6 +84,17 @@ int step_epilogue_multistep(const float* x_t, const float* eps_cond, const float
                             const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
                             float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
                             float* out, float* s_out, float* x0_ws, cudaStream_t st);
+// guidance rescale (step.cu header): f [B] from the conditional and guidance predictions, then the step with eps * f[b]
+long long guidance_rescale_workspace_doubles(int B, int n_per_img);
+int guidance_rescale_factor(const float* eps_cond, const float* eps_null, const float* w, const float* w_sched,
+                            const long long* t, const float* phi, int B, int n_per_img, float* f, double* ws,
+                            cudaStream_t st);
+int step_epilogue_rescaled(const float* x_t, const float* eps_cond, const float* eps_null, const float* w,
+                           const float* w_sched, const float* f, const long long* t, const float* tab_recip,
+                           const float* tab_recipm1, const float* tab_c1, const float* tab_c2, const float* tab_sigma,
+                           const float* tab_c3, const float* noise, float* x0_hist, int B, int n_per_img, int rank_lo,
+                           int rank_hi, float weight, float min_s, float* out, float* s_out, float* x0_ws,
+                           cudaStream_t st);
 int step_advance_t(long long* t, int B, cudaStream_t st);
 int step_advance_t_table(long long* t, const long long* next_t, int T, int B, cudaStream_t st);
 int step_finalize(const float* x, long long n, int unnormalize, float* out, cudaStream_t st);

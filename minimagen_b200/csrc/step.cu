@@ -12,6 +12,13 @@
 // entry points): one captured step then serves every scale and every per-image scale vector.  The _ws entry points also
 // take a guidance table w_sched [T] (Imagen.sample(guidance_interval=, guidance_schedule=)): image b then combines with
 // w_b(t[b]) = w[b] where w_sched[t[b]] == 1, else 1 + (w[b] - 1) * w_sched[t[b]], rounded op by op.
+// Guidance rescale (mi_guidance_rescale_factor, mi_step_epilogue_rescaled; Imagen.sample(guidance_rescale=), Lin et al.
+// 2024): with g the guided prediction as above (fp32, op by op) and c = eps_cond, per image b
+//   SS_c = sum (c - mean c)^2, SS_g = sum (g - mean g)^2   in fp64 (fixed-order chunked two-pass sums, no atomics),
+//   f_b  = fp32(phi_b * sqrt(SS_c / SS_g) + (1 - phi_b))  the whole expression in fp64, rounded once; 1 where SS_g == 0,
+//          NaN where the image has a NaN,
+// and the rescaled step uses eps = fp32(g * f_b) (the kRescale instances of guided_x0); x0, threshold and posterior are
+// unchanged, so it is bit for bit the plain step fed fp32(g * f) with no guidance pass.
 // Steps 1 and 3 are written once (guided_x0, posterior_elem) and shared by the three-kernel form and the fused kernel.
 // The select of step 2 exists twice, and each is the other's test reference: quantile_kernel (one CTA per image, keys
 // streamed from global memory, any n) and the one inside step_epilogue_kernel (an 8-CTA cluster per image, keys held in
@@ -54,14 +61,17 @@ __device__ __forceinline__ float image_scale(const float* w, const float* w_sche
     return s == 1.f ? wb : __fadd_rn(1.f, __fmul_rn(__fsub_rn(wb, 1.f), s));
 }
 
+// The guidance combine g = null + (cond - null) * w, rounded op by op.
+__device__ __forceinline__ float guide(float c, float nl, float w) { return __fadd_rn(nl, __fmul_rn(__fsub_rn(c, nl), w)); }
+
 // Step 1 at element idx: eps = null + (cond - null) * w when eps_null is given, then x0 = a[t] * x_t - b[t] * eps.
+// kRescale (guidance rescale): eps <- eps * f, f the image's factor from rescale_factor_kernel.
+template <bool kRescale = false>
 __device__ __forceinline__ float guided_x0(const float* x_t, const float* eps_cond, const float* eps_null,
-                                           float cond_scale, float a, float b, long long idx) {
+                                           float cond_scale, float a, float b, long long idx, float f = 1.f) {
     float e = eps_cond[idx];
-    if (eps_null) {
-        const float nl = eps_null[idx];
-        e = __fadd_rn(nl, __fmul_rn(__fsub_rn(e, nl), cond_scale));
-    }
+    if (eps_null) e = guide(e, eps_null[idx], cond_scale);
+    if constexpr (kRescale) e = __fmul_rn(e, f);
     return __fsub_rn(__fmul_rn(a, x_t[idx]), __fmul_rn(b, e));
 }
 
@@ -95,11 +105,13 @@ __device__ __forceinline__ void posterior_elem(float x0, float s, float c1, floa
     out[idx] = __fadd_rn(mean, __fmul_rn(sig, noise[idx]));
 }
 
+// kRescale: the guided eps times rescale[b] (guided_x0); the extra argument comes last.
+template <bool kRescale>
 __global__ void __launch_bounds__(256)
 x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
           float cond_scale, const long long* __restrict__ t, const float* __restrict__ tab_recip,
           const float* __restrict__ tab_recipm1, int n_per_img, float* __restrict__ x0, const float* __restrict__ w,
-          const float* __restrict__ w_sched) {
+          const float* __restrict__ w_sched, const float* __restrict__ rescale) {
     pdl_wait();
     pdl_trigger();
     const int b = blockIdx.y;
@@ -107,8 +119,8 @@ x0_kernel(const float* __restrict__ x_t, const float* __restrict__ eps_cond, con
     if (i >= n_per_img) return;
     const long long idx = (long long)b * n_per_img + i;
     const long long tb = t[b];
-    x0[idx] = guided_x0(x_t, eps_cond, eps_null, image_scale(w, w_sched, cond_scale, b, tb), tab_recip[tb],
-                        tab_recipm1[tb], idx);
+    x0[idx] = guided_x0<kRescale>(x_t, eps_cond, eps_null, image_scale(w, w_sched, cond_scale, b, tb), tab_recip[tb],
+                                  tab_recipm1[tb], idx, kRescale ? rescale[b] : 1.f);
 }
 
 // One CTA per image.  Exact k-th order statistics of |x| by 4 x 8-bit radix passes over the float bit patterns.
@@ -228,9 +240,10 @@ posterior_kernel(const float* __restrict__ x0, const float* x_t, const float* __
 // two reads of the image less than the three-kernel form) and two launches disappear from the step.  `out` may alias
 // `x_t` (in-place update of the sampling state): every element is read and written by the same thread.
 // kHist: the multistep form, as posterior_kernel<true>; the history is only touched in the final register loop.
+// kRescale: guidance rescale, the guided eps times rescale[img] (guided_x0).
 constexpr int kSelCluster = 8, kSelPerThread = 24;
 
-template <bool kHist>
+template <bool kHist, bool kRescale>
 __global__ void __cluster_dims__(kSelCluster, 1, 1) __launch_bounds__(kSelThreads)
 step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
                      float cond_scale, const long long* __restrict__ t, const float* __restrict__ tab_recip,
@@ -238,7 +251,8 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
                      const float* __restrict__ tab_c2, const float* __restrict__ tab_sigma,
                      const float* __restrict__ noise, int n, int rank_lo, int rank_hi, float weight, float min_s,
                      float* out, float* __restrict__ s_out, const float* __restrict__ tab_c3,
-                     float* __restrict__ x0_hist, const float* __restrict__ w, const float* __restrict__ w_sched) {
+                     float* __restrict__ x0_hist, const float* __restrict__ w, const float* __restrict__ w_sched,
+                     const float* __restrict__ rescale) {
     pdl_wait();
     pdl_trigger();
     namespace cg = cooperative_groups;
@@ -259,13 +273,14 @@ step_epilogue_kernel(const float* x_t, const float* __restrict__ eps_cond, const
     const long long tb = t[img];
     const float ca = tab_recip[tb], cb = tab_recipm1[tb];
     const float scale = image_scale(w, w_sched, cond_scale, img, tb);
+    const float fac = kRescale ? rescale[img] : 1.f;
 
     float x0v[kSelPerThread];
     bool nan_key = false;
 #pragma unroll
     for (int j = 0; j < kSelPerThread; ++j) {
         const int i = tid + j * kSelThreads;
-        x0v[j] = i < cnt ? guided_x0(x_t, eps_cond, eps_null, scale, ca, cb, base + i) : 0.f;
+        x0v[j] = i < cnt ? guided_x0<kRescale>(x_t, eps_cond, eps_null, scale, ca, cb, base + i, fac) : 0.f;
         nan_key |= isnan(x0v[j]);       // (not absbits(.) > kInfBits: ptxas would keep those keys for pass 0, and spill)
     }
     // Each pass reads its mask from shared memory.  With the mask a compile-time constant of the unrolled passes, ptxas
@@ -521,6 +536,94 @@ randn_keyed_kernel(float* __restrict__ out, const long long* __restrict__ seeds,
         if (j + k < n) row[j + k] = z[k];
 }
 
+
+// ------------------------------------------------------------------------------------------------ guidance rescale factor
+// Per image b: SS_c = sum (c - mean c)^2 and SS_g = sum (g - mean g)^2 in fp64 over its n values, g = guide(c, null, w_b(t)),
+// then f[b] = fp32(phi_b sqrt(SS_c / SS_g) + (1 - phi_b)) (1 where SS_g == 0).  Deterministic, no atomics:
+//   rescale_partial_kernel  one CTA per (kRsChunk-value chunk, image): the chunk's sums and, in a second pass over the
+//                           (L2-hot) chunk, its sums of squares about the chunk mean; both reduced in a fixed order;
+//   rescale_factor_kernel   one CTA per image: the chunks merged in a fixed order (Chan et al.: M2 = sum M2_k +
+//                           n_k (m_k - m)^2, which an offset mean cannot cancel), then f.
+constexpr int kRsThreads = 256, kRsChunk = 8192;
+
+// (a, b) summed over the CTA in a fixed order (shuffle tree per warp, then the warps in order); every thread gets it.
+__device__ __forceinline__ double2 block_sum2(double a, double b, double2* sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, o);
+        b += __shfl_xor_sync(0xffffffffu, b, o);
+    }
+    const int warp = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) sh[warp] = make_double2(a, b);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double2 tot = sh[0];
+        for (int i = 1; i < kRsThreads / 32; ++i) { tot.x += sh[i].x; tot.y += sh[i].y; }
+        sh[kRsThreads / 32] = tot;
+    }
+    __syncthreads();
+    const double2 r = sh[kRsThreads / 32];
+    __syncthreads();                                  // sh is reused by the caller's next reduction
+    return r;
+}
+
+__global__ void __launch_bounds__(kRsThreads)
+rescale_partial_kernel(const float* __restrict__ eps_cond, const float* __restrict__ eps_null,
+                       const float* __restrict__ w, const float* __restrict__ w_sched, const long long* __restrict__ t,
+                       int n, int nchunks, double4* __restrict__ part) {
+    pdl_wait();
+    pdl_trigger();
+    __shared__ double2 sh[kRsThreads / 32 + 1];
+    const int b = blockIdx.y, k = blockIdx.x;
+    const int beg = k * kRsChunk, cnt = min(kRsChunk, n - beg);
+    const long long base = (long long)b * n + beg;
+    const float wb = image_scale(w, w_sched, 1.f, b, t[b]);
+    double sc = 0., sg = 0.;
+    for (int i = threadIdx.x; i < cnt; i += kRsThreads) {
+        const float c = eps_cond[base + i];
+        sc += c;
+        sg += guide(c, eps_null[base + i], wb);
+    }
+    const double2 s = block_sum2(sc, sg, sh);
+    const double mc = s.x / cnt, mg = s.y / cnt;
+    double qc = 0., qg = 0.;
+    for (int i = threadIdx.x; i < cnt; i += kRsThreads) {
+        const float c = eps_cond[base + i];
+        const double dc = (double)c - mc, dg = (double)guide(c, eps_null[base + i], wb) - mg;
+        qc += dc * dc;
+        qg += dg * dg;
+    }
+    const double2 q = block_sum2(qc, qg, sh);
+    if (threadIdx.x == 0) part[(long long)b * nchunks + k] = make_double4(s.x, q.x, s.y, q.y);
+}
+
+__global__ void __launch_bounds__(kRsThreads)
+rescale_factor_kernel(const double4* __restrict__ part, const float* __restrict__ phi, int n, int nchunks,
+                      float* __restrict__ f) {
+    pdl_wait();
+    pdl_trigger();
+    __shared__ double2 sh[kRsThreads / 32 + 1];
+    const int b = blockIdx.x;
+    const double4* p = part + (long long)b * nchunks;
+    double sc = 0., sg = 0.;
+    for (int k = threadIdx.x; k < nchunks; k += kRsThreads) { sc += p[k].x; sg += p[k].z; }
+    const double2 s = block_sum2(sc, sg, sh);
+    const double mc = s.x / n, mg = s.y / n;
+    double qc = 0., qg = 0.;
+    for (int k = threadIdx.x; k < nchunks; k += kRsThreads) {
+        const double4 v = p[k];
+        const double cnt = (double)min(kRsChunk, n - k * kRsChunk);
+        const double dc = v.x / cnt - mc, dg = v.z / cnt - mg;
+        qc += v.y + cnt * dc * dc;
+        qg += v.w + cnt * dg * dg;
+    }
+    const double2 q = block_sum2(qc, qg, sh);
+    if (threadIdx.x == 0) {
+        const double ph = phi[b];
+        f[b] = q.y == 0. ? 1.f : (float)(ph * sqrt(q.x / q.y) + (1. - ph));
+    }
+}
+
 }  // namespace
 
 int randn_keyed(float* out, const long long* seeds, int B, long long n, int kind, int stage, const long long* t,
@@ -568,13 +671,21 @@ int inpaint_finalize(const float* x, const float* k, const float* m, int B, int 
     return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
+template <bool kRescale>
+static int step_x0_impl(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
+                        const float* w_sched, const long long* t, const float* tab_recip, const float* tab_recipm1, int B,
+                        int n_per_img, float* x0, const float* rescale, cudaStream_t st) {
+    dim3 grid((n_per_img + 255) / 256, B);
+    launch_k(x0_kernel<kRescale>, grid, 256, 0, st, x_t, eps_cond, eps_null, cond_scale, t, tab_recip, tab_recipm1,
+             n_per_img, x0, w, w_sched, rescale);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
 int step_x0(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale, const float* w,
             const float* w_sched, const long long* t, const float* tab_recip, const float* tab_recipm1, int B,
             int n_per_img, float* x0, cudaStream_t st) {
-    dim3 grid((n_per_img + 255) / 256, B);
-    launch_k(x0_kernel, grid, 256, 0, st, x_t, eps_cond, eps_null, cond_scale, t, tab_recip, tab_recipm1, n_per_img, x0, w,
-             w_sched);
-    return cudaGetLastError() == cudaSuccess ? 0 : -2;
+    return step_x0_impl<false>(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, B, n_per_img,
+                               x0, nullptr, st);
 }
 
 int step_quantile(const float* x0, int B, int n_per_img, int rank_lo, int rank_hi, float weight, float min_s,
@@ -605,22 +716,24 @@ bool step_epilogue_fused_ok(int n_per_img) {
     return (n_per_img + kSelCluster - 1) / kSelCluster <= kSelThreads * kSelPerThread;
 }
 
-template <bool kHist>
+template <bool kHist, bool kRescale = false>
 static int step_epilogue_impl(const float* x_t, const float* eps_cond, const float* eps_null, float cond_scale,
                               const float* w, const float* w_sched, const long long* t, const float* tab_recip,
                               const float* tab_recipm1, const float* tab_c1, const float* tab_c2, const float* tab_sigma, const float* tab_c3, const float* noise,
                               float* x0_hist, int B, int n_per_img, int rank_lo, int rank_hi, float weight,
-                              float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st) {
+                              float min_s, float* out, float* s_out, float* x0_ws, cudaStream_t st,
+                              const float* rescale = nullptr) {
     if (rank_lo < 0 || rank_hi < rank_lo || rank_hi >= n_per_img) return -1;
     if (step_epilogue_fused_ok(n_per_img)) {
-        launch_k(step_epilogue_kernel<kHist>, B * kSelCluster, kSelThreads, 0, st, x_t, eps_cond, eps_null, cond_scale,
-                 t, tab_recip, tab_recipm1, tab_c1, tab_c2, tab_sigma, noise, n_per_img, rank_lo, rank_hi, weight, min_s,
-                 out, s_out, tab_c3, x0_hist, w, w_sched);
+        launch_k(step_epilogue_kernel<kHist, kRescale>, B * kSelCluster, kSelThreads, 0, st, x_t, eps_cond, eps_null,
+                 cond_scale, t, tab_recip, tab_recipm1, tab_c1, tab_c2, tab_sigma, noise, n_per_img, rank_lo, rank_hi,
+                 weight, min_s, out, s_out, tab_c3, x0_hist, w, w_sched, rescale);
         return cudaGetLastError() == cudaSuccess ? 0 : -2;
     }
     // images beyond the register-resident select (> 196 608 values, e.g. 3 x 1024 x 1024): x0 through the caller's scratch
     if (!x0_ws || !s_out) return -1;
-    int rc = step_x0(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, B, n_per_img, x0_ws, st);
+    int rc = step_x0_impl<kRescale>(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, B,
+                                    n_per_img, x0_ws, rescale, st);
     if (rc) return rc;
     rc = step_quantile(x0_ws, B, n_per_img, rank_lo, rank_hi, weight, min_s, s_out, st);
     if (rc) return rc;
@@ -648,6 +761,42 @@ int step_epilogue_multistep(const float* x_t, const float* eps_cond, const float
     return step_epilogue_impl<true>(x_t, eps_cond, eps_null, cond_scale, w, w_sched, t, tab_recip, tab_recipm1, tab_c1, tab_c2,
                                     tab_sigma, tab_c3, noise, x0_hist, B, n_per_img, rank_lo, rank_hi, weight, min_s,
                                     out, s_out, x0_ws, st);
+}
+
+int step_epilogue_rescaled(const float* x_t, const float* eps_cond, const float* eps_null, const float* w,
+                           const float* w_sched, const float* f, const long long* t, const float* tab_recip,
+                           const float* tab_recipm1, const float* tab_c1, const float* tab_c2, const float* tab_sigma,
+                           const float* tab_c3, const float* noise, float* x0_hist, int B, int n_per_img, int rank_lo,
+                           int rank_hi, float weight, float min_s, float* out, float* s_out, float* x0_ws,
+                           cudaStream_t st) {
+    if (!eps_null || !w || !f || (tab_c3 == nullptr) != (x0_hist == nullptr)) return -1;
+    if (tab_c3)
+        return step_epilogue_impl<true, true>(x_t, eps_cond, eps_null, 1.f, w, w_sched, t, tab_recip, tab_recipm1, tab_c1,
+                                              tab_c2, tab_sigma, tab_c3, noise, x0_hist, B, n_per_img, rank_lo, rank_hi,
+                                              weight, min_s, out, s_out, x0_ws, st, f);
+    return step_epilogue_impl<false, true>(x_t, eps_cond, eps_null, 1.f, w, w_sched, t, tab_recip, tab_recipm1, tab_c1,
+                                           tab_c2, tab_sigma, nullptr, noise, nullptr, B, n_per_img, rank_lo, rank_hi,
+                                           weight, min_s, out, s_out, x0_ws, st, f);
+}
+
+long long guidance_rescale_workspace_doubles(int B, int n_per_img) {
+    if (B <= 0 || n_per_img <= 0) return 0;
+    return 4LL * B * ((n_per_img + kRsChunk - 1) / kRsChunk);
+}
+
+int guidance_rescale_factor(const float* eps_cond, const float* eps_null, const float* w, const float* w_sched,
+                            const long long* t, const float* phi, int B, int n_per_img, float* f, double* ws,
+                            cudaStream_t st) {
+    if (B < 0 || n_per_img <= 0 || B > 65535) return -1;
+    if (B == 0) return 0;
+    if (!eps_cond || !eps_null || !w || !t || !phi || !f || !ws) return -1;
+    const int nchunks = (n_per_img + kRsChunk - 1) / kRsChunk;
+    double4* part = reinterpret_cast<double4*>(ws);
+    launch_k(rescale_partial_kernel, dim3(nchunks, B), kRsThreads, 0, st, eps_cond, eps_null, w, w_sched, t, n_per_img,
+             nchunks, part);
+    if (cudaGetLastError() != cudaSuccess) return -2;
+    launch_k(rescale_factor_kernel, B, kRsThreads, 0, st, (const double4*)part, phi, n_per_img, nchunks, f);
+    return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
 int step_advance_t(long long* t, int B, cudaStream_t st) {

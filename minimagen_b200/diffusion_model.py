@@ -23,6 +23,21 @@ def _betas_fp64(timesteps):
     return torch.linspace(scale * 0.0001, scale * 0.02, timesteps, dtype=torch.float64)
 
 
+def _zero_terminal_snr(betas):
+    """Lin et al. 2024 ("Common Diffusion Noise Schedules and Sample Steps are Flawed"), Algorithm 1, in fp64: with
+    s = sqrt(alphas_cumprod), s <- (s - s_last) s_0 / (s_0 - s_last), alphas_cumprod = s^2, alpha_t = acp_t / acp_{t-1}
+    (alpha_0 = acp_0) and beta = 1 - alpha.  The first alphas_cumprod is kept as it was (the map fixes it, exactly rather
+    than up to rounding), the last becomes exactly 0 and the last beta exactly 1."""
+    acp = torch.cumprod(1. - betas, dim=0)
+    s = acp.sqrt()
+    s0, sl = s[0].clone(), s[-1].clone()
+    s = (s - sl) * s0 / (s0 - sl)
+    acp_new = s * s
+    acp_new[0], acp_new[-1] = acp[0], 0.
+    alphas = torch.cat((acp_new[:1], acp_new[1:] / acp_new[:-1]))
+    return 1. - alphas
+
+
 class SamplingSchedule(NamedTuple):
     """A respaced (DDIM) sampling walk, see `GaussianDiffusion.sampling_schedule`.  The tables are indexed by the step's
     own timestep t and feed the fused step epilogue in place of posterior_mean_coef1 / posterior_mean_coef2 / sigma.
@@ -36,6 +51,9 @@ class SamplingSchedule(NamedTuple):
 
 
 class GaussianDiffusion(nn.Module):
+    # the reference's linear schedule; ZeroTerminalSNRDiffusion rescales it (the constructor keeps the reference's signature)
+    zero_terminal_snr = False
+
     def __init__(self, *, timesteps: int):
         super().__init__()
         # fewer than 20 steps makes the scaled linear schedule's last beta exceed 1 (diffusion_model.py:23-24)
@@ -43,8 +61,11 @@ class GaussianDiffusion(nn.Module):
         self.num_timesteps = timesteps
 
         betas = _betas_fp64(timesteps)
+        if self.zero_terminal_snr:
+            betas = _zero_terminal_snr(betas)
         alphas = 1. - betas
         acp = torch.cumprod(alphas, axis=0)
+        self.alphas_cumprod_fp64 = acp           # host-side fp64, the source of every respaced table below
         acp_prev = F.pad(acp[:-1], (1, 0), value=1.)
         post_var = betas * (1. - acp_prev) / (1. - acp)
 
@@ -65,6 +86,8 @@ class GaussianDiffusion(nn.Module):
         reg('posterior_mean_coef2', (1. - acp_prev) * torch.sqrt(alphas) / (1. - acp))
         # what `(0.5 * model_log_variance).exp()` (Imagen.py:370) evaluates to on the fp32 table, op by op in fp32
         reg('sigma', (0.5 * self.posterior_log_variance_clipped).exp())
+        # the tables of the v target sqrt(a) eps - sqrt(1 - a) x0, as q_sample's (tab_a, tab_b) = (-sqrt(1 - a), sqrt(a))
+        self.register_buffer('neg_sqrt_one_minus_alphas_cumprod', -self.sqrt_one_minus_alphas_cumprod, persistent=False)
         self._schedules = {}
 
     # ---- respaced sampling (no reference counterpart)
@@ -88,7 +111,7 @@ class GaussianDiffusion(nn.Module):
             return sched
         grid_up = torch.linspace(0, T - 1, steps, dtype=torch.float64).round().long()
         assert bool((grid_up[1:] > grid_up[:-1]).all()) and grid_up[0] == 0 and grid_up[-1] == T - 1
-        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        acp = self.alphas_cumprod_fp64
         a_t = acp[grid_up]
         a_prev = torch.cat((torch.ones(1, dtype=torch.float64), acp[grid_up[:-1]]))
         sig2 = eta ** 2 * (1. - a_prev) / (1. - a_t) * (1. - a_t / a_prev)
@@ -136,7 +159,7 @@ class GaussianDiffusion(nn.Module):
         sched = self._schedules.get(key)
         if sched is not None:
             return sched
-        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        acp = self.alphas_cumprod_fp64
         lam = 0.5 * (acp.log() - (1. - acp).log())
         # at T = 20 the last beta is 1, so lambda_{T-1} = -inf: the targets then end at lambda_{T-2}, and the last point is
         # still T-1 (for a finite lambda_{T-1} the rule above gives T-1 anyway)
@@ -203,7 +226,7 @@ class GaussianDiffusion(nn.Module):
         if tabs is not None:
             return tabs
         T = self.num_timesteps
-        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        acp = self.alphas_cumprod_fp64
         on = torch.tensor([t for t in walk.grid if t > 0], dtype=torch.long)
         nxt = walk.next_t.cpu()[on]
         ratio = acp[on] / acp[nxt]
@@ -229,7 +252,7 @@ class GaussianDiffusion(nn.Module):
         if tab is not None:
             return tab
         T = self.num_timesteps
-        acp = torch.cumprod(1. - _betas_fp64(T), dim=0)
+        acp = self.alphas_cumprod_fp64
         tau = torch.arange(T, dtype=torch.float64) / (T - 1)
         if schedule is None:
             s = torch.ones(T, dtype=torch.float64)
@@ -272,3 +295,11 @@ class GaussianDiffusion(nn.Module):
     def predict_start_from_noise(self, x_t, t, noise):
         return (extract(self.sqrt_recip_alphas_cumprod, t, x_t.shape) * x_t -
                 extract(self.sqrt_recipm1_alphas_cumprod, t, x_t.shape) * noise)
+
+
+class ZeroTerminalSNRDiffusion(GaussianDiffusion):
+    """GaussianDiffusion on the linear schedule rescaled to zero terminal SNR (no reference counterpart;
+    _zero_terminal_snr): alphas_cumprod[T-1] == 0, so sampling starts from pure noise, and every buffer and walk table is
+    derived from the rescaled betas as for the linear schedule.  Its epsilon tables sqrt_recip_alphas_cumprod /
+    sqrt_recipm1_alphas_cumprod are inf at T-1: the schedule is for v-prediction (Imagen.set_objectives)."""
+    zero_terminal_snr = True

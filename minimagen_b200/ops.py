@@ -319,6 +319,57 @@ class NativeOps:
                N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), *tail, B, n, int(rank_lo), int(rank_hi), float(weight),
                float(min_s), N.ptr(out), N.ptr(s_out), N.ptr(ws), N.stream())
 
+    def guidance_rescale_factor(self, eps_cond, eps_null, cond_scale, w_sched, t, phi, B, n, f):
+        """f [B] <- fp32(phi_b sqrt(SS_c / SS_g) + (1 - phi_b)) per image (1 where SS_g == 0), SS the fp64 sums of squares
+        about the mean of the conditional prediction and of the guided one g = null + (cond - null) w_b(t)
+        (mi_guidance_rescale_factor).  `cond_scale` as in step_epilogue; `w_sched` optional as in
+        step_epilogue_scheduled; phi: fp32 [B]."""
+        for nm, tt in (("eps_cond", eps_cond), ("eps_null", eps_null), ("w_sched", w_sched), ("phi", phi), ("f", f)):
+            _chk(tt, F32, nm)
+        _chk(t, I64, "t")
+        if eps_null is None or phi is None or phi.numel() != B or f.numel() != B:
+            raise ValueError(f"guidance_rescale_factor: eps_null, phi [{B}] and f [{B}] are required")
+        w = self._weights(cond_scale, B, x_t=eps_cond)
+        ws = torch.empty(int(N.load().mi_guidance_rescale_workspace_doubles(B, n)), dtype=F64, device=eps_cond.device)
+        N.call("mi_guidance_rescale_factor", N.ptr(eps_cond), N.ptr(eps_null), N.ptr(w), N.ptr(w_sched), N.ptr(t),
+               N.ptr(phi), int(B), int(n), N.ptr(f), N.ptr(ws), N.stream())
+
+    def step_epilogue_rescaled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, f, t, tab_a, tab_b, c1, c2, sigma, c3,
+                               noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """The guided step with eps = fp32(g * f[b]), g the guided prediction (mi_step_epilogue_rescaled): step_epilogue
+        (c3 = hist = None), step_epilogue_multistep (both given), each optionally with the guidance table `w_sched`.
+        `cond_scale` as in step_epilogue; f: fp32 [B] from guidance_rescale_factor."""
+        for nm, tt in (("x_t", x_t), ("eps_cond", eps_cond), ("eps_null", eps_null), ("w_sched", w_sched), ("f", f),
+                       ("tab_a", tab_a), ("tab_b", tab_b), ("c1", c1), ("c2", c2), ("sigma", sigma), ("c3", c3),
+                       ("noise", noise), ("hist", hist), ("out", out), ("s_out", s_out)):
+            _chk(tt, F32, nm)
+        _chk(t, I64, "t")
+        if eps_null is None or f is None or f.numel() != B:
+            raise ValueError(f"step_epilogue_rescaled: eps_null and f [{B}] are required")
+        if (c3 is None) != (hist is None):
+            raise ValueError("step_epilogue_rescaled: c3 and hist are given together or not at all")
+        if hist is not None and hist.numel() != B * n:
+            raise ValueError(f"hist: expected {B * n} values, got {hist.numel()}")
+        w = self._weights(cond_scale, B, x_t=x_t)
+        ws = None
+        nws = int(N.load().mi_step_epilogue_workspace_floats(B, n))
+        if nws:
+            ws = torch.empty(nws, dtype=F32, device=x_t.device)
+            if s_out is None:
+                s_out = torch.empty(B, dtype=F32, device=x_t.device)
+        N.call("mi_step_epilogue_rescaled", N.ptr(x_t), N.ptr(eps_cond), N.ptr(eps_null), N.ptr(w), N.ptr(w_sched),
+               N.ptr(f), N.ptr(t), N.ptr(tab_a), N.ptr(tab_b), N.ptr(c1), N.ptr(c2), N.ptr(sigma), N.ptr(c3),
+               N.ptr(noise), N.ptr(hist), B, n, int(rank_lo), int(rank_hi), float(weight), float(min_s), N.ptr(out),
+               N.ptr(s_out), N.ptr(ws), N.stream())
+
+    @staticmethod
+    def _weights(cond_scale, B, x_t):
+        """The per-image weight tensor of `cond_scale` (a number becomes B equal weights on x_t's device), checked."""
+        if not torch.is_tensor(cond_scale):
+            cond_scale = torch.full((B,), float(cond_scale), dtype=F32, device=x_t.device)
+        _scale_args(cond_scale, B, "")
+        return cond_scale
+
     def step_advance_t(self, t, B):
         _chk(t, I64, "t")
         N.call("mi_step_advance_t", N.ptr(t), B, N.stream())
