@@ -100,6 +100,13 @@ def _is_guided(cond_scale):
     return cond_scale != 1
 
 
+def bump_versions(params):
+    """Mark `params` as modified in place: one increment of each tensor's version counter.  A CUDA graph replay writes
+    tensors on the device without going through torch's dispatcher, which is what counts versions, so every cache keyed
+    on `_version` would otherwise keep serving what it built from the weights before the replay."""
+    torch.autograd.graph.increment_version(params)
+
+
 def _pad_text(embeds, mask, length):
     """Zero rows and False mask up to `length` rows: exact, since masked rows become null_text_embed either way."""
     pad = length - embeds.shape[1]
@@ -1304,6 +1311,11 @@ class Imagen(nn.Module):
         launches; the timestep / noise /
         conditioning-dropout draws are in-graph RNG calls, so every replay sees fresh randomness.  `optimizer` must be
         capturable (e.g. `torch.optim.Adam(params, lr, capturable=True)`); gradients are left in `.grad` after each step.
+        A replay updates the parameters on the device without torch's dispatcher, so it leaves their version counters
+        as they were; `step` bumps the counter of every parameter in `optimizer.param_groups` after each replay
+        (`bump_versions`), so that the weight caches of the eval and sampling path, which key on `param._version`
+        (the packed fp16 weights, the concatenated time-MLP weights, the static text projection, the captured sampling
+        step graphs), are rebuilt from the trained weights on their next use.
         Drop references to losses of earlier EAGER steps first (`del loss`): a live autograd graph keeps the parameters' gradient
         accumulators bound to the default stream, and CUDA refuses to make the legacy stream wait on a capturing one."""
         assert images.is_cuda, 'graphed_train_step captures a CUDA graph: move the model and the batch to the GPU first'
@@ -1328,6 +1340,7 @@ class Imagen(nn.Module):
         optimizer.zero_grad(set_to_none=True)
         with torch.cuda.graph(graph):
             loss = one(zero=False)
+        params = [p for group in optimizer.param_groups for p in group['params']]
 
         def step(images, text_embeds, text_masks=None):
             static[0].copy_(images, non_blocking=True)
@@ -1335,6 +1348,7 @@ class Imagen(nn.Module):
             if exists(static[2]):
                 static[2].copy_(text_masks, non_blocking=True)
             graph.replay()
+            bump_versions(params)
             return loss.detach()
 
         step.graph = graph
