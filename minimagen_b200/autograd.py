@@ -23,6 +23,32 @@ def _c(t):
     return t.contiguous()
 
 
+# Gradient operands of the fp16 backward routes.  An MSE-mean loss over b * 3 * H * W elements makes dL/dpred ~1e-5 and the
+# gradients deeper in the network smaller still: below fp16's smallest normal (6.1e-5) a plain cast keeps a bit or two of
+# each element.  So a gradient is cast as g * 2^k, with k chosen on the device from its amax (no host sync: the step stays
+# capturable) so that the scaled amax lies in [2^13, 2^14), and the kernels' fp32 outputs (dx, dw) are multiplied by 2^-k.
+# Powers of two are exact both ways.  _SCALES[device][e] = (2^k, 2^-k) for the biased fp32 exponent e of the amax, k =
+# 140 - e clamped to [-126, 126] (both stay normal fp32).
+_SCALES = {}
+
+
+def _grad_scales(g):
+    """(2^k, 2^-k) as a 2-element fp32 device tensor for the gradient g (see above)."""
+    tab = _SCALES.get(g.device)
+    if tab is None:
+        ks = [min(126, max(-126, 140 - e)) for e in range(256)]
+        tab = _SCALES[g.device] = torch.tensor([[2.0 ** k, 2.0 ** -k] for k in ks], dtype=torch.float32, device=g.device)
+    amax = torch.linalg.vector_norm(g, float("inf")).float().reshape(1)
+    return torch.index_select(tab, 0, (amax.view(torch.int32) >> 23) & 255)[0]
+
+
+def _cast_grad16(ops, g, C, B, H, W, out):
+    """out <- fp16(g * 2^k) through cast_act (mode 0); returns 2^-k, the factor of the outputs computed from `out`."""
+    s = _grad_scales(g)
+    ops.cast_act(g * s[0], C, None, 0, 1.0, B, H, W, 0, out)
+    return s[1]
+
+
 class Conv2dFn(torch.autograd.Function):
     """y = conv2d(x, weight, bias) for the reference's geometries: k x k stride 1 'same' (k odd), and any (k, stride, pad)
     on the fp32 path.  x: [B, H, W, C_in] fp32 NHWC; weight: (C_out, C_in, kh, kw); returns [B, Ho, Wo, C_out]."""
@@ -71,13 +97,13 @@ class Conv2dFn(torch.autograd.Function):
         kh, kw = weight.shape[2], weight.shape[3]
         w = weight.detach()
         dx = dw = db = None
-        g16 = None
+        g16 = inv = None
 
         def dy16():
-            nonlocal g16
+            nonlocal g16, inv
             if g16 is None:
                 g16 = torch.empty((B, 1, Ho, Wo, Cout), dtype=F16, device=dy.device)
-                ops.cast_act(dy, Cout, None, 0, 1.0, B, Ho, Wo, 0, g16)
+                inv = _cast_grad16(ops, dy, Cout, B, Ho, Wo, g16)
             return g16
 
         if ctx.needs_input_grad[0]:
@@ -88,6 +114,7 @@ class Conv2dFn(torch.autograd.Function):
                 g16 = dy16()
                 ops.conv_igemm(g16, B, H, W, Cout, 0, Cout, ops.pack_conv_weight_dgrad(w), Cin, kh, kw, 0, None, None, dx, None,
                                (H * W * Cin, W * Cin, Cin))
+                dx.mul_(inv)
             elif tc and down and Cout % 64 == 0 and Cin % 16 == 0 and ops.igemm_supported(Ho, Wo, Cout, Cin):
                 # transposed 4x4 stride-2 conv = four 2x2 convs of dy, one per output parity (a, b): input pixel 2v + a sees
                 # dy[v - 1], dy[v] through kernel rows 3, 1 (a = 0) or dy[v], dy[v + 1] through rows 2, 0 (a = 1) -- the tap
@@ -102,6 +129,7 @@ class Conv2dFn(torch.autograd.Function):
                     off = (a * W + b) * Cin
                     ops.conv_igemm(g16, B, Ho, Wo, Cout, 0, Cout, ops.pack_conv_weight(_c(k)), Cin, 2, 2, 2 + ph, None, None,
                                    dx.reshape(-1)[off:], None, (H * W * Cin, 2 * W * Cin, 2 * Cin))
+                dx.mul_(inv)
             else:
                 ops.conv_dgrad(dy, B, Ho, Wo, Cout, _c(w), Cin, kh, kw, stride, pad, dx, H, W)
         if ctx.needs_input_grad[1]:
@@ -113,6 +141,7 @@ class Conv2dFn(torch.autograd.Function):
                     x16 = torch.empty((B, 1, H, W, Cin), dtype=F16, device=x.device)
                     ops.cast_act(x, Cin, None, 0, 1.0, B, H, W, 0, x16)
                 ops.conv_wgrad_tc(dy16(), x16, B, Ho, Wo, Cin, Cout, kh, kw, dw, stride)
+                dw.mul_(inv)
             elif same and Cout < 32 <= Cin:
                 # few OUTPUT channels (the 3-channel final conv): sum over input pixels q instead,
                 # dW[co][ci][t] = sum_q x[q][ci] * dy[q - (t - pad)][co] -- the same kernel with x and dy swapped computes
@@ -204,8 +233,13 @@ class LinearFn(torch.autograd.Function):
     everything else (time / text MLPs on B rows, ragged widths) stays fp32."""
 
     @staticmethod
+    def _buf16(t, Mp, C):
+        """the fp16 operand of M rows of t, zero-padded to Mp rows"""
+        return (torch.empty if Mp == t.shape[0] else torch.zeros)((1, 1, Mp // 128, 128, C), dtype=F16, device=t.device)
+
+    @staticmethod
     def _rows16(ops, t, M, Mp, C):
-        a = (torch.empty if Mp == M else torch.zeros)((1, 1, Mp // 128, 128, C), dtype=F16, device=t.device)
+        a = LinearFn._buf16(t, Mp, C)
         ops.cast_act(t, C, None, 0, 1.0, 1, 1, M, 0, a)
         return a
 
@@ -243,13 +277,16 @@ class LinearFn(torch.autograd.Function):
         Nn = w.shape[0]
         Mp = (M + 127) // 128 * 128
         dx = dw = db = None
-        g16 = LinearFn._rows16(ops, dy, M, Mp, Nn) if tc else None
+        g16 = inv = None
+        if tc:
+            g16 = LinearFn._buf16(dy, Mp, Nn)
+            inv = _cast_grad16(ops, dy, Nn, 1, 1, M, g16)
         if ctx.needs_input_grad[0]:
             if g16 is not None and Nn % 64 == 0 and K % 16 == 0 and ops.igemm_supported(Mp // 128, 128, Nn, K):
                 dx = torch.empty((Mp, K), dtype=F32, device=x.device)          # dX[M,K] = dY[M,N] W[N,K]
                 ops.conv_igemm(g16, 1, Mp // 128, 128, Nn, 0, Nn, ops.pack_conv_weight_dgrad(w), K, 1, 1, 0, None, None, dx, None,
                                (Mp * K, 128 * K, K))
-                dx = dx[:M]
+                dx = dx[:M].mul_(inv)
             else:
                 dx = torch.empty_like(x)
                 ops.gemm_f32(dy, w, dx, M, K, Nn, (Nn, 1), (K, 1), (K, 1))
@@ -257,6 +294,7 @@ class LinearFn(torch.autograd.Function):
             dw = torch.empty_like(w)                       # dW[N,K] = dY^T[N,M] X[M,K]
             if g16 is not None and ops.conv_wgrad_tc_supported(8, 8, K, Nn, 1, 1):
                 ops.conv_wgrad_tc(g16, ctx.x16, Mp // 64, 8, 8, K, Nn, 1, 1, dw)
+                dw.mul_(inv)
             else:
                 ops.gemm_f32(dy, x, dw, Nn, K, M, (1, Nn), (K, 1), (K, 1))
             dw = dw.reshape(wshape)

@@ -12,7 +12,10 @@ checkers are not vacuous).
     queries), so a kernel added later cannot slip through unchecked;
   * accumulators: in a forward, every statistics accumulator is zero when first handed to a kernel and no two overlap (the
     ZeroArena carving); in a training step (`fresh_accumulators`), where every GroupNorm statistics / dgamma / dbeta
-    accumulator is a fresh torch.zeros that the caching allocator recycles, every accumulator is zero at every hand-off.
+    accumulator is a fresh torch.zeros that the caching allocator recycles, every accumulator is zero at every hand-off;
+  * conditioning: a cast_act that writes the fp16 copy of a gradient inside an autograd backward must hold it to a tensor
+    rel-L2 of 2^-10, as normal-range fp16 does: an exact rounding of a mostly subnormal copy passes the float64 check and
+    still loses the gradient.
 
 `sms` is the SM count the per-kernel summation plans (and so the bounds' accumulation lengths) depend on: the device's
 multi_processor_count, or 132 (an H100 SXM) for the CPU emulation.
@@ -381,6 +384,8 @@ class CheckingOps:
         n_out = B * H * W * C * (4 if mode == 1 else 1)
         o = out.reshape(-1)[:n_out]                                        # mode 0 writes the first B*H*W rows of `out`
         o.fill_(NAN)
+        backward = torch._C._current_graph_task_id() >= 0                  # called from an autograd backward
+        err = nrm = 0.0
         yield
         s0, s1 = src0.reshape(B, H, W, c0), src1.reshape(B, H, W, c1) if c1 else None
         # the output rows of input rows [h0, h1): the same rows, rows [2 h0, 2 h1) of the nearest x2 upsample, or phase
@@ -399,6 +404,15 @@ class CheckingOps:
                 bound = R.U32 * x.abs() if c1 else torch.zeros_like(x)     # the fp32 product with the skip scale
                 ref, bound = R.half_out(x, bound) if out.dtype == F16 else (x, bound)
                 self._note("cast_act", R.check(got, ref, bound, f"cast_act mode {mode}"))
+                if out.dtype == F16 and backward:
+                    err, nrm = err + float((got.to(F64) - x).norm()) ** 2, nrm + float(x.norm()) ** 2
+        if out.dtype == F16 and backward:
+            # conditioning: an fp16 copy of a gradient must still hold it.  A gradient cast unscaled (~1e-5 per element
+            # under an MSE-mean loss) is mostly subnormal in fp16; rounded exactly, it passes the check above and loses
+            # most of its bits.  Normal-range fp16 keeps the tensor's rel-L2 within 2^-11; the limit is 2^-10.
+            rel = (err / nrm) ** 0.5 if nrm else 0.0
+            assert rel <= 2.0 ** -10, (f"cast_act: the fp16 copy of a backward gradient is off by rel-L2 {rel:.3e} "
+                                       f"(> 2^-10): cast it scaled into fp16's normal range")
 
     def _check_ln_rows(self, inp, rows, C, gamma, beta, eps, pre_gelu, residual, out_f32, out_f16):
         self._count("ln_rows")

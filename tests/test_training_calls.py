@@ -214,6 +214,20 @@ def test_planted_kernel_defect_fails_its_call_check(emu_tc, method):
     assert proxy.failures and all(f.startswith(method + "(") for f in proxy.failures)
 
 
+def test_planted_unscaled_gradient_cast_fails_its_conditioning_check(emu_tc, monkeypatch):
+    """The backward's fp16 gradient casts unscaled (scale 1, as before autograd._grad_scales): every such cast is an exact
+    fp16 rounding and passes its float64 check, but the copy no longer holds the gradient, and the conditioning check of
+    cast_act must fail."""
+    import minimagen_b200.autograd as ag
+    monkeypatch.setattr(ag, "_grad_scales", lambda g: torch.ones(2, dtype=torch.float32, device=g.device))
+    proxy = CheckingOps(emu_tc, sms=SMS, fresh_accumulators=True, only={"cast_act"}, strict=False)
+    _step(proxy, "base_d64_mid_attn")
+    with pytest.raises(AssertionError) as e:
+        proxy.raise_failures()
+    print(f"\nplanted unscaled gradient casts: {len(proxy.failures)} failed cast_act calls\n  {str(e.value)[-200:]}")
+    assert proxy.failures and all(f.startswith("cast_act(") and "backward gradient" in f for f in proxy.failures)
+
+
 # ------------------------------------------------------------------------------------------------ coverage
 def test_every_training_method_has_a_checker_and_a_reaching_case():
     """The training-side section of NativeOps (everything after its "training side" banner), plus the two sampling-loop
