@@ -17,6 +17,10 @@ checkers are not vacuous).
     rel-L2 of 2^-10, as normal-range fp16 does: an exact rounding of a mostly subnormal copy passes the float64 check and
     still loses the gradient.
 
+Every kernel-launching method of the ops interface has a checker here, the sampling features' included (the RePaint
+prologue / advance / finalize, the keyed draws, the scheduled and the rescaled step epilogues, the three-kernel step);
+tests/test_sampling_feature_calls.py holds that against NativeOps itself, so one proxy checks a sample that combines them.
+
 `sms` is the SM count the per-kernel summation plans (and so the bounds' accumulation lengths) depend on: the device's
 multi_processor_count, or 132 (an H100 SXM) for the CPU emulation.
 
@@ -35,11 +39,13 @@ import io
 
 import torch
 
+import fp64_ref
 import fp64_ref as R
 
 F16, F32, F64 = torch.float16, torch.float32, torch.float64
 ALLOWED = {"igemm_supported", "conv_res1x1_supported", "conv_gn_supported",
-           "conv_wgrad_tc_supported"}                                       # capability queries: no kernel runs
+           "conv_wgrad_tc_supported",                                       # capability queries: no kernel runs
+           "set_launch_mode"}                                               # a library setting: no kernel runs
 NAN = float("nan")
 
 # The training-side methods of the ops interface (NativeOps' "training side" section) and the two sampling-loop kernels a
@@ -111,6 +117,7 @@ class CheckingOps:
         self.family = {}                       # method -> [calls, worst |err| / bound]
         self.last = 0.0                        # worst |err| / bound of the latest checked call
         self.features = set()                  # call shapes that matter, reached and checked (conv modes, multi-query, ...)
+        self.keyed = []                        # (kind, stage, per-image labels) of every randn_keyed call, in order
         self.accumulators = {}                 # data_ptr -> numel of every statistics accumulator seen
 
     def __getattr__(self, name):
@@ -580,6 +587,160 @@ class CheckingOps:
                                        hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
         return self._step("step_epilogue_multistep", x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, c3,
                           noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def _check_step_epilogue_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2, sigma,
+                                       noise, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """The step epilogue at the scheduled weights w_b(t[b]) (fp64_ref.scheduled_weights, each image at its own t)."""
+        self.features.add("step_epilogue_scheduled per-image w")
+        return self._step("step_epilogue_scheduled", x_t, eps_cond, eps_null, R.scheduled_weights(cond_scale, w_sched, t, B),
+                          t, tab_a, tab_b, c1, c2, sigma, None, noise, None, B, n, rank_lo, rank_hi, weight, min_s, out,
+                          s_out)
+
+    def _check_step_epilogue_multistep_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1,
+                                                 c2, sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out,
+                                                 s_out=None):
+        return self._step("step_epilogue_multistep_scheduled", x_t, eps_cond, eps_null,
+                          R.scheduled_weights(cond_scale, w_sched, t, B), t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist, B,
+                          n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def _check_guidance_rescale_factor(self, eps_cond, eps_null, cond_scale, w_sched, t, phi, B, n, f):
+        """f [B] within one fp32 ulp of the fp64 factor of the fp32 guided prediction (fp64_ref.rescale_factor_ref)."""
+        self._count("guidance_rescale_factor")
+        w = cond_scale.detach().cpu().clone() if torch.is_tensor(cond_scale) else cond_scale
+        ref, bound = R.rescale_factor_ref(eps_cond, eps_null, w, w_sched, t, phi, B, n)
+        f.fill_(NAN)
+        yield
+        self._note("guidance_rescale_factor", R.check(f.reshape(-1)[:B], ref, bound, "guidance_rescale_factor f"))
+
+    def _check_step_epilogue_rescaled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, f, t, tab_a, tab_b, c1, c2,
+                                      sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """The step of the fp32 rescaled prediction fp32(g * f_b) (fp64_ref.rescaled_eps_fp32, formed as the kernel forms
+        it) with no guidance pass: the checks of step_epilogue(_multistep) on that input."""
+        self.features.add("step_epilogue_rescaled " + ("multistep" if hist is not None else "plain") +
+                          (" scheduled" if w_sched is not None else ""))
+        w = cond_scale.detach().cpu().clone() if torch.is_tensor(cond_scale) else cond_scale
+        eps = R.rescaled_eps_fp32(eps_cond, eps_null, w, w_sched, t, f, B, n)
+        return self._step("step_epilogue_rescaled", x_t, eps, None, 1.0, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist,
+                          B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    # the three-kernel form of the step (the step epilogue's pieces), against the same references
+    def _check_step_x0(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0):
+        self._count("step_x0")
+        x0.fill_(NAN)
+        yield
+        ref, bound = R.step_x0_ref(x_t.reshape(B, n), eps_cond.reshape(B, n),
+                                   None if eps_null is None else eps_null.reshape(B, n), cond_scale, t, tab_a, tab_b)
+        self._note("step_x0", R.check(x0.reshape(B, n), ref, bound, "step_x0"))
+
+    def _check_step_quantile(self, x0, B, n, rank_lo, rank_hi, weight, min_s, s):
+        """The threshold of the fp32 x0 the call reads: exact operands (zero input bound)."""
+        self._count("step_quantile")
+        s.fill_(NAN)
+        yield
+        x = R._d(x0.reshape(B, n)).cpu()
+        ref, bound = R.step_threshold_ref(x, torch.zeros_like(x), rank_lo, rank_hi, weight, min_s)
+        self._note("step_quantile", R.check(s.reshape(-1)[:B], ref, bound, "step_quantile s"))
+
+    def _check_step_posterior(self, x0, x_t, noise, s, t, c1, c2, sigma, B, n, out):
+        self._count("step_posterior")
+        xt0 = x_t.detach().reshape(B, n).clone()
+        if out.data_ptr() != x_t.data_ptr():
+            out.fill_(NAN)
+        yield
+        x = R._d(x0.reshape(B, n)).cpu()
+        sv = R._d(s.reshape(-1)[:B]).cpu()
+        ref, bound, _, _ = R.step_posterior_ref(x, torch.zeros_like(x), sv, torch.zeros_like(sv), xt0, noise.reshape(B, n),
+                                                t, c1, c2, sigma)
+        self._note("step_posterior", R.check(out.reshape(B, n), ref, bound, "step_posterior"))
+
+    # ---------------------------------------------------------------- RePaint and keyed draws
+    def _check_inpaint_prologue(self, x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
+        """In place on x: against fp64_ref.inpaint_prologue_ref within its per-element bound, and the pixels neither branch
+        takes bitwise unchanged.  z_renoise must not be read where r == 0: those images of it are NaN during the call (and
+        restored after it), unless it is z_known itself (the eager loop passes the 'inpaint' draw in its place at r = 0)."""
+        self._count("inpaint_prologue")
+        xv, mv = x.reshape(B, C, hw), m.reshape(B, 1, hw)
+        x0, tt, rr = xv.detach().clone(), t[:B].clone(), r[:B].clone()
+        valid = (tt >= 0) & (tt < T)
+        if bool((valid & (rr > 0)).any()):
+            self.features.add("inpaint_prologue re-noise")
+        if bool((valid & (rr == 0)).any()):
+            self.features.add("inpaint_prologue r = 0")
+        if bool((mv == 0.5).any()):
+            self.features.add("inpaint_prologue m = 0.5")
+        zr = z_renoise.reshape(B, C, hw)
+        idle = rr <= 0
+        shared = z_renoise.untyped_storage().data_ptr() == z_known.untyped_storage().data_ptr()
+        saved = None
+        if bool(idle.any()) and not shared:
+            saved = zr[idle].clone()
+            zr[idle] = NAN
+        yield
+        if saved is not None:
+            zr[idle] = saved
+        ref, bound, touched = R.inpaint_prologue_ref(x0, tt, rr, ra, rb, sqrt_acp, sqrt_1m_acp, k.reshape(B, C, hw), mv,
+                                                     zr, z_known.reshape(B, C, hw), T)
+        bits = lambda v: v.detach().view(torch.int32)[~touched]
+        assert torch.equal(bits(xv), bits(x0)), "inpaint_prologue: a pixel neither branch takes must be left bitwise as it was"
+        self._note("inpaint_prologue", R.check(xv, ref, bound, "inpaint_prologue"))
+
+    def _check_inpaint_advance(self, t, r, next_t, R, T, B):
+        """r <- r + 1 while r + 1 < R[0] at 0 < t < T, else r <- 0 and t <- next_t[t] (0 outside [0, T)): exact."""
+        self._count("inpaint_advance")
+        t0, r0 = t[:B].clone(), r[:B].clone()
+        yield
+        valid = (t0 >= 0) & (t0 < T)
+        rep = valid & (t0 > 0) & (r0 + 1 < R.reshape(-1)[0])
+        want_t = torch.where(rep, t0, torch.where(valid, next_t[t0.clamp(0, T - 1)], torch.zeros_like(t0)))
+        want_r = torch.where(rep, r0 + 1, torch.zeros_like(r0))
+        if bool(rep.any()):
+            self.features.add("inpaint_advance repeat")
+        if bool((~rep).any()):
+            self.features.add("inpaint_advance next point")
+        assert torch.equal(t[:B], want_t) and torch.equal(r[:B], want_r), \
+            "inpaint_advance: (t, r) <- the next RePaint iteration is exact"
+        self._note("inpaint_advance", 0.0)
+
+    def _check_inpaint_finalize(self, x, k, m, B, C, hw, unnormalize, out):
+        """clamp(where(m >= 0.5, k, x), -1, 1) with torch's NaN semantics, then (v + 1) * 0.5 when unnormalising: a select
+        and two fp32 roundings in this order, so the result must be bit for bit torch's (NaN in x survives where m < 0.5)."""
+        self._count("inpaint_finalize")
+        xv = x.reshape(B, C, hw)
+        x0 = xv.detach().clone()
+        o = out.reshape(B, C, hw)
+        if o.data_ptr() != x.data_ptr():
+            o.fill_(NAN)
+        yield
+        v = torch.where(m.reshape(B, 1, hw) >= 0.5, k.reshape(B, C, hw), x0).clamp(-1.0, 1.0)
+        want = (v + 1.0) * 0.5 if unnormalize else v
+        same = torch.equal(o.isnan(), want.isnan()) and torch.equal(o[~o.isnan()], want[~want.isnan()])
+        assert same, "inpaint_finalize: a select, a clamp and one fp32 add and product, it must be bitwise torch's"
+        self._note("inpaint_finalize", 0.0)
+
+    def _check_randn_keyed(self, out, seeds, B, n, kind, stage, t=None, r=None, R=None, label=0):
+        """Image b's normals against tests/keyed_noise_restatement.py in float64 from the same Philox bits, within its
+        relative bound (keyed_noise_restatement.ulp_bound, from CUDA's documented ulp errors).  The labels are read as the
+        kernel reads them: t[b] * R[0] + r[b] from the device tensors when t is given (r, R optional), else `label`.  Each
+        call's (kind, stage, labels) goes to `keyed` and to `features`."""
+        import keyed_noise_restatement as K
+        self._count("randn_keyed")
+        if t is None:
+            labels = [int(label)] * B
+        else:
+            lab = t[:B].cpu() * (int(R.reshape(-1)[0]) if R is not None else 1) + (r[:B].cpu() if r is not None else 0)
+            labels = [int(v) for v in lab]
+        name = {v: k for k, v in K.KINDS.items()}[int(kind)]
+        self.keyed.append((name, int(stage), tuple(labels)))
+        self.features.add(f"randn_keyed {name} stage {int(stage)}")
+        if t is not None:
+            self.features.add(f"randn_keyed {name} stage {int(stage)} device labels")
+        self.features |= {f"randn_keyed {name} stage {int(stage)} label {v}" for v in labels}
+        ov = out.reshape(B, n)
+        ov.fill_(NAN)
+        yield
+        z64 = torch.from_numpy(K.randn_keyed([int(s) for s in seeds[:B].cpu()], n, int(kind), int(stage), labels))
+        z64 = z64.to(ov.device)
+        self._note("randn_keyed", fp64_ref.check(ov, z64, K.ulp_bound() * z64.abs() + 2.0 ** -126, f"randn_keyed {name}"))
 
     def _check_step_advance_t(self, t, B):
         """t <- max(t - 1, 0): exact."""

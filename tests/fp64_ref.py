@@ -2,7 +2,8 @@
 direct and stem convolutions, the conv epilogue's GroupNorm statistics, GroupNorm statistics and GroupNorm/FiLM/SiLU, the
 fused GroupNorm conv), of the image-side training kernels (GroupNorm/SiLU backward, convolution weight and data
 gradients, upsample backward) and of the sampling loop's kernels outside the U-Net (the step epilogue's x0, threshold and
-posterior, q_sample, the cascade resize, the timestep embedding and the text-token pooling) with elementwise error bounds.
+posterior, q_sample, the RePaint prologue, the scheduled guidance weights and the guidance-rescale factor, the cascade
+resize, the timestep embedding and the text-token pooling) with elementwise error bounds.
 
 Every reference takes the operands exactly as the kernel reads them (fp16-rounded where the kernel reads fp16, the null
 key/value included), computes in float64 on the operands' device, and returns (reference, bound): |kernel - reference| <=
@@ -883,6 +884,69 @@ def q_sample_ref(x0, noise, t, tab_a, tab_b, post_scale, post_shift):
     ps, sh = _f32(post_scale), _f32(post_shift)
     ref = (a * x + b * z) * ps + sh
     return ref, 4 * U32 * (abs(ps) * ((a * x).abs() + (b * z).abs()) + abs(sh)) + ETA32
+
+
+def inpaint_prologue_ref(x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T):
+    """inpaint_prologue_kernel on x [B, C, hw] (m [B, 1, hw], t and r [B] as the kernel read them): where r > 0,
+    v = ra[t] x + rb[t] z_renoise; then where m >= 0.5, v = sqrt_acp[t] k + sqrt_1m_acp[t] z_known; images with t outside
+    [0, T) and the pixels neither branch takes are left alone.  Each branch is two fp32 products and one sum, so with
+    twin = |p| + |q| for its two products p, q:  |v - v64| <= U32 twin + U32 |fl(p) + fl(q)| <= 2 U32 (1 + U32) twin,
+    + ETA32 for products that underflow.  Returns (ref, bound, touched) [B, C, hw]; the bound is 0 where not touched and
+    z_renoise is not read there (nor where r == 0)."""
+    B = x.shape[0]
+    tt, rr = t.detach()[:B], r.detach()[:B]
+    valid = ((tt >= 0) & (tt < T)).reshape(B, 1, 1)
+    tc = tt.clamp(0, T - 1)
+    col = lambda tab: _d(tab)[tc].reshape(B, 1, 1)
+    xd = _d(x)
+    ren = valid & (rr > 0).reshape(B, 1, 1)
+    paste = valid & (_d(m) >= 0.5)
+    zr = torch.where(ren, _d(z_renoise), torch.zeros((), dtype=F64, device=xd.device))   # NaN where not read is allowed
+    p, q = col(ra) * xd, col(rb) * zr
+    pk, qk = col(sqrt_acp) * _d(k), col(sqrt_1m_acp) * _d(z_known)
+    c = 2 * U32 * (1 + U32)
+    ref = torch.where(paste, pk + qk, torch.where(ren, p + q, xd))
+    zero = torch.zeros((), dtype=F64, device=xd.device)
+    bound = torch.where(paste, c * (pk.abs() + qk.abs()) + ETA32, torch.where(ren, c * (p.abs() + q.abs()) + ETA32, zero))
+    return ref, bound, (paste | ren).expand(xd.shape)
+
+
+# ---------------------------------------------------------------------------------------------- guidance weights
+def scheduled_weights(w, w_sched, t, B):
+    """image_scale (csrc/step.cu) as fp32 [B] on the CPU: w_b, or 1 + (w_b - 1) * w_sched[t_b] rounded op by op where the
+    guidance table is not 1."""
+    wt = w.detach().cpu().to(torch.float32) if torch.is_tensor(w) else torch.full((B,), _f32(w), dtype=torch.float32)
+    if w_sched is None:
+        return wt
+    s = w_sched.detach().cpu()[t.detach().cpu()[:B]]
+    return torch.where(s == 1, wt, 1 + (wt - 1) * s)
+
+
+def guided_fp32(eps_cond, eps_null, w, w_sched, t, B, n):
+    """The guided prediction g = null + (cond - null) * w_b(t) [B, n] exactly as the kernels form it in fp32 (three
+    roundings, op by op), on the CPU."""
+    c, nl = eps_cond.detach().cpu().reshape(B, n), eps_null.detach().cpu().reshape(B, n)
+    return nl + (c - nl) * scheduled_weights(w, w_sched, t, B)[:, None]
+
+
+def rescale_factor_ref(eps_cond, eps_null, w, w_sched, t, phi, B, n):
+    """rescale_factor_kernel: f_b = phi_b sqrt(SS_c / SS_g) + (1 - phi_b) (1 where SS_g == 0), SS the sum of squares about
+    the image mean, from the fp32 g the kernel forms (guided_fp32).  The kernel sums in fp64 over at most ~2^22 values per
+    image and takes a chunked two-pass variance (Chan et al.), relative error ~ n U64 ~ 2^-31 on SS, so f is within its
+    final rounding of the fp64 value plus a margin far below it: |f - f64| <= 2 U32 |f64| (one fp32 ulp).  Returns (f, bound)
+    [B] in float64."""
+    c = eps_cond.detach().cpu().reshape(B, n).to(F64)
+    g = guided_fp32(eps_cond, eps_null, w, w_sched, t, B, n).to(F64)
+    ssc = ((c - c.mean(dim=1, keepdim=True)) ** 2).sum(dim=1)
+    ssg = ((g - g.mean(dim=1, keepdim=True)) ** 2).sum(dim=1)
+    ph = phi.detach().cpu().to(F64).reshape(-1)[:B]
+    f = torch.where(ssg == 0, torch.ones((), dtype=F64), ph * (ssc / ssg).sqrt() + (1. - ph))
+    return f, 2 * U32 * f.abs() + ETA32
+
+
+def rescaled_eps_fp32(eps_cond, eps_null, w, w_sched, t, f, B, n):
+    """The prediction the rescaled step uses in place of g: fp32(g * f_b) [B, n] (g from guided_fp32), on the CPU."""
+    return guided_fp32(eps_cond, eps_null, w, w_sched, t, B, n) * f.detach().cpu().reshape(-1)[:B, None]
 
 
 def resize_ref(x, iy, wy, ix, wx, clamp=None):

@@ -84,3 +84,16 @@ def randn_keyed(seeds, n, kind, stage, labels, dtype=np.float64):
     labels = np.broadcast_to(np.asarray(labels, dtype=object), (len(seeds),))
     f = normals64 if dtype == np.float64 else normals32
     return np.stack([f(s, n, kind, stage, lab) for s, lab in zip(seeds, labels)])
+
+
+def ulp_bound():
+    """The relative error bound of a kernel normal against the same formula in exact arithmetic, from the CUDA C
+    Programming Guide's maximum ulp errors (no fast-math): logf 1 ulp, sqrtf 0 ulp (correctly rounded), sincospif 1 ulp
+    for each of its two results (as cospif / sinpif), and 0.5 ulp for each rounded product.  With eps = 2^-24 (unit roundoff; 1 ulp <= 2 eps relative at normal
+    results) and u, v, 2v and the factor -2 exact: logf gives ln u (1 + d1), |d1| <= 2 eps; the square root halves d1 and
+    rounds once, so rho carries <= eps + eps; the trig value <= 2 eps; the product one more eps.  In total
+    <= 5 eps (1 + O(eps)) < 6 eps = 2^-21.4, inside 2^-20 by a factor of 2.7."""
+    eps = 2.0 ** -24
+    rel = (2 * eps) / 2 + eps + 2 * eps + eps        # logf through the square root, sqrtf, cospif / sinpif, the product
+    assert rel * (1 + 1e-6) < 6 * eps < 2.0 ** -20
+    return 2.0 ** -20

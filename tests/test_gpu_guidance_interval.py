@@ -178,23 +178,6 @@ def test_identity_graph_keys(native):
 
 
 # ------------------------------------------------------------------------------------------------ per-call check
-class IntervalCheckingOps(CheckingOps):
-    """CheckingOps plus the scheduled step epilogues, checked as the step epilogues at the weights w_b(t[b])."""
-
-    def _check_step_epilogue_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2, sigma,
-                                       noise, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
-        return self._step("step_epilogue_scheduled", x_t, eps_cond, eps_null, scheduled_weights(cond_scale, w_sched, t, B),
-                          t, tab_a, tab_b, c1, c2, sigma, None, noise, None, B, n, rank_lo, rank_hi, weight, min_s, out,
-                          s_out)
-
-    def _check_step_epilogue_multistep_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1,
-                                                 c2, sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out,
-                                                 s_out=None):
-        return self._step("step_epilogue_multistep_scheduled", x_t, eps_cond, eps_null,
-                          scheduled_weights(cond_scale, w_sched, t, B), t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist, B,
-                          n, rank_lo, rank_hi, weight, min_s, out, s_out)
-
-
 @pytest.mark.parametrize("sampler", ["ddim", "dpmpp_2m"])
 def test_every_call_of_an_interval_sample(native, sampler):
     """One eager Imagen.sample with an interval and the 'linear' schedule on the tiny golden U-Net: every kernel call
@@ -204,7 +187,7 @@ def test_every_call_of_an_interval_sample(native, sampler):
     im = _tiny_imagen(g, 1000, "cuda")
     im.use_cuda_graph = False
     im.noise_fn = _bank(4)
-    proxy = IntervalCheckingOps(native)
+    proxy = CheckingOps(native)
     ops_mod.set_ops(proxy)                              # the `native` fixture restores the previous backend afterwards
     out = im.sample(text_embeds=g["text_embeds"].cuda(), text_masks=g["text_mask"].cuda(),
                     cond_scale=torch.tensor([2., 4.5]), sampling_timesteps=4, sampler=sampler,

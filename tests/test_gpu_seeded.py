@@ -39,25 +39,12 @@ def test_bits_independent_of_batch_and_launch(native, n):
         assert not torch.equal(_draw(native, SEEDS[:1], n, **other)[0], full[0])
 
 
-def _ulp_bound():
-    """The relative error bound of a kernel normal against the same formula in exact arithmetic, from the CUDA C
-    Programming Guide's maximum ulp errors (no fast-math): logf 1 ulp, sqrtf 0 ulp (correctly rounded), sincospif 1 ulp
-    for each of its two results (as cospif / sinpif), and 0.5 ulp for each rounded product.  With eps = 2^-24 (unit roundoff; 1 ulp <= 2 eps relative at normal
-    results) and u, v, 2v and the factor -2 exact: logf gives ln u (1 + d1), |d1| <= 2 eps; the square root halves d1 and
-    rounds once, so rho carries <= eps + eps; the trig value <= 2 eps; the product one more eps.  In total
-    <= 5 eps (1 + O(eps)) < 6 eps = 2^-21.4, inside 2^-20 by a factor of 2.7."""
-    eps = 2.0 ** -24
-    rel = (2 * eps) / 2 + eps + 2 * eps + eps        # logf through the square root, sqrtf, cospif / sinpif, the product
-    assert rel * (1 + 1e-6) < 6 * eps < 2.0 ** -20
-    return 2.0 ** -20
-
-
 @pytest.mark.parametrize("n", [3 * 64 * 64, 4099, 10])
 @pytest.mark.parametrize("kind,stage,label", [(0, 1, -1), (1, 1, 999), (2, 2, 2), (3, 3, 4001), (4, 1, 2 ** 31 - 1)])
 def test_normals_vs_float64(native, n, kind, stage, label):
     """|z - z64| <= 2^-20 |z64| element by element against the restatement from the same bits (n % 4 != 0 included:
     the tail lanes are the first lanes of the last quad)."""
-    bound = _ulp_bound()
+    bound = K.ulp_bound()
     z = _draw(native, SEEDS, n, kind, stage, label).double().cpu().numpy()
     z64 = K.randn_keyed(SEEDS, n, kind, stage, label)
     err = np.abs(z - z64)

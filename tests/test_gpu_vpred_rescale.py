@@ -12,7 +12,6 @@ import torch
 import fp64_ref as R
 import rescale_ops as RO
 from checking_ops import ALLOWED, CheckingOps
-from rescale_ops import RescaleCheckingOps
 from conftest import load_golden, rel_l2
 from test_gpu_inpaint import _inp
 from test_guidance import _negative
@@ -112,7 +111,7 @@ def test_rescaled_epilogue_is_the_plain_epilogue(native, B, side, multistep, tab
     else:
         native.step_epilogue(x, eps, None, 1.0, t, a, b, sch.c1, sch.c2, sch.sigma, noise, B, n, lo, hi, wq, 1.0, want)
     assert torch.equal(out, want) and (not multistep or torch.equal(h, wh))
-    proxy = RescaleCheckingOps(native)
+    proxy = CheckingOps(native)
     h = hist.clone() if multistep else None
     proxy.step_epilogue_rescaled(x, c, u, w, w_sched, f, t, a, b, sch.c1, sch.c2, sch.sigma, c3, noise, h, B, n, lo, hi,
                                  wq, 1.0, torch.empty_like(x), s_out=torch.empty(B, device="cuda"))
@@ -210,7 +209,7 @@ def test_one_rescaled_cfg3_sampling_step_at_benchmark_size(native):
     tm = torch.ones(b, 20, dtype=torch.bool)
     tm[-1, 5:] = False
     start = torch.rand(b, 3, low, low, generator=g).cuda()
-    proxy = RescaleCheckingOps(native, only=LOOP)
+    proxy = CheckingOps(native, only=LOOP)
     ops_mod.set_ops(proxy)                                  # the `native` fixture restores the previous backend afterwards
     t0 = time.time()
     out = im.sample(text_embeds=te, text_masks=tm.cuda(), cond_scale=5., sampling_timesteps=2, start_at_unet_number=2,

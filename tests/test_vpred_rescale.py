@@ -15,7 +15,8 @@ from torch import nn
 
 import rescale_restatement as RS
 from conftest import load_golden, rel_l2
-from rescale_ops import RescaleCheckingOps, RescaleEmuOps
+from checking_ops import CheckingOps
+from rescale_ops import RescaleEmuOps
 
 F32, F64 = torch.float32, torch.float64
 SHAPE = (2, 3, 64, 64)
@@ -357,13 +358,13 @@ def _factor(defect):
 @pytest.mark.parametrize("table", [False, True])
 def test_factor_passes_and_planted_defects_fail_its_check(table):
     c, u, w, w_sched, t, phi = _call_data(1, table)
-    proxy = RescaleCheckingOps(RescaleEmuOps(), sms=SMS)
+    proxy = CheckingOps(RescaleEmuOps(), sms=SMS)
     f = torch.empty(B)
     proxy.guidance_rescale_factor(c, u, w, w_sched, t, phi, B, N, f)
     assert "guidance_rescale_factor" in proxy.checked and bool((f != 1).all())
     defects = ["biased", "neighbour"] + (["unscheduled"] if table else [])
     for defect in defects:
-        proxy = RescaleCheckingOps(type("P", (), {"guidance_rescale_factor": staticmethod(_factor(defect))})(), sms=SMS,
+        proxy = CheckingOps(type("P", (), {"guidance_rescale_factor": staticmethod(_factor(defect))})(), sms=SMS,
                             strict=False)
         proxy.guidance_rescale_factor(c, u, w, w_sched, t, phi, B, N, torch.empty(B))
         assert proxy.failures and proxy.failures[0].startswith("guidance_rescale_factor("), defect
@@ -399,7 +400,7 @@ def test_rescaled_epilogue_check(multi, defect):
             f = torch.ones_like(f)
         emu.step_epilogue_rescaled(x_t, eps_cond, eps_null, cond_scale, w_sched, f, *rest, **kw)
 
-    proxy = RescaleCheckingOps(type("P", (), {"step_epilogue_rescaled": staticmethod(planted)})(), sms=SMS, strict=False)
+    proxy = CheckingOps(type("P", (), {"step_epilogue_rescaled": staticmethod(planted)})(), sms=SMS, strict=False)
     proxy.step_epilogue_rescaled(x, c, u, w, w_sched, f, t, gd.sqrt_alphas_cumprod, gd.sqrt_one_minus_alphas_cumprod,
                                  s.c1, s.c2, s.sigma, s.c3 if multi else None, z, hist, B, N, lo, hi, wt, 1.0,
                                  torch.empty_like(x), s_out=torch.empty(B))
