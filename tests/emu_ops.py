@@ -3,7 +3,8 @@
 It mirrors the CONTRACT of every C-ABI entry point (layouts, packing order, strides, fp16 operand rounding, in-place
 output semantics) with plain torch ops, so that the host-side orchestration in minimagen_b200/{layers,Unet,Imagen}.py
 can be executed -- and compared against the real reference -- on a box without a GPU.  The product never imports this
-file; on a GPU box the native library is the only backend.
+file; on a GPU box the native library is the only backend.  EmuOps has every public method of NativeOps, with the same
+parameters; the module's `*_ref` functions are contracts the GPU tests also compare the native kernels against.
 
 Two modes, chosen by the storage-dtype pair of the U-Net ops (the sampler's step ops are fp32 in both):
 
@@ -17,10 +18,15 @@ Two modes, chosen by the storage-dtype pair of the U-Net ops (the sampler's step
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
+import fp64_ref
+import keyed_noise_restatement as K
+
 F16, F32, F64 = torch.float16, torch.float32, torch.float64
+KIND_NAMES = {v: k for k, v in K.KINDS.items()}
 
 
 def _strided(out, shape, strides):
@@ -34,6 +40,95 @@ def _cat_src(src0, c0, src1, c1, scale1, lead_shape):
     return torch.cat((a, src1.reshape(*lead_shape, c1) * scale1), dim=-1)
 
 
+# ------------------------------------------------------------------------------------------------ step contracts
+def _guided(eps_cond, eps_null, w, B, n):
+    """The prediction [B, n] the step uses: eps_cond, or null + (cond - null) * w for a number or [B] fp32 weights."""
+    e = eps_cond.reshape(B, n)
+    if eps_null is None:
+        return e
+    if torch.is_tensor(w):
+        assert w.dtype == F32 and w.numel() == B
+        w = w.reshape(B, 1)
+    nl = eps_null.reshape(B, n)
+    return nl + (e - nl) * w
+
+
+def _scheduled(eps_cond, eps_null, cond_scale, w_sched, t, B, n):
+    """_guided at the weights w_b(t[b]) of the guidance table w_sched (None: w_b), formed by fp64_ref.scheduled_weights."""
+    return _guided(eps_cond, eps_null, fp64_ref.scheduled_weights(cond_scale, w_sched, t, B).to(eps_cond.device), B, n)
+
+
+def _x0(x_t, e, t, tab_a, tab_b, B, n):
+    return tab_a[t][:, None] * x_t.reshape(B, n) - tab_b[t][:, None] * e
+
+
+def _quantile(x0, B, n, rank_lo, rank_hi, weight, min_s):
+    srt = x0.reshape(B, n).abs().sort(dim=-1).values
+    # torch.quantile: a row containing NaN (sorted last) takes both order statistics from its last element -> NaN
+    nan = srt[:, -1].isnan()
+    lo = torch.where(nan, srt[:, -1], srt[:, rank_lo])
+    hi = torch.where(nan, srt[:, -1], srt[:, rank_hi])
+    return torch.lerp(lo, hi, torch.tensor(weight, dtype=F32)).clamp(min=min_s)
+
+
+def _posterior(x0, s, x_t, noise, t, c1, c2, sigma, c3, hist, B, n):
+    """(out, clamped x0) [B, n] from x0 [B, n] unclamped and the thresholds s [B]; with c3 and hist the multistep mean, whose
+    c3 term is selected away, not multiplied, where c3[t] == 0."""
+    sb = s[:, None]
+    xs = x0.reshape(B, n).clamp(-sb, sb) / sb
+    mean = c1[t][:, None] * xs + c2[t][:, None] * x_t.reshape(B, n)
+    if c3 is not None:
+        c3t = c3[t][:, None]
+        mean = torch.where(c3t != 0, mean + c3t * hist.reshape(B, n), mean)
+    sig = torch.where(t == 0, torch.zeros_like(sigma[t]), sigma[t])[:, None]
+    return mean + sig * noise.reshape(B, n), xs
+
+
+def _step(x_t, e, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out):
+    """The step epilogue from the prediction e [B, n]: x0 -> quantile -> posterior (out may alias x_t); with c3 and hist
+    the multistep form, hist <- the clamped x0."""
+    x0 = _x0(x_t, e, t, tab_a, tab_b, B, n)
+    s = _quantile(x0, B, n, rank_lo, rank_hi, weight, min_s)
+    res, xs = _posterior(x0, s, x_t, noise, t, c1, c2, sigma, c3, hist, B, n)
+    if hist is not None:
+        hist.copy_(xs.reshape(hist.shape))
+    out.copy_(res.reshape(out.shape))
+    if s_out is not None:
+        s_out.copy_(s)
+
+
+def multistep_ref(x0, s, x_t, noise, hist, t, c1, c2, sigma, c3, B, n):
+    """Contract of mi_step_epilogue_multistep after the x0 prediction (x0 [B, n] unclamped) and the threshold s [B]:
+    (out, new hist), op by op."""
+    out, xs = _posterior(x0, s, x_t, noise, t, c1, c2, sigma, c3, hist, B, n)
+    return out.reshape(x_t.shape), xs.reshape(hist.shape)
+
+
+def prologue_ref(x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
+    """Contract of mi_inpaint_prologue, op for op (x is returned, not modified)."""
+    xv = x.reshape(B, C, hw)
+    valid = ((t >= 0) & (t < T))[:, None, None]
+    tc = t.clamp(0, T - 1)
+    col = lambda tab: tab[tc][:, None, None]
+    v = torch.where((r > 0)[:, None, None], col(ra) * xv + col(rb) * z_renoise.reshape(B, C, hw), xv)
+    v = torch.where(m.reshape(B, 1, hw) >= 0.5, col(sqrt_acp) * k.reshape(B, C, hw) + col(sqrt_1m_acp) *
+                    z_known.reshape(B, C, hw), v)
+    return torch.where(valid, v, xv).reshape(x.shape)
+
+
+def advance_ref(t, r, next_t, R, T):
+    """Contract of mi_inpaint_advance: the new (t, r)."""
+    valid = (t >= 0) & (t < T)
+    rep = valid & (t > 0) & (r + 1 < R.reshape(-1)[0])
+    nt = torch.where(valid, next_t[t.clamp(0, T - 1)], torch.zeros_like(t))
+    return torch.where(rep, t, nt), torch.where(rep, r + 1, torch.zeros_like(r))
+
+
+def finalize_ref(x, k, m, B, C, hw, unnormalize):
+    v = torch.where(m.reshape(B, 1, hw) >= 0.5, k.reshape(B, C, hw), x.reshape(B, C, hw)).clamp(-1., 1.)
+    return ((v + 1) * 0.5 if unnormalize else v).reshape(x.shape)
+
+
 class EmuOps:
     name = "torch-emulation (tests only)"
 
@@ -41,6 +136,7 @@ class EmuOps:
         self.lo, self.hi = lo, hi
         self.calls = []
         self.conv_log = []      # per host call: conv_igemm (mode, kh, kw, c_in, c_out); conv_res1x1 ('res1x1', two x sources, x_cin, c_in, c_out)
+        self.keyed = []         # per randn_keyed call: (kind name, per-image labels, stage)
 
     def _sat16(self, y):
         """hi -> lo; fp32 -> fp16 saturates (csrc/sat_half.cuh): beyond +-65504 -> +-65504, not inf."""
@@ -48,6 +144,9 @@ class EmuOps:
 
     def _log(self, name):
         self.calls.append(name)
+
+    def set_launch_mode(self, pdl):
+        """Launch modes are a property of the native kernels: nothing to emulate."""
 
     # ---------------------------------------------------------------- capability / weights
     def igemm_supported(self, H, W, c_in, c_out):
@@ -345,60 +444,109 @@ class EmuOps:
         o = attn @ vv                                                       # B,h,n,64
         out.as_strided((B, heads, n, 64), (o_bs, 64, ldo, 1), out.storage_offset()).copy_(o.to(self.lo))
 
-    # ---------------------------------------------------------------- DDPM step
+    # ---------------------------------------------------------------- sampling step
     def step_x0(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0):
         self._log("step_x0")
-        e = eps_cond.reshape(B, n)
-        if eps_null is not None:
-            nl = eps_null.reshape(B, n)
-            e = nl + (e - nl) * cond_scale
-        x0.reshape(B, n).copy_(tab_a[t][:, None] * x_t.reshape(B, n) - tab_b[t][:, None] * e)
+        x0.reshape(B, n).copy_(_x0(x_t, _guided(eps_cond, eps_null, cond_scale, B, n), t, tab_a, tab_b, B, n))
 
     def step_quantile(self, x0, B, n, rank_lo, rank_hi, weight, min_s, s):
         self._log("step_quantile")
-        srt = x0.reshape(B, n).abs().sort(dim=-1).values
-        # torch.quantile: a row containing NaN (sorted last) takes both order statistics from its last element -> NaN
-        nan = srt[:, -1].isnan()
-        lo = torch.where(nan, srt[:, -1], srt[:, rank_lo])
-        hi = torch.where(nan, srt[:, -1], srt[:, rank_hi])
-        w = torch.tensor(weight, dtype=F32)
-        s.copy_(torch.lerp(lo, hi, w).clamp(min=min_s))
+        s.copy_(_quantile(x0, B, n, rank_lo, rank_hi, weight, min_s))
 
     def step_posterior(self, x0, x_t, noise, s, t, c1, c2, sigma, B, n, out):
         self._log("step_posterior")
-        sb = s[:, None]
-        xs = x0.reshape(B, n).clamp(-sb, sb) / sb
-        mean = c1[t][:, None] * xs + c2[t][:, None] * x_t.reshape(B, n)
-        sig = torch.where(t == 0, torch.zeros_like(sigma[t]), sigma[t])[:, None]
-        out.reshape(B, n).copy_(mean + sig * noise.reshape(B, n))
+        out.reshape(B, n).copy_(_posterior(x0, s, x_t, noise, t, c1, c2, sigma, None, None, B, n)[0])
 
     def step_epilogue(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, noise, B, n, rank_lo,
                       rank_hi, weight, min_s, out, s_out=None):
-        """contract of mi_step_epilogue == x0 -> quantile -> posterior (out may alias x_t)"""
+        """contract of mi_step_epilogue (cond_scale a number) and mi_step_epilogue_w (a [B] tensor of per-image weights)"""
         self._log("step_epilogue")
-        x0 = torch.empty_like(x_t)
-        s = torch.empty(B, dtype=F32, device=x_t.device)
-        self.step_x0(x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0)
-        self.step_quantile(x0, B, n, rank_lo, rank_hi, weight, min_s, s)
-        res = torch.empty_like(x_t)
-        self.step_posterior(x0, x_t, noise, s, t, c1, c2, sigma, B, n, res)
-        out.copy_(res)
-        if s_out is not None:
-            s_out.copy_(s)
+        _step(x_t, _guided(eps_cond, eps_null, cond_scale, B, n), t, tab_a, tab_b, c1, c2, sigma, None, noise, None, B, n,
+              rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def step_epilogue_multistep(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist,
+                                B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """contract of mi_step_epilogue_multistep(_w)"""
+        self._log("step_epilogue_multistep")
+        _step(x_t, _guided(eps_cond, eps_null, cond_scale, B, n), t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist, B, n,
+              rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def step_epilogue_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2, sigma, noise, B,
+                                n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """contract of mi_step_epilogue_ws: step_epilogue at the weights w_b(t[b])"""
+        self._log("step_epilogue_scheduled")
+        _step(x_t, _scheduled(eps_cond, eps_null, cond_scale, w_sched, t, B, n), t, tab_a, tab_b, c1, c2, sigma, None,
+              noise, None, B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def step_epilogue_multistep_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, tab_a, tab_b, c1, c2,
+                                          sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """contract of mi_step_epilogue_multistep_ws: step_epilogue_multistep at the weights w_b(t[b])"""
+        self._log("step_epilogue_multistep_scheduled")
+        _step(x_t, _scheduled(eps_cond, eps_null, cond_scale, w_sched, t, B, n), t, tab_a, tab_b, c1, c2, sigma, c3,
+              noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
+
+    def guidance_rescale_factor(self, eps_cond, eps_null, cond_scale, w_sched, t, phi, B, n, f):
+        """contract of mi_guidance_rescale_factor: fp64 sums of squares about the mean, f rounded once to fp32"""
+        self._log("guidance_rescale_factor")
+        c = eps_cond.reshape(B, n).double()
+        g = _scheduled(eps_cond, eps_null, cond_scale, w_sched, t, B, n).double()
+        ssc = ((c - c.mean(dim=1, keepdim=True)) ** 2).sum(dim=1)
+        ssg = ((g - g.mean(dim=1, keepdim=True)) ** 2).sum(dim=1)
+        ph = phi.double()
+        f.copy_(torch.where(ssg == 0, torch.ones_like(ssg), ph * (ssc / ssg).sqrt() + (1. - ph)).to(F32))
+
+    def step_epilogue_rescaled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, f, t, tab_a, tab_b, c1, c2, sigma, c3,
+                               noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
+        """contract of mi_step_epilogue_rescaled: the step of fp32(g * f) without a guidance pass, g the guided prediction
+        at w_b(t[b]); with c3 and hist the multistep form"""
+        self._log("step_epilogue_rescaled")
+        e = _scheduled(eps_cond, eps_null, cond_scale, w_sched, t, B, n) * f[:, None]
+        _step(x_t, e, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist, B, n, rank_lo, rank_hi, weight, min_s, out, s_out)
 
     def step_advance_t(self, t, B):
         self._log("step_advance_t")
         t.copy_((t - 1).clamp(min=0))
+
+    def step_advance_t_table(self, t, next_t, T, B):
+        self._log("step_advance_t_table")
+        inside = (t >= 0) & (t < T)
+        t.copy_(torch.where(inside, next_t[t.clamp(0, T - 1)], torch.zeros_like(t)))
 
     def step_finalize(self, x, n, unnormalize, out):
         self._log("step_finalize")
         v = x.clamp(-1., 1.)
         out.copy_((v + 1) * 0.5 if unnormalize else v)
 
+    def inpaint_prologue(self, x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
+        self._log("inpaint_prologue")
+        x.copy_(prologue_ref(x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw))
+
+    def inpaint_advance(self, t, r, next_t, R, T, B):
+        self._log("inpaint_advance")
+        nt, nr = advance_ref(t, r, next_t, R, T)
+        t.copy_(nt)
+        r.copy_(nr)
+
+    def inpaint_finalize(self, x, k, m, B, C, hw, unnormalize, out):
+        self._log("inpaint_finalize")
+        out.copy_(finalize_ref(x, k, m, B, C, hw, unnormalize))
+
     def q_sample(self, x0, noise, t, tab_a, tab_b, B, n, post_scale, post_shift, out):
         self._log("q_sample")
         v = tab_a[t][:, None] * x0.reshape(B, n) + tab_b[t][:, None] * noise.reshape(B, n)
         out.reshape(B, n).copy_(v * post_scale + post_shift)
+
+    def randn_keyed(self, out, seeds, B, n, kind, stage, t=None, r=None, R=None, label=0):
+        """contract of mi_randn_keyed: the restated generator (keyed_noise_restatement.py), rounded to fp32"""
+        self._log("randn_keyed")
+        assert seeds.dtype == torch.int64 and seeds.numel() >= B and out.dtype == torch.float32 and out.numel() == B * n
+        if t is None:
+            labels = [int(label)] * B
+        else:
+            labels = (t * (int(R[0]) if R is not None else 1) + (r if r is not None else 0)).tolist()
+        self.keyed.append((KIND_NAMES[kind], labels, stage))
+        z = K.randn_keyed(seeds.tolist()[:B], n, kind, stage, labels, np.float32)
+        out.reshape(B, n).copy_(torch.from_numpy(z))
 
 
     # ---------------------------------------------------------------- training side (contracts of the backward entry points)

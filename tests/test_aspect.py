@@ -29,12 +29,10 @@ from test_lowering_exact import exact  # noqa: F401  (the float64 host-code fixt
 from conftest import load_golden, rel_l2
 from emu_ops import EmuOps
 from oracle import restatement as R
-from test_dpmpp import DpmEmuOps
 from test_gpu_flagship_calls import pick_block_n
 from test_gpu_flagship_calls import tile_geometry as old_tile_geometry
 from test_gpu_flagship_calls import transposed_ok as old_transposed_ok
 from test_img2img import cascade, shape_bank, spy_stages
-from test_inpaint import InpaintEmuOps
 from test_respaced import _tiny_imagen
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -253,28 +251,12 @@ def _ops(cls):
     return e, prev
 
 
-@pytest.fixture
-def emu_dpm():
-    import minimagen_b200.ops as ops_mod
-    e, prev = _ops(DpmEmuOps)
-    yield e
-    ops_mod.set_ops(prev)
-
-
-@pytest.fixture
-def emu_inp():
-    import minimagen_b200.ops as ops_mod
-    e, prev = _ops(InpaintEmuOps)
-    yield e
-    ops_mod.set_ops(prev)
-
-
 def _unet_kw(g):
     return dict(text_embeds=g["text_embeds"].cpu(), text_mask=g["text_mask"].cpu())
 
 
 @pytest.mark.parametrize("sampler", ["ddim", "dpmpp_2m"])
-def test_rectangular_sample_vs_restatement(emu_dpm, sampler):
+def test_rectangular_sample_vs_restatement(emu, sampler):
     """Imagen.sample(image_sizes=((32, 48),)) on sample_loop.pt's tiny U-Net (CFG w = 3, S = 8 of T = 1000) against the
     DDIM (eta 0.5) and DPM-Solver++(2M) restatements, at the tolerance of their square tests."""
     g = load_golden("sample_loop.pt")
@@ -295,7 +277,7 @@ def test_rectangular_sample_vs_restatement(emu_dpm, sampler):
 
 
 @pytest.mark.parametrize("T,S_,R_", [(25, None, 2), (25, 5, 3)])
-def test_rectangular_inpaint_vs_restatement(emu_inp, T, S_, R_):
+def test_rectangular_inpaint_vs_restatement(emu, T, S_, R_):
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, T)
     im.use_cuda_graph = False
@@ -315,7 +297,7 @@ def test_rectangular_inpaint_vs_restatement(emu_inp, T, S_, R_):
     assert (out - img)[keep].abs().max() <= 1.2e-7
 
 
-def test_rectangular_cascade_vs_restatement(emu_dpm):
+def test_rectangular_cascade_vs_restatement(emu):
     """The tiny cascade of cascade_tiny.pt at (32, 48) -> (64, 96), CFG w = 2, with one init image at 16 x 24 for both
     stages (base on DDPM skipping 10 points, SR on 2M with S = 8 skipping 3); then the SR stage alone from start images at
     48 x 72.  Each stage against the SDEdit restatement on the inputs the product gave it."""
@@ -372,7 +354,7 @@ def test_rectangular_resize_axes():
 
 
 @pytest.mark.parametrize("sampler", ["ddim", "dpmpp_2m"])
-def test_explicit_squares_are_the_default(emu_dpm, sampler):
+def test_explicit_squares_are_the_default(emu, sampler):
     """image_sizes=None, the constructor's sizes as ints and as (s, s) pairs give the same output bit for bit."""
     outs = []
     for sizes in (None, (16, 32), ((16, 16), [32, 32])):
@@ -383,7 +365,7 @@ def test_explicit_squares_are_the_default(emu_dpm, sampler):
     assert torch.equal(outs[1], outs[0]) and torch.equal(outs[2], outs[0])
 
 
-def test_rectangular_asserts(emu_dpm):
+def test_rectangular_asserts(emu):
     im, g = cascade()
     kw = dict(text_embeds=g["text_embeds"], text_masks=g["text_mask"], sampling_timesteps=3)
     assert im.downsample_factor(im.unets[0]) == 2 and im.downsample_factor(im.unets[1]) == 4

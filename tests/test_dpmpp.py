@@ -10,51 +10,10 @@ from torch import nn
 import ddim_restatement as D
 import dpmpp_restatement as P
 from conftest import load_golden, rel_l2
-from emu_ops import EmuOps
 from test_respaced import _bank, _tiny_imagen
 
 F32 = torch.float32
 SHAPE = (2, 3, 64, 64)
-
-
-# ------------------------------------------------------------------------------------------------ torch contract
-def multistep_ref(x0, s, x_t, noise, hist, t, c1, c2, sigma, c3, B, n):
-    """Contract of mi_step_epilogue_multistep after the x0 prediction (x0 [B, n] unclamped) and the threshold s [B]:
-    (out, new hist), op by op.  The c3 term is selected away, not multiplied, where c3[t] == 0."""
-    sb = s[:, None]
-    xs = x0.reshape(B, n).clamp(-sb, sb) / sb
-    mean = c1[t][:, None] * xs + c2[t][:, None] * x_t.reshape(B, n)
-    c3t = c3[t][:, None]
-    mean = torch.where(c3t != 0, mean + c3t * hist.reshape(B, n), mean)
-    sig = torch.where(t == 0, torch.zeros_like(sigma[t]), sigma[t])[:, None]
-    return (mean + sig * noise.reshape(B, n)).reshape(x_t.shape), xs.reshape(hist.shape)
-
-
-class DpmEmuOps(EmuOps):
-    """EmuOps plus the multistep step epilogue."""
-
-    def step_epilogue_multistep(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, c1, c2, sigma, c3, noise, hist,
-                                B, n, rank_lo, rank_hi, weight, min_s, out, s_out=None):
-        self._log("step_epilogue_multistep")
-        x0 = torch.empty_like(x_t)
-        s = torch.empty(B, dtype=F32, device=x_t.device)
-        self.step_x0(x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0)
-        self.step_quantile(x0, B, n, rank_lo, rank_hi, weight, min_s, s)
-        res, h = multistep_ref(x0, s, x_t, noise, hist, t, c1, c2, sigma, c3, B, n)
-        hist.copy_(h)
-        out.copy_(res)
-        if s_out is not None:
-            s_out.copy_(s)
-
-
-@pytest.fixture
-def emu_dpm():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = DpmEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 # ------------------------------------------------------------------------------------------------ analytic denoiser
@@ -178,7 +137,7 @@ def test_two_steps_are_ddim_eta_0(T):
 
 
 # ------------------------------------------------------------------------------------------------ argument checks
-def test_sampler_asserts(emu_dpm):
+def test_sampler_asserts(emu):
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import Unet, BaseTest, SuperTest
     im = Imagen(unets=(Unet(**BaseTest.defaults), Unet(**SuperTest.defaults)), text_encoder_name="t5_small",
@@ -240,7 +199,7 @@ def test_graph_keys_of_the_three_flavours():
 
 
 # ------------------------------------------------------------------------------------------------ emulated sampler
-def test_emulated_loop_vs_restatement(emu_dpm):
+def test_emulated_loop_vs_restatement(emu):
     """S = 8 over T = 1000 with CFG w = 3 on sample_loop.pt's tiny U-Net: the product's tables through the multistep
     contract vs the paper-form restatement over the restated U-Net; one 'step' draw per grid point, like DDIM."""
     g = load_golden("sample_loop.pt")
@@ -250,7 +209,7 @@ def test_emulated_loop_vs_restatement(emu_dpm):
     out = im._p_sample_loop(im.unets[0], SHAPE, noise_scheduler=im.noise_schedulers[0], text_embeds=g["text_embeds"],
                             text_mask=g["text_mask"], cond_scale=3., schedule=sched)
     assert im.noise_fn.calls == [("init", -1)] + [("step", t) for t in P.dpm_grid(1000, 8)]
-    assert emu_dpm.calls.count("step_epilogue_multistep") == 8 and "step_epilogue" not in emu_dpm.calls
+    assert emu.calls.count("step_epilogue_multistep") == 8 and "step_epilogue" not in emu.calls
     ref = P.dpmpp_loop(g["state_dict"], g["cfg"], SHAPE, 1000, 8, _bank(7), text_embeds=g["text_embeds"].cpu(),
                        text_mask=g["text_mask"].cpu())
     err = rel_l2(out, ref)
@@ -261,7 +220,7 @@ def test_emulated_loop_vs_restatement(emu_dpm):
     assert rel_l2(ddim, out) > 1e-3                                   # a different sampler, not DDIM again
 
 
-def test_two_steps_equal_ddim_loop(emu_dpm):
+def test_two_steps_equal_ddim_loop(emu):
     g = load_golden("sample_loop.pt")
     outs = []
     for sched_of in (lambda gd: gd.dpm_solver_schedule(2, "cpu"), lambda gd: gd.sampling_schedule(2, 0., "cpu")):
@@ -273,7 +232,7 @@ def test_two_steps_equal_ddim_loop(emu_dpm):
     assert torch.equal(outs[0], outs[1])
 
 
-def test_cascade_sample_per_stage(emu_dpm):
+def test_cascade_sample_per_stage(emu):
     """sampler='dpmpp_2m' applies to the stages with a sampling_timesteps entry; a None entry keeps the DDPM loop.  Each
     stage makes one U-Net evaluation pair per grid point (CFG w = 2, unbatched)."""
     from test_host_logic import _cascade_from_golden
@@ -290,12 +249,12 @@ def test_cascade_sample_per_stage(emu_dpm):
     assert out.shape == (2, 3, 32, 32) and torch.isfinite(out).all()
     assert [s[1] for s in steps if s[0] == "step"] == list(range(24, -1, -1)) + P.dpm_grid(25, 5)
     assert len(calls) == 2 * (25 + 5)
-    assert emu_dpm.calls.count("step_epilogue") == 25 and emu_dpm.calls.count("step_epilogue_multistep") == 5
+    assert emu.calls.count("step_epilogue") == 25 and emu.calls.count("step_epilogue_multistep") == 5
 
 
 # ------------------------------------------------------------------------------------------------ analytic convergence
 @pytest.mark.parametrize("S", [10, 20, 50])
-def test_analytic_convergence(emu_dpm, S):
+def test_analytic_convergence(emu, S):
     """On the analytic denoiser (cond_scale 1), 2M's final x0 is at least 10x closer to the exact ODE end point than DDIM
     eta = 0's and 5x closer than the first-order walk over the same log-SNR grid (fp64 ratios: 46 / 23 / 69 and
     18 / 8 / 21 at S = 10 / 20 / 50)."""

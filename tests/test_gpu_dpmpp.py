@@ -7,7 +7,8 @@ import torch
 
 import dpmpp_restatement as P
 from conftest import load_golden, rel_l2
-from test_dpmpp import DpmEmuOps, SHAPE, AnalyticEps, analytic_errors, multistep_ref
+from emu_ops import EmuOps, multistep_ref
+from test_dpmpp import SHAPE, AnalyticEps, analytic_errors
 from test_gpu_inpaint import _capture
 from test_respaced import _bank, _tiny_imagen
 
@@ -221,7 +222,7 @@ def test_cascade_vs_cpu_emulation(native):
     for dev in ("cuda", "cpu"):
         prev = ops_mod._OPS
         if dev == "cpu":
-            ops_mod.set_ops(DpmEmuOps())
+            ops_mod.set_ops(EmuOps())
         try:
             im, _ = _cascade_from_golden(g, dev)
             im.noise_fn = noise_fn

@@ -36,7 +36,6 @@ import fp64_ref as R
 from checking_ops import ALLOWED, CheckingOps
 from emu_ops import EmuOps
 from fp64_ref import check, check_rel_l2
-from test_dpmpp import DpmEmuOps
 from test_gpu_conv_transposed import conv_instance
 from test_gpu_lowering_calls import _inputs
 from test_gpu_sampler_ops import FUSED_MAX, _nan_equal, _tabs_cuda
@@ -336,7 +335,7 @@ def test_step_epilogue_many_cluster_waves(native, B, n, kind):
     oe, se, he = torch.empty(B, n), torch.empty(B), hist.clone()
     ct = [v.cpu() if v is not None else None for v in tabs]
     if multi:
-        DpmEmuOps().step_epilogue_multistep(xb, eb, eps0, 3.0, t, *ct, noise, he, B, n, lo, hi, wt, 1.0, oe, s_out=se)
+        EmuOps().step_epilogue_multistep(xb, eb, eps0, 3.0, t, *ct, noise, he, B, n, lo, hi, wt, 1.0, oe, s_out=se)
     else:
         EmuOps().step_epilogue(xb, eb, eps0, 3.0, t, *ct[:5], noise, B, n, lo, hi, wt, 1.0, oe, s_out=se)
     bad = torch.zeros(B, dtype=torch.bool)

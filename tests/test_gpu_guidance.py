@@ -6,8 +6,9 @@ import pytest
 import torch
 
 from conftest import load_golden, rel_l2
+from emu_ops import EmuOps
 from test_gpu_inpaint import _inp
-from test_guidance import GuidanceEmuOps, _negative
+from test_guidance import _negative
 from test_respaced import _bank, _tiny_imagen
 
 pytestmark = pytest.mark.gpu
@@ -143,7 +144,7 @@ def test_native_vs_emulated(native):
     for dev in ("cuda", "cpu"):
         prev = ops_mod._OPS
         if dev == "cpu":
-            ops_mod.set_ops(GuidanceEmuOps())
+            ops_mod.set_ops(EmuOps())
         try:
             im = _tiny_imagen(g, 1000, dev)
             im.noise_fn = _bank(4)

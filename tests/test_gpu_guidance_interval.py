@@ -6,11 +6,11 @@ import pytest
 import torch
 
 import guidance_interval_restatement as G
+from fp64_ref import scheduled_weights
 from checking_ops import ALLOWED, CheckingOps
 from conftest import load_golden, rel_l2
 from test_gpu_inpaint import _inp
 from test_guidance import _negative
-from test_guidance_interval import scheduled_weights
 from test_respaced import _bank, _tiny_imagen
 
 pytestmark = pytest.mark.gpu
@@ -43,7 +43,7 @@ def test_scheduled_is_the_weight_array(native, B, side, multistep):
     w = torch.tensor([3., 0.5, 7.25, 1.][:B], device="cuda")
     if B == 2:
         w[1] = 1.
-    w_eff = scheduled_weights(w, tab, t, B)
+    w_eff = scheduled_weights(w, tab, t, B).cuda()
     assert w_eff.tolist() == [G.weights([wb], sb)[0] for wb, sb in zip(w.tolist(), s)]
 
     def run(scheduled):

@@ -6,8 +6,8 @@ import torch
 
 import inpaint_restatement as P
 from conftest import load_golden, rel_l2
-from test_inpaint import (InpaintEmuOps, SHAPE, advance_ref, finalize_ref, known_and_mask, prologue_ref,
-                          restated_tiny)
+from emu_ops import EmuOps, advance_ref, finalize_ref, prologue_ref
+from test_inpaint import SHAPE, known_and_mask, restated_tiny
 from test_respaced import _bank, _tiny_imagen
 
 pytestmark = pytest.mark.gpu
@@ -253,7 +253,7 @@ def test_cascade_vs_cpu_emulation(native):
     for dev in ("cuda", "cpu"):
         prev = ops_mod._OPS
         if dev == "cpu":
-            ops_mod.set_ops(InpaintEmuOps())
+            ops_mod.set_ops(EmuOps())
         try:
             im, _ = _cascade_from_golden(g, dev)
             im.noise_fn = noise_fn

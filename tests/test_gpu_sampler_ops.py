@@ -8,13 +8,11 @@ import torch
 import fp64_ref as R
 from emu_ops import EmuOps
 from fp64_ref import check, check_rel_l2
-from test_dpmpp import DpmEmuOps
 from test_error_bounds import _schedule
 
 pytestmark = pytest.mark.gpu
 
 EMU = EmuOps()
-DPM_EMU = DpmEmuOps()
 T = 1000
 FUSED_MAX = 196608                          # the largest image the fused cluster kernel holds in registers
 SIZES = [1, 3, 9, 768, 3 * 64 * 64, FUSED_MAX, FUSED_MAX + 1, 3 * 288 * 288]
@@ -209,7 +207,7 @@ def test_step_nan_and_inf_parity(native, n, multi):
         out, s, h = torch.empty(B, n), torch.empty(B), hist.clone()
         ct = [v.cpu() for v in tabs if v is not None]
         if multi:
-            DPM_EMU.step_epilogue_multistep(xx, ee, eps0, 3.0, t, *ct[:5], ct[5], noise, h, B, n, lo, hi, wt, 1.0, out,
+            EMU.step_epilogue_multistep(xx, ee, eps0, 3.0, t, *ct[:5], ct[5], noise, h, B, n, lo, hi, wt, 1.0, out,
                                             s_out=s)
         else:
             EMU.step_epilogue(xx, ee, eps0, 3.0, t, *ct[:5], noise, B, n, lo, hi, wt, 1.0, out, s_out=s)

@@ -8,8 +8,8 @@ import torch
 
 import keyed_noise_restatement as K
 from conftest import load_golden, rel_l2
+from emu_ops import EmuOps
 from test_respaced import _tiny_imagen
-from test_seeded import SeededEmuOps
 
 pytestmark = pytest.mark.gpu
 I64 = torch.int64
@@ -173,7 +173,7 @@ def test_native_vs_emulated(native):
     for dev in ("cuda", "cpu"):
         prev = ops_mod._OPS
         if dev == "cpu":
-            ops_mod.set_ops(SeededEmuOps())
+            ops_mod.set_ops(EmuOps())
         try:
             im = _tiny_imagen(g, 1000, dev)
             outs[dev] = im.sample(text_embeds=g["text_embeds"].to(dev), text_masks=g["text_mask"].to(dev),

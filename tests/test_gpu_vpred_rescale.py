@@ -10,7 +10,6 @@ import pytest
 import torch
 
 import fp64_ref as R
-import rescale_ops as RO
 from checking_ops import ALLOWED, CheckingOps
 from conftest import load_golden, rel_l2
 from test_gpu_inpaint import _inp
@@ -51,7 +50,7 @@ def test_factor_within_one_ulp(native, B, side, table):
     phi = torch.rand(B, generator=gen).cuda()
     f = torch.empty(B, device="cuda")
     native.guidance_rescale_factor(c.cuda(), u.cuda(), w, w_sched, t, phi, B, n, f)
-    ref, bound = RO.rescale_factor_ref(c, u, w, w_sched, t, phi, B, n)
+    ref, bound = R.rescale_factor_ref(c, u, w, w_sched, t, phi, B, n)
     R.check(f, ref, bound, f"factor B={B} n={n}")
     f2 = torch.empty(B, device="cuda")
     native.guidance_rescale_factor(c.cuda(), u.cuda(), w, w_sched, t, phi, B, n, f2)
@@ -68,7 +67,7 @@ def test_factor_edge_images(native, side):
     f = torch.empty(B, device="cuda")
     native.guidance_rescale_factor(c.cuda(), u.cuda(), w, None, t, phi, B, n, f)
     assert f[1] == 1 and torch.isnan(f[2])
-    ref, bound = RO.rescale_factor_ref(c, u, w, None, t, phi, B, n)
+    ref, bound = R.rescale_factor_ref(c, u, w, None, t, phi, B, n)
     keep = torch.tensor([0, 3])
     print(f"offset image: f = {float(f[3]):.9g}, float64 {float(ref[3]):.9g}")
     R.check(f[keep.cuda()], ref[keep], bound[keep], f"factor edge images n={n}")
@@ -103,7 +102,7 @@ def test_rescaled_epilogue_is_the_plain_epilogue(native, B, side, multistep, tab
     out, h, s = torch.empty_like(x), hist.clone() if multistep else None, torch.empty(B, device="cuda")
     native.step_epilogue_rescaled(x, c, u, w, w_sched, f, t, a, b, sch.c1, sch.c2, sch.sigma, c3, noise, h, B, n, lo, hi,
                                   wq, 1.0, out, s_out=s)
-    eps = RO.rescaled_eps_fp32(c, u, w, w_sched, t, f, B, n).cuda()
+    eps = R.rescaled_eps_fp32(c, u, w, w_sched, t, f, B, n).cuda()
     want, wh = torch.empty_like(x), hist.clone() if multistep else None
     if multistep:
         native.step_epilogue_multistep(x, eps, None, 1.0, t, a, b, sch.c1, sch.c2, sch.sigma, c3, noise, wh, B, n, lo, hi,

@@ -15,32 +15,11 @@ import torch.multiprocessing as mp
 
 from conftest import load_golden, rel_l2
 from negprompt_restatement import negprompt_loop
-from test_dpmpp import DpmEmuOps
+from emu_ops import EmuOps
 from test_respaced import _bank, _tiny_imagen
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-F32 = torch.float32
 SHAPE = (2, 3, 64, 64)
-
-
-class GuidanceEmuOps(DpmEmuOps):
-    """DpmEmuOps whose step epilogues also take cond_scale as a [B] tensor of per-image weights (the _w entry points)."""
-
-    def step_x0(self, x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0):
-        if torch.is_tensor(cond_scale):
-            assert cond_scale.dtype == F32 and cond_scale.numel() == B
-            cond_scale = cond_scale.reshape(B, 1)
-        super().step_x0(x_t, eps_cond, eps_null, cond_scale, t, tab_a, tab_b, B, n, x0)
-
-
-@pytest.fixture
-def emu_g():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = GuidanceEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 def _negative(b=2, L=6, seed=11):
@@ -70,7 +49,7 @@ def _count_forwards(unet):
 
 # ------------------------------------------------------------------------------------------------ against the restatement
 @pytest.mark.parametrize("T,steps,eta", [(25, None, 0.), (1000, 8, 0.5)])
-def test_emulated_loop_vs_restatement(emu_g, T, steps, eta):
+def test_emulated_loop_vs_restatement(emu, T, steps, eta):
     """Negative prompt (one row's mask partly False) and per-image weights (2, 4.5) on sample_loop.pt's tiny U-Net, DDPM
     over T = 25 and DDIM S = 8 over T = 1000, vs the restated loop over the restated U-Net."""
     g = load_golden("sample_loop.pt")
@@ -84,10 +63,10 @@ def test_emulated_loop_vs_restatement(emu_g, T, steps, eta):
     err = rel_l2(out, ref)
     print(f"T={T} steps={steps}: rel-L2 vs restated negative-prompt loop = {err:.3e}")
     assert err < 1e-3
-    assert emu_g.calls.count("step_epilogue") == (T if steps is None else steps)
+    assert emu.calls.count("step_epilogue") == (T if steps is None else steps)
 
 
-def test_equal_weights_vector_is_the_scalar(emu_g):
+def test_equal_weights_vector_is_the_scalar(emu):
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 1000)
     nte, ntm = _negative()
@@ -97,7 +76,7 @@ def test_equal_weights_vector_is_the_scalar(emu_g):
         assert torch.equal(a, b)
 
 
-def test_all_ones_runs_one_pass_and_is_cond_scale_1(emu_g):
+def test_all_ones_runs_one_pass_and_is_cond_scale_1(emu):
     """An all-ones weight vector runs one U-Net pass per step, whatever negative is given, and gives cond_scale=1's bits."""
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 1000)
@@ -113,7 +92,7 @@ def test_all_ones_runs_one_pass_and_is_cond_scale_1(emu_g):
     assert len(calls) == 12
 
 
-def test_no_negative_is_the_null_guidance(emu_g):
+def test_no_negative_is_the_null_guidance(emu):
     """Without a negative the guidance pass is the reference's null pass (cond_drop_prob 1): bit for bit the loop of
     Unet.forward_with_cond_scale's combine fed to the step as its model output."""
     g = load_golden("sample_loop.pt")
@@ -141,7 +120,7 @@ def test_no_negative_is_the_null_guidance(emu_g):
 
 
 @pytest.mark.parametrize("case", ["equal", "padded", "no_mask", "no_masks_equal"])
-def test_cfg_batched_with_negative(emu_g, case):
+def test_cfg_batched_with_negative(emu, case):
     """cfg_batched puts the negative pass in the 2B batch when padding is exact (both masks, any lengths; or no masks and
     equal lengths) and falls back to two passes otherwise; either way it matches the unbatched path."""
     g = load_golden("sample_loop.pt")
@@ -170,7 +149,7 @@ def test_cfg_batched_with_negative(emu_g, case):
     assert (4 in batched) == (case != "no_mask")
 
 
-def test_cascade_per_unet_scales_equal_stage_by_stage(emu_g):
+def test_cascade_per_unet_scales_equal_stage_by_stage(emu):
     """cond_scale=(w1, w2) on the tiny cascade == stage 1 alone at w1, then stage 2 alone at w2 from its output."""
     from test_host_logic import _cascade_from_golden
     g = load_golden("cascade_tiny.pt")
@@ -196,7 +175,7 @@ def test_cascade_per_unet_scales_equal_stage_by_stage(emu_g):
     assert not torch.equal(other, both)
 
 
-def test_negative_texts_are_encoded(emu_g, monkeypatch):
+def test_negative_texts_are_encoded(emu, monkeypatch):
     """negative_texts go through t5_encode_text like texts; one str is used for every image."""
     import minimagen_b200.Imagen as I
     nte, ntm = _negative(b=1, L=5)
@@ -222,7 +201,7 @@ def test_negative_texts_are_encoded(emu_g, monkeypatch):
     assert seen[-1] == ["a", "b"]
 
 
-def test_argument_checks(emu_g):
+def test_argument_checks(emu):
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import Unet, BaseTest, SuperTest
     im = Imagen(unets=(Unet(**BaseTest.defaults), Unet(**SuperTest.defaults)), text_encoder_name="t5_small",
@@ -324,7 +303,7 @@ def _worker(rank, world, port, out_path):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     import minimagen_b200.ops as ops_mod
     from test_distributed_cpu import _build, _noise_bank
-    ops_mod.set_ops(GuidanceEmuOps())
+    ops_mod.set_ops(EmuOps())
     g = torch.load(os.path.join(ROOT, "tests", "golden", "sample_loop.pt"), map_location="cpu", weights_only=False)
     im = _build(g)
     B = 4
@@ -340,7 +319,7 @@ def _worker(rank, world, port, out_path):
 
 
 @pytest.mark.timeout(600)
-def test_two_rank_gloo_with_negative_and_per_image_scales(tmp_path, emu_g):
+def test_two_rank_gloo_with_negative_and_per_image_scales(tmp_path, emu):
     from test_distributed_cpu import _build, _noise_bank
     port = 29400 + (os.getpid() % 200)
     out_path = str(tmp_path / "dist_out.pt")

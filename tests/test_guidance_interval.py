@@ -15,50 +15,14 @@ import torch.multiprocessing as mp
 
 import guidance_interval_restatement as G
 from conftest import load_golden, rel_l2
-from test_guidance import GuidanceEmuOps, _count_forwards, _negative
-from test_inpaint import InpaintEmuOps
+from emu_ops import EmuOps
+from test_guidance import _count_forwards, _negative
 from test_respaced import _bank, _tiny_imagen
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32 = torch.float32
 SHAPE = (2, 3, 64, 64)
 INF = float("inf")
-
-
-def scheduled_weights(cond_scale, w_sched, t, B):
-    """w_b(t[b]) as an fp32 [B] tensor, op by op: w_b where the table is 1, else 1 + (w_b - 1) * table[t]."""
-    w = cond_scale.to(F32) if torch.is_tensor(cond_scale) else torch.full((B,), float(cond_scale), dtype=F32)
-    s = w_sched[t].to(w.device)
-    return torch.where(s == 1, w, 1 + (w - 1) * s)
-
-
-class IntervalEmuOps(GuidanceEmuOps, InpaintEmuOps):
-    """GuidanceEmuOps (and the RePaint kernels) plus the scheduled step epilogues: the _w contract at the weights
-    w_b(t[b])."""
-
-    def _as(self, name, fn, *args, **kw):
-        at = len(self.calls)
-        fn(*args, **kw)
-        self.calls[at] = name
-
-    def step_epilogue_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, *rest, **kw):
-        w = scheduled_weights(cond_scale, w_sched, t, x_t.shape[0])
-        self._as("step_epilogue_scheduled", self.step_epilogue, x_t, eps_cond, eps_null, w, t, *rest, **kw)
-
-    def step_epilogue_multistep_scheduled(self, x_t, eps_cond, eps_null, cond_scale, w_sched, t, *rest, **kw):
-        w = scheduled_weights(cond_scale, w_sched, t, x_t.shape[0])
-        self._as("step_epilogue_multistep_scheduled", self.step_epilogue_multistep, x_t, eps_cond, eps_null, w, t, *rest,
-                 **kw)
-
-
-@pytest.fixture
-def emu_i():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = IntervalEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 def _walk(sch, sampler, steps, eta=0.):
@@ -114,7 +78,7 @@ LOOPS = [("ddpm", 25, None, 0., (0.5, 10.)), ("ddim", 1000, 8, 0.5, (0.4, 20.)),
 
 @pytest.mark.parametrize("sampler,T,steps,eta,interval", LOOPS, ids=[c[0] for c in LOOPS])
 @pytest.mark.parametrize("schedule", [None, "linear", "cosine"])
-def test_emulated_loop_vs_restatement(emu_i, sampler, T, steps, eta, interval, schedule):
+def test_emulated_loop_vs_restatement(emu, sampler, T, steps, eta, interval, schedule):
     """Interval and schedule with a negative prompt and per-image weights (2, 4.5), against the restated loop over the
     restated U-Net; the U-Net runs S + k times for k guided points, the scheduled epilogue k times."""
     g = load_golden("sample_loop.pt")
@@ -133,27 +97,27 @@ def test_emulated_loop_vs_restatement(emu_i, sampler, T, steps, eta, interval, s
     assert 0 < len(guided) < S
     assert len(calls) == S + len(guided)
     step = "step_epilogue_multistep" if sampler == "dpmpp_2m" else "step_epilogue"
-    assert emu_i.calls.count(step + "_scheduled") == len(guided)
-    assert emu_i.calls.count(step) == S - len(guided)
+    assert emu.calls.count(step + "_scheduled") == len(guided)
+    assert emu.calls.count(step) == S - len(guided)
 
 
 # ------------------------------------------------------------------------------------------------ identities
 @pytest.mark.parametrize("sampler", ["ddpm", "ddim", "dpmpp_2m"])
-def test_ones_table_is_the_loop_without_it(emu_i, sampler):
+def test_ones_table_is_the_loop_without_it(emu, sampler):
     """A covering interval (no schedule) is bit for bit the loop without arguments, through the same entry points."""
     g = load_golden("sample_loop.pt")
     nte, ntm = _negative()
     outs, logs = [], []
     for interval in (None, (0., INF)):
         im = _tiny_imagen(g, 25)
-        del emu_i.calls[:]
+        del emu.calls[:]
         outs.append(_loop(im, g, sampler, 6, 0.5, torch.tensor([2., 4.5]), interval, None, nte, ntm)[0])
-        logs.append(list(emu_i.calls))
+        logs.append(list(emu.calls))
     assert torch.equal(outs[0], outs[1]) and logs[0] == logs[1]
     assert not any(c.endswith("_scheduled") for c in logs[1])
 
 
-def test_skipped_points_do_not_count(emu_i):
+def test_skipped_points_do_not_count(emu):
     """A table that is 1 on the points a shortened walk visits (and 0 at the first one it skips) runs the loop without
     it, the same entry points and bits; so does one that is 1 at every point but not on all timesteps."""
     g = load_golden("sample_loop.pt")
@@ -169,16 +133,16 @@ def test_skipped_points_do_not_count(emu_i):
     init = torch.rand(SHAPE, generator=torch.Generator().manual_seed(3)) * 2 - 1
     for table in (None, tab):
         im.noise_fn = _bank(7)
-        del emu_i.calls[:]
+        del emu.calls[:]
         outs.append(im._p_sample_loop(im.unets[0], SHAPE, noise_scheduler=sch, text_embeds=g["text_embeds"],
                                       text_mask=g["text_mask"], cond_scale=3., schedule=short, init_image=init,
                                       guidance_table=table))
-        logs.append([c for c in emu_i.calls if c.startswith("step")])     # (the first run also packs the weights)
+        logs.append([c for c in emu.calls if c.startswith("step")])     # (the first run also packs the weights)
     assert torch.equal(outs[0], outs[1]) and logs[0] == logs[1]
 
 
 @pytest.mark.parametrize("sampler", ["ddim", "dpmpp_2m"])
-def test_zeros_table_is_the_unguided_loop(emu_i, sampler):
+def test_zeros_table_is_the_unguided_loop(emu, sampler):
     """An interval that holds no point of the walk runs the cond_scale = 1 loop bit for bit, one U-Net pass per point,
     and never conditions on the negative prompt."""
     g = load_golden("sample_loop.pt")
@@ -192,17 +156,17 @@ def test_zeros_table_is_the_unguided_loop(emu_i, sampler):
     assert len(calls) == 6 and all(kw.get("text_embeds") is g["text_embeds"] for kw in calls)
 
 
-def test_unguided_stage_ignores_the_table(emu_i):
+def test_unguided_stage_ignores_the_table(emu):
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 1000)
     calls = _count_forwards(im.unets[0])
     a, _ = _loop(im, g, "ddim", 6, 0.5, 1.)
     b, _ = _loop(im, g, "ddim", 6, 0.5, torch.ones(2), (0.4, 20.), "cosine")
     assert torch.equal(a, b) and len(calls) == 12
-    assert "step_epilogue_scheduled" not in emu_i.calls
+    assert "step_epilogue_scheduled" not in emu.calls
 
 
-def test_draws_do_not_change(emu_i):
+def test_draws_do_not_change(emu):
     """The same noise_fn calls, in the same order, with and without an interval and a schedule (DDIM eta > 0, RePaint)."""
     g = load_golden("sample_loop.pt")
     gen = torch.Generator().manual_seed(2)
@@ -217,7 +181,7 @@ def test_draws_do_not_change(emu_i):
         assert seqs[0] == seqs[1] and len(seqs[0]) > 6
 
 
-def test_inpainting_iterations_follow_their_t(emu_i):
+def test_inpainting_iterations_follow_their_t(emu):
     """RePaint with R = 2: each iteration (t, r) runs the guidance pass iff t is guided; a covering interval is the loop
     without it."""
     g = load_golden("sample_loop.pt")
@@ -241,7 +205,7 @@ def test_inpainting_iterations_follow_their_t(emu_i):
     assert torch.equal(plain, cover) and rel_l2(out, plain) > 1e-3
 
 
-def test_cfg_batched(emu_i):
+def test_cfg_batched(emu):
     """cfg_batched runs the guidance pass in the 2B batch at the guided points only, and matches the unbatched loop."""
     g = load_golden("sample_loop.pt")
     nte, ntm = _negative(L=9)
@@ -259,7 +223,7 @@ def test_cfg_batched(emu_i):
     assert 0 < k < 8 and batched.count(4) == k
 
 
-def test_cascade_per_unet_entries_equal_stage_by_stage(emu_i):
+def test_cascade_per_unet_entries_equal_stage_by_stage(emu):
     """guidance_interval=(None, pair) and guidance_schedule=('linear', None) on the tiny cascade == stage 1 alone with
     'linear', then stage 2 alone with the pair."""
     from test_host_logic import _cascade_from_golden
@@ -286,7 +250,7 @@ def test_cascade_per_unet_entries_equal_stage_by_stage(emu_i):
     assert not torch.equal(im.sample(**kw), both)
 
 
-def test_argument_checks(emu_i):
+def test_argument_checks(emu):
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import Unet, BaseTest, SuperTest
     im = Imagen(unets=(Unet(**BaseTest.defaults), Unet(**SuperTest.defaults)), text_encoder_name="t5_small",
@@ -368,7 +332,7 @@ def _worker(rank, world, port, out_path):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     import minimagen_b200.ops as ops_mod
     from test_distributed_cpu import _build, _noise_bank
-    ops_mod.set_ops(IntervalEmuOps())
+    ops_mod.set_ops(EmuOps())
     g = torch.load(os.path.join(ROOT, "tests", "golden", "sample_loop.pt"), map_location="cpu", weights_only=False)
     im = _build(g)
     B = 4
@@ -384,7 +348,7 @@ def _worker(rank, world, port, out_path):
 
 
 @pytest.mark.timeout(600)
-def test_two_rank_gloo(tmp_path, emu_i):
+def test_two_rank_gloo(tmp_path, emu):
     from test_distributed_cpu import _build, _noise_bank
     port = 29600 + (os.getpid() % 200)
     out_path = str(tmp_path / "dist_out.pt")

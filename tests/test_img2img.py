@@ -15,20 +15,10 @@ import torch.multiprocessing as mp
 import ddim_restatement as D
 import img2img_restatement as S
 from conftest import load_golden, rel_l2
-from test_dpmpp import MU, SD, SHAPE, AnalyticEps, DpmEmuOps
+from test_dpmpp import MU, SD, SHAPE, AnalyticEps
 from test_respaced import _bank, _tiny_imagen
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture
-def emu_dpm():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = DpmEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 def init_image(seed, shape=SHAPE):
@@ -100,7 +90,7 @@ CASES = [(25, None, 0., "ddim", 10), (1000, 8, 0., "ddim", 3), (1000, 8, 0.5, "d
 
 
 @pytest.mark.parametrize("T,S_,eta,sampler,skip", CASES)
-def test_emulated_sample_vs_restatement(emu_dpm, T, S_, eta, sampler, skip):
+def test_emulated_sample_vs_restatement(emu, T, S_, eta, sampler, skip):
     """Imagen.sample(init_images=, skip_steps=) on sample_loop.pt's tiny U-Net (CFG w = 3) against the SDEdit
     restatement: DDPM, DDIM (eta 0, 0.5) and 2M; the draws are 'init', then one 'step' per point from grid[skip] on."""
     g = load_golden("sample_loop.pt")
@@ -118,7 +108,7 @@ def test_emulated_sample_vs_restatement(emu_dpm, T, S_, eta, sampler, skip):
     assert err < 1e-3
 
 
-def test_cascade_stages_vs_restatement(emu_dpm):
+def test_cascade_stages_vs_restatement(emu):
     """The two-stage cascade of cascade_tiny.pt (16 -> 32, CFG w = 2) with one init image at 32x32 for both stages: the
     base stage on DDPM skipping 10 points, the SR stage on 2M (S = 8) skipping 3.  Each stage against the SDEdit
     restatement on the inputs the product gave it (its resized init image and its low-res conditioning)."""
@@ -183,7 +173,7 @@ def analytic_img2img_errors(device, steps, graph):
     return errs, outs
 
 
-def test_analytic_convergence_from_init_image(emu_dpm):
+def test_analytic_convergence_from_init_image(emu):
     """From grid[S // 2], 2M's final x0 is at least 10x closer to the exact end point than DDIM eta = 0's and 2x closer
     than 2M's tables without the first-order restart (fp64 ratios: 106 / 27 / 75 and 24 / 3.0 / 5.1 at S = 10 / 20 / 50);
     DDIM and 2M are closer at S = 50 than at S = 10."""
@@ -199,7 +189,7 @@ def test_analytic_convergence_from_init_image(emu_dpm):
 
 
 # ------------------------------------------------------------------------------------------------ cascade entry and exit
-def test_cascade_entry_and_exit_bitwise(emu_dpm):
+def test_cascade_entry_and_exit_bitwise(emu):
     """stop_at_unet_number=1 returns the first stage's output of a full run; start_at_unet_number=2 from that output
     returns the full run's output bit for bit, with the SR stage's draws only."""
     im, g = cascade()
@@ -223,7 +213,7 @@ def test_cascade_entry_and_exit_bitwise(emu_dpm):
 
 
 @pytest.mark.parametrize("sampler", ["ddim", "dpmpp_2m"])
-def test_neutral_arguments_change_nothing(emu_dpm, sampler):
+def test_neutral_arguments_change_nothing(emu, sampler):
     """skip_steps 0, no init or start images and the full stage range give the default call's output bit for bit."""
     outs = []
     for extra in ({}, dict(init_images=None, skip_steps=0, start_at_unet_number=1, start_images=None,
@@ -236,7 +226,7 @@ def test_neutral_arguments_change_nothing(emu_dpm, sampler):
 
 
 # ------------------------------------------------------------------------------------------------ argument checks
-def test_img2img_asserts(emu_dpm):
+def test_img2img_asserts(emu):
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import Unet, BaseTest, SuperTest
     im = Imagen(unets=(Unet(**BaseTest.defaults), Unet(**SuperTest.defaults)), text_encoder_name="t5_small",

@@ -9,65 +9,10 @@ import torch
 import ddim_restatement as D
 import inpaint_restatement as P
 from conftest import load_golden, rel_l2
-from emu_ops import EmuOps
 from oracle import restatement as R
 from test_respaced import _bank, _tiny_imagen
 
 SHAPE = (2, 3, 64, 64)
-
-
-# ------------------------------------------------------------------------------------------------ torch contracts
-def prologue_ref(x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
-    """Contract of mi_inpaint_prologue, op for op (x is returned, not modified)."""
-    xv = x.reshape(B, C, hw)
-    valid = ((t >= 0) & (t < T))[:, None, None]
-    tc = t.clamp(0, T - 1)
-    col = lambda tab: tab[tc][:, None, None]
-    v = torch.where((r > 0)[:, None, None], col(ra) * xv + col(rb) * z_renoise.reshape(B, C, hw), xv)
-    v = torch.where(m.reshape(B, 1, hw) >= 0.5, col(sqrt_acp) * k.reshape(B, C, hw) + col(sqrt_1m_acp) *
-                    z_known.reshape(B, C, hw), v)
-    return torch.where(valid, v, xv).reshape(x.shape)
-
-
-def advance_ref(t, r, next_t, R, T):
-    """Contract of mi_inpaint_advance: the new (t, r)."""
-    valid = (t >= 0) & (t < T)
-    rep = valid & (t > 0) & (r + 1 < R.reshape(-1)[0])
-    nt = torch.where(valid, next_t[t.clamp(0, T - 1)], torch.zeros_like(t))
-    return torch.where(rep, t, nt), torch.where(rep, r + 1, torch.zeros_like(r))
-
-
-def finalize_ref(x, k, m, B, C, hw, unnormalize):
-    v = torch.where(m.reshape(B, 1, hw) >= 0.5, k.reshape(B, C, hw), x.reshape(B, C, hw)).clamp(-1., 1.)
-    return ((v + 1) * 0.5 if unnormalize else v).reshape(x.shape)
-
-
-class InpaintEmuOps(EmuOps):
-    """EmuOps plus the inpainting entry points."""
-
-    def inpaint_prologue(self, x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
-        self._log("inpaint_prologue")
-        x.copy_(prologue_ref(x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw))
-
-    def inpaint_advance(self, t, r, next_t, R, T, B):
-        self._log("inpaint_advance")
-        nt, nr = advance_ref(t, r, next_t, R, T)
-        t.copy_(nt)
-        r.copy_(nr)
-
-    def inpaint_finalize(self, x, k, m, B, C, hw, unnormalize, out):
-        self._log("inpaint_finalize")
-        out.copy_(finalize_ref(x, k, m, B, C, hw, unnormalize))
-
-
-@pytest.fixture
-def emu_inp():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = InpaintEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 def known_and_mask(seed, shape=SHAPE, frac=0.5):
@@ -123,7 +68,7 @@ def test_ddim_tables_follow_the_grid(S):
 
 # ------------------------------------------------------------------------------------------------ plan and draws
 @pytest.mark.parametrize("R_", [1, 3])
-def test_plan_and_draw_sequence(emu_inp, R_):
+def test_plan_and_draw_sequence(emu, R_):
     """(S - 1) R + 1 iterations, draws 'renoise' (r > 0), 'inpaint', 'step' labelled t * R + r; at R = 1 the 'step'
     labels are those of the plain DDIM loop."""
     g = load_golden("sample_loop.pt")
@@ -138,13 +83,13 @@ def test_plan_and_draw_sequence(emu_inp, R_):
         for r in range(R_ if t > 0 else 1):
             want += ([("renoise", t * R_ + r)] if r > 0 else []) + [("inpaint", t * R_ + r), ("step", t * R_ + r)]
     assert im.noise_fn.calls == want
-    assert len(P.plan(25, R_, 4)) == (4 - 1) * R_ + 1 == emu_inp.calls.count("inpaint_prologue")
-    assert emu_inp.calls.count("step_epilogue") == (4 - 1) * R_ + 1
+    assert len(P.plan(25, R_, 4)) == (4 - 1) * R_ + 1 == emu.calls.count("inpaint_prologue")
+    assert emu.calls.count("step_epilogue") == (4 - 1) * R_ + 1
     if R_ == 1:
         assert [c for c in want if c[0] == "step"] == [("step", t) for t in grid]
 
 
-def test_max_steps_counts_iterations(emu_inp):
+def test_max_steps_counts_iterations(emu):
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 25)
     im.use_cuda_graph = False
@@ -201,7 +146,7 @@ def test_graph_key_ignores_the_walk():
 
 
 # ------------------------------------------------------------------------------------------------ argument checks
-def test_inpaint_asserts(emu_inp):
+def test_inpaint_asserts(emu):
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import Unet, BaseTest, SuperTest
     im = Imagen(unets=(Unet(**BaseTest.defaults), Unet(**SuperTest.defaults)), text_encoder_name="t5_small",
@@ -257,7 +202,7 @@ def test_restatement_r1_nothing_known_is_the_plain_loop():
 
 # ------------------------------------------------------------------------------------------------ emulated sampler
 @pytest.mark.parametrize("T,S,R_", [(25, None, 2), (25, 5, 3)])
-def test_emulated_sample_vs_restatement(emu_inp, T, S, R_):
+def test_emulated_sample_vs_restatement(emu, T, S, R_):
     """Imagen.sample with inpainting (CFG w = 3, random mask) on sample_loop.pt's tiny U-Net, DDPM and DDIM (eta 0.5),
     against the RePaint-form restatement over the restated U-Net; the known pixels are the inputs."""
     g = load_golden("sample_loop.pt")

@@ -16,7 +16,7 @@ import torch
 
 from checking_ops import CheckingOps
 from conftest import load_golden
-from test_dpmpp import DpmEmuOps
+from emu_ops import EmuOps
 from test_error_bounds import _schedule, _step_data, step_fp32
 from test_respaced import _tiny_imagen
 
@@ -25,30 +25,13 @@ LOOP = {"step_epilogue", "step_epilogue_multistep", "step_advance_t", "step_adva
         "resize_separable", "q_sample"}
 
 
-class LoopEmuOps(DpmEmuOps):
-    """DpmEmuOps plus the respaced walk's timestep table."""
-
-    def step_advance_t_table(self, t, next_t, T, B):
-        self._log("step_advance_t_table")
-        inside = (t >= 0) & (t < T)
-        t.copy_(torch.where(inside, next_t[t.clamp(0, T - 1)], torch.zeros_like(t)))
-
-
-@pytest.fixture
-def loop_emu():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    yield LoopEmuOps()
-    ops_mod.set_ops(prev)
-
-
 @pytest.mark.parametrize("sampler", ["ddim", "dpmpp_2m"])
-def test_emulated_sampling_loop_passes_every_step_check(loop_emu, sampler):
+def test_emulated_sampling_loop_passes_every_step_check(emu, sampler):
     import minimagen_b200.ops as ops_mod
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 1000)
     im.use_cuda_graph = False
-    proxy = CheckingOps(loop_emu, sms=SMS, only=LOOP)
+    proxy = CheckingOps(emu, sms=SMS, only=LOOP)
     ops_mod.set_ops(proxy)
     torch.manual_seed(4)
     im.sample(text_embeds=g["text_embeds"], text_masks=g["text_mask"], cond_scale=3., sampling_timesteps=4,
@@ -59,9 +42,9 @@ def test_emulated_sampling_loop_passes_every_step_check(loop_emu, sampler):
     proxy.report()
 
 
-def test_emulated_timestep_walks_pass_their_exact_checks(loop_emu):
+def test_emulated_timestep_walks_pass_their_exact_checks():
     from minimagen_b200.diffusion_model import GaussianDiffusion
-    proxy = CheckingOps(loop_emu, sms=SMS)
+    proxy = CheckingOps(EmuOps(), sms=SMS)
     sch = GaussianDiffusion(timesteps=1000).sampling_schedule(6, 0.5, "cpu")
     t = torch.full((3,), 999, dtype=torch.long)
     for _ in range(len(sch.grid) + 1):

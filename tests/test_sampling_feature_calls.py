@@ -1,8 +1,8 @@
 """The sampling features under one CheckingOps (tests/checking_ops.py), on a machine without a GPU:
 
   * completeness over the interface: every public method of minimagen_b200.ops.NativeOps has a `_check_` method in
-    CheckingOps or is in ALLOWED (no kernel: capability queries and the launch-mode setting), so a kernel added to the
-    interface later fails here until it gets a checker;
+    CheckingOps or is in ALLOWED (no kernel: capability queries and the launch-mode setting), and an emulation in
+    tests/emu_ops.py with the same parameters, so a kernel added to the interface later fails here until it gets both;
   * the emulated combined samples of test_gpu_sampling_feature_calls.py on the tiny golden U-Nets, every call checked:
     a non-square two-stage DDIM cascade (RePaint at R = 2 with mask values of exactly 0.5, per-image seeds, weights and
     guidance tables, a negative prompt, then a v-prediction zero-SNR stage with a guidance interval, a cosine schedule,
@@ -20,27 +20,12 @@ import torch
 import keyed_noise_restatement as K
 from checking_ops import ALLOWED, CheckingOps
 from conftest import load_golden
-from rescale_ops import RescaleEmuOps
+from emu_ops import EmuOps
 from test_host_logic import _cascade_from_golden
 from test_respaced import _tiny_imagen
-from test_seeded import SeededEmuOps
 
 SMS = 132
 F32, I64 = torch.float32, torch.int64
-
-
-class FeatureEmuOps(RescaleEmuOps, SeededEmuOps):
-    """The torch emulation of every sampling entry point: per-image weights, the multistep, RePaint, scheduled and
-    rescaled epilogues (RescaleEmuOps), and mi_randn_keyed (SeededEmuOps)."""
-
-
-@pytest.fixture
-def emu_f():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = FeatureEmuOps()
-    yield e
-    ops_mod.set_ops(prev)
 
 
 # ------------------------------------------------------------------------------------------------ completeness
@@ -61,6 +46,17 @@ def test_every_ops_method_has_a_checker():
     for n in set(methods) - ALLOWED:
         src = inspect.getsource(methods[n])
         assert "call(" in src or "self._scheduled(" in src, f"{n} has a checker but launches nothing"
+
+
+def test_emulation_covers_every_ops_method():
+    """Every public method of NativeOps exists on EmuOps with the same parameters (names, order, kinds, defaults), so the
+    CPU tests can run any host code path on the emulation."""
+    params = lambda f: list(inspect.signature(f).parameters.values())
+    methods = _public_methods()
+    missing = sorted(n for n in methods if not hasattr(EmuOps, n))
+    assert not missing, f"NativeOps methods EmuOps does not emulate: {missing}"
+    differ = sorted(n for n, f in methods.items() if params(f) != params(getattr(EmuOps, n)))
+    assert not differ, f"EmuOps methods whose parameters differ from NativeOps's: {differ}"
 
 
 # ------------------------------------------------------------------------------------------------ combined samples
@@ -137,11 +133,11 @@ def _cpu_cascade():
 
 
 @pytest.mark.parametrize("flavour,cfg_batched", [("ddim", False), ("ddim", True), ("dpmpp_2m", False)])
-def test_emulated_combined_cascade_passes_every_call_check(emu_f, flavour, cfg_batched):
+def test_emulated_combined_cascade_passes_every_call_check(emu, flavour, cfg_batched):
     import minimagen_b200.ops as ops_mod
     im, g = _cpu_cascade()
     kw = cascade_case(im, flavour, 2, ((32, 48), (64, 96)), g["text_embeds"].shape[-1], "cpu", cfg_batched)
-    proxy = CheckingOps(emu_f, sms=SMS)
+    proxy = CheckingOps(emu, sms=SMS)
     ops_mod.set_ops(proxy)
     out = im.sample(text_embeds=g["text_embeds"], text_masks=g["text_mask"], **kw)
     print(f"\n{flavour} cascade, cfg_batched={cfg_batched} (emulated)")
@@ -158,12 +154,12 @@ def test_emulated_combined_cascade_passes_every_call_check(emu_f, flavour, cfg_b
         assert steps2 == [t * 2 + r for t, r in ((16, 0), (16, 1), (8, 0), (8, 1), (0, 0))]
 
 
-def test_emulated_ddpm_inpaint_r3_passes_every_call_check(emu_f):
+def test_emulated_ddpm_inpaint_r3_passes_every_call_check(emu):
     import minimagen_b200.ops as ops_mod
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 25)
     im.use_cuda_graph = False
-    proxy = CheckingOps(emu_f, sms=SMS)
+    proxy = CheckingOps(emu, sms=SMS)
     ops_mod.set_ops(proxy)
     gen = torch.Generator().manual_seed(3)
     mask = torch.zeros(2, 64, 64, dtype=torch.bool)
@@ -200,10 +196,10 @@ def device_walk(ops, T, R, B, seeds, n, next_t):
             return walk
 
 
-def test_device_side_repaint_walk_passes_its_checks(emu_f):
+def test_device_side_repaint_walk_passes_its_checks():
     from minimagen_b200.diffusion_model import GaussianDiffusion
     T, R_ = 20, 3
-    proxy = CheckingOps(emu_f, sms=SMS)
+    proxy = CheckingOps(EmuOps(), sms=SMS)
     walk = device_walk(proxy, T, R_, 2, torch.tensor([4, 2 ** 33]), 3 * 8 * 8,
                        GaussianDiffusion(timesteps=T).ddpm_schedule("cpu").next_t)
     assert walk == [(t, r) for t in range(T - 1, -1, -1) for r in range(R_ if t > 0 else 1)]
@@ -213,7 +209,7 @@ def test_device_side_repaint_walk_passes_its_checks(emu_f):
     assert proxy.checked == {"randn_keyed", "inpaint_advance"}
 
 
-def test_three_kernel_step_passes_its_checks(emu_f):
+def test_three_kernel_step_passes_its_checks():
     """mi_step_x0, mi_step_quantile and mi_step_posterior (the pieces of the step the ABI runs for large images) through
     their checkers."""
     from minimagen_b200.Imagen import quantile_rank
@@ -224,7 +220,7 @@ def test_three_kernel_step_passes_its_checks(emu_f):
     x, e, u, z = (torch.randn(B, n, generator=gen) for _ in range(4))
     t = torch.tensor([49, 20, 0])
     lo, hi, wq = quantile_rank(n, 0.9)
-    proxy = CheckingOps(emu_f, sms=SMS)
+    proxy = CheckingOps(EmuOps(), sms=SMS)
     x0, s, out = torch.empty(B, n), torch.empty(B), torch.empty(B, n)
     proxy.step_x0(x, e, u, 3., t, gd.sqrt_recip_alphas_cumprod, gd.sqrt_recipm1_alphas_cumprod, B, n, x0)
     proxy.step_quantile(x0, B, n, lo, hi, wq, 1.0, s)
@@ -239,7 +235,7 @@ class _Planted:
 
 
 def _prologue(defect):
-    """mi_inpaint_prologue's contract op by op (test_inpaint.prologue_ref) with one defect; every t in range."""
+    """mi_inpaint_prologue's contract op by op (emu_ops.prologue_ref) with one defect; every t in range."""
     def run(x, t, r, ra, rb, sqrt_acp, sqrt_1m_acp, k, m, z_renoise, z_known, T, B, C, hw):
         xv = x.reshape(B, C, hw)
         col = lambda tab, tt=t: tab[tt.clamp(0, T - 1)][:, None, None]
@@ -316,7 +312,7 @@ def _randn_call(ops):
 
 
 def _scheduled(defect):
-    emu = FeatureEmuOps()
+    emu = EmuOps()
 
     def run(x_t, eps_cond, eps_null, cond_scale, w_sched, t, *rest, **kw):
         if defect:

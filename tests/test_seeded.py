@@ -16,42 +16,10 @@ import torch.multiprocessing as mp
 
 import keyed_noise_restatement as K
 from conftest import load_golden, rel_l2
-from test_guidance import GuidanceEmuOps
-from test_inpaint import InpaintEmuOps
+from emu_ops import EmuOps
 from test_respaced import _tiny_imagen
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-KIND_NAMES = {v: k for k, v in K.KINDS.items()}
-
-
-class SeededEmuOps(GuidanceEmuOps, InpaintEmuOps):
-    """The emulation with per-image weights, the multistep epilogue, the inpainting entry points and mi_randn_keyed
-    (the restated generator, rounded to fp32).  `keyed` records (kind name, per-image labels, stage) per call."""
-
-    def __init__(self):
-        super().__init__()
-        self.keyed = []
-
-    def randn_keyed(self, out, seeds, B, n, kind, stage, t=None, r=None, R=None, label=0):
-        self._log("randn_keyed")
-        assert seeds.dtype == torch.int64 and seeds.numel() >= B and out.dtype == torch.float32 and out.numel() == B * n
-        if t is None:
-            labels = [int(label)] * B
-        else:
-            labels = (t * (int(R[0]) if R is not None else 1) + (r if r is not None else 0)).tolist()
-        self.keyed.append((KIND_NAMES[kind], labels, stage))
-        z = K.randn_keyed(seeds.tolist()[:B], n, kind, stage, labels, np.float32)
-        out.reshape(B, n).copy_(torch.from_numpy(z))
-
-
-@pytest.fixture
-def emu_s():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = SeededEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 # ------------------------------------------------------------------------------------------------ the generator
@@ -157,7 +125,7 @@ def _plan_kwargs(case):
 
 
 @pytest.mark.parametrize("case", ["ddpm", "ddim_eta", "inpaint", "dpmpp_2m", "img2img"])
-def test_seeded_draws_follow_the_noise_fn_plan(emu_s, case):
+def test_seeded_draws_follow_the_noise_fn_plan(emu, case):
     """A seeded sample takes exactly the (kind, label) draws a noise_fn run requests, in the same order, at stage 1, with
     one label for every image."""
     g = load_golden("sample_loop.pt")
@@ -168,15 +136,15 @@ def test_seeded_draws_follow_the_noise_fn_plan(emu_s, case):
     im.sample(**cond, **kw)
     im.noise_fn = None
     out = im.sample(**cond, seed=17, **kw)
-    got = [(kind, labels[0]) for kind, labels, _ in emu_s.keyed]
+    got = [(kind, labels[0]) for kind, labels, _ in emu.keyed]
     assert got == rec.calls
-    assert all(len(set(labels)) == 1 and stage == 1 for _, labels, stage in emu_s.keyed)
+    assert all(len(set(labels)) == 1 and stage == 1 for _, labels, stage in emu.keyed)
     assert torch.isfinite(out).all()
     if case == "inpaint":
         assert ("renoise", 999 * 2 + 1) in got and ("inpaint", 0) in got
 
 
-def test_cascade_draws_carry_the_stage(emu_s):
+def test_cascade_draws_carry_the_stage(emu):
     """Two-stage cascade: the seeded draws are the noise_fn run's, stage 1's with stage 1, the low-res augmentation
     (label 2) and stage 2's with stage 2."""
     from test_host_logic import _cascade_from_golden
@@ -188,15 +156,15 @@ def test_cascade_draws_carry_the_stage(emu_s):
     im.sample(**kw)
     im.noise_fn = None
     im.sample(seed=[5, 9], **kw)
-    got = [(kind, labels[0]) for kind, labels, _ in emu_s.keyed]
+    got = [(kind, labels[0]) for kind, labels, _ in emu.keyed]
     assert got == rec.calls
-    stages = [stage for _, _, stage in emu_s.keyed]
+    stages = [stage for _, _, stage in emu.keyed]
     lowres = got.index(("lowres", 2))
     assert stages[:lowres] == [1] * lowres and stages[lowres:] == [2] * (len(stages) - lowres)
-    assert all(labels_ == [labels_[0]] * 2 for _, labels_, _ in emu_s.keyed)
+    assert all(labels_ == [labels_[0]] * 2 for _, labels_, _ in emu.keyed)
 
 
-def test_int_seed_is_the_list(emu_s):
+def test_int_seed_is_the_list(emu):
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 1000)
     kw = dict(text_embeds=g["text_embeds"], text_masks=g["text_mask"], cond_scale=3., sampling_timesteps=5,
@@ -205,10 +173,10 @@ def test_int_seed_is_the_list(emu_s):
     assert torch.equal(a, im.sample(seed=[41, 42], **kw))
     assert torch.equal(a, im.sample(seed=torch.tensor([41, 42]), **kw))
     assert not torch.equal(a, im.sample(seed=42, **kw))
-    assert emu_s.keyed[0] == ("init", [-1, -1], 1)
+    assert emu.keyed[0] == ("init", [-1, -1], 1)
 
 
-def test_an_image_regenerates_alone(emu_s):
+def test_an_image_regenerates_alone(emu):
     """Row 1 of a seed-[a, b] batch is the seed-[b] run of row 1 alone: its draws do not depend on the batch."""
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 1000)
@@ -223,7 +191,7 @@ def test_an_image_regenerates_alone(emu_s):
     assert rel_l2(alone[0], both[0]) > 0.1
 
 
-def test_seed_none_is_unchanged(emu_s):
+def test_seed_none_is_unchanged(emu):
     """No keyed draw without a seed, and the graph keys of unseeded loops are those of before."""
     g = load_golden("sample_loop.pt")
     im = _tiny_imagen(g, 25)
@@ -231,7 +199,7 @@ def test_seed_none_is_unchanged(emu_s):
     a = im.sample(text_embeds=g["text_embeds"], text_masks=g["text_mask"], cond_scale=3., sampling_timesteps=4)
     torch.manual_seed(0)
     b = im.sample(text_embeds=g["text_embeds"], text_masks=g["text_mask"], cond_scale=3., sampling_timesteps=4)
-    assert torch.equal(a, b) and "randn_keyed" not in emu_s.calls and not emu_s.keyed
+    assert torch.equal(a, b) and "randn_keyed" not in emu.calls and not emu.keyed
     sch = im.noise_schedulers[0]
     key = lambda **kw: im._graph_key(im.unets[0], (2, 3, 64, 64), sch, g["text_embeds"], g["text_mask"], None, None,
                                      3., **kw)
@@ -240,7 +208,7 @@ def test_seed_none_is_unchanged(emu_s):
     assert key(seeded=True, stage=1)[:len(key())] == key()
 
 
-def test_argument_checks(emu_s):
+def test_argument_checks(emu):
     from minimagen_b200.Imagen import Imagen
     from minimagen_b200.Unet import Unet, BaseTest
     im = Imagen(unets=Unet(**BaseTest.defaults), text_encoder_name="t5_small", image_sizes=(16,), timesteps=25,
@@ -267,7 +235,7 @@ def test_argument_checks(emu_s):
     with pytest.raises(AssertionError, match=r"timesteps \* inpaint_resample_times must be below 2\^31"):
         im.sample(text_embeds=te, seed=1, inpaint_images=torch.zeros(2, 3, 16, 16),
                   inpaint_masks=torch.ones(2, 16, 16, dtype=torch.bool), inpaint_resample_times=2 ** 27)
-    assert not emu_s.keyed
+    assert not emu.keyed
 
 
 # ------------------------------------------------------------------------------------------------ two gloo ranks
@@ -287,8 +255,7 @@ def _worker(rank, world, port, out_path):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     import minimagen_b200.ops as ops_mod
     from test_distributed_cpu import _build
-    from test_seeded import SeededEmuOps
-    ops_mod.set_ops(SeededEmuOps())
+    ops_mod.set_ops(EmuOps())
     g = torch.load(os.path.join(ROOT, "tests", "golden", "sample_loop.pt"), map_location="cpu", weights_only=False)
     im = _build(g)
     out = im.sample(distributed=True, **_dist_inputs(4))
@@ -300,7 +267,7 @@ def _worker(rank, world, port, out_path):
 
 
 @pytest.mark.timeout(600)
-def test_two_rank_gloo_with_seed_only(tmp_path, emu_s):
+def test_two_rank_gloo_with_seed_only(tmp_path, emu):
     """distributed=True with a seed and no noise_fn: the gathered batch is the single-process one."""
     from test_distributed_cpu import _build
     port = 29800 + (os.getpid() % 150)

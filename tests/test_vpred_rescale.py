@@ -1,6 +1,6 @@
 """v-prediction, zero-terminal-SNR schedules and guidance rescale (Imagen.set_objectives(pred_objectives=,
 zero_terminal_snr=), Imagen.sample(guidance_rescale=)) on the CPU, through the torch emulation of the ops interface
-extended by mi_guidance_rescale_factor and mi_step_epilogue_rescaled (tests/rescale_ops.py).  Covers the schedule against Lin et al.'s Algorithm 1 and the
+with mi_guidance_rescale_factor and mi_step_epilogue_rescaled (tests/emu_ops.py).  Covers the schedule against Lin et al.'s Algorithm 1 and the
 finiteness of every walk's tables at alphas_cumprod = 0; an exact v-denoiser under 'v' against the exact eps-denoiser
 under 'noise'; the v training target; the argument checks; the rescaled loop against the float64 restatement
 (rescale_restatement.py) on DDPM, DDIM, DPM-Solver++(2M), a guidance table, per-image phi and a negative prompt, and
@@ -13,24 +13,15 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
+import fp64_ref as R
 import rescale_restatement as RS
 from conftest import load_golden, rel_l2
 from checking_ops import CheckingOps
-from rescale_ops import RescaleEmuOps
+from emu_ops import EmuOps
 
 F32, F64 = torch.float32, torch.float64
 SHAPE = (2, 3, 64, 64)
 INF = float("inf")
-
-
-@pytest.fixture
-def emu():
-    import minimagen_b200.ops as ops_mod
-    prev = ops_mod._OPS
-    e = RescaleEmuOps()
-    ops_mod.set_ops(e)
-    yield e
-    ops_mod.set_ops(prev)
 
 
 def _imagen(T=1000, objective='noise', zero_snr=False, device="cpu"):
@@ -358,7 +349,7 @@ def _factor(defect):
 @pytest.mark.parametrize("table", [False, True])
 def test_factor_passes_and_planted_defects_fail_its_check(table):
     c, u, w, w_sched, t, phi = _call_data(1, table)
-    proxy = CheckingOps(RescaleEmuOps(), sms=SMS)
+    proxy = CheckingOps(EmuOps(), sms=SMS)
     f = torch.empty(B)
     proxy.guidance_rescale_factor(c, u, w, w_sched, t, phi, B, N, f)
     assert "guidance_rescale_factor" in proxy.checked and bool((f != 1).all())
@@ -391,7 +382,7 @@ def test_rescaled_epilogue_check(multi, defect):
     hist = torch.randn(B, N, generator=torch.Generator().manual_seed(6)) * 0.1 if multi else None
     f = torch.tensor([0.8, 1.25, 0.6])
     lo, hi, wt = quantile_rank(N, 0.9)
-    emu = RescaleEmuOps()
+    emu = EmuOps()
 
     def planted(x_t, eps_cond, eps_null, cond_scale, w_sched, f, *rest, **kw):
         if defect == "neighbour":
@@ -416,12 +407,12 @@ def test_rescaled_epilogue_is_the_plain_epilogue_of_the_rescaled_prediction():
     c, u, w, w_sched, t, phi = _call_data(7, True)
     x = torch.randn(B, N, generator=torch.Generator().manual_seed(8))
     z = torch.randn(B, N, generator=torch.Generator().manual_seed(9))
-    emu, lo_hi = RescaleEmuOps(), quantile_rank(N, 0.9)
+    emu, lo_hi = EmuOps(), quantile_rank(N, 0.9)
     f = torch.empty(B)
     emu.guidance_rescale_factor(c, u, w, w_sched, t, phi, B, N, f)
     a, b = gd.sqrt_alphas_cumprod, gd.sqrt_one_minus_alphas_cumprod
     out1, out2 = torch.empty_like(x), torch.empty_like(x)
     emu.step_epilogue_rescaled(x, c, u, w, w_sched, f, t, a, b, s.c1, s.c2, s.sigma, None, z, None, B, N, *lo_hi, 1.0, out1)
-    eps = emu._guided(c, u, w, w_sched, t, B, N) * f[:, None]
+    eps = R.guided_fp32(c, u, w, w_sched, t, B, N) * f[:, None]
     emu.step_epilogue(x, eps, None, 1.0, t, a, b, s.c1, s.c2, s.sigma, z, B, N, *lo_hi, 1.0, out2)
     assert torch.equal(out1, out2)
