@@ -9,7 +9,7 @@ nothing on the host.  Sampling captures three graph flavours: text-only (one gra
 step count and eta), inpainting, and multistep (DPM-Solver++(2M), every step count).  The guidance weights are per-image
 data in a static buffer, so every flavour's graph serves every `cond_scale` and every negative prompt of its shape.
 
-Eleven additions that the reference does not have (all optional, defaults reproduce the reference):
+Twelve additions that the reference does not have (all optional, defaults reproduce the reference):
   * `noise_fn(kind, shape, step)`  -- inject the Gaussian draws (x_T, per-step noise, low-res augmentation noise) so that
     a CPU oracle and this GPU path consume identical numbers (CPU mt19937 and CUDA Philox streams differ);
   * data-parallel sampling over `torch.distributed` ranks: the batch is sharded, each rank runs the whole cascade on
@@ -46,7 +46,11 @@ Eleven additions that the reference does not have (all optional, defaults reprod
     zero_terminal_snr=True)`, `sample(..., guidance_rescale=phi)`; Lin et al. 2024): a U-Net may predict v instead of
     eps, in training and sampling, on a schedule that reaches SNR 0 at T-1 (ZeroTerminalSNRDiffusion); a guided step may
     rescale each image's guided prediction to the conditional prediction's spread (mi_guidance_rescale_factor, then
-    mi_step_epilogue_rescaled), with phi in the captured step's static buffer.
+    mi_step_epilogue_rescaled), with phi in the captured step's static buffer;
+  * DeepCache feature reuse (`sample(..., cache_interval=N)`, Ma et al. 2024): every N-th U-Net evaluation of a stage
+    runs the whole network and keeps the feature entering its last up level; the ones in between run only the
+    shallowest branch (stem, down level 0, the last up level on the kept feature, the final block and conv).  The
+    plan is `deepcache_plan`; a captured stage keeps a full and a cached graph over the same static buffers.
 
 `noise_fn` kinds: 'init' (x_T, step -1; with an init image k, the noise z of the start sqrt(a_t0) k + sqrt(1 - a_t0) z,
 t0 the walk's first point), 'step' (the step's noise, labelled with its timestep t), 'lowres' (the low-res
@@ -66,7 +70,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .Unet import Unet
+from .Unet import DeepCache, Unet
 from .diffusion_model import GaussianDiffusion, ZeroTerminalSNRDiffusion
 from .helpers import (cast_tuple, default, eval_decorator, exists, identity, maybe, module_device,
                       normalize_neg_one_to_one, null_context, resize_image_to, unnormalize_zero_to_one)
@@ -90,6 +94,22 @@ def quantile_rank(n: int, q: float):
 
 def _is_int(v):
     return isinstance(v, int) and not isinstance(v, bool)
+
+
+def deepcache_plan(on, interval):
+    """Which iterations of a sampling loop run the whole U-Net (True) and which the cached shallow branch (False), for
+    DeepCache with `interval` N (None or 1: every iteration is full).  `on[i]`: whether iteration i runs the guidance
+    pass (one entry per iteration of the loop as it runs: after skip_steps and max_steps, a RePaint iteration (t, r)
+    counting as one).  Iteration 0 is full; with j the last full iteration, iteration i is full iff i - j >= N, or it
+    runs the guidance pass and j did not (that pass has no feature kept from j).  A cached iteration's passes read what
+    the same passes stored at j."""
+    full, j = [], None
+    for i, guided in enumerate(on):
+        f = j is None or interval is None or i - j >= interval or (guided and not on[j])
+        if f:
+            j = i
+        full.append(f)
+    return full
 
 
 def _is_guided(cond_scale):
@@ -138,16 +158,21 @@ class _StepGraph:
                 graph serves every interval and schedule); the guided body then steps with mi_step_epilogue_ws(_multistep).
          phi    guidance-rescale graphs only: [B] fp32 per-image rescale weights (`set_cond` refreshes them, so one graph
                 serves every phi); the guided body then runs mi_guidance_rescale_factor and mi_step_epilogue_rescaled.
+    deepcache  DeepCache entries only: the Unet.DeepCache the full graphs store into and the cached graphs read from.
     A guidance-table graph is a pair: `graph`, the guided step, and `graph_unguided`, the same step without the guidance
     pass (one U-Net evaluation, the unguided epilogue), captured when a loop first needs it over the same static buffers,
     in the same memory pool.  The two never run at once: `replay(guided)` picks one per grid point, and the state they
-    carry (x, t, the history of 2M, the RePaint counter) passes from one to the other as it is.
+    carry (x, t, the history of 2M, the RePaint counter) passes from one to the other as it is.  A DeepCache entry adds
+    the cached twin of each (`graph_cached`, `graph_cached_unguided`): the same step with the U-Net passes reading the
+    feature the last full replay stored, so such an entry holds up to four graphs, all in the first one's pool.
     Three flavours: text-only (the step, then mi_step_advance_t_table), inpainting (draws, mi_inpaint_prologue, the step,
     mi_inpaint_advance) and multistep (the draw, mi_step_epilogue_multistep's step, mi_step_advance_t_table).  A whole sampling loop is then `set x, t; replay() * S` for the S grid points of its walk (S = T
     for DDPM; `* ((S-1) R + 1)` when inpainting) -- no per-step host-side tensor ops."""
 
     def __init__(self):
         self.graph = self.graph_unguided = None
+        self.graph_cached = self.graph_cached_unguided = None
+        self.deepcache = None
         self.x = self.t = self.noise = None
         self.cond = {}
         self.sched = None
@@ -201,9 +226,12 @@ class _StepGraph:
             for te in self._static_texts():
                 self.unet.unregister_static_text(te)
 
-    def replay(self, guided=True):
-        """guided=False: the unguided graph of a guidance-table pair."""
-        (self.graph if guided else self.graph_unguided).replay()
+    def replay(self, guided=True, full=True):
+        """guided=False: the unguided graph of a guidance-table pair; full=False: the cached graph of a DeepCache entry."""
+        if full:
+            (self.graph if guided else self.graph_unguided).replay()
+        else:
+            (self.graph_cached if guided else self.graph_cached_unguided).replay()
 
 
 class Imagen(nn.Module):
@@ -404,7 +432,7 @@ class Imagen(nn.Module):
 
     def _step(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
               cond_scale, model_output=None, out=None, schedule=None, hist=None, negative_text_embeds=None,
-              negative_text_mask=None, guided=None, guidance_table=None, rescale=None):
+              negative_text_mask=None, guided=None, guidance_table=None, rescale=None, deepcache=None):
         """x_{t-1} = posterior_mean(x_t, clamp-thresholded x0(x_t, eps)) + [t != 0] * sigma_t * noise.
         eps = g + (cond - g) * w, with w = `cond_scale` (a number, or an fp32 [B] tensor of per-image weights on x's
         device) and g the guidance pass: the U-Net conditioned on `negative_text_embeds` / `negative_text_mask` if given,
@@ -420,6 +448,8 @@ class Imagen(nn.Module):
         `rescale` (an fp32 [B] tensor of guidance-rescale weights phi_b on x's device): a guided step scales image b's
         guided prediction g by f_b = phi_b sqrt(SS_c / SS_g) + (1 - phi_b) (mi_guidance_rescale_factor, then
         mi_step_epilogue_rescaled); an unguided step ignores it.
+        `deepcache` (mode, cache): the U-Net passes store into ('store') or read from ('read') the Unet.DeepCache
+        `cache`, the conditional pass in rows 0 .. B, the guidance pass in rows B .. 2B (a 2B cfg_batched pass: both).
         x0 is formed from the U-Net output by the objective's tables (`_x0_tables`)."""
         with N.device_of(x):
             return self._step_impl(unet, x, t, noise, noise_scheduler=noise_scheduler, text_embeds=text_embeds,
@@ -427,11 +457,13 @@ class Imagen(nn.Module):
                                    lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
                                    model_output=model_output, out=out, schedule=schedule, hist=hist,
                                    negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
-                                   guided=guided, guidance_table=guidance_table, rescale=rescale)
+                                   guided=guided, guidance_table=guidance_table, rescale=rescale,
+                                   deepcache=deepcache)
 
     def _step_impl(self, unet, x, t, noise, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                    lowres_noise_times, cond_scale, model_output=None, out=None, schedule=None, hist=None,
-                   negative_text_embeds=None, negative_text_mask=None, guided=None, guidance_table=None, rescale=None):
+                   negative_text_embeds=None, negative_text_mask=None, guided=None, guidance_table=None, rescale=None,
+                   deepcache=None):
         guided = _is_guided(cond_scale) if guided is None else guided
         assert not (guided and not self.can_classifier_guidance), \
             'imagen was not trained with conditional dropout, and thus one cannot use classifier free guidance ' \
@@ -446,6 +478,11 @@ class Imagen(nn.Module):
         # the guidance pass: the negative prompt (keep = 1, no RNG), or the learned null conditioning
         gkw = dict(kw, text_embeds=negative_text_embeds, text_mask=negative_text_mask) if neg else kw
         eps_null = None
+
+        def forward(x_, t_, row0, **k):
+            if deepcache is None:
+                return unet.forward(x_, t_, **k)
+            return unet._forward_impl(x_, t_, deepcache=(*deepcache, row0), **k)
         if exists(model_output):
             eps = model_output.to(F32).contiguous()
         else:
@@ -466,12 +503,13 @@ class Imagen(nn.Module):
                         L = max(te.shape[1], nte.shape[1])
                         (te, tm), (nte, ntm) = _pad_text(te, tm, L), _pad_text(nte, ntm, L)
                     bkw.update(text_embeds=torch.cat((te, nte)), text_mask=torch.cat((tm, ntm)) if exists(tm) else None)
-                both = unet._forward_impl(two(x), two(t), cond_keep=keep, **bkw)
+                dc = {} if deepcache is None else dict(deepcache=(*deepcache, 0))
+                both = unet._forward_impl(two(x), two(t), cond_keep=keep, **bkw, **dc)
                 eps, eps_null = both[:B], both[B:]
             else:
-                eps = unet.forward(x, t, **kw)
+                eps = forward(x, t, 0, **kw)
                 if guided:
-                    eps_null = unet.forward(x, t, cond_drop_prob=0. if neg else 1., **gkw)
+                    eps_null = forward(x, t, B, cond_drop_prob=0. if neg else 1., **gkw)
         x = x.contiguous()
         lo, hi, w = quantile_rank(n, self.dynamic_thresholding_percentile)
         if out is None:
@@ -520,13 +558,14 @@ class Imagen(nn.Module):
     # -------------------------------------------------------------------------------------------- sampling loop
     def _graph_key(self, unet, shape, noise_scheduler, text_embeds, text_mask, lowres_cond_img, lowres_noise_times,
                    cond_scale, inpaint=False, multistep=False, *, negative_text_embeds=None, negative_text_mask=None,
-                   guided=None, seeded=False, stage=None, scheduled=False, rescaled=False):
+                   guided=None, seeded=False, stage=None, scheduled=False, rescaled=False, deepcache=False):
         """Only whether the step runs the guidance pass is part of the key, not the weights: they are data in the graph's
         static w buffer.  The negative prompt's signature counts when it is used, i.e. when guided.  A seeded graph (keyed
         draws, the seeds in its static buffer) is keyed apart, with the stage its draws carry; an unseeded key is
         unchanged.  So is a guidance-table graph pair (`scheduled`: the table in its static buffer), with a
         'guidance_table' suffix; neither the interval nor the schedule is part of the key.  A guidance-rescale graph
-        (`rescaled`: phi in its static buffer) has a 'rescaled' suffix; phi is not part of the key."""
+        (`rescaled`: phi in its static buffer) has a 'rescaled' suffix; phi is not part of the key.  A DeepCache entry
+        (`deepcache`: full and cached graphs) has a 'deepcache' suffix; the interval is not part of the key."""
         sig = lambda v: None if v is None else (tuple(v.shape), str(v.dtype))
         guided = _is_guided(cond_scale) if guided is None else guided
         p0 = next(unet.parameters())
@@ -541,6 +580,8 @@ class Imagen(nn.Module):
             key = key + ('guidance_table',)
         if rescaled:
             key = key + ('rescaled',)
+        if deepcache:
+            key = key + ('deepcache',)
         if inpaint:
             return key + ('inpaint',)
         return key + ('multistep',) if multistep else key
@@ -555,7 +596,7 @@ class Imagen(nn.Module):
     def _step_graph(self, unet, shape, *, noise_scheduler, text_embeds, text_mask, lowres_cond_img,
                     lowres_noise_times, cond_scale, schedule=None, inpaint=None, negative_text_embeds=None,
                     negative_text_mask=None, guided=None, seeds=None, stage=None, guidance_table=None, unguided=False,
-                    rescale=None):
+                    rescale=None, deepcache=False, reads=()):
         """The captured step for this (unet, shape, conditioning signature, weights version): captured once, then reused by
         every later sampling loop of the same signature.  Every lookup refreshes the conditioning tensors in its static
         buffers and installs the walk `schedule` (a SamplingSchedule; None: the DDPM walk) in its static tables: the step
@@ -579,7 +620,11 @@ class Imagen(nn.Module):
         the guided graph's memory pool.  The pair is one entry of `max_cached_graphs`.
         `rescale` ([B] fp32 guidance-rescale weights, for a guided loop with some phi_b > 0) selects the rescaled variant
         of the flavour, keyed apart: phi lives in its static buffer (`_StepGraph.set_cond` installs it), so one graph
-        serves every phi."""
+        serves every phi.
+        `deepcache` selects the DeepCache entry of the flavour, keyed apart: its full graphs also store the U-Net feature
+        in the entry's Unet.DeepCache, and `reads` (the `replay(guided)` choices of the loop's cached iterations)
+        captures the cached graphs that read it, if they do not exist yet, in the first graph's pool.  One entry serves
+        every interval; it is one entry of `max_cached_graphs`."""
         device = self.device
         schedule = default(schedule, lambda: noise_scheduler.ddpm_schedule(device))
         multistep = exists(schedule.c3)
@@ -593,7 +638,7 @@ class Imagen(nn.Module):
                               lowres_noise_times, cond_scale, exists(inpaint), multistep,
                               negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask,
                               guided=guided, seeded=exists(seeds), stage=stage, scheduled=scheduled,
-                              rescaled=rescaled)
+                              rescaled=rescaled, deepcache=deepcache)
         cond = dict(text_embeds=text_embeds, text_mask=text_mask, lowres_cond_img=lowres_cond_img,
                     lowres_noise_times=lowres_noise_times, negative_text_embeds=negative_text_embeds,
                     negative_text_mask=negative_text_mask)
@@ -620,6 +665,9 @@ class Imagen(nn.Module):
                 g.gtab = guidance_table.to(device=device, dtype=F32).clone()
             if rescaled:
                 g.phi = phi.clone()
+            if deepcache:
+                # rows 0 .. B: the conditional pass, B .. 2B: the guidance pass
+                g.deepcache = DeepCache(2 * shape[0] if guided else shape[0])
             kw = dict(noise_scheduler=noise_scheduler, cond_scale=g.w, guidance_table=g.gtab, rescale=g.phi,
                       **{k: g.cond.get(k) for k in cond})
             g.refresh_static()
@@ -645,7 +693,7 @@ class Imagen(nn.Module):
                                  z_renoise=torch.zeros(shape, dtype=F32, device=device),
                                  z_known=torch.zeros(shape, dtype=F32, device=device))
 
-            def body(step_guided=guided):
+            def body(step_guided=guided, mode='store' if deepcache else None):
                 if exists(g.seeds):
                     # keyed draws at the current t (t * R + r when inpainting): those an eager seeded loop takes
                     n = C * hw
@@ -663,7 +711,8 @@ class Imagen(nn.Module):
                     ops.inpaint_prologue(g.x, g.t, p['r'], p['ra'], p['rb'], noise_scheduler.sqrt_alphas_cumprod,
                                          noise_scheduler.sqrt_one_minus_alphas_cumprod, p['k'], p['m'], p['z_renoise'],
                                          p['z_known'], T, B, C, hw)
-                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, hist=g.hist, guided=step_guided, **kw)
+                self._step(unet, g.x, g.t, g.noise, out=g.x, schedule=g.sched, hist=g.hist, guided=step_guided,
+                           deepcache=None if mode is None else (mode, g.deepcache), **kw)
                 if exists(p):
                     ops.inpaint_advance(g.t, p['r'], g.sched.next_t, p['R'], T, B)   # next repeat, or next grid point
                 else:
@@ -674,6 +723,11 @@ class Imagen(nn.Module):
             self._graphs[key] = g
         if scheduled and unguided and g.graph_unguided is None:
             g.graph_unguided = self._capture(lambda: g.body(False), device, pool=g.graph.pool())
+        # cached graphs after the full ones: the full graphs' warm-up runs allocate the feature buffers they read
+        if deepcache and True in reads and g.graph_cached is None:
+            g.graph_cached = self._capture(lambda: g.body(guided, 'read'), device, pool=g.graph.pool())
+        if deepcache and False in reads and g.graph_cached_unguided is None:
+            g.graph_cached_unguided = self._capture(lambda: g.body(False, 'read'), device, pool=g.graph.pool())
         g.set_schedule(schedule)
         if scheduled:
             g.set_guidance(guidance_table)
@@ -702,7 +756,7 @@ class Imagen(nn.Module):
     def _p_sample_loop(self, unet, shape, *, noise_scheduler, text_embeds=None, text_mask=None, lowres_cond_img=None,
                        lowres_noise_times=None, cond_scale=1., max_steps=None, out=None, schedule=None, inpaint=None,
                        init_image=None, negative_text_embeds=None, negative_text_mask=None, seeds=None, stage=1,
-                       guidance_table=None, guidance_rescale=0.):
+                       guidance_table=None, guidance_rescale=0., cache_interval=None):
         """Reverse diffusion from x_T ~ N(0, I) to x_0 (reference Imagen.py:372-420).  `max_steps` (not in the
         reference) stops after that many iterations -- used by the benchmark / parity harness; `out` (not in the
         reference) receives the finished images (e.g. this rank's slot of the all-gather buffer); `schedule` (not in the
@@ -733,7 +787,10 @@ class Imagen(nn.Module):
         without it, and one that is 0 at every point the unguided loop (as cond_scale = 1).  The draws do not depend on it.
         `guidance_rescale` (not in the reference): phi, a number or an fp32 [B] tensor of per-image weights in [0, 1] on
         the sampling device.  A guided iteration rescales each image's guided prediction as in `_step`; with every
-        phi_b == 0 the loop is exactly the loop without it, on the same entry points."""
+        phi_b == 0 the loop is exactly the loop without it, on the same entry points.
+        `cache_interval` (not in the reference): None, or an int N >= 1, DeepCache's interval.  At N > 1 the iterations
+        `deepcache_plan` marks cached run the U-Net's shallowest branch on the feature the last full iteration kept
+        (Unet.DeepCache); None and 1 run exactly the loop without it.  The draws do not depend on it."""
         device = self.device
         with N.device_of(self._temp):
             ops = get_ops()
@@ -783,9 +840,14 @@ class Imagen(nn.Module):
                       lowres_cond_img=lowres_cond_img, lowres_noise_times=lowres_noise_times, cond_scale=cond_scale,
                       negative_text_embeds=negative_text_embeds, negative_text_mask=negative_text_mask, guided=guided,
                       guidance_table=guidance_table, rescale=rescale)
+            caching = exists(cache_interval) and cache_interval > 1
+            full = deepcache_plan(on, cache_interval) if caching else [True] * len(plan)
             if self.use_cuda_graph and img.is_cuda and len(plan) > 2:
+                # a pair replays the graph each point needs; without a table the graph is the only one of its kind
+                sel = [step_guided or not exists(guidance_table) for step_guided in on]
+                dc = dict(deepcache=True, reads={s for s, f in zip(sel, full) if not f}) if caching else {}
                 g = self._step_graph(unet, tuple(shape), schedule=walk, inpaint=inpaint, unguided=not all(on), **keyed,
-                                     **kw)
+                                     **kw, **dc)
                 static = dict(step=g.noise)
                 if exists(inpaint):
                     static.update(renoise=g.inp['z_renoise'], inpaint=g.inp['z_known'])
@@ -794,20 +856,23 @@ class Imagen(nn.Module):
                     g.hist.zero_()
                 g.x.copy_(img)
                 g.t.fill_(plan[0][0])
-                for iteration, step_guided in zip(draws, on):
+                for iteration, guided_graph, step_full in zip(draws, sel, full):
                     if g.inject_noise:
                         for kind, label in iteration:
                             static[kind].copy_(self._noise(kind, shape, label, device))
-                    # [prologue +] step in place; then t (and r) <- the next iteration's.  Without a table the graph is
-                    # the only one of its key (guided or not as the whole loop); a pair replays the one this point needs
-                    g.replay(step_guided or not exists(guidance_table))
+                    # [prologue +] step in place; then t (and r) <- the next iteration's
+                    if caching:
+                        g.replay(guided_graph, step_full)
+                    else:
+                        g.replay(guided_graph)
                 img = g.x
             else:
                 if exists(inpaint):
                     _, ra, rb = sch.inpaint_tables(walk, device)
                     img = img.clone()           # the prologue works in place; x_T may be the caller's draw
                 hist = torch.zeros(tuple(shape), dtype=F32, device=device) if multistep else None
-                for (t, r), iteration, step_guided in zip(plan, draws, on):
+                cache = DeepCache(2 * B if guided else B) if caching else None
+                for (t, r), iteration, step_guided, step_full in zip(plan, draws, on, full):
                     z = {kind: self._noise(kind, shape, label, device, **keyed) for kind, label in iteration}
                     times = torch.full((B,), t, device=device, dtype=torch.long)
                     if exists(inpaint):
@@ -816,7 +881,9 @@ class Imagen(nn.Module):
                         ops.inpaint_prologue(img, times, reps, ra, rb, sch.sqrt_alphas_cumprod,
                                              sch.sqrt_one_minus_alphas_cumprod, k, m, z.get('renoise', z['inpaint']),
                                              z['inpaint'], sch.num_timesteps, B, C, hw)
-                    img = self._step(unet, img, times, z['step'], schedule=walk, hist=hist, **dict(kw, guided=step_guided))
+                    dc = None if cache is None else ('store' if step_full else 'read', cache)
+                    img = self._step(unet, img, times, z['step'], schedule=walk, hist=hist, deepcache=dc,
+                                     **dict(kw, guided=step_guided))
 
             if out is None:
                 out = torch.empty(tuple(shape), dtype=F32, device=device)
@@ -834,7 +901,7 @@ class Imagen(nn.Module):
                inpaint_masks=None, inpaint_resample_times: int = 5, sampler: str = 'ddim', init_images=None,
                skip_steps=None, start_at_unet_number: int = 1, start_images=None, stop_at_unet_number: int = None,
                negative_texts=None, negative_text_embeds=None, negative_text_masks=None, seed=None,
-               guidance_interval=None, guidance_schedule=None, image_sizes=None, guidance_rescale=0.):
+               guidance_interval=None, guidance_schedule=None, image_sizes=None, guidance_rescale=0., cache_interval=None):
         """Generate images (reference Imagen.py:422-510).  With `distributed=True` inside an initialised
         torch.distributed (NCCL) job, rank r samples rows [r*b/G, (r+1)*b/G) of the conditioning; the last stage's
         finalize kernel writes its images straight into this rank's slot of the gather buffer and ONE in-place
@@ -913,7 +980,17 @@ class Imagen(nn.Module):
         SS and f_b in fp64 (f_b = 1 where SS_g = 0), and the step uses fp32(g * f_b) in place of g (x0, threshold and
         posterior unchanged).  Steps without the guidance pass (cond_scale 1, guidance-table zeros) never rescale.  A
         stage whose phi is 0 for every image runs exactly as without the argument.  Captured graphs are keyed on whether
-        a stage rescales, not on phi."""
+        a stage rescales, not on phi.
+        `cache_interval` (None, an int N >= 1, or one entry per U-Net, each None or such an int) reuses deep U-Net
+        features between neighbouring evaluations (DeepCache, Ma et al. 2024, "DeepCache: Accelerating Diffusion Models
+        for Free").  Every N-th iteration of a stage's loop (iteration 0 first, a RePaint iteration counting as one)
+        runs the whole U-Net and keeps the feature that enters its last up level; the iterations in between run only
+        the shallowest branch -- the stem, down level 0, the last up level on the kept feature and fresh level-0 skips,
+        the final block and conv -- with time and text conditioning recomputed.  An iteration that runs the guidance
+        pass when the last full one did not is full too (`deepcache_plan`).  The conditional and the guidance pass keep
+        a feature each.  It trades sample quality for speed; it needs no training and combines with every argument
+        above, and the draws do not depend on it.  None and 1 (the default: off) run exactly as without it.  A captured
+        stage keeps its full and cached graphs in one entry, keyed on whether the stage caches, not on N."""
         assert sampler in ('ddim', 'dpmpp_2m'), f"sampler must be 'ddim' or 'dpmpp_2m', got {sampler!r}"
         steps = self._sampling_steps(sampling_timesteps, ddim_eta)
         if sampler == 'dpmpp_2m':
@@ -956,6 +1033,9 @@ class Imagen(nn.Module):
             assert sched in (None, 'linear', 'cosine'), \
                 f"guidance_schedule of unet {i} must be None, 'linear' or 'cosine', got {sched!r}"
         sizes = self._stage_sizes(image_sizes, start_at_unet_number, stop_at_unet_number)
+        intervals = self._per_unet(cache_interval, 'cache_interval')
+        for i, v in enumerate(intervals, 1):
+            assert v is None or (_is_int(v) and v >= 1), f'cache_interval of unet {i} must be None or an int >= 1, got {v!r}'
         for i in range(start_at_unet_number, stop_at_unet_number + 1):
             k, walk_len = default(skips[i - 1], 0), default(steps[i - 1], self.noise_schedulers[i - 1].num_timesteps)
             assert _is_int(k) and 0 <= k < walk_len, \
@@ -984,7 +1064,7 @@ class Imagen(nn.Module):
             return self._sample_impl(texts, text_masks, text_embeds, scales, lowres_sample_noise_level,
                                      return_pil_images, device, distributed, steps, ddim_eta, inpaint, sampler,
                                      init_images, skips, start_at_unet_number, stop_at_unet_number, start_images,
-                                     negative, seed, guidance, sizes, phis)
+                                     negative, seed, guidance, sizes, phis, intervals)
 
     @staticmethod
     def downsample_factor(unet):
@@ -1125,7 +1205,7 @@ class Imagen(nn.Module):
     def _sample_impl(self, texts, text_masks, text_embeds, cond_scale, lowres_sample_noise_level, return_pil_images,
                      device, distributed, steps=None, ddim_eta=0., inpaint=None, sampler='ddim', init_images=None,
                      skips=None, start_at=1, stop_at=None, start_images=None, negative=(None, None, None), seed=None,
-                     guidance=None, sizes=None, phis=None):
+                     guidance=None, sizes=None, phis=None, cache_intervals=None):
         if exists(texts) and not exists(text_embeds):
             text_embeds, text_masks = t5_encode_text(texts, name=self.text_encoder_name)
             text_embeds, text_masks = map(lambda t: t.to(device), (text_embeds, text_masks))
@@ -1201,11 +1281,12 @@ class Imagen(nn.Module):
         steps = default(steps, (None,) * n_stages)
         skips = default(skips, (0,) * n_stages)
         intervals, gscheds = default(guidance, ((None,) * n_stages, (None,) * n_stages))
+        cache_intervals = default(cache_intervals, (None,) * n_stages)
         stages = list(zip(range(1, n_stages + 1), self.unets, self.sample_channels, sizes,
                           self.noise_schedulers, steps, init_images, skips, scales, intervals,
-                          gscheds, phis))[start_at - 1:stop_at]
+                          gscheds, phis, cache_intervals))[start_at - 1:stop_at]
         for (unet_number, unet, channel, image_size, noise_scheduler, n_steps, init, skip, stage_scale, interval,
-             gsched, phi) in stages:
+             gsched, phi, cache_interval) in stages:
             with self._one_unet_in_gpu(unet=unet):
                 lowres_cond_img = lowres_noise_times = None
                 if unet.lowres_cond:
@@ -1254,7 +1335,8 @@ class Imagen(nn.Module):
                                           lowres_noise_times=lowres_noise_times, noise_scheduler=noise_scheduler,
                                           out=slot, schedule=schedule, inpaint=stage_inpaint, init_image=stage_init,
                                           negative_text_embeds=neg_embeds, negative_text_mask=neg_masks, seeds=seeds,
-                                          stage=unet_number, guidance_table=gtab, guidance_rescale=phi)
+                                          stage=unet_number, guidance_table=gtab, guidance_rescale=phi,
+                                          cache_interval=cache_interval)
 
         outputs = img
         if gathered is not None:

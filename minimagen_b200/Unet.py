@@ -13,13 +13,46 @@ import torch
 from torch import nn
 
 from .helpers import cast_tuple, default, exists, prob_mask_like
-from .layers import (Attention, Cat, Context, Conv2d, CrossEmbedLayer, Downsample, Identity, Parallel, ResnetBlock,
+from .layers import (Act, Attention, Cat, Context, Conv2d, CrossEmbedLayer, Downsample, Identity, Parallel, ResnetBlock,
                      SinusoidalPosEmb, TokenView, TransformerBlock, Upsample, _no_grad_check, _ResidualAttention)
 from . import _native
 from .ops import get_ops
 from .t5 import get_encoded_dim
 
 F32 = torch.float32
+
+
+class DeepCache:
+    """Static buffers for DeepCache feature reuse (Ma et al. 2024) during sampling: the activation that enters the last up
+    level (`ups[-1]`'s first ResnetBlock reads it as the current half of its skip concatenation), for `rows` batch rows.
+
+    A store pass copies what the producer wrote -- its fp32 and/or fp16 NHWC copy, and the GroupNorm block statistics
+    when its epilogue accumulated them -- into rows row0 .. row0 + b, on the device, before the consumer adds anything.  A read pass hands the consumer an Act over
+    the same rows holding exactly those copies, so it takes the same route over the same bits and statistics: a read
+    at the inputs of the store returns the store pass's output bit for bit.  The buffers are allocated by the first
+    store (outside any graph capture: the capture's warm-up run) and kept until the cache is dropped."""
+
+    def __init__(self, rows):
+        self.rows = rows
+        self.f32 = self.f16 = self.stats = None
+
+    def store(self, act, row0):
+        b = act.shape[0]
+        for name in ('f32', 'f16', 'stats'):
+            src = getattr(act, name)
+            if src is None:
+                setattr(self, name, None)
+                continue
+            buf = getattr(self, name)
+            if buf is None or buf.shape[1:] != src.shape[1:] or buf.dtype != src.dtype:
+                buf = torch.empty((self.rows, *src.shape[1:]), dtype=src.dtype, device=src.device)
+                setattr(self, name, buf)
+            buf[row0:row0 + b].copy_(src)
+
+    def read(self, row0, b):
+        assert self.f32 is not None or self.f16 is not None, 'a read pass needs a feature stored before it'
+        rows = lambda v: None if v is None else v[row0:row0 + b]
+        return Act(rows(self.f32), rows(self.f16), rows(self.stats))
 
 
 class Unet(nn.Module):
@@ -182,15 +215,20 @@ class Unet(nn.Module):
             return self._forward_dev(x, *args, **kwargs)
 
     def _forward_dev(self, x, time, *, lowres_cond_img=None, lowres_noise_times=None, text_embeds=None, text_mask=None,
-                      cond_drop_prob: float = 0., cond_keep=None):
+                      cond_drop_prob: float = 0., cond_keep=None, deepcache=None):
         """x: (b, c, s, s) fp32 NCHW noised images; time: (b,) int64.  Returns the predicted noise, (b, c_out, s, s).
         Orchestration follows the reference's Unet.forward (Unet.py:355-472) block for block.
         `cond_keep` (internal, uint8/bool [b]): explicit per-sample keep mask instead of the Bernoulli(1 - cond_drop_prob)
-        draw of Unet.py:587 -- lets the conditional and the unconditional pass of classifier-free guidance share one batch."""
+        draw of Unet.py:587 -- lets the conditional and the unconditional pass of classifier-free guidance share one batch.
+        `deepcache` (internal, sampling only): (mode, cache, row0) with a DeepCache and the first of its rows this pass
+        uses.  'store' runs the whole network and keeps the feature entering ups[-1] in rows row0 .. row0 + b; 'read'
+        runs only the shallowest branch on the kept feature (DeepCache docstring)."""
         assert not (self.lowres_cond and not exists(lowres_cond_img)), \
             'low resolution conditioning image must be present'
         assert not (self.lowres_cond and not exists(lowres_noise_times)), \
             'low resolution conditioning noise time must be present'
+        assert deepcache is None or (deepcache[0] in ('store', 'read') and not torch.is_grad_enabled()), \
+            'feature caching is for sampling: a store or read pass, under torch.no_grad()'
         B, Cx, H, W = x.shape
         device = x.device
         x = x.to(F32).contiguous()
@@ -205,7 +243,7 @@ class Unet(nn.Module):
         out = torch.empty((B, self.channels_out, H, W), dtype=F32, device=device)
         chunks = self._batch_chunks(B, x.is_cuda)
         if len(chunks) == 1:
-            self._forward_body(x, lowres, t, c, ss, out)
+            self._forward_body(x, lowres, t, c, ss, out, deepcache)
             return out
         # The spatial body is per-sample, so batch halves are independent: run them on two streams.  Tensor-core-bound
         # convs of one half then overlap the HBM-bound GroupNorm/cast/epilogue traffic of the other and fill each
@@ -216,7 +254,8 @@ class Unet(nn.Module):
             s.wait_stream(main)
             with torch.cuda.stream(s):
                 self._forward_body(x[b0:b1], lowres[b0:b1] if exists(lowres) else None, t[b0:b1], c[b0:b1],
-                                   {k: v[b0:b1] for k, v in ss.items()}, out[b0:b1])
+                                   {k: v[b0:b1] for k, v in ss.items()}, out[b0:b1],
+                                   None if deepcache is None else (deepcache[0], deepcache[1], deepcache[2] + b0))
         for s in streams:
             main.wait_stream(s)
         return out
@@ -238,7 +277,7 @@ class Unet(nn.Module):
             self._streams_key = key
         return self._streams
 
-    def _forward_body(self, x, lowres, t, c, ss, out):
+    def _forward_body(self, x, lowres, t, c, ss, out, deepcache=None):
         """Stem -> down path -> middle -> up path -> final block/conv for a batch slice; writes NCHW into `out`."""
         from . import layers as _layers
         ops = get_ops()
@@ -250,20 +289,23 @@ class Unet(nn.Module):
         if x.is_cuda:
             _layers._ARENA = _layers.ZeroArena(device, B * (self.dim * max(8, 1)) // 8 * 4 * (2 * n_res + 8))
         try:
-            return self._forward_body_impl(x, lowres, t, c, ss, out, ctx)
+            return self._forward_body_impl(x, lowres, t, c, ss, out, ctx, deepcache)
         finally:
             _layers._ARENA = None
 
-    def _forward_body_impl(self, x, lowres, t, c, ss, out, ctx):
+    def _forward_body_impl(self, x, lowres, t, c, ss, out, ctx, deepcache=None):
         ops = get_ops()
         B, _, H, W = x.shape
         device = x.device
+        mode, cache, row0 = deepcache if exists(deepcache) else (None, None, 0)
+        read = mode == 'read'
 
         # torch.cat((x, lowres_cond_img), dim=1) (Unet.py:397) + CrossEmbedLayer stem (Unet.py:400)
         h = self.init_conv.run_stem(x, lowres)
 
         hiddens = []
-        for pre_downsample, init_block, resnet_blocks, attn_block, post_downsample in self.downs:
+        # a read pass runs level 0 only: its skips are all the last up level pops
+        for pre_downsample, init_block, resnet_blocks, attn_block, post_downsample in self.downs[:1] if read else self.downs:
             if exists(pre_downsample):
                 h = pre_downsample.run(h)
             h = init_block.run(h, t, ctx, ss[init_block])
@@ -272,16 +314,24 @@ class Unet(nn.Module):
                 hiddens.append(h)
             h = attn_block.run(h)
             hiddens.append(h)
-            if exists(post_downsample):
+            if exists(post_downsample) and not read:
                 h = post_downsample.run(h)
 
-        h = self.mid_block1.run(h, t, ctx, ss[self.mid_block1])
-        if exists(self.mid_attn):
-            h = self.mid_attn.run(h)
-        h = self.mid_block2.run(h, t, ctx, ss[self.mid_block2])
+        if not read:
+            h = self.mid_block1.run(h, t, ctx, ss[self.mid_block1])
+            if exists(self.mid_attn):
+                h = self.mid_attn.run(h)
+            h = self.mid_block2.run(h, t, ctx, ss[self.mid_block2])
 
         skip = lambda cur: Cat(cur, hiddens.pop(), self.skip_connect_scale)
-        for init_block, resnet_blocks, attn_block, upsample in self.ups:
+        last = len(self.ups) - 1
+        for level, (init_block, resnet_blocks, attn_block, upsample) in enumerate(self.ups):
+            if read and level < last:
+                continue
+            if level == last and mode == 'store':
+                cache.store(h, row0)
+            elif level == last and read:
+                h = cache.read(row0, B)
             h = init_block.run(skip(h), t, ctx, ss[init_block])
             for resnet_block in resnet_blocks:
                 h = resnet_block.run(skip(h), t, None, ss[resnet_block])
