@@ -325,10 +325,10 @@ class EmuOps:
         if mode == 0:
             out.reshape(-1)[:B * H * W * C].reshape(B, H, W, C).copy_(x.to(out.dtype))     # the kernel writes the first B*H*W rows
         elif mode == 1:
-            out.reshape(B, 2 * H, 2 * W, C).copy_(
+            out.reshape(-1)[:4 * B * H * W * C].reshape(B, 2 * H, 2 * W, C).copy_(
                 x.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2).to(out.dtype))
         else:
-            o = out.reshape(B, 4, H // 2, W // 2, C)
+            o = out.reshape(-1)[:B * H * W * C].reshape(B, 4, H // 2, W // 2, C)
             for p in range(4):
                 o[:, p].copy_(x[:, (p >> 1)::2, (p & 1)::2].to(out.dtype))
 
@@ -505,12 +505,13 @@ class EmuOps:
 
     def step_advance_t(self, t, B):
         self._log("step_advance_t")
-        t.copy_((t - 1).clamp(min=0))
+        t[:B] = (t[:B] - 1).clamp(min=0)                                   # the kernel advances t[:B] only
 
     def step_advance_t_table(self, t, next_t, T, B):
         self._log("step_advance_t_table")
-        inside = (t >= 0) & (t < T)
-        t.copy_(torch.where(inside, next_t[t.clamp(0, T - 1)], torch.zeros_like(t)))
+        tb = t[:B]
+        inside = (tb >= 0) & (tb < T)
+        tb.copy_(torch.where(inside, next_t[tb.clamp(0, T - 1)], torch.zeros_like(tb)))
 
     def step_finalize(self, x, n, unnormalize, out):
         self._log("step_finalize")
@@ -523,9 +524,9 @@ class EmuOps:
 
     def inpaint_advance(self, t, r, next_t, R, T, B):
         self._log("inpaint_advance")
-        nt, nr = advance_ref(t, r, next_t, R, T)
-        t.copy_(nt)
-        r.copy_(nr)
+        nt, nr = advance_ref(t[:B], r[:B], next_t, R, T)
+        t[:B] = nt
+        r[:B] = nr
 
     def inpaint_finalize(self, x, k, m, B, C, hw, unnormalize, out):
         self._log("inpaint_finalize")
@@ -543,7 +544,7 @@ class EmuOps:
         if t is None:
             labels = [int(label)] * B
         else:
-            labels = (t * (int(R[0]) if R is not None else 1) + (r if r is not None else 0)).tolist()
+            labels = (t[:B] * (int(R[0]) if R is not None else 1) + (r[:B] if r is not None else 0)).tolist()
         self.keyed.append((KIND_NAMES[kind], labels, stage))
         z = K.randn_keyed(seeds.tolist()[:B], n, kind, stage, labels, np.float32)
         out.reshape(B, n).copy_(torch.from_numpy(z))

@@ -35,7 +35,7 @@ pytestmark = pytest.mark.gpu
 
 
 # ------------------------------------------------------------------------------------------------ the cases
-def _inputs(cfg, s, b, L=20, seed=3):
+def _inputs(cfg, s, b, L=20, seed=3, device="cuda"):
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(b, 3, s, s, generator=g)
     tm = torch.ones(b, L, dtype=torch.bool)
@@ -44,7 +44,7 @@ def _inputs(cfg, s, b, L=20, seed=3):
     if cfg.get("lowres_cond"):
         kw.update(lowres_cond_img=torch.randn(b, 3, s, s, generator=g), lowres_noise_times=torch.full((b,), 200))
     t = torch.randint(0, 1000, (b,), generator=g)
-    return x.cuda(), t.cuda(), {k: v.cuda() for k, v in kw.items()}
+    return x.to(device), t.to(device), {k: v.to(device) for k, v in kw.items()}
 
 
 def _cases():
@@ -62,25 +62,36 @@ def _cases():
 CASES = list(_cases()) if torch.cuda.is_available() else []
 
 
-@pytest.mark.parametrize("name,cfg,s,b,opt", CASES, ids=[c[0] for c in CASES])
-def test_every_call_of_a_forward(native, name, cfg, s, b, opt):
-    import minimagen_b200.ops as ops_mod
+def forward_case(name, device="cuda"):
+    """(U-Net, x, t, conditioning, b, options) of the forward case `name` of _cases(), on `device`."""
     from minimagen_b200.Unet import Unet
+    _, cfg, s, b, opt = next(c for c in _cases() if c[0] == name)
     torch.manual_seed(0)
-    u = Unet(**cfg).eval().cuda()
-    x, t, kw = _inputs(cfg, s, b)
-    proxy = CheckingOps(native)
-    ops_mod.set_ops(proxy)                      # the `native` fixture restores the previous backend afterwards
-    t0 = time.time()
+    u = Unet(**cfg).eval().to(device)
+    x, t, kw = _inputs(cfg, s, b, device=device)
+    return u, x, t, kw, b, opt
+
+
+def run_forward(ops, u, x, t, kw, b, opt):
+    """One forward of a case with `ops` installed as the backend (left installed: the caller restores it)."""
+    import minimagen_b200.ops as ops_mod
+    ops_mod.set_ops(ops)
     with torch.no_grad():
         if opt.get("cfg_batched"):               # Imagen.cfg_batched: conditional and unconditional pass as one 2B batch
             two = lambda v: torch.cat((v, v))
-            keep = torch.cat((torch.ones(b, dtype=torch.uint8), torch.zeros(b, dtype=torch.uint8))).cuda()
-            out = u._forward_impl(two(x), two(t), cond_keep=keep, **{k: two(v) for k, v in kw.items()})
-        else:
-            u.batch_streams = opt.get("batch_streams", 1)
-            assert len(u._batch_chunks(b, True)) == u.batch_streams
-            out = u(x, t, **kw)
+            keep = torch.cat((torch.ones(b, dtype=torch.uint8), torch.zeros(b, dtype=torch.uint8))).to(x.device)
+            return u._forward_impl(two(x), two(t), cond_keep=keep, **{k: two(v) for k, v in kw.items()})
+        u.batch_streams = opt.get("batch_streams", 1)
+        assert len(u._batch_chunks(b, x.is_cuda)) == u.batch_streams
+        return u(x, t, **kw)
+
+
+@pytest.mark.parametrize("name,cfg,s,b,opt", CASES, ids=[c[0] for c in CASES])
+def test_every_call_of_a_forward(native, name, cfg, s, b, opt):
+    u, x, t, kw, b, opt = forward_case(name)
+    proxy = CheckingOps(native)
+    t0 = time.time()
+    out = run_forward(proxy, u, x, t, kw, b, opt)   # the `native` fixture restores the previous backend afterwards
     torch.cuda.synchronize()
     assert torch.isfinite(out).all()
     n_acc = proxy.assert_accumulators_disjoint()
